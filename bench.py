@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — imagined frames/s of the DIAMOND sampler hot path on B200 (BASELINE.json metric).
+"""bench.py — imagined frames/s of the DIAMOND sampler hot path on H100 (BASELINE.json metric).
 
 A "step" = one DiffusionSampler.sample() call over a batch of `--envs` imagined environments per GPU
 (frame-stack 4 x 64x64x3 fp32 + 4 actions -> next frame, 3 Euler denoising steps = 3 U-Net forwards).
@@ -10,10 +10,12 @@ roofline), `imagination_update` (cfg 3: 32 envs x horizon 15 through WorldModelE
 `gpu_baseline` (the reference's GPU path on this GPU: eager and torch.compile), `cpu_baseline` (its CPU path on the host cores).
 Multi-GPU is weak scaling: imagination needs no collective (SURVEY.md 8e); both training blocks all-reduce their gradients.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--envs B] [--impl native|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--envs B] [--impl native|reference] [--dump-outputs DIR]
 
 Prints ONE JSON line (rank 0).  `--impl reference` times the reference algorithm's CPU path (the oracle port — the
-reference is pure Python and /root/reference does not travel to the GPU box) on the host cores.
+reference is pure Python and is not part of this repository) on the host cores.  `--dump-outputs DIR` writes what the last
+timed sample() returned (rank 0) as DIR/<name>.npy in float32; the noise is seeded, so the same arguments give the same
+inputs on every run and two builds can be compared output for output.
 """
 import argparse
 import json
@@ -38,7 +40,7 @@ def load_peaks():
             p = json.load(f)
         return p, "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet (dense, 700 W)"
 
 
 class ClockSampler(threading.Thread):
@@ -145,23 +147,19 @@ def run_reference(args):
     torch.set_num_threads(cores)
     cfg, sc = O.DenoiserCfg(inner=inner), O.SamplerCfg(3)
     obs, act, x0 = O.synthetic_inputs(envs, inner, 64, 64, 5)
-    steps = min(args.steps, 8)  # bounded: K x 32 envs x 3 U-Net forwards on the host cores
-    warmups = 0
+    steps, warmups = args.steps, args.warmup   # exactly as given: K x `envs` x 3 U-Net forwards on the host cores
+    result = None
     with torch.no_grad():
-        for _ in range(max(1, min(args.warmup, 2))):
-            t0 = time.perf_counter()
+        for _ in range(warmups):
             O.sample(obs, act, x0, sd, cfg, sc)
-            t_one = time.perf_counter() - t0
-            warmups += 1
-            if t_one > 15.0:      # a host shared with other jobs: keep the whole arm within ~2 minutes
-                break
-        steps = max(1, min(steps, int(90.0 / max(t_one, 1e-3))))
         t0 = time.perf_counter()
         for _ in range(steps):
-            O.sample(obs, act, x0, sd, cfg, sc)
+            result = O.sample(obs, act, x0, sd, cfg, sc)
         dt = time.perf_counter() - t0
+    if args.dump_outputs and result is not None:
+        dump_outputs(args.dump_outputs, result)
     val = envs * steps / dt
-    sample = f"{envs} envs x {steps} sample() calls (the full {args.envs}-env workload per step; steps capped at 8 and at ~90 s of work), torch {torch.__version__} CPU fp32, {cores} threads (fastest of 8/16/32/64/{avail} available)"
+    sample = f"{envs} envs x {steps} sample() calls, torch {torch.__version__} CPU fp32, {cores} threads (fastest of 8/16/32/64/{avail} available)"
     print(json.dumps({
         "impl": "reference", "metric": METRIC, "value": val, "unit": "frames/s", "n_gpus": args.gpus, "steps": steps,
         "warmup": warmups, "ms_per_step": 1e3 * dt / steps, "higher_is_better": True, "scaling": "weak",
@@ -215,7 +213,7 @@ def conv_roofline(dev, envs, peaks, peaks_src):
     wt = (torch.randn(64, 64, 3, 3, generator=g) / 24).to(dev)
     wpk, cp = ops.pack_conv_weight(wt, 64, trs=TRS)
     bias = torch.zeros(64, device=dev)
-    nset = 6  # rotating operand / output sets: 6 x (17 MB operand + 33.5 MB output) at 32 envs > 126 MB L2
+    nset = 6  # rotating operand / output sets: 6 x (17 MB operand + 33.5 MB output) at 32 envs > 50 MB L2
     xs = [torch.randn(envs, 64, 64, 64, device=dev) for _ in range(nset)]
     film = torch.randn(envs, 128, device=dev) * 0.1
     sts = [ops.gn_stats(x, 32) for x in xs]
@@ -260,25 +258,25 @@ def conv_roofline(dev, envs, peaks, peaks_src):
     flops = 2.0 * 576 * 64 * 4096 * envs
     traffic, traffic_src = conv_traffic_from_profile()
     achieved = flops / (ms * 1e-3) / 1e12
-    peak = float(peaks.get("bf16_tflops", 1590.0))
-    return {"bound": "tensor", "kernel": ("conv_tc_kernel<256,3> (tap-row-stacked: 3 MMAs of N=192 per slab)" if TRS else "conv_tc_kernel<64,0> (tap-major: 9 MMAs of N=64 per slab)") + " 3x3 64->64 @64x64 on a PLC16 fp16 operand, bias + GroupNorm-stats epilogue",
+    peak = float(peaks.get("bf16_tflops", 989.0))
+    return {"bound": "tensor", "kernel": "conv_tc_kernel<64> (9 wgmma of N=64 per slab and warpgroup" + (", tap-row-stacked weights)" if TRS else ")") + " 3x3 64->64 @64x64 on a PLC16 fp16 operand, bias + GroupNorm-stats epilogue",
             "prep_us_per_launch": ms_prep * 1e3,
             # the operand pass that precedes every conv (GroupNorm / FiLM / SiLU -> fp16 PLC16): HBM-bound; algorithmic bytes =
             # 256 B read (fp32 NHWC, 64 channels) + 128 B written per pixel
             "prep": {"bound": "hbm", "kernel": "prep_fast_kernel<8,0>", "achieved": (256.0 + 128.0) * 4096.0 * envs / (ms_prep * 1e-3) / 1e9,
-                     "peak": float(peaks.get("hbm_gbs", 6650.0)), "unit": "GB/s",
-                     "frac": (256.0 + 128.0) * 4096.0 * envs / (ms_prep * 1e-3) / 1e9 / float(peaks.get("hbm_gbs", 6650.0))},
+                     "peak": float(peaks.get("hbm_gbs", 3350.0)), "unit": "GB/s",
+                     "frac": (256.0 + 128.0) * 4096.0 * envs / (ms_prep * 1e-3) / 1e9 / float(peaks.get("hbm_gbs", 3350.0))},
             "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
             "traffic": traffic, "traffic_source": traffic_src, "algorithmic_bytes": (128 * 1.0 + 256) * 4096.0 * envs,
             "us_per_launch": ms * 1e3, "flop_per_launch": flops, "peak_source": peaks_src + " bf16 burst (fp16 and bf16 share the tensor-pipe rate)"}
 
 
 def gpu_baseline(dev, envs: int, steps: int = 5):
-    """The reference's own GPU path on this B200 (what north_star's ">= 50x" is stated against, SURVEY.md 8d): the oracle
+    """The reference's own GPU path on this GPU (what north_star's ">= 50x" is stated against, SURVEY.md 8d): the oracle
     port of DiffusionSampler.sample (same torch ops as the reference modules: cuDNN convs, ATen norms, cuBLAS linears) on
     `dev`, fp32 with TF32 matmul (src/trainer.py:41), in the reference's two modes: eager, and the per-step denoise under
-    torch.compile(mode="reduce-overhead") (src/trainer.py:182-184, its default).  /root/reference cannot travel to the GPU
-    box, so the port stands in for it; it runs the reference's per-step device->host syncs (diffusion_sampler.py:39,47)."""
+    torch.compile(mode="reduce-overhead") (src/trainer.py:182-184, its default).  The reference is not part of this
+    repository, so the port stands in for it; it runs the reference's per-step device->host syncs (diffusion_sampler.py:39,47)."""
     import torch
 
     O, inner, sd = build_oracle_model()
@@ -339,13 +337,14 @@ def gpu_baseline(dev, envs: int, steps: int = 5):
     return out
 
 
-def conv_traffic_from_profile():
-    """roofline.traffic = dram__bytes_read.sum + dram__bytes_write.sum of conv_tc_kernel, parsed from the newest committed
-    `profiles/r*_prof_conv_*_summary.csv` (one `ncu --set full` capture of the same kernel); None when no capture exists."""
+def conv_traffic_from_profile(root=ROOT):
+    """roofline.traffic = dram__bytes_read.sum + dram__bytes_write.sum of conv_tc_kernel, parsed from the newest
+    `profiles/r*_prof_conv_*_summary.csv` under `root` (one `ncu --set full` capture of the same kernel); None when no capture
+    exists."""
     import csv
     import glob
 
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_prof_conv_*_summary.csv")))
+    files = sorted(glob.glob(os.path.join(root, "profiles", "r*_prof_conv_*_summary.csv")))
     for path in reversed(files):
         try:
             vals = {}
@@ -357,7 +356,7 @@ def conv_traffic_from_profile():
                             mult = {"byte": 1.0, "kbyte": 1e3, "mbyte": 1e6, "gbyte": 1e9}.get(unit, 1.0)
                             vals[cell] = num * mult
             if len(vals) == 2:
-                return vals["dram__bytes_read.sum"] + vals["dram__bytes_write.sum"], os.path.relpath(path, ROOT)
+                return vals["dram__bytes_read.sum"] + vals["dram__bytes_write.sum"], os.path.relpath(path, root)
         except Exception:
             continue
     return None, None
@@ -492,7 +491,7 @@ def imagination_block(dev, world, rank, envs=32, horizon=15, updates=3, warmup=1
 
 
 def wgrad_roofline(dev, batch, peaks):
-    """tcgen05 wgrad kernel, 3x3 64->64 at 64x64 over `batch` images (the dominant backward-filter shape), timed alone."""
+    """wgmma wgrad kernel, 3x3 64->64 at 64x64 over `batch` images (the dominant backward-filter shape), timed alone."""
     import torch
 
     from diamond_b200 import ops
@@ -513,7 +512,7 @@ def wgrad_roofline(dev, batch, peaks):
     torch.cuda.synchronize()
     us = e0.elapsed_time(e1) / reps * 1e3
     flops = 2.0 * 576 * 64 * 4096 * batch
-    peak = float(peaks.get("bf16_tflops", 1590.0))
+    peak = float(peaks.get("bf16_tflops", 989.0))
     return {"kernel": "wgrad_tc_kernel + fixed-order reduce, 3x3 64->64 @64x64, %d images" % batch, "us_per_launch": us,
             "achieved": flops / (us * 1e-6) / 1e12, "peak": peak, "unit": "TFLOP/s", "frac": flops / (us * 1e-6) / 1e12 / peak}
 
@@ -550,6 +549,20 @@ class SecondaryBlocks:
             timer.cancel()
 
 
+def dump_outputs(out_dir, result):
+    """What the last timed sample() returned: the next frame and the denoising trajectory (B x 3 x 64 x 64 fp32 each).  At most
+    64 MB in all: a larger batch is cut to its first environments."""
+    import numpy as np
+
+    x, traj = result
+    arrays = {"next_obs": x, **{f"trajectory_{i}": t for i, t in enumerate(traj)}}
+    per_env = sum(t[0].numel() * 4 for t in arrays.values())
+    n = max(1, min(x.shape[0], (64 << 20) // per_env))
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t[:n].float().cpu().numpy())
+
+
 def run_native(args):
     import torch
     import torch.distributed as dist
@@ -568,7 +581,7 @@ def run_native(args):
     dev = torch.device("cuda", local)
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
-    lib = _lib.lib()  # no fallback: raises if the sm_100a library is missing
+    lib = _lib.lib()  # no fallback: raises if the sm_90a library is missing
 
     from diamond_b200.synthetic import randomize_module_
 
@@ -577,6 +590,7 @@ def run_native(args):
     den = den.to(dev).eval()
     sampler = DiffusionSampler(den, DiffusionSamplerConfig(3))
     B = args.envs
+    torch.manual_seed(1234 + rank)  # the initial noise of every sample(): same arguments, same inputs
     obs, act = rank_inputs(B, rank)
     obs_d, act_d = obs.to(dev), act.to(dev)
     obs_h, act_h = obs.pin_memory(), act.pin_memory()
@@ -595,17 +609,20 @@ def run_native(args):
     lib.dmd_launch_count(1)
     evs = []
     t_wall0 = time.perf_counter()
+    result = None
     for _ in range(args.steps):
         flush.zero_()
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
-        sampler.sample(obs_d, act_d)
+        result = sampler.sample(obs_d, act_d)
         b.record()
         evs.append((a, b))
     barrier()
     t_wall = time.perf_counter() - t_wall0
     launches = int(lib.dmd_launch_count(0))
     dev_ms = sum(a.elapsed_time(b) for a, b in evs)
+    if args.dump_outputs and rank == 0 and result is not None:
+        dump_outputs(args.dump_outputs, result)
 
     # ---- end to end through the public API with host buffers (H2D of the frame stack + actions, D2H of the frame)
     for _ in range(3):
@@ -641,7 +658,7 @@ def run_native(args):
                     "d2h_bytes_per_step": int(out_h.numel() * 4)},
             "gpu_launches": launches, "clocks": clocks, "roofline": roof,
             "model_flop_util": {"gflop_per_frame": GFLOP_PER_FRAME, "achieved_tflops": value * GFLOP_PER_FRAME / 1e3 / world,
-                                "frac_of_peak": value * GFLOP_PER_FRAME / 1e3 / world / float(peaks.get("bf16_tflops_sustained", 1400.0))},
+                                "frac_of_peak": value * GFLOP_PER_FRAME / 1e3 / world / float(peaks.get("bf16_tflops_sustained", 989.0))},
             "wall_s_timed_loop": t_wall,
             "parity": {"tolerance": "1e-3 RELATIVE L2 over the whole pre-quantisation model-output tensor vs the reference-pinned oracle "
                                     "(not max-per-element); outputs behind the truncating uint8 quantiser: never more than one level off",
@@ -699,8 +716,11 @@ def main():
     ap.add_argument("--skip-train", action="store_true", help="omit the denoiser-training block (cfg 2)")
     ap.add_argument("--train-batch", type=int, default=256, help="denoiser training batch per GPU (config/trainer.yaml: 32; BASELINE cfg 2: 256)")
     ap.add_argument("--skip-gpu-baseline", action="store_true", help="omit the reference-GPU-path leg (eager + torch.compile of the oracle port)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     ap.add_argument("--secondary-budget", type=float, default=200.0, help="seconds shared by the blocks that follow the headline numbers (training, imagination, baselines); ~55 s are used on a healthy box")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,4 +1,4 @@
-"""diamond_b200 — B200-native (sm_100a) implementation of DIAMOND's data-parallel hot path.
+"""diamond_b200 — GPU-native (H100, sm_90a) implementation of DIAMOND's data-parallel hot path.
 
 Host code is Python/PyTorch and mirrors the reference's module surface (eloialonso/diamond, src/models/...);
 every conv / norm / attention / SiLU on the path runs in hand-written CUDA kernels behind the C ABI declared in

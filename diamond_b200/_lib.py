@@ -66,7 +66,7 @@ class WgradDesc(C.Structure):  # dmd_wgrad_desc
 
 
 class ConvPlanInfo(C.Structure):  # dmd_conv_plan_info
-    _fields_ = [("tiles", _i), ("kslabs", _i), ("stages", _i), ("tmem_cols", _i),
+    _fields_ = [("tiles", _i), ("kslabs", _i), ("stages", _i), ("acc_cols", _i),
                 ("smem_bytes", C.c_ulonglong), ("weight_bytes", C.c_ulonglong)]
 
 

@@ -1,4 +1,4 @@
-// libdiamond_b200.so — C ABI (include/diamond_b200.h) over the sm_100a kernels.
+// libdiamond_b200.so — C ABI (include/diamond_b200.h) over the sm_90a kernels.
 #include <cstdlib>
 #include <memory>
 #include <mutex>
@@ -15,7 +15,6 @@
 #include "../../include/diamond_b200.h"
 #include "aux_kernels.cuh"
 #include "conv_tc.cuh"
-#include "conv_fused.cuh"
 #include "wgrad_tc.cuh"
 #include "bwd_kernels.cuh"
 
@@ -91,6 +90,9 @@ extern "C" int dmd_ktrace_end(long long* stamps, int capacity) {
 extern "C" const char* dmd_ktrace_name(int i) { return (i >= 0 && i < (int)g_kt_names.size()) ? g_kt_names[i].c_str() : ""; }
 
 static inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
+// SM count of the H100 SXM the launch shapes of the memory-bound kernels are planned for (grids of >= 2 blocks per SM).  A plan
+// does not depend on the device it is built on, so host-only planning (dmd_prep_plan) gives the same answer as a launch.
+constexpr int kPlanSms = 132;
 static inline int gn_group_size(int C) {  // blocks.py:12,27: num_groups = max(1, C // 32)
   int G = C / 32 > 1 ? C / 32 : 1;
   return C / G;
@@ -116,9 +118,10 @@ static int tune_int(const char* name, int dflt) {
   return r;
 }
 
-static int conv_fill(const dmd_conv_desc* d, ConvParams* p, size_t* smem, int* tmem_cols) {
+static int conv_fill(const dmd_conv_desc* d, ConvParams* p, size_t* smem, int* acc_cols) {
   DMD_CHECK(d->src0 && d->out && d->wpk, "conv: null src0/out/wpk");
   DMD_CHECK(d->taps == 9 || d->taps == 1, "conv: taps must be 1 or 9 (got %d)", d->taps);
+  DMD_CHECK(d->debug == 0 && d->debug_buf == nullptr, "conv: debug / debug_buf must be 0 / NULL (the kernel has no bring-up switches)");
   DMD_CHECK(d->stride == 1 || d->stride == 2, "conv: stride must be 1 or 2");
   DMD_CHECK(d->C0 > 0 && d->C0 % 16 == 0 && d->C1 % 16 == 0 && d->C0 + d->C1 <= kMaxCin, "conv: operand channels must be multiples of 16, total <= %d (C0=%d C1=%d)", kMaxCin, d->C0, d->C1);
   DMD_CHECK((d->C1 == 0) == (d->src1 == nullptr), "conv: src1/C1 mismatch");
@@ -159,17 +162,14 @@ static int conv_fill(const dmd_conv_desc* d, ConvParams* p, size_t* smem, int* t
   if (d->stride == 2) DMD_CHECK(p->H % 2 == 0 && p->W % 2 == 0, "conv: stride 2 needs even H,W");
   p->wpk = reinterpret_cast<const __half*>(d->wpk); p->bias = d->bias; p->Cout = d->Cout; p->CoutPad = d->CoutPad;
   p->resid = d->residual; p->out = d->out; p->ostats = d->out_stats; p->ogs = d->out_gs > 0 ? d->out_gs : d->Cout;
-  p->dbg = d->debug; p->dbg_buf = (long long*)d->debug_buf;
   const Plc g = plc_geometry(d->B, d->H, d->W);
   p->PW = g.PW; p->PH = g.PH; p->Q = g.Q; p->G = g.G; p->plane_bytes = (unsigned long long)g.Qalloc * 16;
   DMD_CHECK((long long)g.Q * (g.PW > g.PH ? g.PW : g.PH) < (1ll << 32), "conv: problem too large for 32-bit position math");
-  // tap-row-stacked mode (TrsEpilogue, conv_tc.cuh): weights packed with dmd_pack_conv_weight(precise = 3)
+  // tap-row-stacked weights: dmd_pack_conv_weight(precise = 3); the kernel addresses tap (dy, dx) inside kernel row dy
   p->trs = d->wpk_layout == 1 ? 1 : 0;
   if (p->trs) DMD_CHECK(d->taps == 9 && !d->precise && 3 * d->CoutPad <= 256, "conv: row-stacked weights need a 3x3, non-split conv with CoutPad <= 80");
-  p->tile_stride = p->trs ? 126 : kTileM;
-  const int halo = p->trs ? g.PW : (d->taps == 9 ? g.PW + 1 : 0);
+  const int halo = d->taps == 9 ? g.PW + 1 : 0;
   p->P = kTileM + 2 * halo; p->Palloc = p->P | 1;
-  if (tune_int("DMD_CONV_PALLOC8", 0)) p->Palloc = round_up(p->P, 8);   // experiment: 128-byte aligned slab / chunk bases
   if (d->out_stats) {
     const int L4 = d->Cout / 4;
     DMD_CHECK(g.PH * g.PW >= 64, "conv: image too small for the statistics epilogue (a tile may touch at most %d images)", kStatSlots);
@@ -178,33 +178,19 @@ static int conv_fill(const dmd_conv_desc* d, ConvParams* p, size_t* smem, int* t
     DMD_CHECK(d->Cout % d->out_gs == 0 && d->Cout / d->out_gs <= kMaxOutGroups, "conv: bad output groups");
   }
   p->dPW.init(g.PW); p->dPH.init(g.PH);
-  p->num_tiles = (g.Q + p->tile_stride - 1) / p->tile_stride;
-  // slab ring: everything that fits next to the resident weights, at most four tiles' worth.  Two epilogue groups (each with
-  // its own staging tile) when the ring still gets >= 4 slabs and a CTA sees at least two tiles; else one group.
+  p->num_tiles = (g.Q + kTileM - 1) / kTileM;
+  // slab ring: everything that fits next to the resident weights (227 KB of shared memory per block), at most four tiles' worth
   const int kslabs = p->Cin / 16 + p->xslabs;
   const uint32_t w_bytes = conv_weight_bytes(p->taps, p->Cin, p->Cextra, p->CoutPad);
-  // epilogue organisation: direct (0) unless switched off (DMD_CONV_EPI=0) or a warp's columns would span several GroupNorm groups
-  const bool direct = tune_int("DMD_CONV_EPI", 1) != 0 && (!d->out_stats || d->CoutPad <= 64);
-  if (p->trs) DMD_CHECK(!d->out_stats || d->CoutPad <= 64, "conv: row-stacked mode computes statistics for CoutPad <= 64");
-  int groups = p->trs ? 3 : (direct ? 0 : (tune_int("DMD_CONV_GROUPS", 2) >= 2 ? 2 : 1));
-  int stages = 0;
-  for (;; groups = 1) {
-    const ConvSmemLayout L0 = conv_smem_layout(w_bytes, p->CoutPad, p->Palloc, 0, groups);
-    const long long budget = 227ll * 1024 - (long long)L0.total;
-    stages = budget > 0 ? (int)(budget / (long long)L0.slab_bytes) : 0;
-    if (groups <= 1 || groups == 3 || stages >= (kslabs < 4 ? kslabs + 1 : 4)) break;
-  }
+  const ConvSmemLayout L0 = conv_smem_layout(w_bytes, p->Palloc, 0);
+  const long long budget = 227ll * 1024 - (long long)L0.total;
+  int stages = budget > 0 ? (int)(budget / (long long)L0.slab_bytes) : 0;
   if (stages > 4 * kslabs) stages = 4 * kslabs;
   if (stages > kMaxStages) stages = kMaxStages;
-  { const int cap = tune_int("DMD_CONV_MAX_STAGES", kMaxStages); if (cap >= 2 && stages > cap) stages = cap; }
   DMD_CHECK(stages >= 2, "conv: shared memory too small for W=%d Cin=%d CoutPad=%d", p->W, p->Cin, p->CoutPad);
   p->stages = stages;
-  p->egroups = groups;
-  // row-stacked mode: two epilogue groups on alternate tiles once a CTA sees more than one tile
-  p->trs_groups = (p->trs && tune_int("DMD_TRS_GROUPS", 2) == 2 && p->num_tiles > 148) ? 2 : 1;
-  *smem = conv_smem_layout(w_bytes, p->CoutPad, p->Palloc, stages, groups).total;
-  *tmem_cols = d->CoutPad <= 32 ? 32 : (d->CoutPad <= 64 ? 64 : 128);
-  if (p->trs) *tmem_cols = 3 * d->CoutPad <= 64 ? 64 : (3 * d->CoutPad <= 128 ? 128 : 256);   // accumulator = three column blocks
+  *smem = conv_smem_layout(w_bytes, p->Palloc, stages).total;
+  *acc_cols = d->CoutPad <= 16 ? 16 : (d->CoutPad <= 32 ? 32 : (d->CoutPad <= 64 ? 64 : 128));   // wgmma N: a power of two
   return 0;
 }
 
@@ -224,22 +210,17 @@ static int init_kernels() {
   if (it == states.end()) {
     DevState st;
     DMD_CUDA(cudaDeviceGetAttribute(&st.num_sms, cudaDevAttrMultiProcessorCount, dev));
-    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<64, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<128, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<256, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<32, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<64, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<128, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<16, 9>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<32, 9>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<64, 9>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<128, 9>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<16, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<32, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<128, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<32, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<128, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(conv_fused_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(conv_fused_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(conv_fused_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    DMD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    DMD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    DMD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(attn_cluster_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(attn_cluster_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(attn_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
@@ -280,8 +261,7 @@ static int conv_launch_t(const ConvParams& p0, size_t smem, cudaStream_t st) {
   const int grid = p0.num_tiles < g_num_sms ? p0.num_tiles : g_num_sms;  // persistent: one CTA per SM
   ConvParams p = p0;
   p.ktrace = kt_slot(p.taps == 9 ? "conv3x3" : "conv1x1", p.num_tiles, (p.Cin + p.Cextra) * 1000 + p.W);
-  if (p.egroups == 0) return launch_pdl(conv_tc_kernel<kCols, 0>, dim3(grid), dim3(kConvThreads), smem, st, p);
-  if (p.egroups == 2) return launch_pdl(conv_tc_kernel<kCols, 2>, dim3(grid), dim3(kConvThreads), smem, st, p);
+  if (p.taps == 9) return launch_pdl(conv_tc_kernel<kCols, 9>, dim3(grid), dim3(kConvThreads), smem, st, p);
   return launch_pdl(conv_tc_kernel<kCols, 1>, dim3(grid), dim3(kConvThreads), smem, st, p);
 }
 
@@ -321,7 +301,7 @@ static int prep_fill(const dmd_prep_desc* d, PrepParams* p, int* nsrc) {
   DMD_CHECK(g.PH * g.PW >= 32, "prep: image too small");
   // a block touches at most 2 images; low-resolution levels get smaller blocks so that the grid still covers the SMs
   int ppb = g.PH * g.PW >= 256 ? 256 : (g.PH * g.PW / 32) * 32;
-  while (ppb > 64 && (g.Qalloc + ppb - 1) / ppb < tune_int("DMD_PREP_MIN_BLOCKS", 2 * 148)) ppb >>= 1;
+  while (ppb > 64 && (g.Qalloc + ppb - 1) / ppb < tune_int("DMD_PREP_MIN_BLOCKS", 2 * kPlanSms)) ppb >>= 1;
   ppb = (ppb / 32) * 32;
   p->pos_per_block = ppb;
   DMD_CHECK(d->C0 / (d->gs0 > 0 ? d->gs0 : 8) <= 4 || d->mode == 0, "prep: at most 4 groups per source");
@@ -366,7 +346,7 @@ extern "C" int dmd_conv_plan(const dmd_conv_desc* d, dmd_conv_plan_info* out) {
   DMD_CHECK(d && out, "conv_plan: null argument");
   ConvParams p; size_t smem; int cols;
   if (conv_fill(d, &p, &smem, &cols)) return 1;
-  out->tiles = p.num_tiles; out->kslabs = p.Cin / 16 + p.xslabs; out->stages = p.stages; out->tmem_cols = cols;
+  out->tiles = p.num_tiles; out->kslabs = p.Cin / 16 + p.xslabs; out->stages = p.stages; out->acc_cols = cols;
   out->smem_bytes = smem; out->weight_bytes = conv_weight_bytes(p.taps, p.Cin, p.Cextra, p.CoutPad);
   return 0;
 }
@@ -376,36 +356,12 @@ extern "C" int dmd_prep_act(const dmd_prep_desc* d, void* stream) {
   return prep_launch(p, nsrc, (cudaStream_t)stream);
 }
 
-static int conv_launch_trs(const ConvParams& p0, size_t smem, int tmem_cols, cudaStream_t st) {
-  if (init_kernels()) return 1;
-  const int grid = p0.num_tiles < g_num_sms ? p0.num_tiles : g_num_sms;
-  ConvParams p = p0;
-  p.ktrace = kt_slot("conv3x3rs", p.num_tiles, (p.Cin + p.Cextra) * 1000 + p.W);
-  switch (tmem_cols) {
-    case 64: return launch_pdl(conv_tc_kernel<64, 3>, dim3(grid), dim3(kConvThreads), smem, st, p);
-    case 128: return launch_pdl(conv_tc_kernel<128, 3>, dim3(grid), dim3(kConvThreads), smem, st, p);
-    default: return launch_pdl(conv_tc_kernel<256, 3>, dim3(grid), dim3(kConvThreads), smem, st, p);
-  }
-}
-
-static int conv_launch(const ConvParams& p, size_t smem, int tmem_cols, cudaStream_t st) {
-  if (p.trs) return conv_launch_trs(p, smem, tmem_cols, st);
-  switch (tmem_cols) {
+static int conv_launch(const ConvParams& p, size_t smem, int acc_cols, cudaStream_t st) {
+  switch (acc_cols) {
+    case 16: return conv_launch_t<16>(p, smem, st);
     case 32: return conv_launch_t<32>(p, smem, st);
     case 64: return conv_launch_t<64>(p, smem, st);
     default: return conv_launch_t<128>(p, smem, st);
-  }
-}
-
-static int fused_launch(const FusedParams& f0, size_t smem, int tmem_cols, cudaStream_t st) {
-  if (init_kernels()) return 1;
-  FusedParams f = f0;
-  f.c.ktrace = kt_slot(f.c.taps == 9 ? "fused3x3" : "fused1x1", f.c.num_tiles, (f.c.Cin + f.c.Cextra) * 1000 + f.c.W);
-  const dim3 grid(f.c.num_tiles), block(kConvThreads);
-  switch (tmem_cols) {
-    case 32: return launch_pdl(conv_fused_kernel<32>, grid, block, smem, st, f);
-    case 64: return launch_pdl(conv_fused_kernel<64>, grid, block, smem, st, f);
-    default: return launch_pdl(conv_fused_kernel<128>, grid, block, smem, st, f);
   }
 }
 
@@ -416,11 +372,11 @@ extern "C" int dmd_conv2d_fprop(const dmd_conv_desc* d, void* stream) {
 }
 
 // ---------------------------------------------------------------------------------------------- wgrad launcher
-// Fills the tcgen05 weight-gradient launch for one (gradient operand, activation operand) pair.  grad: PLC16, Cg stored
+// Fills the wgmma weight-gradient launch for one (gradient operand, activation operand) pair.  grad: PLC16, Cg stored
 // channels (<= 64); act: PLC16, Ca stored channels (16 / 32 / 64), both over B images of H x W (conv INPUT size; a
 // stride-2 conv passes its zero-inserted gradient).
 struct WgradLaunch { WgradParams wp; WgradReduceParams rp; size_t smem; int grid; };
-static size_t wgrad_partial_bytes(int num_sms) { return (size_t)num_sms * kWgMaxMma * kTileM * 64 * sizeof(float); }
+static size_t wgrad_partial_bytes(int num_sms) { return (size_t)num_sms * kWgTaps * 64 * 64 * sizeof(float); }
 
 static int wgrad_fill(const void* grad, int Cg, const void* act, int Ca, int B, int H, int W, int taps, float* partial,
                       int Cout, int Cin, int CinTot, int ci_off, const float* inv_scale, int accumulate, int debug, WgradLaunch* L) {
@@ -435,47 +391,34 @@ static int wgrad_fill(const void* grad, int Cg, const void* act, int Ca, int B, 
   const size_t plane = (size_t)g.Qalloc * 16;
   WgradParams& wp = L->wp;
   const int ng = Cg / 8;
-  for (int k = 0; k < 16; ++k) {
-    const int j = k & 7;
-    const bool second = k >= 8;
-    wp.a_plane[k] = (j < ng && !(second && taps == 1)) ? (const uint8_t*)grad + (size_t)j * plane : nullptr;
-    wp.a_shift[k] = second ? -g.PW : 0;
-  }
+  for (int j = 0; j < 8; ++j) wp.a_plane[j] = j < ng ? (const uint8_t*)grad + (size_t)j * plane : nullptr;
   wp.zeros = g_zeros;
   wp.nB = Ca / 8;
   for (int j = 0; j < wp.nB; ++j) wp.b_plane[j] = (const uint8_t*)act + (size_t)j * plane;
-  WgradReduceParams& rp = L->rp;
-  for (int i = 0; i < kWgMaxMma; ++i) rp.tap_of[i][0] = rp.tap_of[i][1] = -1;
-  if (taps == 9) {
-    wp.n_mma = 6; wp.halo = g.PW + 1;
-    for (int i = 0; i < 3; ++i) {
-      wp.b_shift[i] = -g.PW - 1 + i;      // rows 0-63: tap (ky = 0, kx = i); rows 64-127 (window shifted by -PW): tap (1, i)
-      rp.tap_of[i][0] = i; rp.tap_of[i][1] = 3 + i;
-      wp.b_shift[3 + i] = g.PW - 1 + i;   // rows 0-63: tap (2, i); rows 64-127 unused
-      rp.tap_of[3 + i][0] = 6 + i;
-    }
-  } else {
-    wp.n_mma = 1; wp.halo = 0; wp.b_shift[0] = 0; rp.tap_of[0][0] = 0;
-  }
+  wp.taps = taps; wp.PW = g.PW; wp.halo = taps == 9 ? g.PW + 1 : 0;
   wp.G = g.G; wp.num_tiles = (g.Q + kTileM - 1) / kTileM; wp.Pb = kTileM + 2 * wp.halo;
   const WgradSmem one = wgrad_smem(wp.nB, wp.halo, 1);
-  int stages = (int)((227ll * 1024 - 512) / (long long)(one.a_bytes + one.b_bytes));
+  int stages = (int)((227ll * 1024 - 256) / (long long)(one.a_bytes + one.b_bytes));
   if (stages > kWgStagesMax) stages = kWgStagesMax;
   DMD_CHECK(stages >= 2, "wgrad: image too wide for the shared-memory stage (W=%d)", W);
   wp.stages = stages;
   wp.partial = partial; wp.dbg = debug;
   L->smem = wgrad_smem(wp.nB, wp.halo, stages).total;
   L->grid = wp.num_tiles < g_num_sms ? wp.num_tiles : g_num_sms;
-  rp.partial = partial; rp.nparts = L->grid; rp.n_mma = wp.n_mma; rp.N = Ca;
+  WgradReduceParams& rp = L->rp;
+  rp.partial = partial; rp.nparts = L->grid; rp.N = Ca;
   rp.Cout = Cout; rp.Cin = Cin; rp.CinTot = CinTot; rp.ci_off = ci_off; rp.taps = taps;
   rp.inv_scale = inv_scale; rp.accumulate = accumulate;
   return 0;
 }
 static int wgrad_launch(const WgradLaunch& L, float* dW, cudaStream_t st) {
-  if (launch_pdl(wgrad_tc_kernel, dim3(L.grid), dim3(kWgThreads), L.smem, st, L.wp)) return 1;
+  const int N = L.wp.nB * 8;
+  if (N == 16) { if (launch_pdl(wgrad_tc_kernel<16>, dim3(L.grid), dim3(kWgThreads), L.smem, st, L.wp)) return 1; }
+  else if (N == 32) { if (launch_pdl(wgrad_tc_kernel<32>, dim3(L.grid), dim3(kWgThreads), L.smem, st, L.wp)) return 1; }
+  else if (launch_pdl(wgrad_tc_kernel<64>, dim3(L.grid), dim3(kWgThreads), L.smem, st, L.wp)) return 1;
   WgradReduceParams rp = L.rp;
   rp.dW = dW;
-  const int total = rp.n_mma * 2 * 64 * rp.N;
+  const int total = rp.taps * 64 * rp.N;
   wgrad_reduce_kernel<<<(total + 63) / 64, 256, 0, st>>>(rp);
   DMD_LAUNCH_OK();
   return 0;
@@ -561,9 +504,9 @@ static int linear_launch(const float* in, const float* W, const float* bias, flo
   // enough blocks to cover the SMs: 8, 16 or 32 output features per block
   const int by = (B + 31) / 32;
   const int forceJ = tune_int("DMD_LINEAR_J", 0);
-  if (forceJ == 4 || (forceJ == 0 && (long long)((F + 31) / 32) * by >= 296))
+  if (forceJ == 4 || (forceJ == 0 && (long long)((F + 31) / 32) * by >= 2 * kPlanSms))
     linear_kernel<4><<<dim3((F + 31) / 32, by), 256, (size_t)(32 + 32) * kLinChunk * sizeof(float), st>>>(in, W, bias, out, B, K, F, silu, accumulate, hw_perm);
-  else if (forceJ == 2 || (forceJ == 0 && (long long)((F + 15) / 16) * by >= 148))
+  else if (forceJ == 2 || (forceJ == 0 && (long long)((F + 15) / 16) * by >= kPlanSms))
     linear_kernel<2><<<dim3((F + 15) / 16, by), 256, (size_t)(16 + 32) * kLinChunk * sizeof(float), st>>>(in, W, bias, out, B, K, F, silu, accumulate, hw_perm);
   else
     linear_kernel<1><<<dim3((F + 7) / 8, by), 256, (size_t)(8 + 32) * kLinChunk * sizeof(float), st>>>(in, W, bias, out, B, K, F, silu, accumulate, hw_perm);
@@ -594,7 +537,7 @@ extern "C" int dmd_nhwc_to_nchw(const float* in, float* out, int B, int C, int C
 static int resize_launch(const ResizeParams& p, cudaStream_t st) {
   const long long total = (long long)p.B * p.Hd * p.Wd * (p.C / 4);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kPlanSms * 16) blocks = kPlanSms * 16;
   resize_nhwc_kernel<<<(int)blocks, 256, 0, st>>>(p);
   DMD_LAUNCH_OK();
   if (p.stats) return dmd_gn_stats(p.dst, p.stats, p.B, p.Hd * p.Wd, p.C, p.gs, st);
@@ -626,16 +569,14 @@ struct ResBlockW {
 
 struct Tens { float* data; double* stats; int C, H, W, gs; float* grad = nullptr; int gid = -1; };
 
-enum OpKind { OP_CONV = 0, OP_ATTN = 1, OP_PREP = 2, OP_FUSED = 3, OP_RESIZE = 4 };
-struct Op { int kind; ConvParams conv; size_t smem; int cols; AttnParams attn; PrepParams prep; int prep_nsrc; FusedParams fused; ResizeParams rs; };
+enum OpKind { OP_CONV = 0, OP_ATTN = 1, OP_PREP = 2, OP_RESIZE = 4 };
+struct Op { int kind; ConvParams conv; size_t smem; int cols; AttnParams attn; PrepParams prep; int prep_nsrc; ResizeParams rs; };
 constexpr int kScratchSlots = 10;  // round-robin pool of PLC16 operand buffers (each lives from its prep to the next conv)
 
 // PLC16 operands produced by one prep launch (op = index of that launch in Plan::ops, replayed by the backward pass)
 struct Operand {
   uint8_t *n0 = nullptr, *n1 = nullptr, *r0 = nullptr, *r1 = nullptr, *nl0 = nullptr, *rl0 = nullptr, *rl1 = nullptr; int C0 = 0, C1 = 0, H = 0, W = 0, op = -1;
-  // description of the transform (always filled).  lazy: no prep launch has been emitted -- the consumer either runs the
-  // transform inside its own kernel (conv_fused_kernel, small problems) or materialises the operand first
-  bool lazy = false;
+  // description of the transform (always filled)
   Tens a{}, b{}; bool has_b = false;
   int upsample = 0, mode = 0; const FilmW* film = nullptr; int gamma_idx = 0, beta_idx = 0; bool silu = false, also_raw = false, split = false;
 };
@@ -745,8 +686,8 @@ struct Walker {  // assigns state_dict indices in module registration order and 
     ConvW c; c.w_idx = next((long long)cout * cin_real * taps); c.b_idx = next(cout);
     c.Cout = cout; c.CoutPad = round_up(cout, 16); c.CinReal = cin_real; c.taps = taps;
     c.c0_real = c0_real; c.c0_store = c0_store; c.Cin = round_up(c0_store + c1, 16); c.precise = precise;
-    // tap-row-stacked layout: opt-in (DMD_CONV_TRS=1).  Correct (tests/test_gpu_conv.py runs it), but measured slower on the B200:
-    // 25 us vs 20 us for the 64->64 conv at 64x64 -- see DESIGN.md section 4
+    // tap-row-stacked weight layout: opt-in (DMD_CONV_TRS=1).  The conv kernel addresses each tap inside it, so the layout
+    // changes the weight packing only, not the tensor-core work
     c.trs = (taps == 9 && !precise && 3 * c.CoutPad <= 256 && tune_int("DMD_CONV_TRS", 0) != 0) ? 1 : 0;
     c.pk_off = pk; pk += (size_t)taps * c.Cin * c.CoutPad * 2 * (precise ? 3 : 1); pk = (pk + 255) & ~(size_t)255;
     if (dgrad) {
@@ -860,19 +801,11 @@ struct PlanBuilder {
     o.upsample = upsample; o.mode = mode; o.film = film; o.gamma_idx = gamma_idx; o.beta_idx = beta_idx; o.silu = silu; o.also_raw = also_raw; o.split = split;
     o.C0 = round_up(a.C, 16); o.C1 = b ? round_up(b->C, 16) : 0;
     o.H = upsample ? 2 * a.H : a.H; o.W = upsample ? 2 * a.W : a.W;
-    // small problems (at most one tile per SM) may leave the transform to the consuming conv (conv_fused_kernel, DMD_FUSE_SMALL=1;
-    // measured in the CUDA graph at B=32: one 8.7 us launch instead of 4.0 + 4.6 us -- no gain yet, so it is opt-in); never in
-    // training plans, whose backward replays the prep launches
-    const Plc g = plc_geometry(pl->B, o.H, o.W);
-    const int tiles = (g.Q + kTileM - 1) / kTileM;
-    o.lazy = !pl->train && g_num_sms > 0 && tiles <= g_num_sms && tune_int("DMD_FUSE_SMALL", 0) != 0 && upsample != 2 &&
-             a.C % 16 == 0 && (!b || b->C % 16 == 0);
-    if (!o.lazy) materialize(o);
+    materialize(o);
     return o;
   }
   void materialize(Operand& o) {
-    if (!o.lazy && o.n0) return;
-    o.lazy = false;
+    if (o.n0) return;
     const Tens& a = o.a; const Tens* b = o.has_b ? &o.b : nullptr;
     dmd_prep_desc d; memset(&d, 0, sizeof(d));
     d.src0 = a.data ? a.data : (const float*)1; d.C0 = a.C; d.src1 = b ? (b->data ? b->data : (const float*)1) : nullptr; d.C1 = b ? b->C : 0;
@@ -895,61 +828,8 @@ struct PlanBuilder {
     pl->ops.push_back(op);
   }
 
-  // the conv with its input transform inside the kernel (conv_fused.cuh); false: not applicable (the caller materialises)
-  bool try_fused(const ConvW& cw, Operand& in, int stride, const Tens* resid, Tens& out, bool out_stats, const ConvW* xproj, Operand* xin) {
-    if (!in.lazy || cw.precise || cw.trs || (xproj && !(xin && xin->lazy))) return false;   // (the fused kernel reads tap-major weights)
-    if (in.mode != 0 && (in.a.C / in.a.gs > 4 || (in.has_b && in.b.C / in.b.gs > 4))) return false;   // coefficient table: 4 groups per source
-    Op op; op.kind = OP_FUSED;
-    FusedParams& f = op.fused; memset(&f, 0, sizeof(f));
-    ConvParams& c = f.c;
-    const int Cmain = in.C0 + in.C1, Cx = xproj ? xin->C0 + xin->C1 : 0;
-    if (Cmain != cw.Cin || Cmain > kMaxCin || Cx > kMaxCin) return false;
-    c.Cin = Cmain; c.Cextra = 3 * Cx;
-    c.B = pl->B; c.H = in.H; c.W = in.W; c.taps = cw.taps; c.stride = stride;
-    if (stride == 2 && (c.H % 2 || c.W % 2)) return false;
-    c.wpk = reinterpret_cast<const __half*>(h->packed ? h->packed + cw.pk_off : (const uint8_t*)1); c.bias = P(cw.b_idx);
-    c.Cout = cw.Cout; c.CoutPad = cw.CoutPad;
-    if (xproj) { c.wpk_extra = reinterpret_cast<const __half*>(h->packed ? h->packed + xproj->pk_off : (const uint8_t*)1); c.bias_extra = P(xproj->b_idx); }
-    c.resid = resid ? (resid->data ? resid->data : (const float*)1) : nullptr; c.out = out.data ? out.data : (float*)1;
-    c.ostats = out_stats ? (out.stats ? out.stats : (double*)1) : nullptr; c.ogs = out.gs > 0 ? out.gs : cw.Cout;
-    if (out_stats && (cw.CoutPad > 64 || (cw.Cout != 16 && cw.Cout != 32 && cw.Cout != 64) || cw.Cout % c.ogs)) return false;
-    const Plc g = plc_geometry(pl->B, in.H, in.W);
-    c.PW = g.PW; c.PH = g.PH; c.Q = g.Q; c.G = g.G;
-    const int halo = cw.taps == 9 ? g.PW + 1 : 0;
-    c.P = kTileM + 2 * halo; c.Palloc = c.P | 1;
-    c.dPW.init(g.PW); c.dPH.init(g.PH);
-    c.num_tiles = (g.Q + kTileM - 1) / kTileM;
-    if (out_stats && g.PH * g.PW < 64) return false;                              // epilogue: a tile touches at most 3 images
-    if ((c.P - 1) / (g.PH * g.PW) + 2 > kFusedCoefSlots) return false;          // the halo window touches at most 4 images
-    const uint32_t w_bytes = conv_weight_bytes(cw.taps, c.Cin, c.Cextra, c.CoutPad);
-    const FusedSmem L = fused_smem_layout(w_bytes, Cmain, Cx, c.Palloc);
-    if (L.total > 227u * 1024u) return false;
-    f.coef_off = L.coef_off; f.a_off = L.a_off; f.xa_off = L.xa_off; f.w_off = L.w_off; f.slab_bytes = L.slab_bytes; f.xslab_bytes = L.xslab_bytes;
-    f.Cmain = Cmain; f.Cx = Cx;
-    auto src = [&](const Tens& t, int c_off, bool with_stats) {
-      FusedSrc q; q.src = t.data ? t.data : (const float*)1; q.C = t.C; q.stats = with_stats ? (t.stats ? t.stats : (const double*)1) : nullptr;
-      q.gs = t.gs > 0 ? t.gs : 8; q.c_offset = c_off; return q;
-    };
-    f.m[0] = src(in.a, 0, in.mode != 0); f.nm = 1;
-    if (in.has_b) { f.m[1] = src(in.b, in.a.C, in.mode != 0); f.nm = 2; }
-    f.mode = in.mode; f.act = in.silu ? 1 : 0; f.ups = in.upsample; f.Hs = in.a.H; f.Ws = in.a.W;
-    if (in.mode == 1) { f.film = pl->film ? pl->film : (const float*)1; f.film_stride = h->film_rows; f.film_off = in.film->off; f.film_ctot = in.a.C + (in.has_b ? in.b.C : 0); }
-    if (in.mode == 2) { f.gamma = P(in.gamma_idx) ? P(in.gamma_idx) : (const float*)1; f.beta = P(in.beta_idx) ? P(in.beta_idx) : (const float*)1; }
-    f.eps = kGnEps;
-    if (xproj) {
-      if (xin->upsample || xin->H != in.H || xin->W != in.W) return false;
-      f.x[0] = src(xin->a, 0, false); f.nx = 1;
-      if (xin->has_b) { f.x[1] = src(xin->b, xin->a.C, false); f.nx = 2; }
-    }
-    op.smem = L.total;
-    op.cols = cw.CoutPad <= 32 ? 32 : (cw.CoutPad <= 64 ? 64 : 128);
-    pl->ops.push_back(op);
-    return true;
-  }
-
   void conv(const ConvW& cw, Operand& in, bool raw, int stride, const Tens* resid, Tens& out, bool out_stats,
             const ConvW* xproj = nullptr, Operand* xin = nullptr) {
-    if (!raw && try_fused(cw, in, stride, resid, out, out_stats, xproj, xin)) return;
     materialize(in);
     if (xin) materialize(*xin);
     if (err) return;
@@ -1200,7 +1080,7 @@ struct BwdBuilder {
     nb.gx = gx; nb.addend = addend; nb.accumulate = accumulate ? 1 : 0;
     // pixels per block: enough blocks to cover the SMs, at least 32 pixels each
     int ppb = nb.HW;
-    while (ppb > 32 && (long long)pl->B * ((nb.HW + ppb - 1) / ppb) < 2 * 148) ppb >>= 1;
+    while (ppb > 32 && (long long)pl->B * ((nb.HW + ppb - 1) / ppb) < 2 * kPlanSms) ppb >>= 1;
     b1.nb = nb; b1.ppb = ppb; b1.chunks = (nb.HW + ppb - 1) / ppb;
     push(b1);
     if (mode == 2) {
@@ -1413,10 +1293,6 @@ int run_forward(dmd_denoiser* h, Plan& pl, const float* noisy, const float* sigm
     else if (op.kind == OP_PREP) {
       if (op.prep.film != nullptr && op.prep.film != film) { PrepParams pp = op.prep; pp.film = film; if (prep_launch(pp, op.prep_nsrc, st)) return 1; }
       else if (prep_launch(op.prep, op.prep_nsrc, st)) return 1;
-    }
-    else if (op.kind == OP_FUSED) {
-      if (op.fused.film != nullptr && op.fused.film != film) { FusedParams fp = op.fused; fp.film = film; if (fused_launch(fp, op.smem, op.cols, st)) return 1; }
-      else if (fused_launch(op.fused, op.smem, op.cols, st)) return 1;
     }
     else if (op.kind == OP_RESIZE) { if (resize_launch(op.rs, st)) return 1; }
     else { if (attn_launch(op.attn, pl.B, st)) return 1; }
@@ -2208,7 +2084,7 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
       nb.gx = gx; nb.addend = lv.has_skip ? nullptr : gy; nb.accumulate = 0;
       DMD_CUDA(cudaMemsetAsync(sc.nsum, 0, (size_t)2 * B * kMaxCin * 4, st));
       int ppb = nb.HW;
-      while (ppb > 32 && (long long)B * ((nb.HW + ppb - 1) / ppb) < 2 * 148) ppb >>= 1;
+      while (ppb > 32 && (long long)B * ((nb.HW + ppb - 1) / ppb) < 2 * kPlanSms) ppb >>= 1;
       const int chunks = (nb.HW + ppb - 1) / ppb;
       norm_bwd_pass1_kernel<<<dim3(chunks, B), kNormThreads, 0, st>>>(nb, ppb);
       DMD_LAUNCH_OK();
@@ -2422,7 +2298,6 @@ extern "C" int dmd_rew_end_predict(dmd_rew_end* h, int b, int t, const float* ob
   for (const Op& op : pl.ops) {
     if (op.kind == OP_CONV) { if (conv_launch(op.conv, op.smem, op.cols, st)) return 1; }
     else if (op.kind == OP_PREP) { if (prep_launch(op.prep, op.prep_nsrc, st)) return 1; }
-    else if (op.kind == OP_FUSED) { if (fused_launch(op.fused, op.smem, op.cols, st)) return 1; }
     else { if (attn_launch(op.attn, pl.B, st)) return 1; }
   }
   // LSTM over time (torch.nn.LSTM, gate order i f g o), rows of step k are the contiguous block [k*b, (k+1)*b)

@@ -384,8 +384,7 @@ __global__ void __launch_bounds__(kAttnThreads) attn_kernel(const AttnParams p) 
 
 // ------------------------------------------------------------------------------------------------
 // SelfAttention2d on a CLUSTER of four CTAs per image (same math as attn_kernel above, same parameter block).
-// The one-CTA-per-image kernel keeps 32 of 148 SMs busy at the benchmark batch and runs ~5 k instructions per thread
-// (32 us in the CUDA graph: 5 % of a sample()).  Here cluster rank r owns C/4 channels = C/32 heads:
+// The one-CTA-per-image kernel keeps only 32 SMs busy at the benchmark batch and runs ~5 k instructions per thread.  Here cluster rank r owns C/4 channels = C/32 heads:
 //   every CTA   : GroupNorm(x) for all channels (its q/k/v rows contract over all of them)
 //   rank r      : q, k, v rows of its heads -> softmax(q k^T / sqrt(d)) v with the 64 keys split over 2 (C=64) or 4 (C=32)
 //                 threads per (head, query) and merged with shuffles -> its C/4 channels of y in ITS shared memory
@@ -636,7 +635,7 @@ __global__ void pack_conv_weight_kernel(const float* __restrict__ w, __half* __r
   }
 }
 
-// Tap-row-stacked packing (TrsEpilogue, conv_tc.cuh): [dy 3][Cin/8][3 * CoutPad][8] fp16, column n = dx * CoutPad + co of kernel
+// Tap-row-stacked packing (conv_tc.cuh addresses tap (dy, dx) inside it): [dy 3][Cin/8][3 * CoutPad][8] fp16, column n = dx * CoutPad + co of kernel
 // row dy holds W[co][ci][dy][dx]; channel mapping (c0_real / c0_store / concat) as in pack_conv_weight_kernel.
 __global__ void pack_conv_weight_trs_kernel(const float* __restrict__ w, __half* __restrict__ wpk, int Cout, int CoutPad, int CinReal,
                                             int Cin, int c0_real, int c0_store) {

@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution on tcgen05 tensor cores (sm_100a).  Persistent, warp-specialised, TMA-fed.
+// Implicit-GEMM convolution on Hopper tensor cores (sm_90a wgmma).  Persistent, warp-specialised, TMA-fed.
 //
 // Replaces, on the hot path, every nn.Conv2d of the reference (blocks.py:18-19 Conv1x1/Conv3x3, :96 Downsample,
 // :109-110 Upsample conv, inner_model.py:36,41 conv_in/conv_out) plus its epilogue neighbours: bias, residual add
@@ -12,33 +12,27 @@
 // stored as one plane per 8-channel chunk:   plane[j][G + q] = 8 fp16 channels = 16 bytes   (G = PW+1 zero guard
 // positions in front, PW+1 behind the last tile).  A 128-row tile needs, per 16 input channels ("slab"), positions
 // [q0-PW-1, q0+128+PW+1) of two planes: two CONTIGUOUS byte ranges.  They are fetched with cp.async.bulk straight
-// into the UMMA no-swizzle K-major shared-memory layout  [2 chunks][P positions][16 B]  (LBO = Palloc*16, SBO = 128),
+// into the wgmma no-swizzle K-major shared-memory layout  [2 chunks][P positions][16 B]  (LBO = Palloc*16, SBO = 128),
 // and every tap reads the same slab through a descriptor whose start address is shifted by (dy*PW+dx)*16 B.
 //
-// Roles (320 threads, one CTA per SM, contiguous balanced tile ranges):
-//   warp 0      producer: mbarrier expect_tx + 2 bulk copies per slab into a deep ring (empty/full mbarriers)
-//   warp 1      MMA     : tcgen05.mma (M=128, N=CoutPad, K=16) per (slab, tap) from precomputed descriptor words;
-//                         tcgen05.commit frees the slab / publishes the TMEM accumulator.  A fused 1x1 skip projection
-//                         is extra centre-tap slabs on the same accumulator.
-//               Both warps walk their loops CONVERGED and an elect.sync lane issues (uniform-register operands).
-//   warps 2-9   epilogue: TMEM -> registers (+bias) -> shared staging (transpose) -> coalesced 16-byte global stores with
-//                         the (prefetched) residual added on the way; GroupNorm partial sums run in registers across the
-//                         single-image tiles of the CTA and are reduced once per image -> fp64 atomics
+// Roles (384 threads = three warpgroups, one CTA per SM, contiguous balanced tile ranges):
+//   warps 0, 1       producers: mbarrier expect_tx + 2 bulk copies per slab into a deep ring (empty/full mbarriers); the two
+//                    warps take alternate slabs (warps 2 and 3 have no work)
+//   warpgroups 1, 2  consumers: warpgroup c owns rows 64c .. 64c+63 of the tile.  Per (slab, tap) one wgmma m64 x N x k16 with
+//                    both operands in shared memory and the fp32 accumulator in registers; a fused 1x1 skip projection is
+//                    extra centre-tap slabs on the same accumulator.  After the last slab of a tile the warpgroup stores its
+//                    rows (+bias, +residual) from the registers straight to NHWC global memory (RegEpilogue) while the
+//                    producers already fill the ring with the next tile's slabs.
 // Weights (fp16, [tap][Cin/8][CoutPad][8]) are bulk-copied into shared memory once per CTA and stay resident.
-// TMEM holds two accumulators so the epilogue of tile i overlaps the MMAs of tile i+1.
 #pragma once
-#include <type_traits>
 #include "ptx.cuh"
 
 namespace dmd {
 
-constexpr int kEpiWarps = 8;
-constexpr int kEpiThreads = kEpiWarps * 32;
-constexpr int kConvThreads = (3 + kEpiWarps) * 32;  // 352: warp 0 producer, warp 1 MMA issuer, warps 2-9 epilogue, warp 10 second producer
-constexpr int kProdWarp2 = 2 + kEpiWarps;
+constexpr int kConvThreads = 384;
+constexpr int kConvConsumerWarps = 8;  // warpgroups 1 and 2; each warp releases a ring slot once its wgmma reads retired
 constexpr int kTileM = 128;
 constexpr int kMaxCin = 128;        // channels of one activation source
-constexpr int kMaxKChannels = 384;  // K extent per tap: up to 3 x 128 (split-fp16 "precise" convs)
 constexpr int kMaxSegs = 8;
 constexpr int kMaxStages = 24;
 constexpr int kStatSlots = 3;   // images a 128-row tile can touch
@@ -61,7 +55,7 @@ struct Plc {
 __host__ __device__ inline Plc plc_geometry(int B, int H, int W) {
   Plc g;
   g.PW = W + 1; g.PH = H + 1; g.Q = B * g.PH * g.PW; g.G = g.PW + 1;
-  g.Qalloc = g.G + ((g.Q + kTileM - 1) / kTileM) * kTileM + kTileM + g.PW + 1;   // + one tile: 126-row (tap-row-stacked) tiling reads further
+  g.Qalloc = g.G + ((g.Q + kTileM - 1) / kTileM) * kTileM + kTileM + g.PW + 1;
   return g;
 }
 
@@ -73,14 +67,14 @@ struct ConvParams {
   int nseg;
   int Cin;              // K channels per tap of the main weights
   int Cextra;           // trailing K channels that use ONLY the centre tap with their own weights: the fused 1x1 skip
-                        // projection r = proj(cat(x, skip)) accumulated into the same TMEM tile (blocks.py:133,142,145)
+                        // projection r = proj(cat(x, skip)) accumulated into the same tile (blocks.py:133,142,145)
   const __half* wpk_extra;  // [1][Cextra/8][CoutPad][8]
   const float* bias_extra;  // [Cout] or null
   int xslabs;               // operand slabs of the projection that are LOADED: hi and lo parts once each (2 * channels / 16)
   int B, H, W;          // conv input size
   int taps;             // 9 (3x3, pad 1) or 1 (1x1)
   int stride;           // 1 or 2 (stride 2 == stride-1 result sampled at even (y,x); exact for k=3,p=1)
-  const __half* wpk;    // [taps][Cin/8][CoutPad][8]
+  const __half* wpk;    // [taps][Cin/8][CoutPad][8], or [dy][Cin/8][3*CoutPad][8] when trs
   const float* bias;    // [Cout] or null
   int Cout, CoutPad;
   const float* resid;   // NHWC [B][Ho][Wo][Cout] or null
@@ -92,130 +86,91 @@ struct ConvParams {
   unsigned long long plane_bytes;  // bytes of one chunk plane (same geometry for both sources)
   int P, Palloc;        // halo positions, odd allocation pitch
   int num_tiles, stages;
-  int trs;              // tap-row-stacked mode (see TrsEpilogue): weights [dy][Cin/8][3*CoutPad][8], tiles advance by 126 positions
-  int tile_stride;      // 128, or 126 in trs mode
-  int trs_groups;       // trs mode: 1 = eight warps per tile, 2 = two groups of four warps on alternate tiles
-  int egroups;          // epilogue groups: 1 = eight warps share every tile; 2 = two groups of four warps take alternate tiles
+  int trs;              // weights in the tap-row-stacked layout (dmd_pack_conv_weight precise = 3): tap (dy, dx) is the column
+                        // block dx * CoutPad of kernel row dy
   FastDiv dPW, dPH;
-  int dbg;
-  long long* dbg_buf;   // bring-up: clock64 timeline of CTA 0, [role 3][tile 16][event 16]
   long long* ktrace;    // diagnostics: globaltimer stamp when the kernel's inputs are ready, or null
 };
 
 struct ConvSmemLayout {
-  uint32_t bias_off, rowinfo_off, sstat_off, stage_off, w_off, a_off, slab_bytes, stage_pitch, total;
+  uint32_t bias_off, w_off, a_off, slab_bytes, total;
 };
 
-// barriers live in the first 512 bytes: wbar, full[24], empty[24], tfull[2], tempty[2], tmem slot
+// barriers live in the first 512 bytes: wbar, full[24], empty[24]
 __host__ __device__ inline uint32_t conv_weight_bytes(int taps, int Cin, int Cextra, int CoutPad) {
   return (((uint32_t)taps * Cin * CoutPad * 2 + 127u) & ~127u) + (uint32_t)Cextra * CoutPad * 2;
 }
-// groups == 0: direct epilogue (registers -> global), no staging tile, row table or statistics scratch
-__host__ __device__ inline ConvSmemLayout conv_smem_layout(uint32_t w_bytes, int CoutPad, int Palloc, int stages, int groups = 1) {
+// The slab ring follows the weights: a wgmma of N > CoutPad columns (N is a power of two) reads up to N - CoutPad rows past
+// the end of a weight block, which stay inside the allocation and only feed accumulator columns that are never stored.
+__host__ __device__ inline ConvSmemLayout conv_smem_layout(uint32_t w_bytes, int Palloc, int stages) {
   ConvSmemLayout L;
   L.bias_off = 512;
-  L.rowinfo_off = L.bias_off + 128 * 4;              // [groups][128] int2 (out pixel or -1, stat slot)
-  L.sstat_off = L.rowinfo_off + (uint32_t)groups * kTileM * 8;   // [epilogue warp 8][slot 3][group 4][2] floats
-  L.stage_pitch = (uint32_t)CoutPad * 4 + 16;
-  L.stage_off = (L.sstat_off + (groups ? kEpiWarps * kStatSlots * kMaxOutGroups * 2 * 4 : 0) + 127u) & ~127u;
-  if (groups == 3) {   // tap-row-stacked: no staging, a boundary-row exchange buffer (16 KB) instead
-    L.rowinfo_off = L.sstat_off = L.bias_off + 128 * 4;
-    L.stage_off = L.rowinfo_off;
-    L.w_off = (L.stage_off + 2u * 2u * 2u * 4u * 128u * 4u + 127u) & ~127u;   // [group 2][parity 2][kind 2][quarter 4][128] floats
-    L.a_off = (L.w_off + w_bytes + 127u) & ~127u;
-    L.slab_bytes = 2u * Palloc * 16;
-    L.total = L.a_off + (uint32_t)stages * L.slab_bytes + 16;
-    return L;
-  }
-  L.w_off = (L.stage_off + (uint32_t)groups * kTileM * L.stage_pitch + 127u) & ~127u;   // one staging tile per group
+  L.w_off = L.bias_off + 128 * 4;
   L.a_off = (L.w_off + w_bytes + 127u) & ~127u;
   L.slab_bytes = 2u * Palloc * 16;
   L.total = L.a_off + (uint32_t)stages * L.slab_bytes + 16;
   return L;
 }
 
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-// Bring-up instrumentation (clock64 role timeline, "skip" switches) exists only in -DDMD_TIMELINE builds: the producer and
-// MMA warps are latency-bound on their own scalar instructions, so even a not-taken debug test per slab is measurable.
-#ifdef DMD_TIMELINE
-#define DMD_DBG(bit) (p.dbg & (bit))
-#define DMD_TS(role, it_, ev) \
-  do { if (p.dbg_buf && blockIdx.x == 0 && (it_) < 16) p.dbg_buf[((role) * 16 + (it_)) * 16 + (ev)] = clock64(); } while (0)
-#else
-#define DMD_DBG(bit) 0
-#define DMD_TS(role, it_, ev) do { } while (0)
-#endif
-
 // ------------------------------------------------------------------------------------------------------------------
-// Direct epilogue (shared by conv_tc_kernel and conv_fused_kernel): the eight epilogue warps read the accumulator with the
-// 16-lane x 256-bit TMEM pattern -- four neighbouring threads hold 32 contiguous bytes of one output row -- and store
-// (+bias, +residual) straight to NHWC global memory as full 32-byte sectors.  No shared-memory staging, no row table, no named
-// barriers; GroupNorm partial sums run in registers across the single-image tiles of a CTA and are reduced with shuffles.
-// Two warps share a TMEM lane quarter and split the columns; the host guarantees that all columns of a warp lie in ONE
-// GroupNorm group whenever statistics are requested (CoutPad <= 64).
-template <int kAccCols>
-struct DirectEpilogue {
-  int quarter, blk_begin, blk_end, lr, lc, G, my_grp, lane;
-  bool vec2;
-  float s0, s1, s2, ss0, ss1, ss2;
+// Register epilogue: a consumer thread holds two accumulator rows (r0, r0 + 8) of the tile, columns 8j + 2(lane%4) + {0,1}
+// (the wgmma fragment, ptx.cuh): four neighbouring threads hold 32 contiguous bytes of one output row, which go to NHWC global
+// memory as full 32-byte sectors (+bias, +residual), with no shared-memory staging.  GroupNorm partial sums run in registers
+// across the single-image tiles of a CTA and are reduced with warp shuffles once per image -> fp64 atomics.
+template <int N>
+struct RegEpilogue {
+  int lane, r0, lgs, G;
+  float s[kStatSlots][kMaxOutGroups], ss[kStatSlots][kMaxOutGroups];
   int n_cur;
 
-  __device__ __forceinline__ void init(const ConvParams& p, int warp, int lane_) {
+  __device__ __forceinline__ void init(const ConvParams& p, int row0, int lane_) {
     lane = lane_;
-    const int ew = warp - 2;                   // 0..7
-    quarter = warp & 3;                        // TMEM lane quarter this warp may access
-    const int half = ew >> 2;                  // two warps share a quarter and split the columns
-    const int nblk = p.CoutPad >> 3;           // 8-column blocks of the accumulator
-    const int hb = (nblk + 1) >> 1;
-    blk_begin = half ? hb : 0; blk_end = half ? nblk : hb;
-    lr = lane >> 2; lc = (lane & 3) * 2;
-    vec2 = (p.Cout & 1) == 0;
+    r0 = row0;
     G = p.ostats ? p.Cout / p.ogs : 1;
-    my_grp = p.ostats ? min(G - 1, (blk_begin * 8) / p.ogs) : 0;
-    s0 = s1 = s2 = ss0 = ss1 = ss2 = 0.f;
+    lgs = p.ostats ? 31 - __clz(p.ogs >> 3) : 0;   // 8-column block j lies in group j >> lgs (ogs is 16/32/64/128)
+#pragma unroll
+    for (int k = 0; k < kStatSlots; ++k)
+#pragma unroll
+      for (int g = 0; g < kMaxOutGroups; ++g) s[k][g] = ss[k][g] = 0.f;
     n_cur = -1;
   }
 
-  __device__ __forceinline__ void flush_stats(const ConvParams& p, int img0, bool multi) {
+  // whole warp, converged
+  __device__ __forceinline__ void flush_stats(const ConvParams& p, int img0, int nslots) {
 #pragma unroll
-    for (int m = 16; m > 0; m >>= 1) {
-      s0 += __shfl_xor_sync(0xffffffffu, s0, m);
-      ss0 += __shfl_xor_sync(0xffffffffu, ss0, m);
-      if (multi) {
-        s1 += __shfl_xor_sync(0xffffffffu, s1, m);
-        ss1 += __shfl_xor_sync(0xffffffffu, ss1, m);
-        s2 += __shfl_xor_sync(0xffffffffu, s2, m);
-        ss2 += __shfl_xor_sync(0xffffffffu, ss2, m);
+    for (int k = 0; k < kStatSlots; ++k) {
+#pragma unroll
+      for (int g = 0; g < kMaxOutGroups; ++g) {
+        if (k < nslots && g < G) {
+          float a = s[k][g], b = ss[k][g];
+#pragma unroll
+          for (int m = 16; m > 0; m >>= 1) {
+            a += __shfl_xor_sync(0xffffffffu, a, m);
+            b += __shfl_xor_sync(0xffffffffu, b, m);
+          }
+          if (lane == 0 && img0 + k < p.B && (a != 0.f || b != 0.f)) {
+            double* dst = p.ostats + ((size_t)(img0 + k) * G + g) * 2;
+            atomicAdd(dst, (double)a);
+            atomicAdd(dst + 1, (double)b);
+          }
+        }
+        s[k][g] = ss[k][g] = 0.f;
       }
     }
-    if (lane == 0) {
-      double* dst = p.ostats + ((size_t)img0 * G + my_grp) * 2;
-      if (img0 < p.B && (s0 != 0.f || ss0 != 0.f)) { atomicAdd(dst, (double)s0); atomicAdd(dst + 1, (double)ss0); }
-      if (multi) {
-        if (img0 + 1 < p.B && (s1 != 0.f || ss1 != 0.f)) { atomicAdd(dst + (size_t)G * 2, (double)s1); atomicAdd(dst + (size_t)G * 2 + 1, (double)ss1); }
-        if (img0 + 2 < p.B && (s2 != 0.f || ss2 != 0.f)) { atomicAdd(dst + (size_t)G * 4, (double)s2); atomicAdd(dst + (size_t)G * 4 + 1, (double)ss2); }
-      }
-    }
-    s0 = s1 = s2 = ss0 = ss1 = ss2 = 0.f;
   }
 
-  // one 128-row tile starting at padded-linear position q0; accumulator at TMEM address tmem_acc; tfull/parity: accumulator
-  // ready; tempty: arrived on (once per warp) as soon as the accumulator has been read
-  __device__ __forceinline__ void tile(const ConvParams& p, const float* sbias, uint32_t tmem_acc, int q0, uint64_t* tfull,
-                                       uint32_t parity, uint64_t* tempty) {
+  // the tile starting at padded-linear position q0; acc: this thread's wgmma accumulator fragment
+  __device__ __forceinline__ void tile(const ConvParams& p, const float* sbias, const float (&acc)[N / 2], int q0) {
     const int n_lo = (int)p.dPH.div(p.dPW.div((uint32_t)q0));
     const int q_last = min(q0 + kTileM, p.Q) - 1;
     const bool single_image = (int)p.dPH.div(p.dPW.div((uint32_t)q_last)) == n_lo;
-    if (n_cur >= 0 && (!single_image || n_lo != n_cur)) { flush_stats(p, n_cur, false); n_cur = -1; }
-    // the four accumulator rows of this thread: j = 2*h + s -> row quarter*32 + 16*h + lane/4 + 8*s
-    int opix[4], slot[4];
+    if (p.ostats != nullptr && n_cur >= 0 && (!single_image || n_lo != n_cur)) { flush_stats(p, n_cur, 1); n_cur = -1; }
+    const int c0 = 2 * (lane & 3);
+    const bool vec = (p.Cout & 1) == 0;   // 8-byte accesses (every layer but conv_out / the 15-channel dgrad)
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int q = q0 + quarter * 32 + (j >> 1) * 16 + lr + (j & 1) * 8;
-      opix[j] = -1; slot[j] = 0;
+    for (int h = 0; h < 2; ++h) {
+      const int q = q0 + r0 + 8 * h;
+      int opix = -1, slot = 0;
       if (q < p.Q) {
         const uint32_t R = p.dPW.div((uint32_t)q);
         const int x = q - (int)R * p.PW;
@@ -227,377 +182,69 @@ struct DirectEpilogue {
           valid = valid && ((x & 1) == 0) && ((y & 1) == 0);
           yo = y >> 1; xo = x >> 1; Ho = p.H >> 1; Wo = p.W >> 1;
         }
-        if (valid) { opix[j] = (n * Ho + yo) * Wo + xo; slot[j] = n - n_lo; }
+        if (valid) { opix = (n * Ho + yo) * Wo + xo; slot = n - n_lo; }
       }
-    }
-    bool waited = false;
-    auto chunk = [&](auto nbc, auto vecc, int blk) {
-      constexpr int NB = decltype(nbc)::value;
-      constexpr bool VEC = decltype(vecc)::value;   // even Cout: 8-byte accesses (every layer but conv_out / the 15-channel dgrad)
-      const int col0 = blk * 8 + lc;           // first of this thread's two columns in block 0 of the chunk
-      // residual first: it does not depend on the accumulator, so for the first chunk its latency hides behind the MMAs
-      float2 rr[4][NB];
+      if (opix < 0) continue;
+      float* op = p.out + (size_t)opix * p.Cout;
+      const float* rp = p.resid != nullptr ? p.resid + (size_t)opix * p.Cout : nullptr;
+      float gs[kMaxOutGroups], gss[kMaxOutGroups];
 #pragma unroll
-      for (int j = 0; j < 4; ++j)
+      for (int g = 0; g < kMaxOutGroups; ++g) gs[g] = gss[g] = 0.f;
 #pragma unroll
-        for (int k = 0; k < NB; ++k) {
-          rr[j][k] = make_float2(0.f, 0.f);
-          const int col = col0 + 8 * k;
-          if (p.resid != nullptr && opix[j] >= 0 && col < p.Cout) {
-            const float* rp = p.resid + (size_t)opix[j] * p.Cout + col;
-            if (VEC) rr[j][k] = __ldg(reinterpret_cast<const float2*>(rp));
-            else { rr[j][k].x = __ldg(rp); if (col + 1 < p.Cout) rr[j][k].y = __ldg(rp + 1); }
-          }
-        }
-      if (!waited) {
-        mbar_wait(tfull, parity);
-        tc_fence_after_sync();
-        waited = true;
-      }
-      uint32_t r[8 * NB];
-      const uint32_t ta = tmem_acc + (uint32_t)(blk * 8) + ((uint32_t)(quarter * 32) << 16);
-      tmem_ld_16x256b_pair<NB>(ta, ta + (16u << 16), r);
-      if (blk + NB >= blk_end) {               // last chunk of this warp: the accumulator may be overwritten
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0 && tempty != nullptr) mbar_arrive(tempty);
-      }
-      float2 bv[NB];
-#pragma unroll
-      for (int k = 0; k < NB; ++k) bv[k] = (col0 + 8 * k < p.Cout) ? *reinterpret_cast<const float2*>(sbias + col0 + 8 * k) : make_float2(0.f, 0.f);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        if (opix[j] >= 0) {
-          float* op = p.out + (size_t)opix[j] * p.Cout + col0;
-          float ps = 0.f, pss = 0.f;
-#pragma unroll
-          for (int k = 0; k < NB; ++k) {
-            if (col0 + 8 * k < p.Cout) {
-              const int ri = (j >> 1) * 4 * NB + 4 * k + 2 * (j & 1);
-              float2 o;
-              o.x = __uint_as_float(r[ri]) + bv[k].x + rr[j][k].x;
-              o.y = __uint_as_float(r[ri + 1]) + bv[k].y + rr[j][k].y;
-              if (VEC) *reinterpret_cast<float2*>(op + 8 * k) = o;
-              else { op[8 * k] = o.x; if (col0 + 8 * k + 1 < p.Cout) op[8 * k + 1] = o.y; }
-              ps += o.x + o.y;
-              pss = fmaf(o.x, o.x, fmaf(o.y, o.y, pss));
-            }
+      for (int j = 0; j < N / 8; ++j) {
+        const int col = 8 * j + c0;
+        if (col < p.Cout) {
+          float2 o = make_float2(acc[4 * j + 2 * h] + sbias[col], acc[4 * j + 2 * h + 1] + sbias[col + 1]);
+          if (vec) {
+            if (rp) { const float2 r = __ldg(reinterpret_cast<const float2*>(rp + col)); o.x += r.x; o.y += r.y; }
+            *reinterpret_cast<float2*>(op + col) = o;
+          } else {
+            if (rp) o.x += __ldg(rp + col);
+            op[col] = o.x;
+            if (col + 1 < p.Cout) { if (rp) o.y += __ldg(rp + col + 1); op[col + 1] = o.y; } else o.y = 0.f;
           }
           if (p.ostats != nullptr) {
-            const int sl = single_image ? 0 : slot[j];
-            s0 += (sl == 0) ? ps : 0.f;  ss0 += (sl == 0) ? pss : 0.f;
-            s1 += (sl == 1) ? ps : 0.f;  ss1 += (sl == 1) ? pss : 0.f;
-            s2 += (sl == 2) ? ps : 0.f;  ss2 += (sl == 2) ? pss : 0.f;
+            const int gi = j >> lgs;
+            const float ps = o.x + o.y, pss = fmaf(o.x, o.x, o.y * o.y);
+#pragma unroll
+            for (int g = 0; g < kMaxOutGroups; ++g) { gs[g] += (g == gi) ? ps : 0.f; gss[g] += (g == gi) ? pss : 0.f; }
           }
         }
       }
-    };
-    for (int blk = blk_begin; blk < blk_end;) {
-      const int rem = blk_end - blk;
-      if (!vec2) { chunk(std::integral_constant<int, 1>{}, std::false_type{}, blk); blk += 1; }   // odd Cout: narrow outputs only
-      else if (rem >= 4) { chunk(std::integral_constant<int, 4>{}, std::true_type{}, blk); blk += 4; }
-      else if (rem >= 2) { chunk(std::integral_constant<int, 2>{}, std::true_type{}, blk); blk += 2; }
-      else { chunk(std::integral_constant<int, 1>{}, std::true_type{}, blk); blk += 1; }
+      if (p.ostats != nullptr) {
+        const int sl = single_image ? 0 : slot;
+#pragma unroll
+        for (int k = 0; k < kStatSlots; ++k)
+#pragma unroll
+          for (int g = 0; g < kMaxOutGroups; ++g) { s[k][g] += (sl == k) ? gs[g] : 0.f; ss[k][g] += (sl == k) ? gss[g] : 0.f; }
+      }
     }
     if (p.ostats != nullptr) {
       if (single_image) n_cur = n_lo;            // keep running across the single-image tiles of this CTA
-      else { flush_stats(p, n_lo, true); n_cur = -1; }
+      else { flush_stats(p, n_lo, kStatSlots); n_cur = -1; }
     }
   }
 
   __device__ __forceinline__ void finish(const ConvParams& p) {
-    if (n_cur >= 0) flush_stats(p, n_cur, false);
+    if (p.ostats != nullptr && n_cur >= 0) flush_stats(p, n_cur, 1);
   }
 };
 
-// ------------------------------------------------------------------------------------------------------------------
-// Tap-row-stacked (TRS) 3x3 convolution.  Measured (clock64 timeline, scripts/timeline_conv.py): a tcgen05.mma M128 x N64 x K16
-// with both operands in shared memory takes ~72 cycles on this part independent of operand alignment -- the 4 KB A-operand read
-// per instruction is the bound (N = 64 gives the tensor pipe 32 cycles of work) -- so nine taps x four slabs cost ~2.6 k cycles
-// per 128-row tile.  The three taps of one kernel ROW (dy fixed, dx = -1, 0, +1) read windows that differ by ONE position, so they
-// can share one A read if the dx shift is moved to the OUTPUT side:
-//     D[r][dx*Cout + co] = sum_c X[w0 + r + dy*PW][c] * W[dy][dx][c][co]        one MMA, N = 3 * Cout, per (slab, dy)
-//     out[w0 + m][co]    = D[m - 1][co] + D[m][Cout + co] + D[m + 1][2*Cout + co]      m = 1 .. 126
-// Three MMAs of N = 192 per slab instead of nine of N = 64: a third of the A reads, the tensor pipe becomes the bound.  The price:
-// a tile yields 126 outputs from 128 window rows (tiles advance by 126 positions), the accumulator is 3x wider (2 x 192 TMEM
-// columns), and the epilogue adds three row-shifted accumulator blocks.  With the 16-lane x 256-bit TMEM load pattern the rows
-// m - 1 / m + 1 of a thread's four rows live four lanes away (one shuffle each) except at the edges of a warp's 32-row quarter,
-// which are exchanged through a 4 KB shared-memory buffer (one named barrier per 16-column chunk).
-template <int kAccCols>
-struct TrsEpilogue {
-  int quarter, blk_begin, blk_end, g, lc, G, my_grp, lane;
-  int grp, bar_id, bar_threads;       // epilogue group (two groups of four warps take alternate tiles), its named barrier
-  bool vec2;
-  float s0, s1, s2, ss0, ss1, ss2;   // partial sums of the warp's first GroupNorm group ...
-  float t0, t1, t2, tt0, tt1, tt2;   // ... and of its second one (a warp that owns all 64 columns spans two groups)
-  int n_cur;
-
-  // ngroups == 1: the eight warps share every tile (two warps per TMEM lane quarter split the columns).
-  // ngroups == 2: two groups of four warps take alternate tiles / accumulators, each warp owns all columns of its quarter: the
-  //               stores of one tile (32 KB at ~16 B/clk/SM: ~2 k cycles, the longest phase) drain while the other group loads
-  //               and combines the next tile.
-  __device__ __forceinline__ void init(const ConvParams& p, int warp, int lane_, int ngroups) {
-    lane = lane_;
-    const int ew = warp - 2;
-    quarter = warp & 3;
-    const int nblk = p.CoutPad >> 3;
-    if (ngroups == 2) {
-      grp = ew >> 2; blk_begin = 0; blk_end = nblk; bar_id = 1 + grp; bar_threads = kEpiThreads / 2;
-    } else {
-      const int half = ew >> 2;
-      const int hb = nblk >> 1;                // CoutPad is a multiple of 16: equal halves (every warp runs the same number of chunks)
-      grp = 0; blk_begin = half ? hb : 0; blk_end = half ? nblk : hb; bar_id = 1; bar_threads = kEpiThreads;
-    }
-    g = lane >> 2; lc = (lane & 3) * 2;
-    vec2 = (p.Cout & 1) == 0;
-    G = p.ostats ? p.Cout / p.ogs : 1;
-    my_grp = p.ostats ? min(G - 1, (blk_begin * 8) / p.ogs) : 0;
-    s0 = s1 = s2 = ss0 = ss1 = ss2 = 0.f;
-    t0 = t1 = t2 = tt0 = tt1 = tt2 = 0.f;
-    n_cur = -1;
-  }
-
-  __device__ __forceinline__ void flush_stats(const ConvParams& p, int img0, bool multi) {
-#pragma unroll
-    for (int m = 16; m > 0; m >>= 1) {
-      s0 += __shfl_xor_sync(0xffffffffu, s0, m);
-      ss0 += __shfl_xor_sync(0xffffffffu, ss0, m);
-      if (multi) {
-        s1 += __shfl_xor_sync(0xffffffffu, s1, m);
-        ss1 += __shfl_xor_sync(0xffffffffu, ss1, m);
-        s2 += __shfl_xor_sync(0xffffffffu, s2, m);
-        ss2 += __shfl_xor_sync(0xffffffffu, ss2, m);
-      }
-    }
-    if (lane == 0) {
-      double* dst = p.ostats + ((size_t)img0 * G + my_grp) * 2;
-      if (img0 < p.B && (s0 != 0.f || ss0 != 0.f)) { atomicAdd(dst, (double)s0); atomicAdd(dst + 1, (double)ss0); }
-      if (multi) {
-        if (img0 + 1 < p.B && (s1 != 0.f || ss1 != 0.f)) { atomicAdd(dst + (size_t)G * 2, (double)s1); atomicAdd(dst + (size_t)G * 2 + 1, (double)ss1); }
-        if (img0 + 2 < p.B && (s2 != 0.f || ss2 != 0.f)) { atomicAdd(dst + (size_t)G * 4, (double)s2); atomicAdd(dst + (size_t)G * 4 + 1, (double)ss2); }
-      }
-    }
-    s0 = s1 = s2 = ss0 = ss1 = ss2 = 0.f;
-    if (my_grp + 1 < G && (blk_end - blk_begin) * 8 > p.ogs) {   // the warp's columns reach into a second group
-#pragma unroll
-      for (int m = 16; m > 0; m >>= 1) {
-        t0 += __shfl_xor_sync(0xffffffffu, t0, m);
-        tt0 += __shfl_xor_sync(0xffffffffu, tt0, m);
-        if (multi) {
-          t1 += __shfl_xor_sync(0xffffffffu, t1, m);
-          tt1 += __shfl_xor_sync(0xffffffffu, tt1, m);
-          t2 += __shfl_xor_sync(0xffffffffu, t2, m);
-          tt2 += __shfl_xor_sync(0xffffffffu, tt2, m);
-        }
-      }
-      if (lane == 0) {
-        double* dst = p.ostats + ((size_t)img0 * G + my_grp + 1) * 2;
-        if (img0 < p.B && (t0 != 0.f || tt0 != 0.f)) { atomicAdd(dst, (double)t0); atomicAdd(dst + 1, (double)tt0); }
-        if (multi) {
-          if (img0 + 1 < p.B && (t1 != 0.f || tt1 != 0.f)) { atomicAdd(dst + (size_t)G * 2, (double)t1); atomicAdd(dst + (size_t)G * 2 + 1, (double)tt1); }
-          if (img0 + 2 < p.B && (t2 != 0.f || tt2 != 0.f)) { atomicAdd(dst + (size_t)G * 4, (double)t2); atomicAdd(dst + (size_t)G * 4 + 1, (double)tt2); }
-        }
-      }
-      t0 = t1 = t2 = tt0 = tt1 = tt2 = 0.f;
-    }
-  }
-
-  // tile index ti: window rows r = 0..127 are positions w0 + r, w0 = 126 * ti - 1; outputs are rows 1..126.
-  // bnd: shared exchange buffer [parity 2][kind 2 (0: row 31 of D_-1, 1: row 0 of D_+1)][quarter 4][128] floats
-  __device__ __forceinline__ void tile(const ConvParams& p, const float* sbias, float* bnd, uint32_t tmem_acc, int ti, uint64_t* tfull,
-                                       uint32_t parity, uint64_t* tempty, int it = 0, int xpar = 0) {
-    (void)it;
-    const bool ts = threadIdx.x == 64;   // timeline stamps (DMD_TIMELINE builds): first epilogue thread
-    (void)ts;
-    const int w0 = ti * 126 - 1;
-    const int q_first = w0 + 1;
-    const int n_lo = (int)p.dPH.div(p.dPW.div((uint32_t)q_first));
-    const int q_last = min(q_first + 126, p.Q) - 1;
-    const bool single_image = (int)p.dPH.div(p.dPW.div((uint32_t)q_last)) == n_lo;
-    if (n_cur >= 0 && (!single_image || n_lo != n_cur)) { flush_stats(p, n_cur, false); n_cur = -1; }
-    // the four window rows of this thread: m = quarter*32 + 8*j + g, j = 0..3
-    int opix[4], slot[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int m = quarter * 32 + 8 * j + g;
-      const int q = w0 + m;
-      opix[j] = -1; slot[j] = 0;
-      if (m >= 1 && m <= 126 && q < p.Q) {
-        const uint32_t R = p.dPW.div((uint32_t)q);
-        const int x = q - (int)R * p.PW;
-        const int n = (int)p.dPH.div(R);
-        const int y = (int)R - n * p.PH;
-        bool valid = (x < p.W) && (y < p.H);
-        int yo = y, xo = x, Ho = p.H, Wo = p.W;
-        if (p.stride == 2) {
-          valid = valid && ((x & 1) == 0) && ((y & 1) == 0);
-          yo = y >> 1; xo = x >> 1; Ho = p.H >> 1; Wo = p.W >> 1;
-        }
-        if (valid) { opix[j] = (n * Ho + yo) * Wo + xo; slot[j] = n - n_lo; }
-      }
-    }
-    float* bup = bnd + (size_t)(((grp * 2 + xpar) * 2 + 0) * 4) * 128;    // [quarter][col]: row 31 of the D_-1 block
-    float* bdn = bnd + (size_t)(((grp * 2 + xpar) * 2 + 1) * 4) * 128;    //                 row 0 of the D_+1 block
-    bool waited = false;
-    auto chunk = [&](auto nbc, auto vecc, int blk) {
-      constexpr int NB = decltype(nbc)::value;
-      constexpr bool VEC = decltype(vecc)::value;
-      const int col0 = blk * 8 + lc;
-      float2 rr[4][NB];
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-#pragma unroll
-        for (int k = 0; k < NB; ++k) {
-          rr[j][k] = make_float2(0.f, 0.f);
-          const int col = col0 + 8 * k;
-          if (p.resid != nullptr && opix[j] >= 0 && col < p.Cout) {
-            const float* rp = p.resid + (size_t)opix[j] * p.Cout + col;
-            if (VEC) rr[j][k] = __ldg(reinterpret_cast<const float2*>(rp));
-            else { rr[j][k].x = __ldg(rp); if (col + 1 < p.Cout) rr[j][k].y = __ldg(rp + 1); }
-          }
-        }
-      if (!waited) {
-        if (ts) DMD_TS(2, it, 0);
-        mbar_wait(tfull, parity);
-        if (ts) DMD_TS(2, it, 1);
-        tc_fence_after_sync();
-        waited = true;
-      }
-      uint32_t rm[8 * NB], rz[8 * NB], rp_[8 * NB];   // D_-1, D_0, D_+1 blocks: columns dx * CoutPad + blk*8 ...
-      const uint32_t ta = tmem_acc + (uint32_t)(blk * 8) + ((uint32_t)(quarter * 32) << 16);
-      tmem_ld_16x256b_pair<NB>(ta, ta + (16u << 16), rm);
-      tmem_ld_16x256b_pair<NB>(ta + (uint32_t)p.CoutPad, ta + (uint32_t)p.CoutPad + (16u << 16), rz);
-      tmem_ld_16x256b_pair<NB>(ta + 2u * (uint32_t)p.CoutPad, ta + 2u * (uint32_t)p.CoutPad + (16u << 16), rp_);
-      if (blk + NB >= blk_end) {
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0 && tempty != nullptr) mbar_arrive(tempty);
-      }
-      // ---- edge rows of this warp's quarter for the neighbouring quarters
-      if (g == 7) {   // window row 31 of the quarter (j = 3 -> register block h = 1, s = 1)
-#pragma unroll
-        for (int k = 0; k < NB; ++k) {
-          bup[quarter * 128 + col0 + 8 * k] = __uint_as_float(rm[4 * NB + 4 * k + 2]);
-          bup[quarter * 128 + col0 + 8 * k + 1] = __uint_as_float(rm[4 * NB + 4 * k + 3]);
-        }
-      }
-      if (g == 0) {   // window row 0 of the quarter (j = 0 -> h = 0, s = 0)
-#pragma unroll
-        for (int k = 0; k < NB; ++k) {
-          bdn[quarter * 128 + col0 + 8 * k] = __uint_as_float(rp_[4 * k]);
-          bdn[quarter * 128 + col0 + 8 * k + 1] = __uint_as_float(rp_[4 * k + 1]);
-        }
-      }
-      if (ts && blk == blk_begin) DMD_TS(2, it, 2);
-      named_bar_sync(bar_id, bar_threads);
-      if (ts && blk == blk_begin) DMD_TS(2, it, 8);
-      const int src_up = (lane - 4) & 31, src_dn = (lane + 4) & 31;
-      float2 bv[NB];
-#pragma unroll
-      for (int k = 0; k < NB; ++k) bv[k] = (col0 + 8 * k < p.Cout) ? *reinterpret_cast<const float2*>(sbias + col0 + 8 * k) : make_float2(0.f, 0.f);
-#pragma unroll
-      for (int k = 0; k < NB; ++k) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          // register of window row 8*j + g: index (j >> 1) * 4 * NB + 4 * k + 2 * (j & 1) + e
-          float tm[4], tp[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int idx = (j >> 1) * 4 * NB + 4 * k + 2 * (j & 1) + e;
-            tm[j] = __shfl_sync(0xffffffffu, __uint_as_float(rm[idx]), src_up);    // D_-1 at the lane four below (row - 1 when g >= 1)
-            tp[j] = __shfl_sync(0xffffffffu, __uint_as_float(rp_[idx]), src_dn);   // D_+1 at the lane four above (row + 1 when g <= 6)
-          }
-          const int col = col0 + 8 * k + e;
-          const float e_up = (quarter > 0) ? bup[(quarter - 1) * 128 + col] : 0.f;   // row -1 of this quarter = row 31 of the previous one
-          const float e_dn = (quarter < 3) ? bdn[(quarter + 1) * 128 + col] : 0.f;   // row 32 = row 0 of the next one
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int idx = (j >> 1) * 4 * NB + 4 * k + 2 * (j & 1) + e;
-            const float up = (g >= 1) ? tm[j] : (j >= 1 ? tm[j >= 1 ? j - 1 : 0] : e_up);
-            const float dn = (g <= 6) ? tp[j] : (j <= 2 ? tp[j <= 2 ? j + 1 : 3] : e_dn);
-            const float o = (up + __uint_as_float(rz[idx])) + dn + (e ? bv[k].y : bv[k].x) + (e ? rr[j][k].y : rr[j][k].x);
-            rz[idx] = __float_as_uint(o);      // the output value replaces the centre block register
-          }
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        if (opix[j] >= 0) {
-          float* op = p.out + (size_t)opix[j] * p.Cout + col0;
-          float sps = 0.f, spss = 0.f;
-#pragma unroll
-          for (int k = 0; k < NB; ++k) {
-            if (col0 + 8 * k < p.Cout) {
-              const int idx = (j >> 1) * 4 * NB + 4 * k + 2 * (j & 1);
-              const float ox = __uint_as_float(rz[idx]), oy = __uint_as_float(rz[idx + 1]);
-              if (VEC) *reinterpret_cast<float2*>(op + 8 * k) = make_float2(ox, oy);
-              else { op[8 * k] = ox; if (col0 + 8 * k + 1 < p.Cout) op[8 * k + 1] = oy; }
-              sps += ox + ((VEC || col0 + 8 * k + 1 < p.Cout) ? oy : 0.f);
-              spss = fmaf(ox, ox, spss); if (VEC || col0 + 8 * k + 1 < p.Cout) spss = fmaf(oy, oy, spss);
-            }
-          }
-          if (p.ostats != nullptr) {
-            const int sl = single_image ? 0 : slot[j];
-            if ((blk - blk_begin) * 8 < p.ogs) {     // chunk inside the warp's first group (uniform per chunk)
-              s0 += (sl == 0) ? sps : 0.f;  ss0 += (sl == 0) ? spss : 0.f;
-              s1 += (sl == 1) ? sps : 0.f;  ss1 += (sl == 1) ? spss : 0.f;
-              s2 += (sl == 2) ? sps : 0.f;  ss2 += (sl == 2) ? spss : 0.f;
-            } else {
-              t0 += (sl == 0) ? sps : 0.f;  tt0 += (sl == 0) ? spss : 0.f;
-              t1 += (sl == 1) ? sps : 0.f;  tt1 += (sl == 1) ? spss : 0.f;
-              t2 += (sl == 2) ? sps : 0.f;  tt2 += (sl == 2) ? spss : 0.f;
-            }
-          }
-        }
-      }
-    };
-    for (int blk = blk_begin; blk < blk_end;) {
-      const int rem = blk_end - blk;
-      if (!vec2) { chunk(std::integral_constant<int, 1>{}, std::false_type{}, blk); blk += 1; }
-      else if (rem >= 2) { chunk(std::integral_constant<int, 2>{}, std::true_type{}, blk); blk += 2; }
-      else { chunk(std::integral_constant<int, 1>{}, std::true_type{}, blk); blk += 1; }
-    }
-    if (p.ostats != nullptr) {
-      if (single_image) n_cur = n_lo;
-      else { flush_stats(p, n_lo, true); n_cur = -1; }
-    }
-    if (ts) DMD_TS(2, it, 3);
-  }
-
-  __device__ __forceinline__ void finish(const ConvParams& p) {
-    if (n_cur >= 0) flush_stats(p, n_cur, false);
-  }
-};
-
-// kAccCols: TMEM columns per accumulator (>= CoutPad); two accumulators are allocated.
-// kGroups : epilogue organisation.  0: DIRECT -- the eight warps read the accumulator with the 16-lane x 256-bit TMEM pattern, whose
-//           register layout puts 32 contiguous bytes of an output row into four neighbouring threads, and store (+bias, +residual)
-//           straight to global memory as full 32-byte sectors: no shared-memory staging, no row table, no named barriers; the
-//           GroupNorm partial sums are reduced with warp shuffles.  The tile loop is bound by the shared-memory port (operand
-//           re-reads of the nine taps), so taking the epilogue's 64 KB per tile off that port is what this buys.
-//           1: the eight epilogue warps work on one tile at a time through a staging tile.  2: two independent groups of four
-//           warps (each covers the four TMEM lane quarters) own accumulator 0 / 1 and take alternate tiles, with their own
-//           staging tile and named barriers -- the epilogue is latency-bound (0.84 IPC per SM in the round-1 profile), so two
-//           tiles in flight hide each other's TMEM / shared-memory / barrier latencies.
-template <int kAccCols, int kGroups>
+// N: accumulator columns (power of two >= CoutPad); kTaps: 9 (3x3) or 1 (1x1), equal to p.taps
+template <int N, int kTaps>
 __global__ void __launch_bounds__(kConvThreads, 1) conv_tc_kernel(const ConvParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint64_t* wbar = reinterpret_cast<uint64_t*>(smem);
   uint64_t* full = wbar + 1;                 // [kMaxStages]
   uint64_t* empty = full + kMaxStages;       // [kMaxStages]
-  uint64_t* tfull = empty + kMaxStages;      // [2]
-  uint64_t* tempty = tfull + 2;              // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  const ConvSmemLayout L = conv_smem_layout(conv_weight_bytes(p.taps, p.Cin, p.Cextra, p.CoutPad), p.CoutPad, p.Palloc, p.stages, kGroups);
+  const ConvSmemLayout L = conv_smem_layout(conv_weight_bytes(p.taps, p.Cin, p.Cextra, p.CoutPad), p.Palloc, p.stages);
   float* sbias = reinterpret_cast<float*>(smem + L.bias_off);
   uint8_t* sW = smem + L.w_off;
   uint8_t* sA = smem + L.a_off;
 
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
-  // halo positions in front of the tile's first window row (row-stacked mode: one image row; the dx shift lives on the output side)
-  const int halo = p.trs ? p.PW : ((p.taps == 9) ? (p.PW + 1) : 0);
-  const int lead = p.trs ? 1 : 0;            // window rows in front of the first output row
+  const int halo = (kTaps == 9) ? (p.PW + 1) : 0;   // positions in front of the tile's first row
   const int S = p.stages;
   const int main_slabs = p.Cin >> 4;
   const int kslabs = main_slabs + p.xslabs;   // slabs that travel through the ring (the projection's hi slabs feed two MMAs)
@@ -611,8 +258,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_tc_kernel(const ConvPara
   pdl_launch_dependents();
   if (tid == 0) {
     mbar_init(wbar, 1);
-    for (int s = 0; s < S; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(tfull + b, 1); mbar_init(tempty + b, kGroups == 3 ? kEpiWarps / p.trs_groups : (kGroups == 0 ? kEpiWarps : kEpiWarps / kGroups)); }
+    for (int s = 0; s < S; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, kConvConsumerWarps); }
     fence_mbar_init();
     const uint32_t tap_bytes = (uint32_t)p.Cin * p.CoutPad * 2;
     const uint32_t extra_bytes = (uint32_t)p.Cextra * p.CoutPad * 2;
@@ -621,422 +267,113 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_tc_kernel(const ConvPara
       bulk_g2s(sW + (size_t)t * tap_bytes, reinterpret_cast<const uint8_t*>(p.wpk) + (size_t)t * tap_bytes, tap_bytes, wbar);
     if (extra_bytes) bulk_g2s(sW + w_main_bytes, p.wpk_extra, extra_bytes, wbar);
   }
-  if (warp == 1) tmem_alloc<2 * kAccCols>(tmem_slot);
   for (int i = tid; i < 128; i += blockDim.x)
     sbias[i] = ((p.bias != nullptr && i < p.Cout) ? __ldg(p.bias + i) : 0.f) + ((p.bias_extra != nullptr && i < p.Cout) ? __ldg(p.bias_extra + i) : 0.f);
-  if (kGroups == 1 || kGroups == 2)
-    for (int i = tid; i < kEpiWarps * kStatSlots * kMaxOutGroups * 2; i += blockDim.x) reinterpret_cast<float*>(smem + L.sstat_off)[i] = 0.f;
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();  // operands / residual / statistics come from earlier kernels
-  if (blockIdx.x == 0 && tid == 64) ktrace_stamp(p.ktrace);
+  if (blockIdx.x == 0 && tid == 128) ktrace_stamp(p.ktrace);
 
-  if (warp == 0 || warp == kProdWarp2) {
+  if (warp < 2) {
     // =========================================================================================== PRODUCERS (TMA)
-    // Two producer warps take alternate slabs of the global slab sequence.  One warp spends ~200 cycles per slab (the wait on
-    // the `empty` barrier alone is ~130 even when the phase has completed), which is slower than the tensor pipe consumes the
-    // centre-tap slabs of a fused projection (one MMA each): with 28 slabs per tile and a 12-stage ring the single producer
-    // set the tile time of those convs (11.6 k cycles per tile measured vs ~2.9 k of MMA work).
-    {  // converged warp, one elected lane issues the copies (uniform-register operands)
-      const uint32_t pid = (warp == 0) ? 0u : 1u;
-      const uint32_t chunk_bytes = (uint32_t)p.P * 16;
-      uint32_t stage = 0, phase = 0, nslab = 0;
-      for (int it = 0; it < my_tiles; ++it) {
-        // first halo position of this tile inside a plane (guard G keeps it non-negative)
-        const size_t pos0 = (size_t)((tile_begin + it) * p.tile_stride - lead - halo + p.G) * 16;
-        int seg = 0, seg_ks = 0;  // current operand segment and slab index inside it
-        for (int ks = 0; ks < kslabs; ++ks, ++nslab) {
-          if ((nslab & 1u) == pid) {
-            DMD_TS(0, it, (ks & 3) * 3 + 0);
-            mbar_wait(empty + stage, phase ^ 1u);
-            DMD_TS(0, it, (ks & 3) * 3 + 1);
-            if (elect_one_sync()) {
-              uint8_t* slab = sA + (size_t)stage * L.slab_bytes;
-              // projection slabs (centre tap only): the tile's own 128 rows, no halo
-              const bool xs = ks >= main_slabs;
-              const uint32_t bytes = xs ? (uint32_t)kTileM * 16 : chunk_bytes;
-              mbar_expect_tx(full + stage, 2 * bytes);
-              const uint8_t* plane = p.seg_base[seg] + (size_t)(2 * seg_ks) * p.plane_bytes + pos0 + (xs ? (size_t)halo * 16 : 0);
-              bulk_g2s(slab, plane, bytes, full + stage);
-              bulk_g2s(slab + (size_t)p.Palloc * 16, plane + p.plane_bytes, bytes, full + stage);
-            }
-            __syncwarp();
-            DMD_TS(0, it, (ks & 3) * 3 + 2);
-          }
-          if (++seg_ks == p.seg_slabs[seg]) { seg_ks = 0; ++seg; }
-          if (++stage == (uint32_t)S) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // =========================================================================================== MMA ISSUER
-    // The whole warp walks the loop CONVERGED and one elected lane issues (elect.sync): every loop variable is warp-uniform,
-    // so the descriptors live in uniform registers and each tcgen05.mma is a single predicated UTCHMMA.  (Issuing from a
-    // divergent `lane == 0` branch makes ptxas wrap every MMA in an R2UR + ELECT uniformisation loop; the issuing thread is
-    // latency-bound on its own scalar instructions, so that overhead -- not the tensor pipe -- set the tile time.)
-    // Descriptor words are precomputed: per MMA only the 14-bit start-address fields change (A: ring stage + tap shift,
-    // both in 16-byte units; B: tap + slab).
-    if (my_tiles > 0) {
-      mbar_wait(wbar, 0);
-      const uint32_t idesc = umma_idesc_f16(kTileM, (uint32_t)p.CoutPad, 0, 0);
-      const uint32_t a_lbo = (uint32_t)p.Palloc * 16, b_lbo = (uint32_t)p.CoutPad * 16;
-      const uint32_t hi = (128u >> 4) | (1u << 14);                       // SBO = 128 B, descriptor version 1
-      const uint32_t a_lo0 = ((smem_u32(sA) >> 4) & 0x3FFFu) | (((a_lbo >> 4) & 0x3FFFu) << 16);
-      const uint32_t b_lo0 = ((smem_u32(sW) >> 4) & 0x3FFFu) | (((b_lbo >> 4) & 0x3FFFu) << 16);
-      const uint32_t b_x0 = (((smem_u32(sW) + w_main_bytes) >> 4) & 0x3FFFu) | (((b_lbo >> 4) & 0x3FFFu) << 16);
-      const uint32_t slab16 = L.slab_bytes >> 4;
-      const uint32_t tap16 = ((uint32_t)p.Cin * p.CoutPad * 2) >> 4;     // bytes of one tap of weights, /16
-      const uint32_t kstep16 = (2u * b_lbo) >> 4;                          // one 16-channel slab of weights, /16
-      const bool nine = p.taps == 9;
-      uint32_t shift[9], b_tap[9];
-#pragma unroll
-      for (int t = 0; t < 9; ++t) {
-        shift[t] = (uint32_t)(halo + (nine ? (t / 3 - 1) * p.PW + (t % 3 - 1) : 0));
-        b_tap[t] = (uint32_t)t * tap16;
-      }
-      if constexpr (kGroups == 3) {
-        // ---- tap-row-stacked: per slab three MMAs (dy = -1, 0, +1) of N = 3 * CoutPad, A shifted by whole image rows only
-        const uint32_t idesc3 = umma_idesc_f16(kTileM, 3u * (uint32_t)p.CoutPad, 0, 0);
-        const uint32_t b3_lbo = 3u * (uint32_t)p.CoutPad * 16;
-        const uint32_t b3_lo0 = ((smem_u32(sW) >> 4) & 0x3FFFu) | (((b3_lbo >> 4) & 0x3FFFu) << 16);
-        const uint32_t row16 = ((uint32_t)p.Cin * 3u * p.CoutPad * 2) >> 4;   // one kernel row (three taps) of weights, /16
-        const uint32_t k3step16 = (2u * b3_lbo) >> 4;
-        const uint32_t pw = (uint32_t)p.PW;
-        uint32_t stage = 0, phase = 0, a_lo = a_lo0;
-        uint32_t tph0 = 1u, tph1 = 1u;
-        for (int it = 0; it < my_tiles; ++it) {
-          const int b = it & 1;
-          DMD_TS(1, it, 12);
-          mbar_wait(tempty + b, b ? tph1 : tph0);
-          DMD_TS(1, it, 13);
-          if (b) tph1 ^= 1u; else tph0 ^= 1u;
-          tc_fence_after_sync();
-          const uint32_t d_tmem = tmem_base + (uint32_t)b * kAccCols;
-          uint32_t b_lo = b3_lo0;
-          for (int ks = 0; ks < kslabs; ++ks) {
-            DMD_TS(1, it, (ks & 3) * 3 + 0);
-            mbar_wait(full + stage, phase);
-            DMD_TS(1, it, (ks & 3) * 3 + 1);
-            tc_fence_after_sync();
-            if (elect_one_sync()) {
-              if (ks >= main_slabs) {
-                // fused 1x1 projection: centre tap, N = CoutPad, accumulated into the dx = 0 column block (hi slabs: two MMAs)
-                const uint32_t e = (uint32_t)(ks - main_slabs), ng = (uint32_t)p.xslabs >> 1;
-                const uint64_t ad = ((uint64_t)hi << 32) | (uint64_t)a_lo;
-                const uint64_t bd = ((uint64_t)hi << 32) | (uint64_t)(b_x0 + e * kstep16);
-                umma_f16(d_tmem + (uint32_t)p.CoutPad, ad, bd, idesc, 1u);
-                if (e < ng) {
-                  const uint64_t bd2 = ((uint64_t)hi << 32) | (uint64_t)(b_x0 + (2u * ng + e) * kstep16);
-                  umma_f16(d_tmem + (uint32_t)p.CoutPad, ad, bd2, idesc, 1u);
-                }
-              } else {
-#pragma unroll
-                for (int dy = 0; dy < 3; ++dy) {
-                  const uint64_t ad = ((uint64_t)hi << 32) | (uint64_t)(a_lo + (uint32_t)dy * pw);
-                  const uint64_t bd = ((uint64_t)hi << 32) | (uint64_t)(b_lo + (uint32_t)dy * row16);
-                  umma_f16(d_tmem, ad, bd, idesc3, (ks | dy) != 0 ? 1u : 0u);
-                }
-              }
-              umma_commit(empty + stage);
-              if (ks == kslabs - 1) umma_commit(tfull + b);
-            }
-            __syncwarp();
-            DMD_TS(1, it, (ks & 3) * 3 + 2);
-            b_lo += k3step16;
-            a_lo += slab16;
-            if (++stage == (uint32_t)S) { stage = 0; phase ^= 1u; a_lo = a_lo0; }
-          }
-          DMD_TS(1, it, 14);
-        }
-      } else {
-      uint32_t stage = 0, phase = 0, a_lo = a_lo0;
-      uint32_t tph0 = 1u, tph1 = 1u;  // parity to wait on for tempty[b]: first use passes immediately
-      for (int it = 0; it < my_tiles; ++it) {
-        const int b = it & 1;
-        DMD_TS(1, it, 12);
-        mbar_wait(tempty + b, b ? tph1 : tph0);
-        DMD_TS(1, it, 13);
-        if (b) tph1 ^= 1u; else tph0 ^= 1u;
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + (uint32_t)b * kAccCols;
-        uint32_t b_lo = b_lo0;
-        for (int ks = 0; ks < kslabs; ++ks) {
-          DMD_TS(1, it, (ks & 3) * 3 + 0);
-          mbar_wait(full + stage, phase);
-          DMD_TS(1, it, (ks & 3) * 3 + 1);
-          tc_fence_after_sync();
+    // Two producer warps take alternate slabs of the global slab sequence: one warp alone spends ~200 cycles per slab (mostly
+    // the wait on the `empty` barrier), more than the tensor cores need for the centre-tap slabs of a fused projection.
+    // The warp stays converged and one elected lane issues the copies (uniform-register operands).
+    const uint32_t pid = (uint32_t)warp;
+    const uint32_t chunk_bytes = (uint32_t)p.P * 16;
+    uint32_t stage = 0, phase = 0, nslab = 0;
+    for (int it = 0; it < my_tiles; ++it) {
+      // first halo position of this tile inside a plane (guard G keeps it non-negative)
+      const size_t pos0 = (size_t)((tile_begin + it) * kTileM - halo + p.G) * 16;
+      int seg = 0, seg_ks = 0;  // current operand segment and slab index inside it
+      for (int ks = 0; ks < kslabs; ++ks, ++nslab) {
+        if ((nslab & 1u) == pid) {
+          mbar_wait(empty + stage, phase ^ 1u);
           if (elect_one_sync()) {
-            if (!DMD_DBG(2)) {
-              if (ks >= main_slabs) {
-                // fused projection (centre tap, slab = the tile's rows): weights [W_hi | W_hi | W_lo] along K; a hi slab of group g
-                // meets W_hi (block g) and W_lo (block 2*ng + g), a lo slab W_hi (block ng + g)
-                const uint32_t e = (uint32_t)(ks - main_slabs), ng = (uint32_t)p.xslabs >> 1;
-                const uint64_t ad = ((uint64_t)hi << 32) | (uint64_t)a_lo;
-                const uint64_t bd = ((uint64_t)hi << 32) | (uint64_t)(b_x0 + e * kstep16);
-                umma_f16(d_tmem, ad, bd, idesc, 1u);
-                if (e < ng) {
-                  const uint64_t bd2 = ((uint64_t)hi << 32) | (uint64_t)(b_x0 + (2u * ng + e) * kstep16);
-                  umma_f16(d_tmem, ad, bd2, idesc, 1u);
-                }
-              } else if (nine) {
-#pragma unroll
-                for (int t = 0; t < 9; ++t) {
-                  const uint64_t ad = ((uint64_t)hi << 32) | (uint64_t)(a_lo + (DMD_DBG(16) ? 0u : shift[t]));   // dbg 16: every tap at the (aligned) slab base -- timing experiment, wrong results
-                  const uint64_t bd = ((uint64_t)hi << 32) | (uint64_t)(b_lo + b_tap[t]);
-                  umma_f16(d_tmem, ad, bd, idesc, (ks | t) != 0 ? 1u : 0u);
-                }
-              } else {
-                const uint64_t ad = ((uint64_t)hi << 32) | (uint64_t)(a_lo + shift[0]);
-                const uint64_t bd = ((uint64_t)hi << 32) | (uint64_t)b_lo;
-                umma_f16(d_tmem, ad, bd, idesc, ks != 0 ? 1u : 0u);
-              }
-            }
-            umma_commit(empty + stage);                       // slab reusable once these MMAs retire
-            if (ks == kslabs - 1) umma_commit(tfull + b);     // accumulator complete (same lane: commits track its MMAs)
+            uint8_t* slab = sA + (size_t)stage * L.slab_bytes;
+            // projection slabs (centre tap only): the tile's own 128 rows, no halo
+            const bool xs = ks >= main_slabs;
+            const uint32_t bytes = xs ? (uint32_t)kTileM * 16 : chunk_bytes;
+            mbar_expect_tx(full + stage, 2 * bytes);
+            const uint8_t* plane = p.seg_base[seg] + (size_t)(2 * seg_ks) * p.plane_bytes + pos0 + (xs ? (size_t)halo * 16 : 0);
+            bulk_g2s(slab, plane, bytes, full + stage);
+            bulk_g2s(slab + (size_t)p.Palloc * 16, plane + p.plane_bytes, bytes, full + stage);
           }
           __syncwarp();
-          DMD_TS(1, it, (ks & 3) * 3 + 2);
-          b_lo += kstep16;
-          a_lo += slab16;
-          if (++stage == (uint32_t)S) { stage = 0; phase ^= 1u; a_lo = a_lo0; }
         }
-        DMD_TS(1, it, 14);
+        if (++seg_ks == p.seg_slabs[seg]) { seg_ks = 0; ++seg; }
+        if (++stage == (uint32_t)S) { stage = 0; phase ^= 1u; }
       }
-      }  // generic tap loop
     }
-    __syncwarp();
-  } else {
-    // =========================================================================================== EPILOGUE (8 warps)
-    if constexpr (kGroups == 3) {
-      // ---- tap-row-stacked epilogue: three row-shifted accumulator blocks -> registers -> global (TrsEpilogue above)
-      TrsEpilogue<kAccCols> epi;
-      epi.init(p, warp, lane, p.trs_groups);
-      float* bnd = reinterpret_cast<float*>(smem + L.stage_off);
-      for (int it = epi.grp; it < my_tiles; it += p.trs_groups) {
-        const int b = it & 1;                    // two groups: accumulator b belongs to group b
-        const int xpar = p.trs_groups == 2 ? ((it >> 1) & 1) : (it & 1);
-        epi.tile(p, sbias, bnd, tmem_base + (uint32_t)b * kAccCols, tile_begin + it, tfull + b, ((uint32_t)it >> 1) & 1u, tempty + b, it, xpar);
-      }
-      epi.finish(p);
-    } else if constexpr (kGroups == 0) {
-      // ---- direct epilogue: TMEM (16 lanes x 256 bit pattern) -> registers -> (+bias, +residual) -> global (DirectEpilogue above)
-      DirectEpilogue<kAccCols> epi;
-      epi.init(p, warp, lane);
-      for (int it = 0; it < my_tiles; ++it) {
-        const int b = it & 1;
-        epi.tile(p, sbias, tmem_base + (uint32_t)b * kAccCols, (tile_begin + it) * kTileM, tfull + b, ((uint32_t)it >> 1) & 1u, tempty + b);
-      }
-      epi.finish(p);
-    } else {
-    constexpr int GT = kEpiThreads / (kGroups ? kGroups : 1);  // threads per epilogue group
-    constexpr int GW = kEpiWarps / (kGroups ? kGroups : 1);    // warps per group (8 or 4): GW / 4 warps share one TMEM lane quarter
-    const int et_all = tid - 64;               // 0..255
-    const int grp = et_all / GT;               // epilogue group of this thread
-    const int et = et_all - grp * GT;          // thread index inside the group
-    const int ew = et >> 5;                    // warp inside the group
-    const int bar0 = 8 + grp * 4;              // named barriers of this group: bar0 .. bar0+3
-    int2* rowinfo = reinterpret_cast<int2*>(smem + L.rowinfo_off) + grp * kTileM;
-    float* sstat = reinterpret_cast<float*>(smem + L.sstat_off) + grp * GW * kStatSlots * kMaxOutGroups * 2;
-    uint8_t* sStage = smem + L.stage_off + (size_t)grp * kTileM * L.stage_pitch;
-    const int quarter = warp & 3;              // TMEM lane quarter this warp may access
-    const int nchunks = p.CoutPad >> 4;
-    constexpr int kShare = GW / 4;             // warps of the group per quarter: they split the columns
-    const int ch_per = (nchunks + kShare - 1) / kShare;
-    const int ch_begin = (ew >> 2) * ch_per, ch_end = min(nchunks, ch_begin + ch_per);
-    const int G = p.ostats ? p.Cout / p.ogs : 1;
-    const int L4 = p.Cout >> 2;                // float4 per output row (vector path)
-    const bool vec_ok = (p.Cout & 3) == 0 && (L4 & (L4 - 1)) == 0 && L4 <= 32;  // 16/32/64/128 channels
-    const int lg = 31 - __clz(L4 > 0 ? L4 : 1);
-    const int c4 = et & (L4 - 1), r0 = et >> lg, rstep = GT >> lg;
-    const int ogrp = p.ostats ? (c4 * 4) / p.ogs : 0;   // a thread's channel quad, hence its group, is fixed
-    const int lanes_per_group = p.ogs >> 2;            // lanes (float4s) covering one group inside a row
-    // GroupNorm partial sums (scalars: arrays indexed by the image slot end up in local memory).  A CTA owns a contiguous
-    // range of tiles and an image spans many tiles, so (s0, ss0) RUN across consecutive single-image tiles of image n_cur and
-    // are reduced / flushed only when the image changes; a tile that straddles images uses the three slots and flushes at once.
-    float s0 = 0.f, s1 = 0.f, s2 = 0.f, ss0 = 0.f, ss1 = 0.f, ss2 = 0.f;
-    int n_cur = -1;
-    auto flush_stats = [&](int img0, bool multi) {
-      bool leader = true;
+  } else if (warp >= 4) {
+    // =========================================================================================== CONSUMERS (wgmma)
+    const int m0 = ((warp >> 2) - 1) * 64;     // first tile row of this warpgroup
+    RegEpilogue<N> epi;
+    epi.init(p, m0 + 16 * (warp & 3) + (lane >> 2), lane);
+    if (my_tiles > 0) mbar_wait(wbar, 0);
+    // Descriptor words: per wgmma only the 14-bit start-address fields change (A: ring stage + tap shift, B: tap + slab), all in
+    // 16-byte units.  K-major operands: LBO = stride of the 8-channel chunks, SBO = 128 B (eight 16-byte rows).
+    const uint64_t hi = gmma_desc_hi(128);
+    const uint32_t a_lbo = (uint32_t)p.Palloc * 16;
+    const uint32_t b_lbo = (uint32_t)(p.trs ? 3 * p.CoutPad : p.CoutPad) * 16;
+    const uint32_t x_lbo = (uint32_t)p.CoutPad * 16;
+    const uint32_t a_lo0 = (((smem_u32(sA) + (uint32_t)m0 * 16) >> 4) & 0x3FFFu) | (((a_lbo >> 4) & 0x3FFFu) << 16);
+    const uint32_t b_lo0 = ((smem_u32(sW) >> 4) & 0x3FFFu) | (((b_lbo >> 4) & 0x3FFFu) << 16);
+    const uint32_t b_x0 = (((smem_u32(sW) + w_main_bytes) >> 4) & 0x3FFFu) | (((x_lbo >> 4) & 0x3FFFu) << 16);
+    const uint32_t slab16 = L.slab_bytes >> 4;
+    const uint32_t kstep16 = (2u * b_lbo) >> 4;                          // one 16-channel slab of main weights, /16
+    const uint32_t xstep16 = (2u * x_lbo) >> 4;                          // one 16-channel slab of projection weights, /16
+    uint32_t shift[kTaps], b_tap[kTaps];
 #pragma unroll
-      for (int m = 1; m < 32; m <<= 1) {
-        // the xor-m partner lane is in the same group iff m stays inside the group span or jumps whole rows
-        const bool same = (m < lanes_per_group && m < L4) || (m >= L4);
-        if (same) {
-          s0 += __shfl_xor_sync(0xffffffffu, s0, m);
-          ss0 += __shfl_xor_sync(0xffffffffu, ss0, m);
-          if (multi) {
-            s1 += __shfl_xor_sync(0xffffffffu, s1, m);
-            ss1 += __shfl_xor_sync(0xffffffffu, ss1, m);
-            s2 += __shfl_xor_sync(0xffffffffu, s2, m);
-            ss2 += __shfl_xor_sync(0xffffffffu, ss2, m);
-          }
-          if (lane & m) leader = false;
-        }
-      }
-      if (leader) {  // exactly one leader lane per (warp, group): plain stores, summed in fixed order below
-        float* dstp = sstat + ((size_t)ew * kStatSlots * kMaxOutGroups + ogrp) * 2;
-        *reinterpret_cast<float2*>(dstp) = make_float2(s0, ss0);
-        if (multi) {
-          *reinterpret_cast<float2*>(dstp + kMaxOutGroups * 2) = make_float2(s1, ss1);
-          *reinterpret_cast<float2*>(dstp + 2 * kMaxOutGroups * 2) = make_float2(s2, ss2);
-        }
-      }
-      named_bar_sync(bar0 + 3, GT);   // every reuse of sstat is separated from these reads by barrier bar0 or bar0+1
-      if (et < (multi ? kStatSlots : 1) * G * 2) {
-        const int k = et / (G * 2), r = et - k * (G * 2);
-        const int og = r >> 1, which = r & 1;
-        float pw[GW];
-#pragma unroll
-        for (int w = 0; w < GW; ++w) pw[w] = sstat[(((size_t)w * kStatSlots + k) * kMaxOutGroups + og) * 2 + which];
-        // fixed-order pairwise tree: deterministic within the group
-        float tsum = (pw[0] + pw[1]) + (pw[2] + pw[3]);
-        if (GW == 8) tsum += (pw[4 % GW] + pw[5 % GW]) + (pw[6 % GW] + pw[7 % GW]);
-        const double val = (double)tsum;
-        const int img = img0 + k;
-        if (val != 0.0 && img < p.B) atomicAdd(p.ostats + ((size_t)img * G + og) * 2 + which, val);
-      }
-      s0 = s1 = s2 = ss0 = ss1 = ss2 = 0.f;
+    for (int t = 0; t < kTaps; ++t) {
+      shift[t] = (uint32_t)(halo + (kTaps == 9 ? (t / 3 - 1) * p.PW + (t % 3 - 1) : 0));
+      b_tap[t] = p.trs ? ((uint32_t)(t / 3) * p.Cin * 3u * p.CoutPad * 2 + (uint32_t)(t % 3) * p.CoutPad * 16) >> 4
+                       : ((uint32_t)t * p.Cin * p.CoutPad * 2) >> 4;
+    }
+    const int ng = p.xslabs >> 1;   // projection: hi slabs, then as many lo slabs
+    float acc[N / 2];
+    uint32_t stage = 0, phase = 0, prev = 0;
+    int done = 0;                   // slabs of the current tile consumed so far
+    // One ring slot: wait for its data, issue the wgmma of `issue` (a fixed, straight-line set: wgmma in a divergent path
+    // between fence and commit would make ptxas serialise every wgmma of the kernel), then release the previous slot as soon
+    // as its wgmma have retired.
+    auto slab = [&](auto issue) {
+      mbar_wait(full + stage, phase);
+      wgmma_fence();
+      issue(a_lo0 + stage * slab16);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (done > 0 && lane == 0) mbar_arrive(empty + prev);
+      prev = stage;
+      ++done;
+      if (++stage == (uint32_t)S) { stage = 0; phase ^= 1u; }
     };
-    for (int it = grp; it < my_tiles; it += (kGroups ? kGroups : 1)) {
-      const int b = it & 1;                    // kGroups == 2: accumulator b belongs to group b
-      const int q0 = (tile_begin + it) * kTileM;
-      const int n_lo = (int)p.dPH.div(p.dPW.div((uint32_t)q0));
-      const int q_last = min(q0 + kTileM, p.Q) - 1;
-      const bool single_image = (int)p.dPH.div(p.dPW.div((uint32_t)q_last)) == n_lo;  // all rows of the tile in one image
-      if (et == 0) DMD_TS(2, it, 7);
-      if (n_cur >= 0 && (!single_image || n_lo != n_cur)) { flush_stats(n_cur, false); n_cur = -1; }
-      // ---- row bookkeeping (one thread per row)
-      if (et < kTileM) {
-        const int q = q0 + et;
-        int opix = -1, slot = 0;
-        if (q < p.Q) {
-          const uint32_t R = p.dPW.div((uint32_t)q);
-          const int x = q - (int)R * p.PW;
-          const int n = (int)p.dPH.div(R);
-          const int y = (int)R - n * p.PH;
-          bool valid = (x < p.W) && (y < p.H);
-          int yo = y, xo = x, Ho = p.H, Wo = p.W;
-          if (p.stride == 2) {
-            valid = valid && ((x & 1) == 0) && ((y & 1) == 0);
-            yo = y >> 1; xo = x >> 1; Ho = p.H >> 1; Wo = p.W >> 1;
-          }
-          if (valid && !DMD_DBG(8)) { opix = (n * Ho + yo) * Wo + xo; slot = n - n_lo; }
-        }
-        rowinfo[et] = make_int2(opix, slot);
+    for (int it = 0; it < my_tiles; ++it) {
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+      done = 0;
+      for (int ks = 0; ks < main_slabs; ++ks) {
+        const uint32_t b_lo = b_lo0 + (uint32_t)ks * kstep16;
+        slab([&](uint32_t a_lo) {
+#pragma unroll
+          for (int t = 0; t < kTaps; ++t) Wgmma<N>::template mma<0, 0>(acc, hi | (a_lo + shift[t]), hi | (b_lo + b_tap[t]), 1u);
+        });
       }
-      // ---- residual prefetch: it does not depend on the accumulator, so its latency hides behind the MMAs of this tile
-      const int iters = vec_ok ? kTileM / rstep : 0;  // 2..16
-      float4 rpre[8];
-      const bool prefetch = vec_ok && p.resid != nullptr && iters <= 8;
-      if (prefetch) {
-        named_bar_sync(bar0 + 2, GT);  // rowinfo visible
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          rpre[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (u < iters) {
-            const int2 ri = rowinfo[r0 + u * rstep];
-            if (ri.x >= 0) rpre[u] = __ldg(reinterpret_cast<const float4*>(p.resid + (size_t)ri.x * p.Cout + (size_t)c4 * 4));
-          }
-        }
-      }
-      // ---- pass 1: TMEM -> (+bias) -> staging
-      if (et == 0) DMD_TS(2, it, 0);
-      mbar_wait(tfull + b, ((uint32_t)it >> 1) & 1u);
-      if (et == 0) DMD_TS(2, it, 1);
-      tc_fence_after_sync();
-      {
-        const int row = quarter * 32 + lane;
-        const uint32_t trow = tmem_base + (uint32_t)b * kAccCols + ((uint32_t)(quarter * 32) << 16);
-        uint8_t* srow = sStage + (size_t)row * L.stage_pitch;
-        for (int ch = ch_begin; ch < ch_end; ++ch) {
-          float v[16];
-          tmem_ld16(trow + (uint32_t)ch * 16, v);
-          const float4* bp = reinterpret_cast<const float4*>(sbias + ch * 16);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float4 bv = bp[i];
-            *reinterpret_cast<float4*>(srow + (size_t)(ch * 16 + 4 * i) * 4) =
-                make_float4(v[4 * i] + bv.x, v[4 * i + 1] + bv.y, v[4 * i + 2] + bv.z, v[4 * i + 3] + bv.w);
-          }
-        }
-      }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty + b);   // TMEM accumulator may be overwritten
-      named_bar_sync(bar0, GT);
-      if (et == 0) DMD_TS(2, it, 2);
-      // ---- pass 2: staging -> (+residual) -> coalesced global stores, GroupNorm partial sums
-      if (vec_ok) {
-        // L4 is a power of two (host-checked for the vector path): thread owns channel quad c4 of rows r0, r0+rstep, ...
-#pragma unroll
-        for (int k0 = 0; k0 < 16; k0 += 4) {
-          if (k0 < iters) {
-            int2 ri[4]; float4 v[4], rr[4];
-            // all shared-memory (and, if not prefetched, residual) loads of the batch first, then the math and the stores
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              const int row = r0 + (k0 + u) * rstep;
-              ri[u] = (k0 + u < iters) ? rowinfo[row] : make_int2(-1, 0);
-              rr[u] = (prefetch && k0 + u < 8) ? rpre[(k0 + u) & 7] : make_float4(0.f, 0.f, 0.f, 0.f);
-              if (ri[u].x >= 0) {
-                v[u] = *reinterpret_cast<const float4*>(sStage + (size_t)row * L.stage_pitch + (size_t)c4 * 16);
-                if (p.resid && !prefetch) rr[u] = __ldg(reinterpret_cast<const float4*>(p.resid + (size_t)ri[u].x * p.Cout + (size_t)c4 * 4));
-              }
-            }
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              if (ri[u].x >= 0) {
-                float4 o = v[u];
-                o.x += rr[u].x; o.y += rr[u].y; o.z += rr[u].z; o.w += rr[u].w;
-                *reinterpret_cast<float4*>(p.out + (size_t)ri[u].x * p.Cout + (size_t)c4 * 4) = o;
-                if (p.ostats != nullptr) {
-                  const float ps = (o.x + o.y) + (o.z + o.w);
-                  const float pss = (o.x * o.x + o.y * o.y) + (o.z * o.z + o.w * o.w);
-                  if (single_image) { s0 += ps; ss0 += pss; }
-                  else {
-                    const int sl = ri[u].y;
-                    s0 += (sl == 0) ? ps : 0.f;  ss0 += (sl == 0) ? pss : 0.f;
-                    s1 += (sl == 1) ? ps : 0.f;  ss1 += (sl == 1) ? pss : 0.f;
-                    s2 += (sl == 2) ? ps : 0.f;  ss2 += (sl == 2) ? pss : 0.f;
-                  }
-                }
-              }
-            }
-          }
-        }
-        if (et == 0) DMD_TS(2, it, 4);
-        if (p.ostats != nullptr) {
-          if (single_image) n_cur = n_lo;            // keep running
-          else { flush_stats(n_lo, true); n_cur = -1; }
-        }
-      } else {
-        // narrow outputs (conv_out: 3 channels): scalar stores, no statistics
-        const int total = kTileM * p.Cout;
-        for (int idx = et; idx < total; idx += GT) {
-          const int row = idx / p.Cout, c = idx - row * p.Cout;
-          const int2 ri = rowinfo[row];
-          if (ri.x >= 0) {
-            float v = *reinterpret_cast<const float*>(sStage + (size_t)row * L.stage_pitch + (size_t)c * 4);
-            const size_t off = (size_t)ri.x * p.Cout + c;
-            if (p.resid) v += __ldg(p.resid + off);
-            p.out[off] = v;
-          }
-        }
-      }
-      if (et == 0) DMD_TS(2, it, 5);
-      named_bar_sync(bar0 + 1, GT);   // staging / rowinfo may be reused; sstat complete
-      if (et == 0) DMD_TS(2, it, 6);
-      if (et == 0) DMD_TS(2, it, 3);
+      // fused projection (centre tap, slab = the tile's rows): weights [W_hi | W_hi | W_lo] along K; hi slab g meets W_hi
+      // (block g) and W_lo (block 2*ng + g), lo slab g meets W_hi (block ng + g)
+      for (int g = 0; g < ng; ++g)
+        slab([&](uint32_t a_lo) {
+          Wgmma<N>::template mma<0, 0>(acc, hi | a_lo, hi | (b_x0 + (uint32_t)g * xstep16), 1u);
+          Wgmma<N>::template mma<0, 0>(acc, hi | a_lo, hi | (b_x0 + (uint32_t)(2 * ng + g) * xstep16), 1u);
+        });
+      for (int g = 0; g < ng; ++g)
+        slab([&](uint32_t a_lo) { Wgmma<N>::template mma<0, 0>(acc, hi | a_lo, hi | (b_x0 + (uint32_t)(ng + g) * xstep16), 1u); });
+      wgmma_wait<0>();
+      wgmma_fence_operands(acc);
+      if (done > 0 && lane == 0) mbar_arrive(empty + prev);
+      epi.tile(p, sbias, acc, (tile_begin + it) * kTileM);
     }
-    if (n_cur >= 0) flush_stats(n_cur, false);
-    }  // staged epilogue
+    epi.finish(p);
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_free<2 * kAccCols>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------------------------

@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, bulk async copy, tcgen05 (MMA / TMEM / commit / ld).
-// Everything here is hand-written for Blackwell; there is no fallback path.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, bulk async copy (TMA), wgmma.
+// Everything here is hand-written for Hopper; there is no fallback path.
 #pragma once
 #include <cstdint>
 #include <cuda_fp16.h>
@@ -47,15 +47,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ---------------------------------------------------------------- proxies / fences
-// generic-proxy smem writes (st.shared) -> visible to the async proxy (tcgen05.mma operand reads, TMA)
+// generic-proxy smem writes (st.shared) -> visible to the async proxy (wgmma operand reads, TMA)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- bulk async copy (TMA 1-D), global -> smem
@@ -67,125 +61,106 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
       : "memory");
 }
 
-// ---------------------------------------------------------------- TMEM alloc / free (one full warp executes)
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "TMEM columns: pow2 in [32,512]");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------- wgmma shared-memory matrix descriptors
+// SWIZZLE_NONE ("interleave") canonical layouts, 16-byte units:
+//   K-major : core matrix = 8 MN-rows x 16 B (8 k-elements), contiguous 128 B; LBO = stride of the 8-element K chunks,
+//             SBO = stride of the 8-row MN groups
+//   MN-major: core matrix = 8 k-rows x 16 B (8 MN-elements), contiguous 128 B; LBO = stride of the 8-row K groups,
+//             SBO = stride of the 8-element MN groups
+// bits [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout (0 = no swizzle).  The start address only has to be
+// 16-byte aligned, so a descriptor can address a window shifted by any whole number of 16-byte rows (the conv taps).
+__host__ __device__ __forceinline__ uint64_t gmma_desc_hi(uint32_t sbo_bytes) {
+  return (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
 }
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_free(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-
-// ---------------------------------------------------------------- UMMA descriptors
-// Shared-memory matrix descriptor, SWIZZLE_NONE ("interleave") canonical layouts (16-byte units):
-//   K-major : ((8,m),2):((1,SBO),LBO)   8 rows x 16 B contiguous core matrix; m-groups at SBO; 2 k-chunks at LBO
-//   MN-major: ((1,m),(8,k)):((X,SBO),(1,LBO))  core matrix = 8 k-rows x 16 B (8 mn-elems); m-groups SBO; k-groups LBO
-// bits [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout (0 = no swizzle)
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return gmma_desc_hi(sbo_bytes) | (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16);
 }
 
-// Instruction descriptor for kind::f16 (fp16 x fp16 -> fp32), dense, no negate.
-//   [4,6) c_format=1 (F32) | [7,10) a_format=0 (F16) | [10,13) b_format=0 (F16) | [15] a_major | [16] b_major
-//   [17,23) N>>3 | [24,29) M>>4          major: 0 = K-major, 1 = MN-major
-__host__ __device__ __forceinline__ uint32_t umma_idesc_f16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                            uint32_t b_mn_major) {
-  uint32_t d = 0;
-  d |= 1u << 4;
-  d |= (a_mn_major & 1u) << 15;
-  d |= (b_mn_major & 1u) << 16;
-  d |= ((N >> 3) & 0x3F) << 17;
-  d |= ((M >> 4) & 0x1F) << 24;
-  return d;
-}
+// ---------------------------------------------------------------- wgmma (one warpgroup, fp16 x fp16 -> fp32 registers)
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], both operands in shared memory.  Fragment of D held by thread t of the warpgroup
+// (warp w = t / 32, lane l):  d[4j + 2s + e] = D[16w + l/4 + 8s][8j + 2(l%4) + e].  kTransA / kTransB: 0 = K-major,
+// 1 = MN-major operand.
+template <int N>
+struct Wgmma;
+template <>
+struct Wgmma<16> {
+  template <int kTransA, int kTransB>
+  __device__ __forceinline__ static void mma(float (&d)[8], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+        "%8, %9, p, 1, 1, %11, %12;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(kTransA), "n"(kTransB)
+        : "memory");
+  }
+};
+template <>
+struct Wgmma<32> {
+  template <int kTransA, int kTransB>
+  __device__ __forceinline__ static void mma(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1, %19, %20;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(kTransA), "n"(kTransB)
+        : "memory");
+  }
+};
+template <>
+struct Wgmma<64> {
+  template <int kTransA, int kTransB>
+  __device__ __forceinline__ static void mma(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(kTransA), "n"(kTransB)
+        : "memory");
+  }
+};
+template <>
+struct Wgmma<128> {
+  template <int kTransA, int kTransB>
+  __device__ __forceinline__ static void mma(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(kTransA), "n"(kTransB)
+        : "memory");
+  }
+};
 
-// D[tmem] (+)= A[smem] * B[smem];  issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory");
 }
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// ---------------------------------------------------------------- TMEM -> registers (32 lanes x 16 columns, fp32)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  // ld + wait in ONE asm statement so the compiler cannot consume r[] before the wait retires.
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+// Orders the compiler's accesses of accumulator registers against the asynchronous wgmma (no instruction is emitted).
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operands(float (&d)[R]) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// ---------------------------------------------------------------- TMEM -> registers, 16 lanes x 256 bit pattern (x NB column blocks)
-// One instruction reads 16 TMEM lanes x (8 * NB) fp32 columns.  Thread i of the warp receives, for column block k:
-//   r[4k + 0..1] = (lane0 + i/4    , col0 + 8k + 2*(i%4) + {0,1})
-//   r[4k + 2..3] = (lane0 + i/4 + 8, col0 + 8k + 2*(i%4) + {0,1})
-// i.e. four neighbouring threads hold 32 contiguous bytes of one accumulator row: the registers can go straight to NHWC
-// global memory as full 32-byte sectors, with no shared-memory transpose.  The pair form issues the two 16-lane halves of the
-// warp's 32-lane quarter and waits once (loads + wait in ONE asm statement: the registers cannot be consumed early).
-template <int NB>
-__device__ __forceinline__ void tmem_ld_16x256b_pair(uint32_t taddr_lo, uint32_t taddr_hi, uint32_t* r);
-template <>
-__device__ __forceinline__ void tmem_ld_16x256b_pair<1>(uint32_t taddr_lo, uint32_t taddr_hi, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.16x256b.x1.b32 {%0, %1, %2, %3}, [%8];\n\t"
-      "tcgen05.ld.sync.aligned.16x256b.x1.b32 {%4, %5, %6, %7}, [%9];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-      : "r"(taddr_lo), "r"(taddr_hi)
-      : "memory");
-}
-template <>
-__device__ __forceinline__ void tmem_ld_16x256b_pair<2>(uint32_t taddr_lo, uint32_t taddr_hi, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.16x256b.x2.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%16];\n\t"
-      "tcgen05.ld.sync.aligned.16x256b.x2.b32 {%8, %9, %10, %11, %12, %13, %14, %15}, [%17];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr_lo), "r"(taddr_hi)
-      : "memory");
-}
-template <>
-__device__ __forceinline__ void tmem_ld_16x256b_pair<4>(uint32_t taddr_lo, uint32_t taddr_hi, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.16x256b.x4.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%32];\n\t"
-      "tcgen05.ld.sync.aligned.16x256b.x4.b32 {%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%33];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr_lo), "r"(taddr_hi)
-      : "memory");
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // ---------------------------------------------------------------- programmatic dependent launch (PDL)
 // launch_dependents: the next kernel in the stream (launched with the programmatic-serialization attribute) may start
 // its prologue now.  wait: block until the previous kernel has completed and its memory is visible.
 // elect.sync: one lane of a CONVERGED warp (deterministic for a given mask).  Code under `if (elect_one_sync())` keeps
-// warp-uniform values in uniform registers, which is what tcgen05.mma / cp.async.bulk / tcgen05.commit want.
+// warp-uniform values in uniform registers, which is what cp.async.bulk wants.
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred;
   asm volatile(

@@ -1,4 +1,4 @@
-"""ActorCritic (reference: src/models/actor_critic.py) with a native sm_100a forward for predict_act_value."""
+"""ActorCritic (reference: src/models/actor_critic.py) with a native sm_90a forward for predict_act_value."""
 import ctypes as C
 import math
 from collections import namedtuple
@@ -96,7 +96,7 @@ class ActorCritic(NativeStateMixin, nn.Module):
         lib = _lib.lib()
         dev = self.device
         if dev.type != "cuda":
-            raise RuntimeError("diamond_b200 runs on CUDA (sm_100a) only; move the model to a cuda device")
+            raise RuntimeError("diamond_b200 runs on CUDA (sm_90a) only; move the model to a cuda device")
         self.require_current_device(dev)
         if self._h is None:
             c = self.cfg

@@ -27,7 +27,7 @@ def conv1x1(cin: int, cout: int) -> nn.Conv2d:  # blocks.py:18
 class _NativeOnly(nn.Module):
     def forward(self, *args, **kwargs):
         raise RuntimeError(
-            f"{type(self).__name__} is a parameter container; it is executed by the native sm_100a executor of the "
+            f"{type(self).__name__} is a parameter container; it is executed by the native sm_90a executor of the "
             "enclosing model (InnerModel / ActorCritic), not called directly"
         )
 
@@ -79,7 +79,7 @@ class FourierFeatures(_NativeOnly):  # blocks.py:78-87
 
 
 class Downsample(_NativeOnly):  # blocks.py:93-100
-    """3x3 stride-2 conv, orthogonal init.  Executed as the stride-1 tcgen05 conv stored at even (y, x) (exact for k = 3, p = 1);
+    """3x3 stride-2 conv, orthogonal init.  Executed as the stride-1 wgmma conv stored at even (y, x) (exact for k = 3, p = 1);
     backward-data through `zero_insert_prep_kernel` (the adjoint of the subsampling) + the transposed conv."""
 
     def __init__(self, in_channels: int) -> None:

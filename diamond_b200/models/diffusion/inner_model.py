@@ -62,7 +62,7 @@ class InnerModel(NativeStateMixin, nn.Module):
         lib = _lib.lib()
         dev = self.noise_emb.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("diamond_b200 runs on CUDA (sm_100a) only; move the model to a cuda device")
+            raise RuntimeError("diamond_b200 runs on CUDA (sm_90a) only; move the model to a cuda device")
         self.require_current_device(dev)
         key = (float(sigma_data), float(sigma_offset_noise), dev.index)
         if self._h is None or self._h_key != key:

@@ -1,4 +1,4 @@
-"""RewEndModel (reference: src/models/rew_end_model.py) with a native sm_100a `predict_rew_end` (SURVEY.md 8 f1).
+"""RewEndModel (reference: src/models/rew_end_model.py) with a native sm_90a `predict_rew_end` (SURVEY.md 8 f1).
 
 The reward / termination model runs once per imagined step between the sampler and the policy (world_model_env.py:97) and
 over the burn-in frames of every fresh episode (:120-129).  Parameters live under the reference's names (state_dict keys,
@@ -75,7 +75,7 @@ class RewEndModel(NativeStateMixin, nn.Module):
         lib = _lib.lib()
         dev = self.device
         if dev.type != "cuda":
-            raise RuntimeError("diamond_b200 runs on CUDA (sm_100a) only; move the model to a cuda device")
+            raise RuntimeError("diamond_b200 runs on CUDA (sm_90a) only; move the model to a cuda device")
         self.require_current_device(dev)
         if self._h is None or self._h_dev != dev.index:
             if self._h is not None:

@@ -98,7 +98,7 @@ def conv2d_operand(n0: Tensor, n1: Optional[Tensor], c0: int, c1: int, b: int, h
                    residual: Optional[Tensor] = None, out_gs: int = 0, out: Optional[Tensor] = None,
                    ostats: Optional[Tensor] = None, debug: int = 0, debug_buf: Optional[Tensor] = None,
                    lo0: Optional[Tensor] = None, lo1: Optional[Tensor] = None, xproj=None, trs: bool = False):
-    """tcgen05 conv on already prepared PLC16 operand(s) (one kernel launch)."""
+    """wgmma conv on already prepared PLC16 operand(s) (one kernel launch)."""
     _cuda(n0, n1, wpk, bias, residual)
     ho, wo = h // stride, w // stride
     if out is None:
@@ -128,7 +128,7 @@ def conv2d_fprop(src0: Tensor, wpk: Tensor, cout: int, cout_pad: int, cin_pad: i
                  gamma: Optional[Tensor] = None, beta: Optional[Tensor] = None, eps: float = 1e-5,
                  residual: Optional[Tensor] = None, out_gs: int = 0, debug: int = 0, debug_buf: Optional[Tensor] = None,
                  precise: bool = False, trs: bool = False) -> Tuple[Tensor, Optional[Tensor]]:
-    """The reference's `conv(act(norm(cat(x, skip))))` on NHWC fp32 tensors: one prep launch + one tcgen05 conv launch.
+    """The reference's `conv(act(norm(cat(x, skip))))` on NHWC fp32 tensors: one prep launch + one wgmma conv launch.
     precise=True: split-fp16 operands (weights must be packed with precise=True)."""
     res = prep_act(src0, src1=src1, upsample=upsample, mode=prologue, silu=silu, stats0=stats0, stats1=stats1,
                    gs0=gs0, gs1=gs1, film=film, film_off=film_off, gamma=gamma, beta=beta, eps=eps, split=precise)
@@ -171,7 +171,7 @@ _partial = {}
 def conv2d_wgrad(grad_op: Tensor, cg: int, act_op: Tensor, ca: int, b: int, h: int, w: int, cout: int, cin: int, taps: int = 9, *,
                  dw: Optional[Tensor] = None, cin_tot: Optional[int] = None, ci_off: int = 0, inv_scale: Optional[Tensor] = None,
                  accumulate: bool = False, debug: int = 0) -> Tensor:
-    """tcgen05 weight gradient from two PLC16 operands (dL/dy with `cg` stored channels, conv input with `ca`)."""
+    """wgmma weight gradient from two PLC16 operands (dL/dy with `cg` stored channels, conv input with `ca`)."""
     _cuda(grad_op, act_op)
     lib = _lib.lib()
     cin_tot = cin if cin_tot is None else cin_tot

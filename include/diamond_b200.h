@@ -1,4 +1,4 @@
-/* diamond_b200 — C ABI of the B200-native DIAMOND hot path (libdiamond_b200.so).
+/* diamond_b200 — C ABI of the GPU-native DIAMOND hot path (libdiamond_b200.so, H100 / sm_90a).
  *
  * The reference (eloialonso/diamond @ 5bcd159) is pure Python and has no FFI of its own (SURVEY.md section 8b); the
  * seam is its Python module surface.  Every entry point below therefore names the reference call site it replaces.
@@ -48,8 +48,8 @@ int dmd_pack_conv_weight(const float* w, void* wpk, int Cout, int CoutPad, int C
 /* precise = 1: split-fp16 packing [W_hi | W_hi | W_lo] (3*Cin channels per tap) for dmd_conv_desc.precise convs: the
  * product is evaluated as A_hi W_hi + A_lo W_hi + A_hi W_lo on the tensor cores, i.e. to ~2^-22 instead of 2^-11.  Used
  * for the layers whose input is the raw residual stream (1x1 skip projections, conv_in) and for conv_out.
- * precise = 3: the tap-row-stacked layout [dy][Cin/8][3*CoutPad][8] of 3x3 kernels (dmd_conv_desc.wpk_layout = 1): one
- * tensor-core instruction per kernel ROW with N = 3*CoutPad, the dx shift applied on the output side (conv_tc.cuh). */
+ * precise = 3: the tap-row-stacked layout [dy][Cin/8][3*CoutPad][8] of 3x3 kernels (dmd_conv_desc.wpk_layout = 1): the
+ * three taps of a kernel row side by side as column blocks dx*CoutPad (conv_tc.cuh addresses each tap inside its row). */
 
 /* Activation operand ("PLC16": padded-linear, chunk-major fp16; layout in diamond_b200/csrc/conv_tc.cuh).  One pass over
  * an NHWC fp32 tensor applies what the reference runs on a conv INPUT — GroupNorm (blocks.py:28) or AdaGroupNorm
@@ -99,8 +99,8 @@ typedef struct dmd_conv_desc {
   float* out;            /* NHWC [B][Ho][Wo][Cout] */
   double* out_stats;     /* [B][Cout/out_gs][2], accumulated (caller zeroes) or NULL */
   int out_gs;
-  int debug;             /* bring-up only; 0 */
-  void* debug_buf;       /* bring-up only; NULL */
+  int debug;             /* reserved: must be 0 (rejected otherwise) */
+  void* debug_buf;       /* reserved: must be NULL (rejected otherwise) */
   int precise;           /* 1: split-fp16 (needs src*_lo and weights packed with precise = 1) */
   int wpk_layout;        /* 0: tap-major weights ; 1: tap-row-stacked (dmd_pack_conv_weight precise = 3; 3x3, non-split only) */
   const void* src0_lo;
@@ -122,7 +122,7 @@ int dmd_conv2d_fprop(const dmd_conv_desc* d, void* stream);
 int dmd_pack_conv_weight_dgrad(const float* w, void* wpk, int CoutF, int CinTotF, int ci_off, int CinK, int taps, void* stream);
 
 /* Backward-filter of nn.Conv2d (torch autograd conv2d_weight; reference forward src/models/blocks.py:18-19,96,109-110) on
- * tcgen05: dW[co][ci_off+ci][t] (+)= inv_scale * sum_q GY[q][co] * X[q + o_t][ci] over the padded-linear positions of the
+ * wgmma: dW[co][ci_off+ci][t] (+)= inv_scale * sum_q GY[q][co] * X[q + o_t][ci] over the padded-linear positions of the
  * two PLC16 operands (layout and kernel: diamond_b200/csrc/wgrad_tc.cuh).  Deterministic: per-CTA partial sums are reduced in
  * a fixed order.  A stride-2 conv passes its gradient zero-inserted (dmd_prep_desc.upsample = 2) at the conv INPUT size. */
 typedef struct dmd_wgrad_desc {
@@ -149,7 +149,7 @@ typedef struct dmd_conv_plan_info {
   int tiles;             /* 128-row tiles (one CTA per SM walks a contiguous range of them) */
   int kslabs;            /* 16-channel K slabs per tile, fused projection included */
   int stages;            /* depth of the shared-memory slab ring */
-  int tmem_cols;         /* TMEM columns per accumulator (two are allocated) */
+  int acc_cols;          /* accumulator columns of one wgmma (power of two >= CoutPad) */
   unsigned long long smem_bytes;    /* dynamic shared memory of the launch */
   unsigned long long weight_bytes;  /* resident packed weights */
 } dmd_conv_plan_info;
@@ -220,7 +220,7 @@ int dmd_inner_model_forward(dmd_denoiser* h, int B, int H, int W, const float* n
  * dmd_inner_model_forward_train = dmd_inner_model_forward that keeps every activation (and the GroupNorm statistics) in the
  * training workspace; dmd_denoiser_backward consumes them: given dL/d(model output) (B,C,H,W) it writes the gradient of
  * EVERY parameter into one flat fp32 buffer (16-byte aligned slices, layout from dmd_denoiser_grad_layout, state_dict
- * order; buffers such as noise_emb.weight get zeros).  Convolutions run on tcgen05 (dgrad = fprop with transposed weights,
+ * order; buffers such as noise_emb.weight get zeros).  Convolutions run on wgmma (dgrad = fprop with transposed weights,
  * wgrad = dmd_conv2d_wgrad), gradients carry a power-of-two loss scale chosen from max|grad_out| on the device.  The flat
  * buffer is what a data-parallel step all-reduces in ONE collective (utils.py:105-106 wraps each model in DDP instead). */
 size_t dmd_denoiser_train_workspace_bytes(const dmd_denoiser* h, int B, int H, int W);

@@ -26,7 +26,7 @@ def wgrad_over_positions(x: Tensor, gy: Tensor) -> Tensor:
     """Weight gradient of a 3x3 / stride-1 / pad-1 conv as nine GEMMs with K = positions (blocks.py:18 backward):
         gw[co, ci, dy+1, dx+1] = sum_q  GY[q, co] * X[q + dy*(W+1) + dx, ci]
     over ALL positions q of the padded line.  No boundary tests: out-of-image taps read the shared zero pads, and GY is zero
-    at pad positions because its operand is written by the same prep kernel.  This is the tcgen05 formulation: both operands
+    at pad positions because its operand is written by the same prep kernel.  This is the wgmma formulation: both operands
     are the PLC16 planes the forward already uses, read as MN-major (K = position) tiles."""
     b, c, h, w = x.shape
     pw = w + 1
@@ -43,7 +43,7 @@ def wgrad_over_positions(x: Tensor, gy: Tensor) -> Tensor:
 
 def dgrad_as_forward_conv(gy: Tensor, w: Tensor) -> Tensor:
     """Backward-data of the same conv = the forward implicit GEMM on gy with weights transposed and taps flipped
-    (verified on the tcgen05 kernel itself in tests/test_gpu_conv.py)."""
+    (verified on the wgmma kernel itself in tests/test_gpu_conv.py)."""
     return F.conv2d(gy, w.transpose(0, 1).flip(2, 3), padding=1)
 
 

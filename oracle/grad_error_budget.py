@@ -1,4 +1,4 @@
-"""Test-infrastructure tool (CPU): error budget of the BACKWARD pass when conv operands are rounded the way the tcgen05
+"""Test-infrastructure tool (CPU): error budget of the BACKWARD pass when conv operands are rounded the way the wgmma
 kernels round them (fp16 operands, fp32 accumulate), measured on the oracle against exact fp32 autograd.
 
     python oracle/grad_error_budget.py [small|default]

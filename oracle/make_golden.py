@@ -1,7 +1,7 @@
-"""Generates tests/golden/*.npz by running the UNMODIFIED reference (imported from /root/reference/src with test-side
-stub modules, oracle/ref_import.py) on seeded inputs and seeded 'de-zeroed' weights.  Run in the build container:
+"""Generates tests/golden/*.npz by running the UNMODIFIED reference (imported from its source tree with test-side
+stub modules, oracle/ref_import.py) on seeded inputs and seeded 'de-zeroed' weights.  Run where the reference tree is:
 
-    python oracle/make_golden.py
+    DIAMOND_REFERENCE_SRC=<reference checkout>/src python oracle/make_golden.py
 
 The fixtures pin oracle/torch_oracle.py (CPU tests) and the CUDA path (GPU tests) to the reference itself.
 Weights are NOT stored (17 MB); they are regenerated from the seed by torch_oracle.seeded_state_dict and guarded by a

@@ -1,9 +1,9 @@
-"""Test-only helper: import the UNMODIFIED reference (eloialonso/diamond) from /root/reference/src.
+"""Test-only helper: import the UNMODIFIED reference (eloialonso/diamond) from its source tree, given by
+DIAMOND_REFERENCE_SRC.
 
 ORACLE / TEST INFRASTRUCTURE ONLY.  Nothing in the product path (diamond_b200/) may import this.
-/root/reference does not exist on the GPU box, so this module is only used (a) by
-oracle/make_golden.py to generate tests/golden/*.npz in the build container and (b) by CPU tests
-that are skipped when the reference tree is absent.
+The reference is not part of this repository, so this module is only used by oracle/make_golden.py and
+oracle/make_reference_records.py to record tests/golden/* where the reference tree is available; no test needs it.
 
 The reference needs omegaconf / hydra / gymnasium / ale_py / torcheval at *import* time only
 (utils.py:11, trainer.py:7, envs/env.py:4-6, models/rew_end_model.py:8); none of them is used on the
@@ -14,11 +14,11 @@ import os
 import sys
 import types
 
-REF_SRC = os.environ.get("DIAMOND_REFERENCE_SRC", "/root/reference/src")
+REF_SRC = os.environ.get("DIAMOND_REFERENCE_SRC", "")   # the reference checkout's src/ directory; no default
 
 
 def available() -> bool:
-    return os.path.isdir(os.path.join(REF_SRC, "models"))
+    return bool(REF_SRC) and os.path.isdir(os.path.join(REF_SRC, "models"))
 
 
 def _stub(name, **attrs):
@@ -77,7 +77,7 @@ def install_stubs() -> None:
 def load():
     """Returns a namespace with the reference modules (models, envs, agent, data, utils)."""
     if not available():
-        raise RuntimeError(f"reference tree not found at {REF_SRC}")
+        raise RuntimeError(f"reference tree not found: set DIAMOND_REFERENCE_SRC to its src/ directory (now {REF_SRC!r})")
     install_stubs()
     if REF_SRC not in sys.path:
         sys.path.insert(0, REF_SRC)

@@ -1,5 +1,5 @@
 """CPU: host-side logic of bench.py that does not need a GPU -- the watchdog / time-budget wrapper around the secondary blocks
-of the bench line, and the parser that takes roofline.traffic from the committed ncu summary."""
+of the bench line, and the parser that takes roofline.traffic from an ncu summary."""
 import io
 import json
 import time
@@ -35,7 +35,14 @@ def test_secondary_block_watchdog_prints_the_line_and_exits():
     assert exits2 == [0] and out2.getvalue() == ""
 
 
-def test_roofline_traffic_comes_from_the_committed_ncu_summary():
-    traffic, src = bench.conv_traffic_from_profile()
-    assert src is not None and src.startswith("profiles/r") and "_prof_conv_" in src
-    assert 4.0e7 < traffic < 8.0e7          # DRAM read + write bytes of one 3x3 64->64 @64x64 launch at B = 32 (algorithmic: 50.3 MB)
+def test_roofline_traffic_is_parsed_from_the_newest_ncu_summary(tmp_path):
+    assert bench.conv_traffic_from_profile(str(tmp_path)) == (None, None)   # no capture: no traffic figure
+    prof = tmp_path / "profiles"
+    prof.mkdir()
+    rows = [["Section Name", "Metric Name", "Metric Unit", "Metric Value"],
+            ["Memory", "dram__bytes_read.sum", "Mbyte", "51.04"], ["Memory", "dram__bytes_write.sum", "Kbyte", "3,300"]]
+    (prof / "r01_prof_conv_a_summary.csv").write_text("Memory,dram__bytes_read.sum,byte,1\nMemory,dram__bytes_write.sum,byte,2\n")
+    (prof / "r02_prof_conv_b_summary.csv").write_text("\n".join(",".join(f'"{c}"' if "," in c else c for c in r) for r in rows) + "\n")
+    traffic, src = bench.conv_traffic_from_profile(str(tmp_path))
+    assert src == "profiles/r02_prof_conv_b_summary.csv"
+    assert traffic == 51.04e6 + 3.3e6

@@ -1,6 +1,7 @@
-"""CPU: index / buffer logic of the WorldModelEnv and env-loop mirrors must be BIT-EXACT against the live reference
-(SURVEY.md 8 a20/a24), driven by identical fake networks and identical RNG streams.  Skipped without the reference tree;
-the oracle-free invariants below it always run."""
+"""CPU: index / buffer logic of the WorldModelEnv and env-loop mirrors must be BIT-EXACT against the reference
+(SURVEY.md 8 a20/a24), driven by identical fake networks and identical RNG streams.  The reference side is recorded in
+tests/golden/reference_records.npz (SHA-256 of every tensor of the stream, oracle/make_reference_records.py); the
+oracle-free invariants below it always run."""
 import random
 from types import SimpleNamespace
 
@@ -10,7 +11,13 @@ import torch
 from diamond_b200.coroutines.env_loop import make_env_loop
 from diamond_b200.envs import world_model_env as mine
 from diamond_b200.models.actor_critic import compute_lambda_returns
-from oracle import ref_import
+from oracle.make_reference_records import digest, load_records
+
+LAMBDAS = (0.0, 0.95)
+
+
+def _records(golden_dir):
+    return load_records(golden_dir)
 
 
 class FakeDenoiser:
@@ -67,15 +74,12 @@ def _run_env(envmod, cfg_cls, sampler_cfg, steps=40, seed=3):
     return out
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree absent")
-def test_world_model_env_matches_reference_bit_for_bit():
-    ns = ref_import.load()
-    ref_env = ns.envs.world_model_env
-    a = _run_env(ref_env, ref_env.WorldModelEnvConfig, ns.diffusion.DiffusionSamplerConfig(3))
-    b = _run_env(mine, mine.WorldModelEnvConfig, mine.DiffusionSamplerConfig(3))
-    assert len(a) == len(b)
-    for x, y in zip(a, b):
-        assert x.dtype == y.dtype and x.shape == y.shape and torch.equal(x, y)
+def test_world_model_env_matches_reference_bit_for_bit(golden_dir):
+    want = _records(golden_dir)["world_model_env"]
+    got = [digest(t) for t in _run_env(mine, mine.WorldModelEnvConfig, mine.DiffusionSamplerConfig(3))]
+    assert len(got) == len(want)
+    for i, (x, y) in enumerate(zip(got, want)):
+        assert x == y, (i, x, y)
 
 
 class FakePolicy(torch.nn.Module):
@@ -107,20 +111,22 @@ def _run_loop(loop_factory, envmod, cfg_cls, sampler_cfg):
     return res
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree absent")
-def test_env_loop_and_lambda_returns_match_reference_bit_for_bit():
-    ns = ref_import.load()
-    ref_env = ns.envs.world_model_env
-    a = _run_loop(ns.env_loop.make_env_loop, ref_env, ref_env.WorldModelEnvConfig, ns.diffusion.DiffusionSamplerConfig(3))
-    b = _run_loop(make_env_loop, mine, mine.WorldModelEnvConfig, mine.DiffusionSamplerConfig(3))
-    assert len(a) == len(b)
-    for x, y in zip(a, b):
-        assert x.shape == y.shape and torch.equal(x, y)
+def lambda_returns_inputs():
     g = torch.Generator().manual_seed(0)
     rew = torch.randn(4, 9, generator=g) * 2; end = (torch.rand(4, 9, generator=g) < 0.1).long()
     trunc = (torch.rand(4, 9, generator=g) < 0.1).long(); vb = torch.randn(4, 9, generator=g)
-    for lam in (0.0, 0.95):
-        assert torch.equal(compute_lambda_returns(rew, end, trunc, vb, 0.985, lam), ns.actor_critic.compute_lambda_returns(rew, end, trunc, vb, 0.985, lam))
+    return rew, end, trunc, vb
+
+
+def test_env_loop_and_lambda_returns_match_reference_bit_for_bit(golden_dir):
+    rec = _records(golden_dir)
+    got = [digest(t) for t in _run_loop(make_env_loop, mine, mine.WorldModelEnvConfig, mine.DiffusionSamplerConfig(3))]
+    assert len(got) == len(rec["env_loop"])
+    for i, (x, y) in enumerate(zip(got, rec["env_loop"])):
+        assert x == y, (i, x, y)
+    rew, end, trunc, vb = lambda_returns_inputs()
+    for lam in LAMBDAS:
+        assert digest(compute_lambda_returns(rew, end, trunc, vb, 0.985, lam)) == rec["lambda_returns"][str(lam)]
 
 
 def test_world_model_env_invariants_without_reference():

@@ -1,4 +1,4 @@
-"""GPU: tcgen05 conv kernel (C-ABI dmd_conv2d_fprop) vs torch fp32 reference ops of the same op.
+"""GPU: wgmma conv kernel (C-ABI dmd_conv2d_fprop) vs torch fp32 reference ops of the same op.
 
 Operands are rounded to fp16 inside the kernel (fp32 accumulate), so the reference is evaluated both with exact fp32
 operands (tolerance 2e-3 of the output rms: the TF32-class error the reference's own GPU path has, trainer.py:41) and
@@ -111,8 +111,8 @@ def test_conv_plain(case):
 
 @pytest.mark.parametrize("case", [c for c in CASES if c.get("taps", 9) == 9], ids=lambda c: "-".join(f"{k}{v}" for k, v in c.items()))
 def test_conv_row_stacked_taps(case):
-    """The production layout of the 3x3 convs: one tensor-core instruction per kernel row (N = 3 * Cout) with the dx shift on the
-    output side, tiles of 126 outputs (TrsEpilogue, conv_tc.cuh) -- same results as the tap-major kernel."""
+    """The tap-row-stacked weight layout of the 3x3 convs (the three taps of a kernel row side by side, N = 3 * Cout; the kernel
+    addresses each tap inside its row, conv_tc.cuh) -- same results as the tap-major layout."""
     dev = _dev()
     got, ref32, ref16, _ = _run_conv(dev, trs=True, **case)
     assert got.shape == ref32.shape
@@ -164,7 +164,7 @@ def test_conv_precise_split_fp16(case):
 @pytest.mark.parametrize("trs", [False, True], ids=["tap-major", "row-stacked"])
 def test_conv_with_fused_skip_projection(trs):
     """ResBlock tail (blocks.py:142-145): conv2(silu(norm2(t))) + proj(cat(x, skip)) in ONE launch — the 1x1 projection is
-    extra K (split-fp16, centre tap) accumulated into the same TMEM tile."""
+    extra K (split-fp16, centre tap) accumulated into the same accumulator tile."""
     dev = _dev()
     from diamond_b200 import ops
 
@@ -191,7 +191,7 @@ def test_conv_with_fused_skip_projection(trs):
 def test_conv_dgrad_is_the_forward_kernel_with_transposed_flipped_weights(cin, cout):
     """Building block of the training rows (SURVEY.md 8 a18): backward-data of a 3x3 / stride-1 / pad-1 convolution
     (every ResBlock conv, blocks.py:137-139) is the SAME implicit GEMM on the output gradient with the weights transposed
-    (Cin <-> Cout) and the taps flipped, so it runs on the tcgen05 kernel unchanged.  Checked against torch autograd."""
+    (Cin <-> Cout) and the taps flipped, so it runs on the wgmma kernel unchanged.  Checked against torch autograd."""
     dev = _dev()
     from diamond_b200 import ops
 

@@ -1,4 +1,4 @@
-"""GPU: Denoiser.forward + loss.backward() on the native sm_100a path (SURVEY.md 8 a17/a18) against
+"""GPU: Denoiser.forward + loss.backward() on the native sm_90a path (SURVEY.md 8 a17/a18) against
 (1) the reference's own loss / gradient summary (tests/golden/denoiser_*_training.npz, written by the unmodified reference)
 and (2) the reference-pinned oracle's full fp32 autograd gradients, tensor by tensor.
 

@@ -1,4 +1,4 @@
-"""GPU: tcgen05 weight-gradient kernel (diamond_b200/csrc/wgrad_tc.cuh) and the dgrad packing helper against torch
+"""GPU: wgmma weight-gradient kernel (diamond_b200/csrc/wgrad_tc.cuh) and the dgrad packing helper against torch
 autograd's conv2d_weight / conv2d_input (the reference's backward: nn.Conv2d under loss.backward(), blocks.py:18-19,96,109).
 
 Operands are fp16 (PLC16), accumulation fp32: compared (a) with an fp16-operand fp64 reference to 2e-5 and (b) with exact
@@ -50,7 +50,7 @@ def _wgrad_case(dev, b, h, w, cin, cout, taps, seed, stride=1, debug=0):
 
 def test_wgrad_descriptor_probe():
     """Bring-up probe: reports which LBO/SBO reading of the MN-major no-swizzle descriptor matches (debug bit 0 swaps them)
-    and the per-tap errors, so ONE run on the B200 pins the layout.  The shipped setting (debug = 0) must be the exact one."""
+    and the per-tap errors, so ONE run on the GPU pins the layout.  The shipped setting (debug = 0) must be the exact one."""
     dev = _dev()
     res = {}
     for dbg in (0, 1):
@@ -69,7 +69,7 @@ def test_wgrad_descriptor_probe():
 @pytest.mark.parametrize("b,h,w,cin,cout,taps,stride", [
     (2, 16, 16, 64, 64, 9, 1),      # 8 tiles... multi-tile, one image row per ~8 tiles
     (3, 32, 32, 64, 64, 9, 1),      # ResBlock conv at 32x32
-    (5, 64, 64, 64, 64, 9, 1),      # 64x64: 165 tiles > 148 CTAs (uneven tile ranges)
+    (5, 64, 64, 64, 64, 9, 1),      # 64x64: 165 tiles > 132 CTAs (uneven tile ranges)
     (2, 8, 8, 64, 64, 9, 1),        # fewer tiles than SMs
     (2, 32, 32, 32, 64, 9, 1),      # Cin 32 (small config / actor-critic)
     (2, 32, 32, 64, 32, 9, 1),      # Cout 32: zero row groups

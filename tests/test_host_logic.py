@@ -4,7 +4,7 @@ import torch
 
 from diamond_b200.models.diffusion import (Denoiser, DenoiserConfig, DiffusionSamplerConfig, InnerModelConfig)
 from diamond_b200.models.diffusion.diffusion_sampler import build_sigmas
-from oracle import ref_import
+from oracle import make_reference_records as R
 from oracle import torch_oracle as O
 
 
@@ -14,20 +14,20 @@ def _denoiser(inner: O.InnerCfg) -> Denoiser:
                                                     inner.num_actions), 0.5, 0.3))
 
 
-@pytest.mark.parametrize("inner", [O.InnerCfg(), O.InnerCfg(depths=[1, 2, 1], channels=[32, 64, 32], attn_depths=[0, 0, 1],
-                                                             cond_channels=64, num_steps_conditioning=2, num_actions=6)])
-def test_state_dict_keys_and_shapes_match_the_reference_layout(inner):
+def _reference_records(golden_dir):
+    """What the unmodified reference reported (oracle/make_reference_records.py)."""
+    return R.load_records(golden_dir)
+
+
+@pytest.mark.parametrize("inner", [R.LAYOUT_INNERS["default"], R.LAYOUT_INNERS["small"]])
+def test_state_dict_keys_and_shapes_match_the_reference_layout(inner, golden_dir):
+    key = next(k for k, v in R.LAYOUT_INNERS.items() if v is inner)
     den = _denoiser(inner)
     want = O.inner_model_shapes(inner)
     got = [(k, tuple(v.shape)) for k, v in den.inner_model.state_dict().items()]
     assert got == want
-    if ref_import.available():
-        ns = ref_import.load()
-        D = ns.diffusion
-        ref = D.Denoiser(D.DenoiserConfig(D.InnerModelConfig(inner.img_channels, inner.num_steps_conditioning, inner.cond_channels,
-                                                             list(inner.depths), list(inner.channels), list(inner.attn_depths),
-                                                             inner.num_actions), 0.5, 0.3))
-        assert [(k, tuple(v.shape)) for k, v in ref.state_dict().items()] == [(k, tuple(v.shape)) for k, v in den.state_dict().items()]
+    ref = [(k, tuple(s)) for k, s in _reference_records(golden_dir)["state_dict_layout"][key]]
+    assert ref == [(k, tuple(v.shape)) for k, v in den.state_dict().items()]
 
 
 def test_default_denoiser_has_the_reference_parameter_count_and_init():
@@ -42,14 +42,19 @@ def test_default_denoiser_has_the_reference_parameter_count_and_init():
     assert torch.allclose(w @ w.t(), torch.eye(64), atol=1e-4)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree absent")
-def test_reference_configure_opt_accepts_the_mirror():
+def test_reference_configure_opt_accepts_the_mirror(golden_dir):
     """utils.configure_opt classifies parameters by isinstance(owner, nn.Conv2d/Linear/GroupNorm/...) and asserts full
-    coverage (utils.py:129-166): expected split for the denoiser is 114 decay / 121 no-decay (SURVEY.md 8b)."""
-    ns = ref_import.load()
+    coverage (utils.py:129-166): expected split for the denoiser is 114 decay / 121 no-decay (SURVEY.md 8b).  The split the
+    reference made of the mirror is recorded; the mirror must still have exactly those parameters, the decay group being
+    the weights of its Conv2d / Linear modules."""
+    decay, no_decay = _reference_records(golden_dir)["configure_opt_groups"]
+    assert [len(decay), len(no_decay)] == [114, 121]
     den = _denoiser(O.InnerCfg())
-    opt = ns.utils.configure_opt(den, 1e-4, 1e-2, 1e-8)
-    assert [len(g["params"]) for g in opt.param_groups] == [114, 121]
+    params = dict(den.named_parameters())
+    assert sorted(decay + no_decay) == sorted(params)
+    mods = dict(den.named_modules())
+    weights = {n for n in params if n.endswith(".weight") and isinstance(mods[n.rpartition(".")[0]], (torch.nn.Conv2d, torch.nn.Linear))}
+    assert set(decay) == weights
 
 
 def test_sigma_schedule_matches_reference_values():

@@ -37,7 +37,7 @@ def test_dominant_conv_plan():
     rc, i, _ = _conv()
     assert rc == 0
     assert i.tiles == -(-32 * 65 * 65 // 128) == 1057
-    assert i.kslabs == 4 and i.tmem_cols == 64
+    assert i.kslabs == 4 and i.acc_cols == 64
     assert i.stages == 16      # direct epilogue (no staging tile): four tiles' worth of 8.2 KB slabs next to 72 KB of weights
     assert i.weight_bytes == 9 * 64 * 64 * 2
     assert i.smem_bytes <= 227 * 1024
@@ -46,7 +46,7 @@ def test_dominant_conv_plan():
 @pytest.mark.parametrize("kw,kslabs,cols", [
     (dict(C0=64, C1=64, src1=P), 8, 64),                                              # u-block conv1: x || skip
     (dict(C0=16, precise=1, src0_lo=P), 3, 64),                                       # conv_in, split-fp16
-    (dict(C0=64, Cout=3, CoutPad=16), 4, 32),                                         # conv_out
+    (dict(C0=64, Cout=3, CoutPad=16), 4, 16),                                         # conv_out
     (dict(C0=64, xsrc0=P, xsrc0_lo=P, xsrc1=P, xsrc1_lo=P, xC0=64, xC1=64, wpk_x=P), 4 + 16, 64),  # conv2 + fused projection: hi and lo slabs once each (24 MMAs)
     (dict(C0=64, taps=1), 4, 64),
     (dict(C0=64, CoutPad=128, Cout=128, H=32, W=32), 4, 128),                         # 147 KB of weights: narrow images only
@@ -54,7 +54,7 @@ def test_dominant_conv_plan():
 def test_conv_plan_variants(kw, kslabs, cols):
     rc, i, err = _conv(**kw)
     assert rc == 0, err
-    assert i.kslabs == kslabs and i.tmem_cols == cols
+    assert i.kslabs == kslabs and i.acc_cols == cols
     assert 2 <= i.stages <= 24 and i.smem_bytes <= 227 * 1024
 
 
@@ -80,6 +80,7 @@ def test_conv_tiles_per_level(hw, tiles):
     (dict(C0=64, C1=64, src1=P, W=600, H=8, B=1), "shared memory too small"),
     (dict(src0=0), "null src0/out/wpk"),
     (dict(wpk_x=P), "bad fused projection operands"),
+    (dict(debug=1), "debug / debug_buf must be 0"),
 ])
 def test_conv_rejections_fail_loudly(kw, needle):
     rc, _, err = _conv(**kw)
@@ -101,9 +102,9 @@ def test_width_limit_is_the_shared_memory_ring(kw, w_ok, w_bad):
 
 
 def test_prep_plan_block_granularity():
-    """Low-resolution levels get smaller blocks so that the grid still covers the 148 SMs (>= 296 blocks wanted)."""
+    """Low-resolution levels get smaller blocks so that the grid still covers the 132 SMs (>= 264 blocks wanted)."""
     rc, blocks, ppb, nsrc, _ = _prep()
-    assert rc == 0 and ppb == 256 and nsrc == 1 and blocks >= 296
+    assert rc == 0 and ppb == 256 and nsrc == 1 and blocks >= 264
     rc, blocks, ppb, nsrc, _ = _prep(Hs=16, Ws=16)
     assert rc == 0 and ppb == 64
     rc, blocks, ppb, nsrc, _ = _prep(Hs=32, Ws=32, C1=64, src1=P, dst1=P)
