@@ -70,6 +70,16 @@ class ConvPlanInfo(C.Structure):  # dmd_conv_plan_info
                 ("smem_bytes", C.c_ulonglong), ("weight_bytes", C.c_ulonglong)]
 
 
+class NormBwdDesc(C.Structure):  # dmd_norm_bwd_desc
+    _fields_ = [("x", _vp), ("gy", _vp), ("stats", _vp), ("B", _i), ("HW", _i), ("C", _i), ("gs", _i), ("mode", _i), ("act", _i),
+                ("film", _vp), ("film_stride", _i), ("film_off", _i), ("film_ctot", _i), ("c_off", _i),
+                ("gamma", _vp), ("beta", _vp), ("eps", _f), ("sumA", _vp), ("sumB", _vp), ("sum_stride", _i),
+                ("gx", _vp), ("addend", _vp), ("accumulate", _i)]
+
+
+_ll = C.c_longlong
+
+
 # name -> (restype, argtypes); this table is also what tests use to check that every symbol is exported
 SIGNATURES = {
     "dmd_version": (_i, []),
@@ -91,6 +101,21 @@ SIGNATURES = {
     "dmd_attn_fwd": (_i, [_vp] * 10 + [_i, _i, _i, _i, _f, _vp]),
     "dmd_nchw_to_nhwc": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "dmd_nhwc_to_nchw": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
+    "dmd_norm_bwd": (_i, [C.POINTER(NormBwdDesc), _i, _vp]),
+    "dmd_norm_affine_grad": (_i, [C.POINTER(NormBwdDesc), _vp, _vp, _vp, _vp]),
+    "dmd_attn_bwd": (_i, [_vp] * 16 + [_i, _i, _i, _i, _f, _vp]),
+    "dmd_sgemm_partial_floats": (_ll, [_i, _i, _i, _i]),
+    "dmd_sgemm": (_i, [_vp, _ll, _ll, _vp, _ll, _ll, _vp, _ll, _i, _i, _i, _vp, _i, _i, _vp, _vp]),
+    "dmd_film_wgrad": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
+    "dmd_embedding_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "dmd_colsum": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _vp]),
+    "dmd_sumpool2": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "dmd_add": (_i, [_vp, _vp, _ll, _i, _vp]),
+    "dmd_dsilu_mul": (_i, [_vp, _vp, _vp, _ll, _vp]),
+    "dmd_maxpool2_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "dmd_lstm_cell_bwd": (_i, [_vp] * 6 + [_i, _i, _vp]),
+    "dmd_heads_bwd": (_i, [_vp] * 10 + [_i, _i, _i, _vp]),
+    "dmd_loss_scale": (_i, [_vp, _ll, _vp, _vp, _vp]),
     "dmd_denoiser_create": (_vp, [C.POINTER(DenoiserConfigC)]),
     "dmd_denoiser_destroy": (None, [_vp]),
     "dmd_denoiser_num_tensors": (_i, [_vp]),

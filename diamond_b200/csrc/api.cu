@@ -532,6 +532,243 @@ extern "C" int dmd_nhwc_to_nchw(const float* in, float* out, int B, int C, int C
   return 0;
 }
 
+// ---------------------------------------------------------------------------------------------- backward launchers
+// The launch geometry of every CUDA-core backward kernel (bwd_kernels.cuh).  The denoiser and actor-critic executors and the
+// per-op entry points (dmd_norm_bwd, dmd_colsum, ...) all launch through these, so the per-op tests run the executors' shapes.
+
+// loss scale S = scale[0] from max|g| (amax_bits zeroed by the caller), 1/S in scale[1]
+static int loss_scale_launch(const float* g, long long n, unsigned int* amax_bits, float* scale, cudaStream_t st) {
+  absmax_kernel<<<(int)std::min<long long>(std::max<long long>((n + 255) / 256, 1), 1184), 256, 0, st>>>(g, amax_bits, n);
+  DMD_LAUNCH_OK();
+  loss_scale_kernel<<<1, 1, 0, st>>>(amax_bits, scale);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+
+// column sums: up to 592 blocks of 256 / (Cb / 4) row lanes, at least 8 rows per lane
+static int colsum_launch(const float* x, float* out, float* out2, const float* inv, long long rows, int C, int Creal, cudaStream_t st) {
+  const int L4 = (C < 256 ? C : 256) >> 2, lanes = 256 / L4;
+  long long blocks = (rows + (long long)lanes * 8 - 1) / ((long long)lanes * 8);
+  blocks = blocks > 592 ? 592 : (blocks < 1 ? 1 : blocks);
+  colsum_kernel<<<dim3((unsigned)blocks, (C + 255) / 256), 256, 0, st>>>(x, out, out2, inv, rows, C, Creal);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+
+// norm + SiLU backward, pass 1 (per-channel sums) or pass 2 (gx).  Pixels per block: halved from the whole image until the
+// grid covers the SMs twice, but never below 32 pixels
+static int norm_bwd_ppb(int B, int HW) {
+  int ppb = HW;
+  while (ppb > 32 && (long long)B * ((HW + ppb - 1) / ppb) < 2 * kPlanSms) ppb >>= 1;
+  return ppb;
+}
+static int norm_bwd_launch(const NormBwdParams& nb, int pass, cudaStream_t st) {
+  const int ppb = norm_bwd_ppb(nb.B, nb.HW);
+  const dim3 grid((nb.HW + ppb - 1) / ppb, nb.B);
+  if (pass == 1) norm_bwd_pass1_kernel<<<grid, kNormThreads, 0, st>>>(nb, ppb);
+  else norm_bwd_pass2_kernel<<<grid, kNormThreads, 0, st>>>(nb, ppb);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+static int affine_param_grad_launch(const NormBwdParams& nb, float* dgamma, float* dbeta, const float* inv, cudaStream_t st) {
+  affine_param_grad_kernel<<<(nb.C + 127) / 128, 128, 0, st>>>(nb.sumA, nb.sumB, nb.B, nb.C, nb.sum_stride, dgamma, dbeta, inv);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+
+// strided SGEMM; chunks > 1 splits K into 16-aligned ranges whose partial products (splitk_partial_floats of `partial`) are
+// reduced in a fixed order.  The split count is ceil(K / kchunk), which can be fewer than `chunks`.
+static void splitk_plan(int K, int chunks, int* kchunk, int* splits) {
+  *kchunk = ((K + chunks - 1) / chunks + 15) / 16 * 16;
+  *splits = (K + *kchunk - 1) / *kchunk;
+}
+static long long splitk_partial_floats(int M, int N, int K, int chunks) {
+  if (chunks <= 1) return 0;
+  int kchunk, splits;
+  splitk_plan(K, chunks, &kchunk, &splits);
+  return (long long)splits * M * N;
+}
+static int sgemm_launch(const float* A, long long sam, long long sak, const float* Bm, long long sbk, long long sbn, float* C, long long ldc,
+                        int M, int N, int K, const float* alpha, int accumulate, int chunks, float* partial, cudaStream_t st) {
+  if (chunks > 1) {
+    DMD_CHECK(ldc == N && partial, "sgemm: split-K needs a dense result (ldc == N) and a partial buffer");
+    int kchunk, splits;
+    splitk_plan(K, chunks, &kchunk, &splits);
+    const long long count = (long long)M * N;
+    sgemm_kernel<<<dim3((N + 63) / 64, (M + 63) / 64, splits), 256, 0, st>>>(A, sam, sak, Bm, sbk, sbn, partial, N, M, N, K, nullptr, 0, kchunk, count);
+    DMD_LAUNCH_OK();
+    splitk_reduce_kernel<<<(unsigned)((count + 255) / 256), 256, 0, st>>>(partial, splits, count, C, alpha, accumulate);
+    DMD_LAUNCH_OK();
+    return 0;
+  }
+  sgemm_kernel<<<dim3((N + 63) / 64, (M + 63) / 64), 256, 0, st>>>(A, sam, sak, Bm, sbk, sbn, C, ldc, M, N, K, alpha, accumulate);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+
+// attention backward: one CTA per image, the recomputed forward and its gradients in dynamic shared memory
+static size_t attn_bwd_smem(int L, int C) {
+  return sizeof(float) * ((size_t)L * (C + 1) * 4 + (size_t)L * (3 * C + 4) * 2 + (size_t)(C / 8) * L * 3);
+}
+static int attn_bwd_launch(const AttnBwdParams& ab, int B, cudaStream_t st) {
+  DMD_CHECK((ab.C == 64 || ab.C == 32) && ab.L == kAttnL && ab.gs > 0 && ab.C % ab.gs == 0 && ab.C / ab.gs <= 4,
+            "attention backward: unsupported shape L=%d C=%d gs=%d", ab.L, ab.C, ab.gs);
+  const size_t smem = attn_bwd_smem(ab.L, ab.C);
+  if (ab.C == 64) attn_bwd_kernel<64><<<B, kAttnThreads, smem, st>>>(ab);
+  else attn_bwd_kernel<32><<<B, kAttnThreads, smem, st>>>(ab);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+
+static int film_wgrad_launch(const float* dfilm, const float* cond, float* grads, const long long* woff, const long long* boff,
+                             int B, int rows, int CC, const float* inv, cudaStream_t st) {
+  film_wgrad_kernel<<<(rows + 7) / 8, 256, 0, st>>>(dfilm, cond, grads, woff, boff, B, rows, CC, inv);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+static int embedding_bwd_launch(const float* de, const int64_t* act, float* dE, int B, int CC, int T, int num_actions, const float* inv,
+                                cudaStream_t st) {
+  embedding_bwd_kernel<<<(B * CC + 255) / 256, 256, 0, st>>>(de, act, dE, B, CC, T, num_actions, inv);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+// H, W: the pooled (output) size
+static int sumpool2_launch(const float* in, float* out, int B, int H, int W, int C, int accumulate, cudaStream_t st) {
+  const long long total4 = (long long)B * H * W * C / 4;
+  sumpool2_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>(in, out, H, W, C, accumulate, total4);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+static int add_launch(const float* a, float* out, long long total4, int accumulate, cudaStream_t st) {
+  add_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>(a, out, accumulate, total4);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+static int dsilu_mul_launch(const float* pre, const float* dh, float* out, long long n, cudaStream_t st) {
+  dsilu_mul_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pre, dh, out, n);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+// H, W: the pre-pool size
+static int maxpool2_bwd_launch(const float* y, const float* gp, float* gy, int B, int H, int W, int C, cudaStream_t st) {
+  const int total = (H / 2) * (W / 2) * C;
+  maxpool2_bwd_kernel<<<dim3((total + 255) / 256, B), 256, 0, st>>>(y, gp, gy, H, W, C);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+static int lstm_cell_bwd_launch(const float* gates, const float* c_in, const float* g_h, const float* g_c, float* dgates, float* g_c_in,
+                                int B, int Hd, cudaStream_t st) {
+  lstm_cell_bwd_kernel<<<(B * Hd + 255) / 256, 256, 0, st>>>(gates, c_in, g_h, g_c, dgates, g_c_in, B, Hd);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+// actor / critic heads: g_h, and the actor bias (dba) / critic weight and bias (dWc, dbc) gradients of the non-null head gradients
+static int heads_bwd_launch(const float* g_hx, const float* g_logits, const float* g_val, const float* hx_out, const float* Wa, const float* Wc,
+                            float* g_h, float* dba, float* dWc, float* dbc, int B, int Hd, int A, cudaStream_t st) {
+  heads_bwd_kernel<<<(B * Hd + 255) / 256, 256, 0, st>>>(g_hx, g_logits, g_val, Wa, Wc, g_h, B, Hd, A);
+  DMD_LAUNCH_OK();
+  if (g_logits) {
+    small_colsum_kernel<<<(A + 31) / 32, 32, 0, st>>>(g_logits, B, A, dba);   // A need not be a multiple of 4
+    DMD_LAUNCH_OK();
+  }
+  if (g_val) {
+    vec_outer_sum_kernel<<<(Hd + 127) / 128, 128, 0, st>>>(g_val, hx_out, dWc, dbc, B, Hd);
+    DMD_LAUNCH_OK();
+  }
+  return 0;
+}
+
+// ---- per-op entry points of the backward kernels (include/diamond_b200.h): validate, then the launchers above
+static int norm_bwd_params(const dmd_norm_bwd_desc* d, NormBwdParams* nb) {
+  DMD_CHECK(d && d->x && d->gy && d->stats && d->sumA && d->sumB, "norm_bwd: null argument");
+  DMD_CHECK(d->B > 0 && d->HW > 0 && d->C > 0 && d->C % 4 == 0 && d->C <= kMaxCin, "norm_bwd: C=%d must be a positive multiple of 4, <= %d", d->C, kMaxCin);
+  DMD_CHECK(d->gs > 0 && d->gs % 4 == 0 && d->C % d->gs == 0 && d->C / d->gs <= 8, "norm_bwd: bad group size %d for C=%d", d->gs, d->C);
+  DMD_CHECK(d->mode == 1 ? (d->film != nullptr && d->c_off + d->C <= d->film_ctot) : (d->mode == 2 && d->gamma && d->beta),
+            "norm_bwd: mode %d needs %s", d->mode, d->mode == 1 ? "film with c_off + C <= film_ctot" : "gamma and beta (mode 1 or 2)");
+  DMD_CHECK(d->sum_stride >= d->C, "norm_bwd: sum_stride %d < C %d", d->sum_stride, d->C);
+  NormBwdParams p;
+  p.x = d->x; p.gy = d->gy; p.stats = d->stats; p.B = d->B; p.HW = d->HW; p.C = d->C; p.gs = d->gs; p.mode = d->mode; p.act = d->act;
+  p.film = d->film; p.film_stride = d->film_stride; p.film_off = d->film_off; p.film_ctot = d->film_ctot; p.c_off = d->c_off;
+  p.gamma = d->gamma; p.beta = d->beta; p.eps = d->eps; p.sumA = d->sumA; p.sumB = d->sumB; p.sum_stride = d->sum_stride;
+  p.gx = d->gx; p.addend = d->addend; p.accumulate = d->accumulate;
+  *nb = p;
+  return 0;
+}
+extern "C" int dmd_norm_bwd(const dmd_norm_bwd_desc* d, int pass, void* stream) {
+  NormBwdParams nb;
+  if (norm_bwd_params(d, &nb)) return 1;
+  DMD_CHECK(pass == 1 || (pass == 2 && d->gx), "norm_bwd: pass must be 1 or 2 (pass 2 writes gx)");
+  return norm_bwd_launch(nb, pass, (cudaStream_t)stream);
+}
+extern "C" int dmd_norm_affine_grad(const dmd_norm_bwd_desc* d, float* dgamma, float* dbeta, const float* inv_scale, void* stream) {
+  NormBwdParams nb;
+  if (norm_bwd_params(d, &nb)) return 1;
+  DMD_CHECK(dgamma && dbeta, "norm_affine_grad: null dgamma / dbeta");
+  return affine_param_grad_launch(nb, dgamma, dbeta, inv_scale, (cudaStream_t)stream);
+}
+extern "C" int dmd_attn_bwd(const float* x, const double* stats_in, const float* gamma, const float* beta, const float* wqkv,
+                            const float* bqkv, const float* wout, const float* gout, float* gx, float* dgamma, float* dbeta, float* dwqkv,
+                            float* dbqkv, float* dwout, float* dbout, const float* inv_scale, int B, int L, int C, int gs, float eps,
+                            void* stream) {
+  DMD_CHECK(x && stats_in && gamma && beta && wqkv && bqkv && wout && gout && gx && dgamma && dbeta && dwqkv && dbqkv && dwout && dbout,
+            "attn_bwd: null argument");
+  if (init_kernels()) return 1;
+  AttnBwdParams ab{x, stats_in, gamma, beta, wqkv, bqkv, wout, gout, gx, dgamma, dbeta, dwqkv, dbqkv, dwout, dbout, inv_scale, L, C, gs, eps};
+  return attn_bwd_launch(ab, B, (cudaStream_t)stream);
+}
+extern "C" long long dmd_sgemm_partial_floats(int M, int N, int K, int chunks) { return splitk_partial_floats(M, N, K, chunks); }
+extern "C" int dmd_sgemm(const float* A, long long sam, long long sak, const float* Bm, long long sbk, long long sbn, float* C, long long ldc,
+                         int M, int N, int K, const float* alpha, int accumulate, int chunks, float* partial, void* stream) {
+  DMD_CHECK(A && Bm && C && M > 0 && N > 0 && K > 0 && ldc >= N, "sgemm: bad arguments");
+  return sgemm_launch(A, sam, sak, Bm, sbk, sbn, C, ldc, M, N, K, alpha, accumulate, chunks, partial, (cudaStream_t)stream);
+}
+extern "C" int dmd_film_wgrad(const float* dfilm, const float* cond, float* grads, const long long* woff, const long long* boff, int B, int rows,
+                              int CC, const float* inv_scale, void* stream) {
+  DMD_CHECK(dfilm && cond && grads && woff && boff && B > 0 && rows > 0 && CC > 0 && CC <= 256, "film_wgrad: bad arguments (CC <= 256)");
+  return film_wgrad_launch(dfilm, cond, grads, woff, boff, B, rows, CC, inv_scale, (cudaStream_t)stream);
+}
+extern "C" int dmd_embedding_bwd(const float* de, const int64_t* act, float* dE, int B, int CC, int T, int num_actions, const float* inv_scale,
+                                 void* stream) {
+  DMD_CHECK(de && act && dE && B > 0 && T > 0 && CC % T == 0 && num_actions > 0, "embedding_bwd: bad arguments");
+  return embedding_bwd_launch(de, act, dE, B, CC, T, num_actions, inv_scale, (cudaStream_t)stream);
+}
+extern "C" int dmd_colsum(const float* x, float* out, float* out2, const float* inv_scale, long long rows, int C, int Creal, void* stream) {
+  DMD_CHECK(x && out && rows > 0 && C > 0 && C % 4 == 0 && Creal <= C, "colsum: bad arguments (C a multiple of 4, Creal <= C)");
+  return colsum_launch(x, out, out2, inv_scale, rows, C, Creal, (cudaStream_t)stream);
+}
+extern "C" int dmd_sumpool2(const float* in, float* out, int B, int H, int W, int C, int accumulate, void* stream) {
+  DMD_CHECK(in && out && B > 0 && H > 0 && W > 0 && C % 4 == 0, "sumpool2: bad arguments (C a multiple of 4)");
+  return sumpool2_launch(in, out, B, H, W, C, accumulate, (cudaStream_t)stream);
+}
+extern "C" int dmd_add(const float* a, float* out, long long n, int accumulate, void* stream) {
+  DMD_CHECK(a && out && n > 0 && n % 4 == 0, "add: bad arguments (n a multiple of 4)");
+  return add_launch(a, out, n / 4, accumulate, (cudaStream_t)stream);
+}
+extern "C" int dmd_dsilu_mul(const float* pre, const float* dh, float* out, long long n, void* stream) {
+  DMD_CHECK(pre && dh && out && n > 0, "dsilu_mul: bad arguments");
+  return dsilu_mul_launch(pre, dh, out, n, (cudaStream_t)stream);
+}
+extern "C" int dmd_maxpool2_bwd(const float* y, const float* gp, float* gy, int B, int H, int W, int C, void* stream) {
+  DMD_CHECK(y && gp && gy && B > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0 && C > 0, "maxpool2_bwd: bad arguments (even H, W)");
+  return maxpool2_bwd_launch(y, gp, gy, B, H, W, C, (cudaStream_t)stream);
+}
+extern "C" int dmd_lstm_cell_bwd(const float* gates, const float* c_in, const float* g_h, const float* g_c, float* dgates, float* g_c_in,
+                                 int B, int Hd, void* stream) {
+  DMD_CHECK(gates && c_in && dgates && g_c_in && B > 0 && Hd > 0, "lstm_cell_bwd: bad arguments");
+  return lstm_cell_bwd_launch(gates, c_in, g_h, g_c, dgates, g_c_in, B, Hd, (cudaStream_t)stream);
+}
+extern "C" int dmd_heads_bwd(const float* g_hx, const float* g_logits, const float* g_val, const float* hx_out, const float* Wa,
+                             const float* Wc, float* g_h, float* dba, float* dWc, float* dbc, int B, int Hd, int A, void* stream) {
+  DMD_CHECK(Wa && Wc && g_h && B > 0 && Hd > 0 && A > 0, "heads_bwd: bad arguments");
+  DMD_CHECK(!g_logits || dba, "heads_bwd: g_logits needs dba");
+  DMD_CHECK(!g_val || (hx_out && dWc && dbc), "heads_bwd: g_val needs hx_out, dWc, dbc");
+  return heads_bwd_launch(g_hx, g_logits, g_val, hx_out, Wa, Wc, g_h, dba, dWc, dbc, B, Hd, A, (cudaStream_t)stream);
+}
+extern "C" int dmd_loss_scale(const float* g, long long n, unsigned int* amax, float* scale, void* stream) {
+  DMD_CHECK(g && amax && scale && n > 0, "loss_scale: bad arguments");
+  return loss_scale_launch(g, n, amax, scale, (cudaStream_t)stream);
+}
+
 // ---------------------------------------------------------------------------------------------- denoiser executor
 // zero-pad / crop copy of an NHWC tensor, then the GroupNorm partial sums of the result (the consumer's prologue reads them)
 static int resize_launch(const ResizeParams& p, cudaStream_t st) {
@@ -590,7 +827,8 @@ struct BOp {
   ConvParams conv; size_t smem = 0; int cols = 0;
   WgradLaunch wg;
   long long goff = -1, goff2 = -1;            // flat-gradient offsets (floats)
-  NormBwdParams nb; int ppb = 0, chunks = 0;
+  NormBwdParams nb;
+  int chunks = 0;                             // sgemm: split-K chunk count (<= 1: no split)
   const float* src = nullptr; float* dst = nullptr; long long rows = 0; int C = 0, Creal = 0, H = 0, W = 0, acc = 0; long long total4 = 0;
   AttnBwdParams ab; long long goffs[6] = {-1, -1, -1, -1, -1, -1};
   void* ms_ptr = nullptr; size_t ms_bytes = 0;
@@ -1078,10 +1316,7 @@ struct BwdBuilder {
       BOp m; m.kind = B_MEMSET; m.ms_ptr = pl->nsum; m.ms_bytes = (size_t)2 * pl->B * kMaxCin * 4; push(m);
     }
     nb.gx = gx; nb.addend = addend; nb.accumulate = accumulate ? 1 : 0;
-    // pixels per block: enough blocks to cover the SMs, at least 32 pixels each
-    int ppb = nb.HW;
-    while (ppb > 32 && (long long)pl->B * ((nb.HW + ppb - 1) / ppb) < 2 * kPlanSms) ppb >>= 1;
-    b1.nb = nb; b1.ppb = ppb; b1.chunks = (nb.HW + ppb - 1) / ppb;
+    b1.nb = nb;
     push(b1);
     if (mode == 2) {
       BOp a; a.kind = B_AFFINE; a.nb = nb; a.goff = h->goff[gamma_idx]; a.goff2 = h->goff[beta_idx]; push(a);
@@ -1443,10 +1678,7 @@ int run_backward(dmd_denoiser* h, Plan& pl, const float* grad_out, float* grads,
   DMD_CUDA(cudaMemsetAsync(pl.zero_begin, 0, pl.zero_bytes, st));
   // loss scale from the incoming gradient, then the scaled NHWC gradient of the model output
   const long long n_out = (long long)B * c.img_channels * HW;
-  absmax_kernel<<<(int)std::min<long long>((n_out + 255) / 256, 1184), 256, 0, st>>>(grad_out, pl.amax, n_out);
-  DMD_LAUNCH_OK();
-  loss_scale_kernel<<<1, 1, 0, st>>>(pl.amax, pl.scale);
-  DMD_LAUNCH_OK();
+  if (loss_scale_launch(grad_out, n_out, pl.amax, pl.scale, st)) return 1;
   nchw_to_nhwc_scaled_kernel<<<dim3((HW + 255) / 256, B), 256, 0, st>>>(grad_out, pl.gF, pl.scale, c.img_channels, 8, HW);
   DMD_LAUNCH_OK();
   for (const BOp& b : pl.bops) {
@@ -1454,61 +1686,33 @@ int run_backward(dmd_denoiser* h, Plan& pl, const float* grad_out, float* grads,
       case B_PREP: if (prep_launch(b.prep, b.prep_nsrc, st)) return 1; break;
       case B_CONV: if (conv_launch(b.conv, b.smem, b.cols, st)) return 1; break;
       case B_WGRAD: if (wgrad_launch(b.wg, grads + b.goff, st)) return 1; break;
-      case B_COLSUM: {
-        const int L4 = (b.C < 256 ? b.C : 256) >> 2, lanes = 256 / L4;
-        long long blocks = (b.rows + (long long)lanes * 8 - 1) / ((long long)lanes * 8);
-        if (blocks > 592) blocks = 592;
-        if (blocks < 1) blocks = 1;
-        colsum_kernel<<<dim3((unsigned)blocks, (b.C + 255) / 256), 256, 0, st>>>(b.src, grads + b.goff, b.goff2 >= 0 ? grads + b.goff2 : nullptr, inv, b.rows, b.C, b.Creal);
-        DMD_LAUNCH_OK();
+      case B_COLSUM:
+        if (colsum_launch(b.src, grads + b.goff, b.goff2 >= 0 ? grads + b.goff2 : nullptr, inv, b.rows, b.C, b.Creal, st)) return 1;
         break;
-      }
-      case B_NORM1: norm_bwd_pass1_kernel<<<dim3(b.chunks, B), kNormThreads, 0, st>>>(b.nb, b.ppb); DMD_LAUNCH_OK(); break;
-      case B_NORM2: norm_bwd_pass2_kernel<<<dim3(b.chunks, B), kNormThreads, 0, st>>>(b.nb, b.ppb); DMD_LAUNCH_OK(); break;
-      case B_AFFINE:
-        affine_param_grad_kernel<<<(b.nb.C + 127) / 128, 128, 0, st>>>(b.nb.sumA, b.nb.sumB, B, b.nb.C, b.nb.sum_stride, grads + b.goff, grads + b.goff2, inv);
-        DMD_LAUNCH_OK();
-        break;
-      case B_POOL: sumpool2_kernel<<<(unsigned)((b.total4 + 255) / 256), 256, 0, st>>>(b.src, b.dst, b.H, b.W, b.C, b.acc, b.total4); DMD_LAUNCH_OK(); break;
-      case B_ADD: add_kernel<<<(unsigned)((b.total4 + 255) / 256), 256, 0, st>>>(b.src, b.dst, b.acc, b.total4); DMD_LAUNCH_OK(); break;
+      case B_NORM1: if (norm_bwd_launch(b.nb, 1, st)) return 1; break;
+      case B_NORM2: if (norm_bwd_launch(b.nb, 2, st)) return 1; break;
+      case B_AFFINE: if (affine_param_grad_launch(b.nb, grads + b.goff, grads + b.goff2, inv, st)) return 1; break;
+      case B_POOL: if (sumpool2_launch(b.src, b.dst, B, b.H, b.W, b.C, b.acc, st)) return 1; break;
+      case B_ADD: if (add_launch(b.src, b.dst, b.total4, b.acc, st)) return 1; break;
       case B_ATTN: {
         AttnBwdParams ab = b.ab;
         ab.dgamma = grads + b.goffs[0]; ab.dbeta = grads + b.goffs[1]; ab.dwqkv = grads + b.goffs[2]; ab.dbqkv = grads + b.goffs[3];
         ab.dwout = grads + b.goffs[4]; ab.dbout = grads + b.goffs[5];
-        DMD_CHECK((ab.C == 64 || ab.C == 32) && ab.L == kAttnL, "attention backward: unsupported shape L=%d C=%d", ab.L, ab.C);
-        const size_t smem = sizeof(float) * ((size_t)ab.L * (ab.C + 1) * 4 + (size_t)ab.L * (3 * ab.C + 4) * 2 + (size_t)(ab.C / 8) * ab.L * 3);
-        if (ab.C == 64) attn_bwd_kernel<64><<<B, kAttnThreads, smem, st>>>(ab);
-        else attn_bwd_kernel<32><<<B, kAttnThreads, smem, st>>>(ab);
-        DMD_LAUNCH_OK();
+        if (attn_bwd_launch(ab, B, st)) return 1;
         break;
       }
       case B_MEMSET: DMD_CUDA(cudaMemsetAsync(b.ms_ptr, 0, b.ms_bytes, st)); break;
-      case B_SGEMM: {
-        float* C = b.c_goff >= 0 ? grads + b.c_goff : b.gc;
-        if (b.chunks > 1) {   // long-K product (dcond = dfilm Wf, K = all FiLM rows): split-K partials in tA, fixed-order reduce
-          const int kchunk = ((b.K + b.chunks - 1) / b.chunks + 15) / 16 * 16;
-          const int splits = (b.K + kchunk - 1) / kchunk;
-          const long long count = (long long)b.M * b.N;
-          sgemm_kernel<<<dim3((b.N + 63) / 64, (b.M + 63) / 64, splits), 256, 0, st>>>(b.ga, b.sam, b.sak, b.gb, b.sbk, b.sbn, pl.tA, b.N, b.M, b.N, b.K, nullptr, 0, kchunk, count);
-          DMD_LAUNCH_OK();
-          if (b.ldc != b.N) return fail("backward: split-K sgemm needs a dense result");
-          splitk_reduce_kernel<<<(unsigned)((count + 255) / 256), 256, 0, st>>>(pl.tA, splits, count, C, b.use_inv ? inv : nullptr, b.acc);
-          DMD_LAUNCH_OK();
-          break;
-        }
-        sgemm_kernel<<<dim3((b.N + 63) / 64, (b.M + 63) / 64), 256, 0, st>>>(b.ga, b.sam, b.sak, b.gb, b.sbk, b.sbn, C, b.ldc, b.M, b.N, b.K, b.use_inv ? inv : nullptr, b.acc);
-        DMD_LAUNCH_OK();
+      case B_SGEMM:   // the long-K product (dcond = dfilm Wf, K = all FiLM rows) is split; its partials live in tA
+        if (sgemm_launch(b.ga, b.sam, b.sak, b.gb, b.sbk, b.sbn, b.c_goff >= 0 ? grads + b.c_goff : b.gc, b.ldc, b.M, b.N, b.K,
+                         b.use_inv ? inv : nullptr, b.acc, b.chunks, pl.tA, st)) return 1;
         break;
-      }
       case B_FILMW:
-        film_wgrad_kernel<<<(h->film_rows + 7) / 8, 256, 0, st>>>(pl.dfilm, pl.cond, grads, pl.film_woff, pl.film_boff, B, h->film_rows, CC, inv);
-        DMD_LAUNCH_OK();
+        if (film_wgrad_launch(pl.dfilm, pl.cond, grads, pl.film_woff, pl.film_boff, B, h->film_rows, CC, inv, st)) return 1;
         break;
       case B_LINEAR: if (linear_launch(b.lin_in, b.lin_w, b.lin_b, b.lin_out, B, b.lin_K, b.lin_F, 0, st)) return 1; break;
-      case B_DSILU: dsilu_mul_kernel<<<(unsigned)((b.rows + 255) / 256), 256, 0, st>>>(b.src, b.ga, b.dst, b.rows); DMD_LAUNCH_OK(); break;
+      case B_DSILU: if (dsilu_mul_launch(b.src, b.ga, b.dst, b.rows, st)) return 1; break;
       case B_EMB:
-        embedding_bwd_kernel<<<(B * CC + 255) / 256, 256, 0, st>>>(b.src, pl.t_act, grads + b.goff, B, CC, c.num_steps_conditioning, c.num_actions, inv);
-        DMD_LAUNCH_OK();
+        if (embedding_bwd_launch(b.src, pl.t_act, grads + b.goff, B, CC, c.num_steps_conditioning, c.num_actions, inv, st)) return 1;
         break;
       default: return fail("backward: unknown op kind %d", b.kind);
     }
@@ -1983,32 +2187,18 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
   auto G = [&](int idx) { return grads + h->goff[idx]; };
   auto sgemm = [&](const float* Am, long long sam, long long sak, const float* Bm, long long sbk, long long sbn, float* C, long long ldc,
                    int M, int N, int Kd, int acc) -> int {
-    sgemm_kernel<<<dim3((N + 63) / 64, (M + 63) / 64), 256, 0, st>>>(Am, sam, sak, Bm, sbk, sbn, C, ldc, M, N, Kd, nullptr, acc);
-    DMD_LAUNCH_OK();
-    return 0;
+    return sgemm_launch(Am, sam, sak, Bm, sbk, sbn, C, ldc, M, N, Kd, nullptr, acc, 0, nullptr, st);
   };
   auto colsum = [&](const float* x, long long rows, int C, int Creal, float* out, float* out2, const float* inv) -> int {
-    const int L4 = (C < 256 ? C : 256) >> 2, lanes = 256 / L4;
-    long long blocks = (rows + (long long)lanes * 8 - 1) / ((long long)lanes * 8);
-    blocks = blocks > 592 ? 592 : (blocks < 1 ? 1 : blocks);
-    colsum_kernel<<<dim3((unsigned)blocks, (C + 255) / 256), 256, 0, st>>>(x, out, out2, inv, rows, C, Creal);
-    DMD_LAUNCH_OK();
-    return 0;
+    return colsum_launch(x, out, out2, inv, rows, C, Creal, st);
   };
   if (!accumulate) DMD_CUDA(cudaMemsetAsync(grads, 0, (size_t)h->grad_total * 4, st));
   DMD_CUDA(cudaMemsetAsync(sc.amax, 0, 256, st));
   // ---- heads (actor_critic.py:73)
-  heads_bwd_kernel<<<(B * D + 255) / 256, 256, 0, st>>>(g_hx, g_logits, g_val, h->ptrs[h->i_aw], h->ptrs[h->i_cw], sc.g_h, B, D, A);
-  DMD_LAUNCH_OK();
-  if (g_logits) {
-    if (sgemm(g_logits, 1, A, hx_out, D, 1, G(h->i_aw), D, A, D, B, 1)) return 1;          // dWa += g_logits^T h'
-    small_colsum_kernel<<<(A + 31) / 32, 32, 0, st>>>(g_logits, B, A, G(h->i_ab));           // dba (A need not be a multiple of 4)
-    DMD_LAUNCH_OK();
-  }
-  if (g_val) { vec_outer_sum_kernel<<<(D + 127) / 128, 128, 0, st>>>(g_val, hx_out, G(h->i_cw), G(h->i_cb), B, D); DMD_LAUNCH_OK(); }
+  if (heads_bwd_launch(g_hx, g_logits, g_val, hx_out, h->ptrs[h->i_aw], h->ptrs[h->i_cw], sc.g_h, G(h->i_ab), G(h->i_cw), G(h->i_cb), B, D, A, st)) return 1;
+  if (g_logits && sgemm(g_logits, 1, A, hx_out, D, 1, G(h->i_aw), D, A, D, B, 1)) return 1;   // dWa += g_logits^T h'
   // ---- LSTMCell (actor_critic.py:72)
-  lstm_cell_bwd_kernel<<<(B * D + 255) / 256, 256, 0, st>>>(b.gates, cx_in, sc.g_h, g_cx, sc.dgates, g_cx_in, B, D);
-  DMD_LAUNCH_OK();
+  if (lstm_cell_bwd_launch(b.gates, cx_in, sc.g_h, g_cx, sc.dgates, g_cx_in, B, D, st)) return 1;
   const float* feat = b.pooled[h->levels.size()];
   if (dmd_nhwc_to_nchw(feat, sc.x_flat, B, h->feat_c, h->feat_c, h->feat_hw, st)) return 1;   // x.flatten(start_dim=1) of the NCHW feature map
   if (sgemm(sc.dgates, 1, 4 * D, sc.x_flat, K, 1, G(h->i_wih), K, 4 * D, K, B, 1)) return 1;  // dWih += dgates^T x
@@ -2022,10 +2212,7 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
   if (dmd_nchw_to_nhwc(sc.g_xflat, g_cur, B, h->feat_c, h->feat_c, h->feat_hw, st)) return 1;
   {
     const long long n = (long long)B * K;
-    absmax_kernel<<<(int)std::min<long long>((n + 255) / 256, 592), 256, 0, st>>>(g_cur, sc.amax, n);
-    DMD_LAUNCH_OK();
-    loss_scale_kernel<<<1, 1, 0, st>>>(sc.amax, sc.scale);
-    DMD_LAUNCH_OK();
+    if (loss_scale_launch(g_cur, n, sc.amax, sc.scale, st)) return 1;
     scale_inplace_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(g_cur, sc.scale, n);
     DMD_LAUNCH_OK();
   }
@@ -2063,9 +2250,7 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
     const float* gy = g_cur;            // gradient of the SmallResBlock output y[i] (NHWC, S x S x cout)
     float* gx = other(g_cur);           // gradient of the block input pooled[i]
     if (lv.down) {                      // un-pool into the other buffer; the pooled gradient's buffer then takes gx
-      const int total = (S / 2) * (S / 2) * lv.cout;
-      maxpool2_bwd_kernel<<<dim3((total + 255) / 256, B), 256, 0, st>>>(b.y[i], g_cur, other(g_cur), S, S, lv.cout);
-      DMD_LAUNCH_OK();
+      if (maxpool2_bwd_launch(b.y[i], g_cur, other(g_cur), B, S, S, lv.cout, st)) return 1;
       gy = other(g_cur);
       gx = g_cur;
     }
@@ -2083,15 +2268,7 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
       nb.sumA = sc.nsum; nb.sumB = sc.nsum + (size_t)B * kMaxCin; nb.sum_stride = kMaxCin;
       nb.gx = gx; nb.addend = lv.has_skip ? nullptr : gy; nb.accumulate = 0;
       DMD_CUDA(cudaMemsetAsync(sc.nsum, 0, (size_t)2 * B * kMaxCin * 4, st));
-      int ppb = nb.HW;
-      while (ppb > 32 && (long long)B * ((nb.HW + ppb - 1) / ppb) < 2 * kPlanSms) ppb >>= 1;
-      const int chunks = (nb.HW + ppb - 1) / ppb;
-      norm_bwd_pass1_kernel<<<dim3(chunks, B), kNormThreads, 0, st>>>(nb, ppb);
-      DMD_LAUNCH_OK();
-      affine_param_grad_kernel<<<(nb.C + 127) / 128, 128, 0, st>>>(nb.sumA, nb.sumB, B, nb.C, nb.sum_stride, G(lv.gn_w), G(lv.gn_b), inv);
-      DMD_LAUNCH_OK();
-      norm_bwd_pass2_kernel<<<dim3(chunks, B), kNormThreads, 0, st>>>(nb, ppb);
-      DMD_LAUNCH_OK();
+      if (norm_bwd_launch(nb, 1, st) || affine_param_grad_launch(nb, G(lv.gn_w), G(lv.gn_b), inv, st) || norm_bwd_launch(nb, 2, st)) return 1;
     }
     if (lv.has_skip) {  // 1x1 skip projection on the raw input
       if (prep(b.pooled[i], lv.cin, S, 0, 0, 0, nullptr, sc.x_op)) return 1;

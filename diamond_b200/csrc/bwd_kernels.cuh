@@ -5,12 +5,14 @@
 // scale[1] = 1/S) chosen from the incoming gradient so that their fp16 tensor-core operands stay in range; parameter
 // gradients are multiplied by 1/S where they are written.
 #pragma once
+#include "../../include/diamond_b200.h"
 #include "aux_kernels.cuh"
 
 namespace dmd {
 
 // ------------------------------------------------------------------------------------------------ loss scale
-// amax of |g| (non-negative floats order like their bit patterns) -> S = 2^(12 - ceil(log2 amax)), so max |S g| in (2^11, 2^12]
+// amax of |g| (non-negative floats order like their bit patterns) -> S = 2^(E - e) with amax = f * 2^e, f in [0.5, 1) and
+// E = DMD_LOSS_SCALE_EXP, so max |S g| = f * 2^E lies in [2^(E-1), 2^E).  A power of two amax = 2^k gets f = 0.5, e = k + 1.
 __global__ void absmax_kernel(const float* __restrict__ g, unsigned int* __restrict__ amax_bits, long long n) {
   float m = 0.f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) m = fmaxf(m, fabsf(g[i]));
@@ -23,8 +25,8 @@ __global__ void loss_scale_kernel(const unsigned int* __restrict__ amax_bits, fl
   float s = 1.f;
   if (m > 0.f) {
     int e;
-    frexpf(m, &e);                 // m = f * 2^e, f in [0.5, 1)  ->  ceil(log2 m) <= e
-    s = ldexpf(1.f, 12 - e);
+    frexpf(m, &e);                 // m = f * 2^e, f in [0.5, 1)
+    s = ldexpf(1.f, DMD_LOSS_SCALE_EXP - e);
   }
   scale[0] = s;
   scale[1] = 1.f / s;

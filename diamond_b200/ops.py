@@ -187,3 +187,149 @@ def conv2d_wgrad(grad_op: Tensor, cg: int, act_op: Tensor, ca: int, b: int, h: i
     d.inv_scale, d.accumulate, d.partial, d.partial_bytes, d.debug = _lib.ptr(inv_scale), int(accumulate), part.data_ptr(), part.numel(), debug
     _lib.check(lib.dmd_conv2d_wgrad(C.byref(d), _lib.current_stream()))
     return dw
+
+
+# ------------------------------------------------------------------------------------------------ backward kernels
+# One wrapper per C entry point of the CUDA-core backward kernels.  Outputs that the kernels accumulate into are passed in
+# by the caller; the launch geometry is the library's (the same launchers the training executors use).
+
+def _inv(inv_scale):
+    return _lib.ptr(inv_scale)
+
+
+def norm_bwd(x: Tensor, gy: Tensor, stats: Tensor, gs: int, gx: Tensor, sum_a: Tensor, sum_b: Tensor, sum_stride: int, *, mode: int,
+             act: bool = True, film: Optional[Tensor] = None, film_off: int = 0, film_ctot: int = 0, c_off: int = 0,
+             gamma: Optional[Tensor] = None, beta: Optional[Tensor] = None, eps: float = 1e-5, addend: Optional[Tensor] = None,
+             accumulate: bool = False, dgamma: Optional[Tensor] = None, dbeta: Optional[Tensor] = None,
+             inv_scale: Optional[Tensor] = None) -> None:
+    """(Ada)GroupNorm [+ SiLU] backward of NHWC x [B][H][W][C] as the executors run it: pass 1 adds the per-channel sums to
+    sum_a / sum_b (rows of sum_stride floats; they may be views into a larger buffer such as the FiLM gradient), then the
+    affine parameter gradients when dgamma / dbeta are given, then pass 2 writes (or adds to) gx."""
+    _cuda(x, gy, stats, gx, film, gamma, beta, addend)
+    lib = _lib.lib()
+    b, c = x.shape[0], x.shape[-1]
+    d = _lib.NormBwdDesc()
+    d.x, d.gy, d.stats, d.B, d.HW, d.C, d.gs = x.data_ptr(), gy.data_ptr(), stats.data_ptr(), b, x.numel() // (b * c), c, gs
+    d.mode, d.act = mode, int(act)
+    d.film, d.film_stride, d.film_off, d.film_ctot, d.c_off = _lib.ptr(film), (film.shape[1] if film is not None else 0), film_off, film_ctot, c_off
+    d.gamma, d.beta, d.eps = _lib.ptr(gamma), _lib.ptr(beta), eps
+    d.sumA, d.sumB, d.sum_stride = sum_a.data_ptr(), sum_b.data_ptr(), sum_stride
+    d.gx, d.addend, d.accumulate = gx.data_ptr(), _lib.ptr(addend), int(accumulate)
+    st = _lib.current_stream()
+    _lib.check(lib.dmd_norm_bwd(C.byref(d), 1, st))
+    if dgamma is not None:
+        _lib.check(lib.dmd_norm_affine_grad(C.byref(d), dgamma.data_ptr(), dbeta.data_ptr(), _inv(inv_scale), st))
+    _lib.check(lib.dmd_norm_bwd(C.byref(d), 2, st))
+
+
+def attn_bwd(x: Tensor, stats_in: Tensor, gamma: Tensor, beta: Tensor, wqkv: Tensor, bqkv: Tensor, wout: Tensor, gout: Tensor, gs: int,
+             pgrads: Tuple[Tensor, ...], inv_scale: Optional[Tensor] = None, eps: float = 1e-5) -> Tensor:
+    """SelfAttention2d backward of NHWC x [B][8][8][C]: returns g_x; ADDS the parameter gradients to
+    pgrads = (dgamma, dbeta, dwqkv, dbqkv, dwout, dbout)."""
+    _cuda(x, stats_in, gamma, beta, wqkv, bqkv, wout, gout, *pgrads)
+    b, h, w, c = x.shape
+    gx = torch.empty_like(x)
+    _lib.check(_lib.lib().dmd_attn_bwd(x.data_ptr(), stats_in.data_ptr(), gamma.data_ptr(), beta.data_ptr(), wqkv.data_ptr(),
+                                       bqkv.data_ptr(), wout.data_ptr(), gout.data_ptr(), gx.data_ptr(), *[t.data_ptr() for t in pgrads],
+                                       _inv(inv_scale), b, h * w, c, gs, eps, _lib.current_stream()))
+    return gx
+
+
+def sgemm(a: Tensor, sam: int, sak: int, bm: Tensor, sbk: int, sbn: int, c: Tensor, ldc: int, m: int, n: int, k: int, *,
+          alpha: Optional[Tensor] = None, accumulate: bool = False, chunks: int = 0) -> Tensor:
+    """c[i*ldc + j] (+)= alpha * sum_k a[i*sam + k*sak] * bm[k*sbk + j*sbn]; chunks > 1: split-K through a partial buffer."""
+    _cuda(a, bm, c, alpha)
+    lib = _lib.lib()
+    nf = lib.dmd_sgemm_partial_floats(m, n, k, chunks)
+    part = torch.empty(max(nf, 1), device=c.device, dtype=torch.float32) if nf else None
+    _lib.check(lib.dmd_sgemm(a.data_ptr(), sam, sak, bm.data_ptr(), sbk, sbn, c.data_ptr(), ldc, m, n, k, _lib.ptr(alpha),
+                             int(accumulate), chunks, _lib.ptr(part), _lib.current_stream()))
+    return c
+
+
+def film_wgrad(dfilm: Tensor, cond: Tensor, grads: Tensor, woff: Tensor, boff: Tensor, inv_scale: Optional[Tensor] = None) -> Tensor:
+    """grads[woff[f] + k] += sum_n dfilm[n][f] cond[n][k], grads[boff[f]] += sum_n dfilm[n][f] (times inv_scale)."""
+    _cuda(dfilm, cond, grads, woff, boff)
+    b, rows = dfilm.shape
+    _lib.check(_lib.lib().dmd_film_wgrad(dfilm.data_ptr(), cond.data_ptr(), grads.data_ptr(), woff.data_ptr(), boff.data_ptr(), b, rows,
+                                         cond.shape[1], _inv(inv_scale), _lib.current_stream()))
+    return grads
+
+
+def embedding_bwd(de: Tensor, act: Tensor, de_table: Tensor, inv_scale: Optional[Tensor] = None) -> Tensor:
+    """de [B][T*E], act [B][T] int64 -> de_table [num_actions][E] += scattered rows."""
+    _cuda(de, act, de_table)
+    b, t = act.shape
+    _lib.check(_lib.lib().dmd_embedding_bwd(de.data_ptr(), act.data_ptr(), de_table.data_ptr(), b, de.shape[1], t, de_table.shape[0],
+                                            _inv(inv_scale), _lib.current_stream()))
+    return de_table
+
+
+def colsum(x: Tensor, out: Tensor, out2: Optional[Tensor] = None, inv_scale: Optional[Tensor] = None, creal: Optional[int] = None) -> Tensor:
+    """out[c] (and out2[c]) += sum over the rows of x [rows][C] for c < creal (default C)."""
+    _cuda(x, out, out2)
+    rows, c = x.shape
+    _lib.check(_lib.lib().dmd_colsum(x.data_ptr(), out.data_ptr(), _lib.ptr(out2), _inv(inv_scale), rows, c,
+                                     c if creal is None else creal, _lib.current_stream()))
+    return out
+
+
+def sumpool2(inp: Tensor, out: Tensor, accumulate: bool = False) -> Tensor:
+    """out [B][H][W][C] (+)= sum of the 2x2 blocks of inp [B][2H][2W][C]."""
+    _cuda(inp, out)
+    b, h, w, c = out.shape
+    _lib.check(_lib.lib().dmd_sumpool2(inp.data_ptr(), out.data_ptr(), b, h, w, c, int(accumulate), _lib.current_stream()))
+    return out
+
+
+def add(a: Tensor, out: Tensor, accumulate: bool = True) -> Tensor:
+    _cuda(a, out)
+    _lib.check(_lib.lib().dmd_add(a.data_ptr(), out.data_ptr(), out.numel(), int(accumulate), _lib.current_stream()))
+    return out
+
+
+def dsilu_mul(pre: Tensor, dh: Tensor) -> Tensor:
+    _cuda(pre, dh)
+    out = torch.empty_like(pre)
+    _lib.check(_lib.lib().dmd_dsilu_mul(pre.data_ptr(), dh.data_ptr(), out.data_ptr(), pre.numel(), _lib.current_stream()))
+    return out
+
+
+def maxpool2_bwd(y: Tensor, gp: Tensor) -> Tensor:
+    """MaxPool2d(2) backward: y NHWC [B][H][W][C] (pre-pool), gp [B][H/2][W/2][C] -> gradient wrt y."""
+    _cuda(y, gp)
+    b, h, w, c = y.shape
+    gy = torch.empty_like(y)
+    _lib.check(_lib.lib().dmd_maxpool2_bwd(y.data_ptr(), gp.data_ptr(), gy.data_ptr(), b, h, w, c, _lib.current_stream()))
+    return gy
+
+
+def lstm_cell_bwd(gates: Tensor, c_in: Tensor, g_h: Optional[Tensor], g_c: Optional[Tensor]) -> Tuple[Tensor, Tensor]:
+    """LSTMCell backward from the gate pre-activations [B][4H]: returns (dgates, gradient wrt c_in)."""
+    _cuda(gates, c_in, g_h, g_c)
+    b, hd = c_in.shape
+    dgates, gc = torch.empty_like(gates), torch.empty_like(c_in)
+    _lib.check(_lib.lib().dmd_lstm_cell_bwd(gates.data_ptr(), c_in.data_ptr(), _lib.ptr(g_h), _lib.ptr(g_c), dgates.data_ptr(),
+                                            gc.data_ptr(), b, hd, _lib.current_stream()))
+    return dgates, gc
+
+
+def heads_bwd(g_hx: Optional[Tensor], g_logits: Optional[Tensor], g_val: Optional[Tensor], hx_out: Tensor, wa: Tensor, wc: Tensor,
+              dba: Tensor, dwc: Tensor, dbc: Tensor) -> Tensor:
+    """Actor / critic heads backward: returns g_h; adds the actor bias and critic weight / bias gradients of the given heads."""
+    _cuda(g_hx, g_logits, g_val, hx_out, wa, wc, dba, dwc, dbc)
+    b, hd = hx_out.shape
+    g_h = torch.empty_like(hx_out)
+    _lib.check(_lib.lib().dmd_heads_bwd(_lib.ptr(g_hx), _lib.ptr(g_logits), _lib.ptr(g_val), hx_out.data_ptr(), wa.data_ptr(),
+                                        wc.data_ptr(), g_h.data_ptr(), dba.data_ptr(), dwc.data_ptr(), dbc.data_ptr(), b, hd,
+                                        wa.shape[0], _lib.current_stream()))
+    return g_h
+
+
+def loss_scale(g: Tensor) -> Tensor:
+    """The backward loss scale of a gradient tensor: [S, 1/S]."""
+    _cuda(g)
+    amax = torch.zeros(1, device=g.device, dtype=torch.int32)
+    scale = torch.empty(2, device=g.device, dtype=torch.float32)
+    _lib.check(_lib.lib().dmd_loss_scale(g.data_ptr(), g.numel(), amax.data_ptr(), scale.data_ptr(), _lib.current_stream()))
+    return scale

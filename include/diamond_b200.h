@@ -22,6 +22,11 @@ extern "C" {
 #endif
 
 #define DMD_VERSION 100
+/* Headroom of the backward loss scale: max|S * dL/d(output)| is put in [2^(E-1), 2^E), E = DMD_LOSS_SCALE_EXP, so an inner
+ * gradient up to 65504 / 2^E (just under 2^(16-E)) times the largest output gradient is finite in the fp16 tensor-core operands.
+ * E = 8 (headroom 256x) costs nothing measurable against E = 12 (16x) on either training fixture: fp16 keeps its relative
+ * precision down to 2^-14 (oracle/grad_error_budget.py --exp emulates the scheme). */
+#define DMD_LOSS_SCALE_EXP 8
 
 int dmd_version(void);
 const char* dmd_last_error(void);
@@ -166,6 +171,80 @@ int dmd_attn_fwd(const float* x, const double* stats_in, const float* gamma, con
 
 int dmd_nchw_to_nhwc(const float* in, float* out, int B, int C, int CP, int HW, void* stream);
 int dmd_nhwc_to_nchw(const float* in, float* out, int B, int C, int CP, int HW, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * Per-op entry points of the CUDA-core backward kernels (diamond_b200/csrc/bwd_kernels.cuh) that dmd_denoiser_backward and
+ * dmd_actor_critic_backward run, with the launch geometry those executors use.  Gradients are fp32.  `inv_scale` (a device
+ * scalar, or NULL = 1) multiplies parameter gradients: the executors pass 1/S of the loss scale.
+ * ------------------------------------------------------------------------------------------------------------- */
+
+/* GroupNorm (mode 2, blocks.py:28) / AdaGroupNorm (mode 1, blocks.py:41-45) [+ SiLU] backward.  Pass 1 adds the per-(image,
+ * channel) sums A = sum_px gz and Bm = sum_px gz * xhat to sumA / sumB[n * sum_stride + c] (caller zeroes them); pass 2 writes
+ * gx (+ addend) or adds it to gx (accumulate).  Mode 1 reads FiLM scale at film[n * film_stride + film_off + c_off + c] and
+ * shift at ... + film_ctot + c_off + c; one source of a channel concat is one launch at its channel offset c_off. */
+typedef struct dmd_norm_bwd_desc {
+  const float* x;        /* NHWC [B][HW][C] forward input of the norm */
+  const float* gy;       /* NHWC [B][HW][C] gradient wrt the (activated) output */
+  const double* stats;   /* [B][C/gs][2] forward (sum, sumsq) */
+  int B, HW, C, gs;      /* C multiple of 4, <= 128; gs multiple of 4, C / gs <= 8 */
+  int mode;              /* 1 AdaGroupNorm, 2 affine GroupNorm */
+  int act;               /* SiLU after the norm */
+  const float* film;
+  int film_stride, film_off, film_ctot, c_off;
+  const float* gamma;    /* mode 2: [c_off + C] */
+  const float* beta;
+  float eps;
+  float* sumA;
+  float* sumB;
+  int sum_stride;
+  float* gx;             /* NHWC [B][HW][C] */
+  const float* addend;   /* NULL or NHWC [B][HW][C] added to gx */
+  int accumulate;
+} dmd_norm_bwd_desc;
+int dmd_norm_bwd(const dmd_norm_bwd_desc* d, int pass, void* stream);
+/* affine GroupNorm parameters after pass 1: dgamma[c] += inv_scale * sum_n sumB[n][c], dbeta[c] += inv_scale * sum_n sumA[n][c] */
+int dmd_norm_affine_grad(const dmd_norm_bwd_desc* d, float* dgamma, float* dbeta, const float* inv_scale, void* stream);
+
+/* SelfAttention2d backward (blocks.py:62-72), the forward of dmd_attn_fwd: gx (NHWC [B][L][C]) is ASSIGNED; the six parameter
+ * gradients are ADDED (times inv_scale).  L = 64, C in {32, 64}. */
+int dmd_attn_bwd(const float* x, const double* stats_in, const float* gamma, const float* beta, const float* wqkv, const float* bqkv,
+                 const float* wout, const float* gout, float* gx, float* dgamma, float* dbeta, float* dwqkv, float* dbqkv,
+                 float* dwout, float* dbout, const float* inv_scale, int B, int L, int C, int gs, float eps, void* stream);
+
+/* C[m][n] (+)= alpha * sum_k A[m*sam + k*sak] * B[k*sbk + n*sbn] (alpha: device scalar or NULL = 1).  chunks > 1 splits K into
+ * 16-aligned ranges reduced in a fixed order through `partial` (dmd_sgemm_partial_floats floats; needs ldc == N). */
+long long dmd_sgemm_partial_floats(int M, int N, int K, int chunks);
+int dmd_sgemm(const float* A, long long sam, long long sak, const float* B, long long sbk, long long sbn, float* C, long long ldc,
+              int M, int N, int K, const float* alpha, int accumulate, int chunks, float* partial, void* stream);
+
+/* FiLM linear weights (blocks.py:39) batched as rows of one matrix: grads[woff[f] + k] += inv_scale * sum_n dfilm[n][f] cond[n][k],
+ * grads[boff[f]] += inv_scale * sum_n dfilm[n][f].  dfilm [B][rows], cond [B][CC], CC <= 256. */
+int dmd_film_wgrad(const float* dfilm, const float* cond, float* grads, const long long* woff, const long long* boff, int B, int rows,
+                   int CC, const float* inv_scale, void* stream);
+/* act_emb (inner_model.py:27-30): dE[act[n][t]][j] += inv_scale * de[n][t * CC/T + j]; act [B][T] int64 */
+int dmd_embedding_bwd(const float* de, const int64_t* act, float* dE, int B, int CC, int T, int num_actions, const float* inv_scale,
+                      void* stream);
+/* bias gradients: out[c] (and out2[c], if not NULL) += inv_scale * sum_rows x[row][c] for c < Creal; x [rows][C], C multiple of 4 */
+int dmd_colsum(const float* x, float* out, float* out2, const float* inv_scale, long long rows, int C, int Creal, void* stream);
+/* nearest-2x upsample adjoint: out [B][H][W][C] (+)= sum of the 2x2 blocks of in [B][2H][2W][C] */
+int dmd_sumpool2(const float* in, float* out, int B, int H, int W, int C, int accumulate, void* stream);
+/* out (+)= a, n floats (multiple of 4) */
+int dmd_add(const float* a, float* out, long long n, int accumulate, void* stream);
+/* out = dh * silu'(pre) */
+int dmd_dsilu_mul(const float* pre, const float* dh, float* out, long long n, void* stream);
+/* MaxPool2d(2) backward (actor_critic.py:109): y NHWC [B][H][W][C] pre-pool, gp [B][H/2][W/2][C] -> gy [B][H][W][C] (assigned) */
+int dmd_maxpool2_bwd(const float* y, const float* gp, float* gy, int B, int H, int W, int C, void* stream);
+/* LSTMCell backward (actor_critic.py:72): gates [B][4Hd] pre-activations, c_in [B][Hd]; g_h, g_c (either may be NULL) ->
+ * dgates [B][4Hd], g_c_in [B][Hd] */
+int dmd_lstm_cell_bwd(const float* gates, const float* c_in, const float* g_h, const float* g_c, float* dgates, float* g_c_in,
+                      int B, int Hd, void* stream);
+/* actor / critic heads (actor_critic.py:73): g_h = g_hx + g_logits Wa + g_val Wc (g_h assigned); dba += colsum(g_logits) when
+ * g_logits is given; dWc += g_val^T hx_out and dbc += sum g_val when g_val is given.  Wa [A][Hd], Wc [Hd]. */
+int dmd_heads_bwd(const float* g_hx, const float* g_logits, const float* g_val, const float* hx_out, const float* Wa, const float* Wc,
+                  float* g_h, float* dba, float* dWc, float* dbc, int B, int Hd, int A, void* stream);
+/* Loss scale of a backward call: from m = max|g| (amax: one zeroed device word), scale[0] = S (a power of two, 1 when m = 0) and
+ * scale[1] = 1/S, with max|S g| in [2^(DMD_LOSS_SCALE_EXP-1), 2^DMD_LOSS_SCALE_EXP). */
+int dmd_loss_scale(const float* g, long long n, unsigned int* amax, float* scale, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Denoiser executor: InnerModel.forward (inner_model.py:44-49) + Denoiser.denoise (denoiser.py:86-91) +

@@ -1,11 +1,19 @@
 """Test-infrastructure tool (CPU): error budget of the BACKWARD pass when conv operands are rounded the way the wgmma
 kernels round them (fp16 operands, fp32 accumulate), measured on the oracle against exact fp32 autograd.
 
-    python oracle/grad_error_budget.py [small|default]
+    python oracle/grad_error_budget.py [small|default]                 operand-rounding rows, per-tensor gradient scale
+    python oracle/grad_error_budget.py [small|default] --exp 12 8 ...  the kernels' scheme: ONE scale per backward call
 
 It answers, before any backward kernel is written: which backward GEMMs (dgrad, wgrad) can take single-fp16 operands with
 a per-tensor power-of-two scale on the gradient, and which need the split-fp16 treatment the forward uses on the
 residual-stream layers.  Results are quoted in DESIGN.md section 7.
+
+The kernels do not scale per tensor: dmd_denoiser_backward picks one power-of-two S per call from max|dL/d(model output)| so
+that it lands in [2^(E-1), 2^E), E = DMD_LOSS_SCALE_EXP (include/diamond_b200.h), and every conv gradient operand of that call
+is fp16(S * dL/dy).  `--exp` emulates exactly that (conv_out, the first conv the backward meets, fixes S), which shows the cost
+of a smaller E: gradients far below max|dL/d(output)| fall into the fp16 subnormals (2^-24 .. 2^-14) and lose precision.
+`--gain k` multiplies conv_out.weight by k, which makes inner gradients ~0.29 k times the output gradient (default net): the
+headroom a trained network may need; an overflowing operand shows up as a non-finite error.
 """
 import math
 import os
@@ -27,12 +35,18 @@ def _h(t):
     return t.half().float()
 
 
+# the loss-scale scheme: None = a per-tensor scale (max near 2^12); an int E = one scale per backward call, set by conv_out
+_SCALE = {"exp": None, "S": None}
+
+
+def _pow2_scale(m, e):
+    """2^(e - k) for m = f 2^k, f in [0.5, 1): loss_scale_kernel's choice, max |S g| in [2^(e-1), 2^e)."""
+    return 1.0 if m == 0.0 else 2.0 ** (e - math.frexp(m)[1])
+
+
 def _scaled_h(g):
-    """fp16 rounding of a gradient tensor with a per-tensor power-of-two scale that puts its max near 2^12."""
-    m = float(g.abs().max())
-    if m == 0.0:
-        return g
-    s = 2.0 ** (12 - math.ceil(math.log2(m)))
+    """fp16 rounding of a gradient tensor under the loss scale of _SCALE."""
+    s = _SCALE["S"] if _SCALE["exp"] is not None else _pow2_scale(float(g.abs().max()), 12)
     return _h(g * s) / s
 
 
@@ -40,9 +54,10 @@ class QConv(torch.autograd.Function):
     """conv2d whose forward / dgrad / wgrad operands are rounded per `mode` = (fwd, dgrad, wgrad), each in {0: exact, 1: fp16}."""
 
     @staticmethod
-    def forward(ctx, x, w, b, stride, padding, mode):
+    def forward(ctx, x, w, b, stride, padding, mode, is_out=False):
         ctx.save_for_backward(x, w)
         ctx.cfg = (stride, padding, mode, b is not None)
+        ctx.is_out = is_out
         xq, wq = (_h(x), _h(w)) if mode[0] else (x, w)
         return _real_conv2d(xq, wq, b, stride=stride, padding=padding)
 
@@ -50,16 +65,20 @@ class QConv(torch.autograd.Function):
     def backward(ctx, gy):
         x, w = ctx.saved_tensors
         stride, padding, mode, has_b = ctx.cfg
+        if ctx.is_out and _SCALE["exp"] is not None:   # conv_out: its dL/dy is the gradient of the model output
+            _SCALE["S"] = _pow2_scale(float(gy.abs().max()), _SCALE["exp"])
         gd = _scaled_h(gy) if mode[1] else gy
         gx = torch.nn.grad.conv2d_input(x.shape, _h(w) if mode[1] else w, gd, stride=stride, padding=padding)
         gwy = _scaled_h(gy) if mode[2] else gy
         gw = torch.nn.grad.conv2d_weight(_h(x) if mode[2] else x, w.shape, gwy, stride=stride, padding=padding)
         gb = gy.sum(dim=(0, 2, 3)) if has_b else None
-        return gx, gw, gb, None, None, None
+        return gx, gw, gb, None, None, None, None
 
 
-def run(case_name, mode_main, mode_stream):
-    """mode_main: 3x3 ResBlock / up / down convs; mode_stream: 1x1 projections, conv_in (read the raw residual stream)."""
+def run(case_name, mode_main, mode_stream, exp=None, gain=1.0):
+    """mode_main: 3x3 ResBlock / up / down convs; mode_stream: 1x1 projections, conv_in (read the raw residual stream).
+    exp: None = per-tensor gradient scale, else one scale per backward call with max|S dL/d(output)| in [2^(exp-1), 2^exp).
+    gain: multiplies conv_out.weight."""
     tc = TRAIN_CASES[case_name]
     c = CASES[tc["case"]]
     g = np.load(os.path.join(ROOT, "tests", "golden", case_name + ".npz"))
@@ -67,6 +86,7 @@ def run(case_name, mode_main, mode_stream):
 
     def grads(patched):
         sd = O.seeded_state_dict(O.inner_model_shapes(inner), c["wseed"])
+        sd["conv_out.weight"] *= gain
         for k, v in sd.items():
             if k != "noise_emb.weight":
                 v.requires_grad_(True)
@@ -74,9 +94,10 @@ def run(case_name, mode_main, mode_stream):
 
         def conv2d(x, w, b=None, stride=1, padding=0):
             stream = w.shape[-1] == 1 or w.shape[1] == (inner.num_steps_conditioning + 1) * inner.img_channels
-            return QConv.apply(x, w, b, stride, padding, mode_stream if stream else mode_main)
+            return QConv.apply(x, w, b, stride, padding, mode_stream if stream else mode_main, w.shape[0] == inner.img_channels)
 
         F.conv2d = conv2d if patched else _real_conv2d
+        _SCALE["exp"], _SCALE["S"] = exp, None
         try:
             loss = O.denoiser_loss(torch.from_numpy(g["obs"]), torch.from_numpy(g["act"]), torch.from_numpy(g["mask_padding"]),
                                    draws, sd, O.DenoiserCfg(inner=inner), O.SigmaDistCfg())
@@ -93,10 +114,30 @@ def run(case_name, mode_main, mode_stream):
     return abs(l1 - l0) / abs(l0), num / den, per[:3]
 
 
+def per_call_rows(name, exps, gain=1.0):
+    """The kernels' operand rounding (forward fp16 with exact stream layers, backward fp16 everywhere) under a per-tensor scale
+    and under one scale per call for each E in exps: [(label, loss error, whole-gradient error, worst tensors)]."""
+    rows = [("per-tensor scale", *run(name, (1, 1, 1), (0, 1, 1), None, gain))]
+    for e in exps:
+        rows.append((f"one scale per call, E = {e}", *run(name, (1, 1, 1), (0, 1, 1), e, gain)))
+    return rows
+
+
 if __name__ == "__main__":
     torch.set_num_threads(8)
-    which = sys.argv[1] if len(sys.argv) > 1 else "small"
+    args = sys.argv[1:]
+    which = args[0] if args and not args[0].startswith("--") else "small"
     name = {"small": "denoiser_small_training", "default": "denoiser_default_training"}[which]
+    if "--exp" in args:
+        i = args.index("--exp") + 1
+        exps = []
+        while i < len(args) and not args[i].startswith("--"):
+            exps.append(int(args[i])); i += 1
+        gain = float(args[args.index("--gain") + 1]) if "--gain" in args else 1.0
+        print(f"case {name}, conv_out.weight x {gain}: relative error of the loss / of the whole gradient (L2) / worst tensors")
+        for label, dl, dg, worst in per_call_rows(name, exps, gain):
+            print(f"{label:30s} loss {dl:.2e}  grad {dg:.2e}  worst {[(round(e, 5), k) for e, k in worst]}")
+        sys.exit(0)
     E, H = (0, 0, 0), (1, 1, 1)
     rows = [
         ("forward fp16 (stream layers exact), backward exact", (1, 0, 0), E),

@@ -6,6 +6,7 @@ Tolerance: loss and the WHOLE gradient (relative L2 over all parameters) within 
 reported and bounded at 4e-3 (fp16 tensor-core operands: the CPU error budget oracle/grad_error_budget.py predicts
 <= 1.2e-3 for the worst tensor of the default net, 1.9e-3 for the small net)."""
 import os
+import time
 
 import numpy as np
 import pytest
@@ -42,24 +43,18 @@ def _replay_rng(draws, dev):
     return randn, randn_like, q
 
 
-def _run_native(name, golden_dir, dev):
+def _native_step(inner, sd, obs, act, mask, draws, dev):
+    """Denoiser.forward + loss.backward() on the native path with the reference's random draws replayed."""
     from diamond_b200.models.diffusion import Denoiser, DenoiserConfig, InnerModelConfig, SigmaDistributionConfig
     from oracle import torch_oracle as O
-    from oracle.make_golden import CASES, TRAIN_CASES
 
-    tc = TRAIN_CASES[name]
-    c = CASES[tc["case"]]
-    g = np.load(os.path.join(golden_dir, name + ".npz"))
-    inner = c["inner"]
-    sd = O.seeded_state_dict(O.inner_model_shapes(inner), c["wseed"])
     den = Denoiser(DenoiserConfig(InnerModelConfig(inner.img_channels, inner.num_steps_conditioning, inner.cond_channels,
                                                    list(inner.depths), list(inner.channels), list(inner.attn_depths), inner.num_actions), 0.5, 0.3))
     den.inner_model.load_state_dict(sd)
     den = den.to(dev).train()
     sc = O.SigmaDistCfg()
     den.setup_training(SigmaDistributionConfig(sc.loc, sc.scale, sc.sigma_min, sc.sigma_max))
-    draws = [tuple(torch.from_numpy(g[k][i]) for k in ("raw_sigma", "raw_offset", "raw_noise")) for i in range(tc["seq"])]
-    batch = _Batch(torch.from_numpy(g["obs"]).to(dev), torch.from_numpy(g["act"]).to(dev), torch.from_numpy(g["mask_padding"]).to(dev))
+    batch = _Batch(obs.to(dev), act.to(dev), mask.to(dev))
     randn, randn_like, q = _replay_rng(draws, dev)
     o1, o2 = torch.randn, torch.randn_like
     torch.randn, torch.randn_like = randn, randn_like
@@ -70,25 +65,49 @@ def _run_native(name, golden_dir, dev):
     assert not q, "the native Denoiser.forward consumed a different number of random draws than the reference"
     loss.backward()
     torch.cuda.synchronize()
-    grads = {k: p.grad.detach().cpu() for k, p in den.inner_model.named_parameters()}
-    # the checker: full fp32 autograd of the reference-pinned oracle on the host
-    torch.set_num_threads(min(16, max(1, os.cpu_count() or 1)))  # torch CPU convs on these small images collapse with very many threads
-    sd2 = O.seeded_state_dict(O.inner_model_shapes(inner), c["wseed"])
-    for k, v in sd2.items():
+    return float(loss), logs, {k: p.grad.detach().cpu() for k, p in den.inner_model.named_parameters()}
+
+
+def _oracle_params(inner, wseed):
+    from oracle import torch_oracle as O
+
+    sd = O.seeded_state_dict(O.inner_model_shapes(inner), wseed)
+    for k, v in sd.items():
         if k != "noise_emb.weight":
             v.requires_grad_(True)
-    ref_loss = O.denoiser_loss(torch.from_numpy(g["obs"]), torch.from_numpy(g["act"]), torch.from_numpy(g["mask_padding"]), draws, sd2,
-                               O.DenoiserCfg(inner=inner), sc)
+    return sd
+
+
+def _run_native(name, golden_dir, dev):
+    from oracle import torch_oracle as O
+    from oracle.make_golden import CASES, TRAIN_CASES
+
+    tc = TRAIN_CASES[name]
+    c = CASES[tc["case"]]
+    g = np.load(os.path.join(golden_dir, name + ".npz"))
+    inner = c["inner"]
+    draws = [tuple(torch.from_numpy(g[k][i]) for k in ("raw_sigma", "raw_offset", "raw_noise")) for i in range(tc["seq"])]
+    obs, act, mask = (torch.from_numpy(g[k]) for k in ("obs", "act", "mask_padding"))
+    loss, logs, grads = _native_step(inner, O.seeded_state_dict(O.inner_model_shapes(inner), c["wseed"]), obs, act, mask, draws, dev)
+    # the checker: full fp32 autograd of the reference-pinned oracle on the host
+    torch.set_num_threads(min(16, max(1, os.cpu_count() or 1)))  # torch CPU convs on these small images collapse with very many threads
+    sd2 = _oracle_params(inner, c["wseed"])
+    ref_loss = O.denoiser_loss(obs, act, mask, draws, sd2, O.DenoiserCfg(inner=inner), O.SigmaDistCfg())
     ref_loss.backward()
     ref = {k: v.grad for k, v in sd2.items() if v.grad is not None}
-    return float(loss), logs, grads, float(ref_loss), ref, g
+    return loss, logs, grads, float(ref_loss), ref, g
 
 
-@pytest.mark.parametrize("name", ["denoiser_default_training", "denoiser_small_training"])
-def test_denoiser_training_step_matches_reference(golden_dir, name):
-    dev = _dev()
-    loss, logs, grads, ref_loss, ref, g = _run_native(name, golden_dir, dev)
-    print(f"{name}: loss native {loss:.6f} oracle {ref_loss:.6f} reference {float(g['loss']):.6f}")
+# Every tensor's relative error is also capped, whatever its share of the whole gradient: the per-tensor rule
+# `e < 4e-3 or e * |g| < 1e-4 |G|` alone lets a tensor that carries little of the gradient be wrong by any amount.  Measured on
+# an H100 SXM (700 W): no tensor of any training test needs the share rule; the worst are 2.5e-3 (small net), 2.2e-3 (batch
+# 256 and the headroom weights), 1.7e-3 (default net) and 6.6e-4 (actor-critic).  The cap is twice the worst.
+PER_TENSOR_CAP = 5e-3
+
+
+def _compare_grads(label, grads, ref, whole_tol):
+    """Prints every tensor's relative L2 error and bounds the whole gradient, each tensor (4e-3, or negligible against the
+    whole gradient) and every tensor by PER_TENSOR_CAP."""
     assert set(grads) == set(ref)
     num = den = 0.0
     rows = []
@@ -97,28 +116,135 @@ def test_denoiser_training_step_matches_reference(golden_dir, name):
         num += float(d.pow(2).sum()); den += float(ref[k].double().pow(2).sum())
         rows.append((float(d.norm() / ref[k].double().norm().clamp_min(1e-30)), k, float(ref[k].norm())))
     whole = (num / den) ** 0.5
-    print(f"{name}: whole-gradient relative L2 error {whole:.3e}")
+    total = den ** 0.5
+    print(f"{label}: whole-gradient relative L2 error {whole:.3e}")
     for e, k, n in rows:
-        print(f"   {e:9.3e}  |g|={n:9.3e}  {k}")
+        print(f"   {e:9.3e}  |g|={n:9.3e}  {'(small: share rule)' if e >= 4e-3 else '':20s} {k}")
     worst = sorted(rows, reverse=True)[:5]
-    print("worst:", worst)
+    print(f"{label} worst:", worst)
+    assert whole < whole_tol, whole
+    for e, k, n in rows:
+        assert e < 4e-3 or e * n < 1e-4 * total, (k, e, n, total)
+        assert e < PER_TENSOR_CAP, (k, e, n, total)
+    return whole, worst
+
+
+@pytest.mark.parametrize("name", ["denoiser_default_training", "denoiser_small_training"])
+def test_denoiser_training_step_matches_reference(golden_dir, name):
+    dev = _dev()
+    loss, logs, grads, ref_loss, ref, g = _run_native(name, golden_dir, dev)
+    print(f"{name}: loss native {loss:.6f} oracle {ref_loss:.6f} reference {float(g['loss']):.6f}")
     assert abs(loss - float(g["loss"])) <= 2e-3 * abs(float(g["loss"])), (loss, float(g["loss"]))
     assert float(logs["loss_denoising"]) == pytest.approx(loss)
     # north_star's 1e-3 holds for the default network.  The small fixture (32x32 images, batch 3) averages the operand rounding
     # over 16x fewer terms: oracle/grad_error_budget.py (CPU emulation of 10-bit-mantissa operands, which is ALSO what the
     # reference's own GPU path computes with: TF32, src/trainer.py:41) predicts 9.7e-4 for it, 8.8e-4 of that from the FORWARD
     # operand rounding alone -- the bound there is the budget plus 25 %.
-    tol = 1e-3 if name == "denoiser_default_training" else 1.25e-3
-    assert whole < tol, whole
-    total = den ** 0.5
-    for e, k, n in rows:  # tensors that carry almost none of the gradient are bounded relative to the whole gradient
-        assert e < 4e-3 or e * n < 1e-4 * total, (k, e, n, total)
+    _compare_grads(name, grads, ref, 1e-3 if name == "denoiser_default_training" else 1.25e-3)
     # the reference's own summary: per-tensor L2 norms
     keys = [str(k) for k in g["grad_keys"]]
     norms = np.array([float(grads[k].double().norm()) for k in keys])
     ref_n = g["grad_norms"]
     tot = float(np.sqrt((ref_n ** 2).sum()))
     assert np.all(np.abs(norms - ref_n) <= 4e-3 * ref_n + 1e-4 * tot), float(np.max(np.abs(norms - ref_n) / (ref_n + 1e-12)))
+
+
+def test_denoiser_training_batch256_matches_oracle():
+    """The benchmarked training batch (bench.py cfg 2): default net, 64x64, B = 256, one autoregressive step, every sample
+    valid, frames and random draws from a seed.  At this batch the FiLM weight gradient walks four 64-sample chunks, the norm
+    backward runs 2048-pixel blocks, the bias column sums hit their grid cap and the split-K dcond GEMM has four row tiles.
+    The checker accumulates the oracle's fp32 gradient over chunks of 16 samples (O.denoiser_loss_grads_chunked).
+
+    Whole-gradient bound 1.25e-3, the budget plus 25 % as for the small fixture: emulating the kernels' fp16 operands on the
+    oracle at exactly these inputs (oracle/grad_error_budget.py's QConv over the chunked loss) gives 1.01e-3, worst tensor
+    2.1e-3 (u_blocks.1.resblocks.1.norm1.linear.bias) -- this batch draws sigmas down to 0.016, whose samples dominate the
+    gradient.  The kernels measure the same (1.01e-3, same worst tensor)."""
+    dev = _dev()
+    from oracle import torch_oracle as O
+
+    inner, wseed = O.InnerCfg(), 1234
+    b, n, hw = 256, inner.num_steps_conditioning, 64
+    rng = np.random.default_rng(2560)
+    obs = torch.from_numpy(rng.integers(0, 256, size=(b, n + 1, inner.img_channels, hw, hw)).astype(np.float32)).div(255).mul(2).sub(1)
+    act = torch.from_numpy(rng.integers(0, inner.num_actions, size=(b, n + 1)).astype(np.int64))
+    mask = torch.ones(b, n + 1, dtype=torch.bool)
+    g = torch.Generator().manual_seed(2561)
+    draws = [(torch.randn(b, generator=g), torch.randn(b, inner.img_channels, 1, 1, generator=g),
+              torch.randn(b, inner.img_channels, hw, hw, generator=g))]
+    loss, logs, grads = _native_step(inner, O.seeded_state_dict(O.inner_model_shapes(inner), wseed), obs, act, mask, draws, dev)
+    # a second run differs only by the order of fp32 / fp64 atomic additions (DESIGN.md section 2): ~1e-7 of the whole gradient
+    _, _, again = _native_step(inner, O.seeded_state_dict(O.inner_model_shapes(inner), wseed), obs, act, mask, draws, dev)
+    flat, flat2 = (torch.cat([d[k].flatten() for k in sorted(d)]).double() for d in (grads, again))
+    noise = float((flat2 - flat).norm() / flat.norm())
+    print(f"B=256: run-to-run relative L2 difference {noise:.2e}")
+    assert noise < 1e-6, noise
+    torch.set_num_threads(min(16, max(1, os.cpu_count() or 1)))
+    t0 = time.perf_counter()
+    ref_loss, ref = O.denoiser_loss_grads_chunked(obs, act, mask, draws, _oracle_params(inner, wseed), O.DenoiserCfg(inner=inner),
+                                                  O.SigmaDistCfg(), 16)
+    print(f"B=256: loss native {loss:.6f} oracle {ref_loss:.6f}; chunked oracle {time.perf_counter() - t0:.1f} s on {torch.get_num_threads()} threads")
+    assert abs(loss - ref_loss) <= 2e-3 * abs(ref_loss), (loss, ref_loss)
+    assert float(logs["loss_denoising"]) == pytest.approx(loss)
+    _compare_grads("denoiser B=256", grads, ref, 1.25e-3)
+
+
+def _oracle_conv_grad_maxima(inner, sd, obs, act, mask, draws):
+    """Oracle loss.backward() recording max|dL/dy| of every conv output in forward order (the last one, conv_out, is the model
+    output, whose gradient sets the loss scale)."""
+    import torch.nn.functional as F
+
+    from oracle import torch_oracle as O
+
+    real, maxima = F.conv2d, []
+
+    def conv2d(x, w, bias=None, stride=1, padding=0):
+        y = real(x, w, bias, stride=stride, padding=padding)
+        i = len(maxima)
+        maxima.append(0.0)
+        y.register_hook(lambda gy: maxima.__setitem__(i, float(gy.abs().max())))
+        return y
+
+    F.conv2d = conv2d
+    try:
+        loss = O.denoiser_loss(obs, act, mask, draws, sd, O.DenoiserCfg(inner=inner), O.SigmaDistCfg())
+        loss.backward()
+    finally:
+        F.conv2d = real
+    return maxima
+
+
+def test_loss_scale_headroom(golden_dir):
+    """The backward picks ONE power-of-two loss scale per call from max|dL/d(model output)| and feeds fp16 tensor-core operands
+    that do not saturate, so it must leave room for inner gradients much larger than the output gradient (small activation
+    variance or large norm gains in a trained network).  conv_out.weight x 256 on the default fixture makes an inner conv
+    gradient > 32x max|dL/d(output)| (asserted on the oracle): past the 16-32x that a scale target of 2^12 left, which turned
+    those operands into inf and every gradient into NaN.  The gradients must stay finite and match the oracle; the whole-gradient
+    bound is 2e-3 because oracle/grad_error_budget.py predicts 1.35e-3 for this weighting (`default --exp 8 --gain 256`, fp16
+    operand rounding alone), above the 1e-3 of the unscaled fixture."""
+    dev = _dev()
+    from oracle import torch_oracle as O
+    from oracle.make_golden import CASES
+
+    c = CASES["denoiser_default"]
+    inner = c["inner"]
+    g = np.load(os.path.join(golden_dir, "denoiser_default_training.npz"))
+    draws = [tuple(torch.from_numpy(g[k][0]) for k in ("raw_sigma", "raw_offset", "raw_noise"))]
+    obs, act, mask = (torch.from_numpy(g[k]) for k in ("obs", "act", "mask_padding"))
+    sd = O.seeded_state_dict(O.inner_model_shapes(inner), c["wseed"])
+    sd["conv_out.weight"] *= 256
+    loss, _, grads = _native_step(inner, sd, obs, act, mask, draws, dev)
+    torch.set_num_threads(min(16, max(1, os.cpu_count() or 1)))
+    sd2 = _oracle_params(inner, c["wseed"])
+    with torch.no_grad():
+        sd2["conv_out.weight"] *= 256
+    maxima = _oracle_conv_grad_maxima(inner, sd2, obs, act, mask, draws)
+    ratio = max(maxima[:-1]) / maxima[-1]
+    bad = [k for k, v in grads.items() if not torch.isfinite(v).all()]
+    print(f"headroom: max inner conv gradient / max output gradient = {ratio:.1f}; native loss {loss:.4f}; "
+          f"non-finite gradients in {len(bad)} of {len(grads)} tensors")
+    assert ratio > 32, ratio
+    assert not bad, bad[:5]
+    _compare_grads("headroom (conv_out.weight x 256)", grads, {k: v.grad for k, v in sd2.items() if v.grad is not None}, 2e-3)
 
 
 def test_training_step_is_usable_by_an_optimizer_and_repacks_weights():
@@ -233,6 +359,7 @@ def test_actor_critic_training_step_matches_reference(golden_dir):
     total = den ** 0.5
     for e, k, n in rows:
         assert e < 4e-3 or e * n < 1e-4 * total, (k, e, n)
+        assert e < PER_TENSOR_CAP, (k, e, n, total)
     keys = [str(k) for k in g["grad_keys"]]
     grads = dict(ac.named_parameters())
     norms = np.array([float(grads[k].grad.double().norm()) for k in keys])
