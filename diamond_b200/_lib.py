@@ -101,6 +101,10 @@ SIGNATURES = {
     "dmd_attn_fwd": (_i, [_vp] * 10 + [_i, _i, _i, _i, _f, _vp]),
     "dmd_nchw_to_nhwc": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "dmd_nhwc_to_nchw": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
+    "dmd_linear": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "dmd_maxpool2_stats": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "dmd_lstm_gates": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp]),
+    "dmd_resize_nhwc": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "dmd_norm_bwd": (_i, [C.POINTER(NormBwdDesc), _i, _vp]),
     "dmd_norm_affine_grad": (_i, [C.POINTER(NormBwdDesc), _vp, _vp, _vp, _vp]),
     "dmd_attn_bwd": (_i, [_vp] * 16 + [_i, _i, _i, _i, _f, _vp]),

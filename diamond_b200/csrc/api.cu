@@ -304,7 +304,9 @@ static int prep_fill(const dmd_prep_desc* d, PrepParams* p, int* nsrc) {
   while (ppb > 64 && (g.Qalloc + ppb - 1) / ppb < tune_int("DMD_PREP_MIN_BLOCKS", 2 * kPlanSms)) ppb >>= 1;
   ppb = (ppb / 32) * 32;
   p->pos_per_block = ppb;
-  DMD_CHECK(d->C0 / (d->gs0 > 0 ? d->gs0 : 8) <= 4 || d->mode == 0, "prep: at most 4 groups per source");
+  // both kernels keep (mean, rstd) of at most 4 groups per image slot in shared memory, for every source
+  DMD_CHECK(d->mode == 0 || (d->C0 / (d->gs0 > 0 ? d->gs0 : 8) <= 4 && d->C1 / (d->gs1 > 0 ? d->gs1 : 8) <= 4),
+            "prep: at most 4 groups per source (C0=%d gs0=%d, C1=%d gs1=%d)", d->C0, d->gs0, d->C1, d->gs1);
   DMD_CHECK((long long)g.Q * (g.PW > g.PH ? g.PW : g.PH) < (1ll << 32), "prep: problem too large for 32-bit position math");
   p->PW = g.PW; p->PH = g.PH; p->Q = g.Q; p->G = g.G; p->Qalloc = g.Qalloc; p->plane_bytes = (unsigned long long)g.Qalloc * 16;
   p->dPW.init(g.PW); p->dPH.init(g.PH);
@@ -512,6 +514,43 @@ static int linear_launch(const float* in, const float* W, const float* bias, flo
     linear_kernel<1><<<dim3((F + 7) / 8, by), 256, (size_t)(8 + 32) * kLinChunk * sizeof(float), st>>>(in, W, bias, out, B, K, F, silu, accumulate, hw_perm);
   DMD_LAUNCH_OK();
   return 0;
+}
+
+// MaxPool2d(2) + GroupNorm partial sums of the pooled tensor; H, W: the pre-pool size.  The statistics are reduced over aligned
+// segments of min(gs, 32) lanes, i.e. consecutive channels of one pixel: a segment stays inside one group when gs is a power
+// of two <= 32 or a multiple of 32, and warps start on a group boundary when C % 32 == 0 or 256 % C == 0.
+static int maxpool2_stats_launch(const float* x, float* y, double* stats, int B, int H, int W, int C, int gs, cudaStream_t st) {
+  DMD_CHECK(H % 2 == 0 && W % 2 == 0, "maxpool2_stats: H=%d, W=%d must be even", H, W);
+  DMD_CHECK((long long)(H / 2) * (W / 2) * C < (1ll << 31), "maxpool2_stats: image too large for 32-bit indices");
+  if (stats) DMD_CHECK(gs > 0 && C % gs == 0 && (gs % 32 == 0 || (gs <= 32 && (gs & (gs - 1)) == 0)) && (C % 32 == 0 || 256 % C == 0),
+                       "maxpool2_stats: statistics need gs a power of two <= 32 or a multiple of 32, and C %% 32 == 0 or 256 %% C == 0 (C=%d gs=%d)", C, gs);
+  const int total = (H / 2) * (W / 2) * C;
+  maxpool2_stats_kernel<<<dim3((total + 255) / 256, B), 256, 0, st>>>(x, y, stats, H, W, C, gs);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+
+// LSTMCell pointwise part: gates [B][4Hd] (pre-activations, gate order i, f, g, o) and c_in -> h_out, c_out (c_out may be c_in)
+static int lstm_gates_launch(const float* gates, const float* c_in, float* h_out, float* c_out, int B, int Hd, cudaStream_t st) {
+  lstm_gates_kernel<<<(B * Hd + 255) / 256, 256, 0, st>>>(gates, c_in, h_out, c_out, B, Hd);
+  DMD_LAUNCH_OK();
+  return 0;
+}
+
+// ---- per-op entry points of the forward CUDA-core kernels (include/diamond_b200.h): validate, then the launchers the executors use
+extern "C" int dmd_linear(const float* in, const float* W, const float* bias, float* out, int B, int K, int F, int silu, int accumulate,
+                          int hw_perm, void* stream) {
+  DMD_CHECK(in && W && out && B > 0 && K > 0 && F > 0 && hw_perm >= 0, "linear: bad arguments");
+  return linear_launch(in, W, bias, out, B, K, F, silu, (cudaStream_t)stream, accumulate, hw_perm);
+}
+extern "C" int dmd_maxpool2_stats(const float* x, float* y, double* stats, int B, int H, int W, int C, int gs, void* stream) {
+  DMD_CHECK(x && y && B > 0 && H > 0 && W > 0 && C > 0, "maxpool2_stats: bad arguments");
+  return maxpool2_stats_launch(x, y, stats, B, H, W, C, gs, (cudaStream_t)stream);
+}
+extern "C" int dmd_lstm_gates(const float* gates, const float* c_in, float* h_out, float* c_out, int B, int Hd, void* stream) {
+  DMD_CHECK(gates && c_in && h_out && c_out && B > 0 && Hd > 0, "lstm_gates: bad arguments");
+  DMD_CHECK((long long)B * Hd <= (1ll << 30), "lstm_gates: too many cells for 32-bit indices");
+  return lstm_gates_launch(gates, c_in, h_out, c_out, B, Hd, (cudaStream_t)stream);
 }
 
 extern "C" int dmd_attn_fwd(const float* x, const double* stats_in, const float* gamma, const float* beta,
@@ -779,6 +818,12 @@ static int resize_launch(const ResizeParams& p, cudaStream_t st) {
   DMD_LAUNCH_OK();
   if (p.stats) return dmd_gn_stats(p.dst, p.stats, p.B, p.Hd * p.Wd, p.C, p.gs, st);
   return 0;
+}
+extern "C" int dmd_resize_nhwc(const float* src, float* dst, int B, int Hs, int Ws, int Hd, int Wd, int C, double* stats, int gs, void* stream) {
+  DMD_CHECK(src && dst && B > 0 && Hs > 0 && Ws > 0 && Hd > 0 && Wd > 0 && C > 0 && C % 4 == 0, "resize_nhwc: bad arguments (C a multiple of 4)");
+  DMD_CHECK(!stats || (gs > 0 && C % gs == 0), "resize_nhwc: statistics need C %% gs == 0 (C=%d gs=%d)", C, gs);
+  ResizeParams p{src, dst, B, Hs, Ws, Hd, Wd, C, stats, gs};
+  return resize_launch(p, (cudaStream_t)stream);
 }
 
 namespace {
@@ -2096,10 +2141,8 @@ extern "C" int dmd_actor_critic_forward(dmd_actor_critic* h, int B, const float*
     double* st_y = lv.down ? nullptr : b.st_in[i + 1];
     if (run_conv(lv.conv, x, lv.cin, S, 2, lv.gn_w, lv.gn_b, b.st_in[i], r, b.y[i], st_y)) return 1;
     if (lv.down) {
-      const int total = (S / 2) * (S / 2) * lv.cout;
-      maxpool2_stats_kernel<<<dim3((total + 255) / 256, B), 256, 0, st>>>(b.y[i], b.pooled[i + 1], i + 1 < h->levels.size() ? b.st_in[i + 1] : nullptr,
-                                                                         S, S, lv.cout, gn_group_size(lv.cout));
-      DMD_LAUNCH_OK();
+      if (maxpool2_stats_launch(b.y[i], b.pooled[i + 1], i + 1 < h->levels.size() ? b.st_in[i + 1] : nullptr, B, S, S, lv.cout,
+                                gn_group_size(lv.cout), st)) return 1;
       S /= 2;
     }
   }
@@ -2107,8 +2150,7 @@ extern "C" int dmd_actor_critic_forward(dmd_actor_critic* h, int B, const float*
   const int K = h->feat_c * h->feat_hw, D = c.lstm_dim;
   if (linear_launch(feat, h->ptrs[h->i_wih], h->ptrs[h->i_bih], b.gates, B, K, 4 * D, 0, st, 0, h->feat_hw)) return 1;
   if (linear_launch(hx_in, h->ptrs[h->i_whh], h->ptrs[h->i_bhh], b.gates, B, D, 4 * D, 0, st, 1, 0)) return 1;
-  lstm_gates_kernel<<<(B * D + 255) / 256, 256, 0, st>>>(b.gates, cx_in, hx_out, cx_out, B, D);
-  DMD_LAUNCH_OK();
+  if (lstm_gates_launch(b.gates, cx_in, hx_out, cx_out, B, D, st)) return 1;
   if (linear_launch(hx_out, h->ptrs[h->i_aw], h->ptrs[h->i_ab], logits, B, D, c.num_actions, 0, st)) return 1;
   if (linear_launch(hx_out, h->ptrs[h->i_cw], h->ptrs[h->i_cb], val, B, D, 1, 0, st)) return 1;
   return 0;
@@ -2487,8 +2529,7 @@ extern "C" int dmd_rew_end_predict(dmd_rew_end* h, int b, int t, const float* ob
     if (linear_launch(xk, core->ptrs[h->i_wih], core->ptrs[h->i_bih], h->x_gates, b, K, 4 * D, 0, st, 0, h->feat_hw)) return 1;
     if (linear_launch(hprev, core->ptrs[h->i_whh], core->ptrs[h->i_bhh], h->x_gates, b, D, 4 * D, 0, st, 1, 0)) return 1;
     float* hk = h->y + (size_t)k * b * D;   // y rows of step k (time-major); also the next step's h
-    lstm_gates_kernel<<<(b * D + 255) / 256, 256, 0, st>>>(h->x_gates, cprev, hk, cx_out, b, D);
-    DMD_LAUNCH_OK();
+    if (lstm_gates_launch(h->x_gates, cprev, hk, cx_out, b, D, st)) return 1;
     hprev = hk; cprev = cx_out;
   }
   DMD_CUDA(cudaMemcpyAsync(hx_out, hprev, (size_t)b * D * 4, cudaMemcpyDeviceToDevice, st));

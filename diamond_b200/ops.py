@@ -64,10 +64,14 @@ def gn_stats(x: Tensor, gs: int) -> Tensor:
 def prep_act(src0: Tensor, *, src1: Optional[Tensor] = None, upsample: bool = False, mode: int = 0, silu: bool = False,
              stats0: Optional[Tensor] = None, stats1: Optional[Tensor] = None, gs0: int = 0, gs1: int = 0,
              film: Optional[Tensor] = None, film_off: int = 0, gamma: Optional[Tensor] = None, beta: Optional[Tensor] = None,
-             eps: float = 1e-5, also_raw: bool = False, split: bool = False):
+             eps: float = 1e-5, also_raw: bool = False, split: bool = False, raw_split: bool = False):
     """NHWC fp32 -> PLC16 fp16 operand(s) with the conv-input transform fused.  Returns (n0, n1, r0, r1, H, W); with
-    split=True the low fp16 parts of the main operands are returned as extra elements (l0, l1)."""
+    split=True the low fp16 parts of the main operands are returned as extra elements (l0, l1).  raw_split=True (needs
+    also_raw) also writes the low parts of the raw operands, the split-fp16 operand of a fused skip projection, and returns
+    (n0, n1, r0, r1, H, W, l0, l1, rl0, rl1) with l0 = l1 = None unless split."""
     _cuda(src0, src1, stats0, stats1, film, gamma, beta)
+    if raw_split and not also_raw:
+        raise ValueError("raw_split needs also_raw")
     lib = _lib.lib()
     b, hs, ws, c0 = src0.shape
     h, w = (2 * hs, 2 * ws) if upsample else (hs, ws)
@@ -87,7 +91,11 @@ def prep_act(src0: Tensor, *, src1: Optional[Tensor] = None, upsample: bool = Fa
     d.dst0, d.dst1, d.dst_raw0, d.dst_raw1 = n0.data_ptr(), _lib.ptr(n1), _lib.ptr(r0), _lib.ptr(r1)
     l0, l1 = (buf(c0) if split else None), (buf(c1) if (split and c1) else None)
     d.dst_lo0, d.dst_lo1 = _lib.ptr(l0), _lib.ptr(l1)
+    rl0, rl1 = (buf(c0) if raw_split else None), (buf(c1) if (raw_split and c1) else None)
+    d.dst_raw_lo0, d.dst_raw_lo1 = _lib.ptr(rl0), _lib.ptr(rl1)
     _lib.check(lib.dmd_prep_act(C.byref(d), _lib.current_stream()))
+    if raw_split:
+        return n0, n1, r0, r1, h, w, l0, l1, rl0, rl1
     if split:
         return n0, n1, r0, r1, h, w, l0, l1
     return n0, n1, r0, r1, h, w
@@ -151,6 +159,52 @@ def attn_fwd(x: Tensor, stats_in: Tensor, gamma: Tensor, beta: Tensor, wqkv: Ten
                                        wqkv.data_ptr(), bqkv.data_ptr(), wout.data_ptr(), bout.data_ptr(), out.data_ptr(),
                                        _lib.ptr(ostats), b, h * w, c, gs, eps, _lib.current_stream()))
     return out, ostats
+
+
+# ------------------------------------------------------------------------------------------------ forward CUDA-core kernels
+# One wrapper per C entry point; the launch geometry is the library's (the launchers the executors use).
+
+def linear(x: Tensor, w: Tensor, bias: Optional[Tensor] = None, *, out: Optional[Tensor] = None, silu: bool = False,
+           accumulate: bool = False, hw_perm: int = 0) -> Tensor:
+    """out [B][F] (+)= silu?(x W^T + bias) for x [B][K] (or NHWC [B][H][W][C] read in NCHW-flatten order with hw_perm = H*W),
+    W [F][K]; accumulate adds to `out` before the SiLU."""
+    _cuda(x, w, bias, out)
+    b, k, f = x.shape[0], x[0].numel(), w.shape[0]
+    if out is None:
+        if accumulate:
+            raise ValueError("accumulate needs out")
+        out = torch.empty(b, f, device=x.device, dtype=torch.float32)
+    _lib.check(_lib.lib().dmd_linear(x.data_ptr(), w.data_ptr(), _lib.ptr(bias), out.data_ptr(), b, k, f, int(silu), int(accumulate),
+                                     hw_perm, _lib.current_stream()))
+    return out
+
+
+def maxpool2_stats(x: Tensor, y: Tensor, stats: Optional[Tensor] = None, gs: int = 0) -> Tensor:
+    """MaxPool2d(2) of NHWC x [B][H][W][C] into y [B][H/2][W/2][C]; with stats [B][C/gs][2] (float64), adds y's GroupNorm
+    (sum, sumsq) to it."""
+    _cuda(x, y, stats)
+    b, h, w, c = x.shape
+    _lib.check(_lib.lib().dmd_maxpool2_stats(x.data_ptr(), y.data_ptr(), _lib.ptr(stats), b, h, w, c, gs, _lib.current_stream()))
+    return y
+
+
+def lstm_gates(gates: Tensor, c_in: Tensor, h_out: Tensor, c_out: Tensor) -> Tuple[Tensor, Tensor]:
+    """LSTMCell pointwise part from the gate pre-activations [B][4H] (order i, f, g, o) into h_out, c_out [B][H] (c_out may be
+    c_in)."""
+    _cuda(gates, c_in, h_out, c_out)
+    b, hd = c_in.shape
+    _lib.check(_lib.lib().dmd_lstm_gates(gates.data_ptr(), c_in.data_ptr(), h_out.data_ptr(), c_out.data_ptr(), b, hd, _lib.current_stream()))
+    return h_out, c_out
+
+
+def resize_nhwc(x: Tensor, out: Tensor, stats: Optional[Tensor] = None, gs: int = 0) -> Tensor:
+    """Zero-pad / crop NHWC x [B][H][W][C] at the bottom / right into out [B][Hd][Wd][C]; with stats [B][C/gs][2] (float64),
+    adds out's GroupNorm (sum, sumsq) to it."""
+    _cuda(x, out, stats)
+    b, h, w, c = x.shape
+    _lib.check(_lib.lib().dmd_resize_nhwc(x.data_ptr(), out.data_ptr(), b, h, w, out.shape[1], out.shape[2], c, _lib.ptr(stats), gs,
+                                          _lib.current_stream()))
+    return out
 
 
 def pack_conv_weight_T(w: Tensor, ci_off: int = 0, cin_k: Optional[int] = None) -> Tuple[Tensor, int, int]:

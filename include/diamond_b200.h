@@ -172,6 +172,24 @@ int dmd_attn_fwd(const float* x, const double* stats_in, const float* gamma, con
 int dmd_nchw_to_nhwc(const float* in, float* out, int B, int C, int CP, int HW, void* stream);
 int dmd_nhwc_to_nchw(const float* in, float* out, int B, int C, int CP, int HW, void* stream);
 
+/* Per-op entry points of the forward CUDA-core kernels (diamond_b200/csrc/aux_kernels.cuh) that the executors run, through
+ * the same launchers, so the launch geometry is the executors'. */
+/* out[n][f] (+)= silu?( sum_k in[n][k] W[f][k] + bias[f] ): the conditioning MLP (blocks.py:84-87), the batched FiLM linears
+ * (blocks.py:39), the LSTM input / recurrent products and the heads (actor_critic.py:71-73, rew_end_model.py:46-55).  K a multiple
+ * of 4; bias may be NULL; accumulate: out += (before the SiLU); hw_perm > 0: `in` is NHWC [B][hw_perm][K/hw_perm] read in
+ * NCHW-flatten order (k = c * hw_perm + pixel, the flatten of actor_critic.py:71). */
+int dmd_linear(const float* in, const float* W, const float* bias, float* out, int B, int K, int F, int silu, int accumulate,
+               int hw_perm, void* stream);
+/* MaxPool2d(2) (actor_critic.py:109): x NHWC [B][H][W][C] (H, W even) -> y [B][H/2][W/2][C]; stats (or NULL) [B][C/gs][2] +=
+ * (sum, sumsq) of y (caller zeroes).  Statistics need gs a power of two <= 32 or a multiple of 32, and C % 32 == 0 or 256 % C == 0. */
+int dmd_maxpool2_stats(const float* x, float* y, double* stats, int B, int H, int W, int C, int gs, void* stream);
+/* LSTMCell pointwise part (actor_critic.py:72): gates [B][4Hd] pre-activations (order i, f, g, o), c_in [B][Hd] -> h_out, c_out
+ * [B][Hd] (c_out may alias c_in). */
+int dmd_lstm_gates(const float* gates, const float* c_in, float* h_out, float* c_out, int B, int Hd, void* stream);
+/* Zero-pad / crop of NHWC [B][Hs][Ws][C] at the bottom / right to [B][Hd][Wd][C] (blocks.py:225-229, :245), C a multiple of 4;
+ * stats (or NULL) [B][C/gs][2] += (sum, sumsq) of the result. */
+int dmd_resize_nhwc(const float* src, float* dst, int B, int Hs, int Ws, int Hd, int Wd, int C, double* stats, int gs, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Per-op entry points of the CUDA-core backward kernels (diamond_b200/csrc/bwd_kernels.cuh) that dmd_denoiser_backward and
  * dmd_actor_critic_backward run, with the launch geometry those executors use.  Gradients are fp32.  `inv_scale` (a device

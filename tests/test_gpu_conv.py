@@ -97,6 +97,11 @@ CASES = [
     dict(b=2, h=32, w=32, c0=32, c1=64, cout=64),                                   # Cin 96 (generic chunk count)
     dict(b=2, h=64, w=64, c0=3, c1=0, cout=32),                                     # actor-critic stem 3 -> 32
     dict(b=2, h=24, w=40, c0=32, c1=0, cout=32),                                    # non-square, non power of two
+    dict(b=2, h=32, w=32, c0=64, c1=0, cout=48),                                    # CoutPad 48 < 64 accumulator columns
+    dict(b=3, h=16, w=24, c0=64, c1=0, cout=96),                                    # CoutPad 96 < 128 accumulator columns
+    dict(b=2, h=32, w=32, c0=64, c1=0, cout=128),                                   # the 128-column kernel (narrow images)
+    dict(b=2, h=32, w=32, c0=64, c1=0, cout=128, taps=1),
+    dict(b=2, h=32, w=32, c0=128, c1=0, cout=64),                                   # one 128-channel source (16 prep chunks)
 ]
 
 
@@ -109,7 +114,9 @@ def test_conv_plain(case):
     assert _rel(got, ref32) < 2e-3, ("fp32 reference", _rel(got, ref32))
 
 
-@pytest.mark.parametrize("case", [c for c in CASES if c.get("taps", 9) == 9], ids=lambda c: "-".join(f"{k}{v}" for k, v in c.items()))
+# row-stacked weights hold 3 * CoutPad columns, at most 256 (CoutPad <= 80)
+@pytest.mark.parametrize("case", [c for c in CASES if c.get("taps", 9) == 9 and c["cout"] <= 80],
+                         ids=lambda c: "-".join(f"{k}{v}" for k, v in c.items()))
 def test_conv_row_stacked_taps(case):
     """The tap-row-stacked weight layout of the 3x3 convs (the three taps of a kernel row side by side, N = 3 * Cout; the kernel
     addresses each tap inside its row, conv_tc.cuh) -- same results as the tap-major layout."""
@@ -135,7 +142,9 @@ def test_conv_row_stacked_norm_prologue_residual_stats(shape):
 
 @pytest.mark.parametrize("prologue,silu", [(1, True), (2, True), (1, False)])
 @pytest.mark.parametrize("shape", [dict(b=2, h=64, w=64, c0=64, c1=0, cout=64), dict(b=3, h=16, w=16, c0=64, c1=64, cout=64),
-                                   dict(b=4, h=8, w=8, c0=64, c1=0, cout=64)], ids=["64x64", "16x16cat", "8x8"])
+                                   dict(b=4, h=8, w=8, c0=64, c1=0, cout=64), dict(b=2, h=32, w=32, c0=128, c1=0, cout=64),
+                                   dict(b=2, h=16, w=16, c0=64, c1=0, cout=128)],
+                         ids=["64x64", "16x16cat", "8x8", "32x32c128", "16x16cout128"])
 def test_conv_fused_norm_prologue_residual_stats(prologue, silu, shape):
     dev = _dev()
     got, ref32, _, st = _run_conv(dev, prologue=prologue, silu=silu, residual=True, want_stats=True, seed=3, **shape)

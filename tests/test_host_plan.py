@@ -50,6 +50,9 @@ def test_dominant_conv_plan():
     (dict(C0=64, xsrc0=P, xsrc0_lo=P, xsrc1=P, xsrc1_lo=P, xC0=64, xC1=64, wpk_x=P), 4 + 16, 64),  # conv2 + fused projection: hi and lo slabs once each (24 MMAs)
     (dict(C0=64, taps=1), 4, 64),
     (dict(C0=64, CoutPad=128, Cout=128, H=32, W=32), 4, 128),                         # 147 KB of weights: narrow images only
+    (dict(Cout=48, CoutPad=48, H=32, W=32), 4, 64),                                   # CoutPad below the accumulator width
+    (dict(Cout=96, CoutPad=96, H=16, W=24), 4, 128),
+    (dict(C0=128, H=32, W=32), 8, 64),                                                # one 128-channel source
 ])
 def test_conv_plan_variants(kw, kslabs, cols):
     rc, i, err = _conv(**kw)
@@ -109,6 +112,9 @@ def test_prep_plan_block_granularity():
     assert rc == 0 and ppb == 64
     rc, blocks, ppb, nsrc, _ = _prep(Hs=32, Ws=32, C1=64, src1=P, dst1=P)
     assert rc == 0 and nsrc == 2
+    # the widest norm the executors build: 4 groups of 32 in each source of an up-path concat
+    rc, *_, err = _prep(Hs=32, Ws=32, mode=1, silu=1, stats0=P, gs0=32, film=P, C0=128, C1=128, src1=P, dst1=P, stats1=P, gs1=32)
+    assert rc == 0, err
 
 
 @pytest.mark.parametrize("kw,needle", [
@@ -123,5 +129,17 @@ def test_prep_plan_block_granularity():
     (dict(dst0=0), "null src0/dst0"),
 ])
 def test_prep_rejections_fail_loudly(kw, needle):
+    rc, *_, err = _prep(**kw)
+    assert rc != 0 and needle in err, err
+
+
+@pytest.mark.parametrize("kw,needle", [
+    (dict(C0=15), "multiples of 8"),                        # 15 image channels are zero-padded to 16 before the prep
+    # both prep kernels keep (mean, rstd) of at most 4 groups per source in shared memory: source 0 and source 1
+    (dict(mode=1, stats0=P, gs0=8, film=P), "at most 4 groups per source"),
+    (dict(mode=1, stats0=P, gs0=32, film=P, C1=64, src1=P, dst1=P, stats1=P, gs1=8), "at most 4 groups per source"),
+    (dict(mode=2, stats0=P, gs0=32, gamma=P, beta=P, C0=32, C1=128, src1=P, dst1=P, stats1=P, gs1=16), "at most 4 groups per source"),
+], ids=["c15", "groups-src0", "groups-src1-ada", "groups-src1-gn"])
+def test_prep_channel_and_group_limits(kw, needle):
     rc, *_, err = _prep(**kw)
     assert rc != 0 and needle in err, err
