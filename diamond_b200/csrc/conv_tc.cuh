@@ -190,24 +190,49 @@ struct RegEpilogue {
       float gs[kMaxOutGroups], gss[kMaxOutGroups];
 #pragma unroll
       for (int g = 0; g < kMaxOutGroups; ++g) gs[g] = gss[g] = 0.f;
+      // Every load of a batch of columns (bias from shared memory, residual from global memory) is issued before the batch's
+      // first store.  The compiler cannot prove that a store to `out` leaves the next load's address alone, so loads placed
+      // after stores would each wait out their whole latency in turn.  A batch is at most 8 column blocks, which bounds the
+      // extra registers at N = 128.
+      constexpr int kBatch = N / 8 < 8 ? N / 8 : 8;
 #pragma unroll
-      for (int j = 0; j < N / 8; ++j) {
-        const int col = 8 * j + c0;
-        if (col < p.Cout) {
-          float2 o = make_float2(acc[4 * j + 2 * h] + sbias[col], acc[4 * j + 2 * h + 1] + sbias[col + 1]);
-          if (vec) {
-            if (rp) { const float2 r = __ldg(reinterpret_cast<const float2*>(rp + col)); o.x += r.x; o.y += r.y; }
-            *reinterpret_cast<float2*>(op + col) = o;
-          } else {
-            if (rp) o.x += __ldg(rp + col);
-            op[col] = o.x;
-            if (col + 1 < p.Cout) { if (rp) o.y += __ldg(rp + col + 1); op[col + 1] = o.y; } else o.y = 0.f;
+      for (int jb = 0; jb < N / 8; jb += kBatch) {
+        float2 bv[kBatch], rv[kBatch];
+#pragma unroll
+        for (int u = 0; u < kBatch; ++u) {
+          const int col = 8 * (jb + u) + c0;
+          bv[u] = rv[u] = make_float2(0.f, 0.f);
+          if (col < p.Cout) {
+            bv[u] = make_float2(sbias[col], sbias[col + 1]);
+            if (rp) {
+              if (vec) rv[u] = __ldg(reinterpret_cast<const float2*>(rp + col));
+              else {
+                rv[u].x = __ldg(rp + col);
+                if (col + 1 < p.Cout) rv[u].y = __ldg(rp + col + 1);
+              }
+            }
           }
-          if (p.ostats != nullptr) {
-            const int gi = j >> lgs;
-            const float ps = o.x + o.y, pss = fmaf(o.x, o.x, o.y * o.y);
+        }
 #pragma unroll
-            for (int g = 0; g < kMaxOutGroups; ++g) { gs[g] += (g == gi) ? ps : 0.f; gss[g] += (g == gi) ? pss : 0.f; }
+        for (int u = 0; u < kBatch; ++u) {
+          const int j = jb + u;
+          const int col = 8 * j + c0;
+          if (col < p.Cout) {
+            float2 o = make_float2(acc[4 * j + 2 * h] + bv[u].x, acc[4 * j + 2 * h + 1] + bv[u].y);
+            if (vec) {
+              if (rp) { o.x += rv[u].x; o.y += rv[u].y; }
+              *reinterpret_cast<float2*>(op + col) = o;
+            } else {
+              if (rp) o.x += rv[u].x;
+              op[col] = o.x;
+              if (col + 1 < p.Cout) { if (rp) o.y += rv[u].y; op[col + 1] = o.y; } else o.y = 0.f;
+            }
+            if (p.ostats != nullptr) {
+              const int gi = j >> lgs;
+              const float ps = o.x + o.y, pss = fmaf(o.x, o.x, o.y * o.y);
+#pragma unroll
+              for (int g = 0; g < kMaxOutGroups; ++g) { gs[g] += (g == gi) ? ps : 0.f; gss[g] += (g == gi) ? pss : 0.f; }
+            }
           }
         }
       }
