@@ -119,7 +119,7 @@ __host__ __device__ inline ConvSmemLayout conv_smem_layout(uint32_t w_bytes, int
 // across the single-image tiles of a CTA and are reduced with warp shuffles once per image -> fp64 atomics.
 template <int N>
 struct RegEpilogue {
-  int lane, r0, lgs, G;
+  int lane, r0, G;
   float s[kStatSlots][kMaxOutGroups], ss[kStatSlots][kMaxOutGroups];
   int n_cur;
 
@@ -127,7 +127,6 @@ struct RegEpilogue {
     lane = lane_;
     r0 = row0;
     G = p.ostats ? p.Cout / p.ogs : 1;
-    lgs = p.ostats ? 31 - __clz(p.ogs >> 3) : 0;   // 8-column block j lies in group j >> lgs (ogs is 16/32/64/128)
 #pragma unroll
     for (int k = 0; k < kStatSlots; ++k)
 #pragma unroll
@@ -159,12 +158,17 @@ struct RegEpilogue {
     }
   }
 
-  // the tile starting at padded-linear position q0; acc: this thread's wgmma accumulator fragment
+  // the tile starting at padded-linear position q0; acc: this thread's wgmma accumulator fragment.  kLgs: 0 without
+  // statistics, else log2 of the 8-column blocks per output group (ogs 16/32/64/128 -> 1..4), so that block j's group j >> kLgs
+  // is known at compile time and each block adds straight into its group's sums.
+  template <int kLgs>
   __device__ __forceinline__ void tile(const ConvParams& p, const float* sbias, const float (&acc)[N / 2], int q0) {
+    constexpr bool kStats = kLgs > 0;
+    constexpr int kGroups = (N / 8) >> kLgs > 0 ? ((N / 8) >> kLgs < kMaxOutGroups ? (N / 8) >> kLgs : kMaxOutGroups) : 1;
     const int n_lo = (int)p.dPH.div(p.dPW.div((uint32_t)q0));
     const int q_last = min(q0 + kTileM, p.Q) - 1;
     const bool single_image = (int)p.dPH.div(p.dPW.div((uint32_t)q_last)) == n_lo;
-    if (p.ostats != nullptr && n_cur >= 0 && (!single_image || n_lo != n_cur)) { flush_stats(p, n_cur, 1); n_cur = -1; }
+    if (kStats && n_cur >= 0 && (!single_image || n_lo != n_cur)) { flush_stats(p, n_cur, 1); n_cur = -1; }
     const int c0 = 2 * (lane & 3);
     const bool vec = (p.Cout & 1) == 0;   // 8-byte accesses (every layer but conv_out / the 15-channel dgrad)
 #pragma unroll
@@ -227,24 +231,28 @@ struct RegEpilogue {
               op[col] = o.x;
               if (col + 1 < p.Cout) { if (rp) o.y += rv[u].y; op[col + 1] = o.y; } else o.y = 0.f;
             }
-            if (p.ostats != nullptr) {
-              const int gi = j >> lgs;
-              const float ps = o.x + o.y, pss = fmaf(o.x, o.x, o.y * o.y);
-#pragma unroll
-              for (int g = 0; g < kMaxOutGroups; ++g) { gs[g] += (g == gi) ? ps : 0.f; gss[g] += (g == gi) ? pss : 0.f; }
+            if (kStats) {
+              gs[j >> kLgs] += o.x + o.y;
+              gss[j >> kLgs] += fmaf(o.x, o.x, o.y * o.y);
             }
           }
         }
       }
-      if (p.ostats != nullptr) {
-        const int sl = single_image ? 0 : slot;
+      if (kStats) {
+        // Groups and slots that a value does not belong to are skipped rather than given +0.0: every sum starts at +0.0 and
+        // so is never -0.0, which makes adding +0.0 an identity, and the sums keep the bits of the select-and-add form.
+        if (single_image) {   // warp-uniform: every row of the tile is in image n_lo
 #pragma unroll
-        for (int k = 0; k < kStatSlots; ++k)
+          for (int g = 0; g < kGroups; ++g) { s[0][g] += gs[g]; ss[0][g] += gss[g]; }
+        } else {
 #pragma unroll
-          for (int g = 0; g < kMaxOutGroups; ++g) { s[k][g] += (sl == k) ? gs[g] : 0.f; ss[k][g] += (sl == k) ? gss[g] : 0.f; }
+          for (int k = 0; k < kStatSlots; ++k)
+#pragma unroll
+            for (int g = 0; g < kGroups; ++g) { s[k][g] += (slot == k) ? gs[g] : 0.f; ss[k][g] += (slot == k) ? gss[g] : 0.f; }
+        }
       }
     }
-    if (p.ostats != nullptr) {
+    if (kStats) {
       if (single_image) n_cur = n_lo;            // keep running across the single-image tiles of this CTA
       else { flush_stats(p, n_lo, kStatSlots); n_cur = -1; }
     }
@@ -334,6 +342,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_tc_kernel(const ConvPara
     const int m0 = ((warp >> 2) - 1) * 64;     // first tile row of this warpgroup
     RegEpilogue<N> epi;
     epi.init(p, m0 + 16 * (warp & 3) + (lane >> 2), lane);
+    const int lgs = p.ostats ? 31 - __clz(p.ogs >> 3) : 0;   // 8-column block j lies in output group j >> lgs
     if (my_tiles > 0) mbar_wait(wbar, 0);
     // Descriptor words: per wgmma only the 14-bit start-address fields change (A: ring stage + tap shift, B: tap + slab), all in
     // 16-byte units.  K-major operands: LBO = stride of the 8-channel chunks, SBO = 128 B (eight 16-byte rows).
@@ -395,7 +404,13 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_tc_kernel(const ConvPara
       wgmma_wait<0>();
       wgmma_fence_operands(acc);
       if (done > 0 && lane == 0) mbar_arrive(empty + prev);
-      epi.tile(p, sbias, acc, (tile_begin + it) * kTileM);
+      // statistics' group size -> template argument (only the sizes an N-column accumulator can hold are instantiated)
+      const int q0 = (tile_begin + it) * kTileM;
+      if (lgs == 0) epi.template tile<0>(p, sbias, acc, q0);
+      else if (lgs == 1 || N == 16) epi.template tile<1>(p, sbias, acc, q0);
+      else if (lgs == 2 || N == 32) epi.template tile<2>(p, sbias, acc, q0);
+      else if (lgs == 3 || N == 64) epi.template tile<3>(p, sbias, acc, q0);
+      else epi.template tile<4>(p, sbias, acc, q0);
     }
     epi.finish(p);
   }
