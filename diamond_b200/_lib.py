@@ -114,7 +114,6 @@ SIGNATURES = {
     "dmd_embedding_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "dmd_colsum": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _vp]),
     "dmd_sumpool2": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp]),
-    "dmd_add": (_i, [_vp, _vp, _ll, _i, _vp]),
     "dmd_dsilu_mul": (_i, [_vp, _vp, _vp, _ll, _vp]),
     "dmd_maxpool2_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "dmd_lstm_cell_bwd": (_i, [_vp] * 6 + [_i, _i, _vp]),

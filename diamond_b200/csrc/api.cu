@@ -678,11 +678,6 @@ static int sumpool2_launch(const float* in, float* out, int B, int H, int W, int
   DMD_LAUNCH_OK();
   return 0;
 }
-static int add_launch(const float* a, float* out, long long total4, int accumulate, cudaStream_t st) {
-  add_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>(a, out, accumulate, total4);
-  DMD_LAUNCH_OK();
-  return 0;
-}
 static int dsilu_mul_launch(const float* pre, const float* dh, float* out, long long n, cudaStream_t st) {
   dsilu_mul_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pre, dh, out, n);
   DMD_LAUNCH_OK();
@@ -779,10 +774,6 @@ extern "C" int dmd_sumpool2(const float* in, float* out, int B, int H, int W, in
   DMD_CHECK(in && out && B > 0 && H > 0 && W > 0 && C % 4 == 0, "sumpool2: bad arguments (C a multiple of 4)");
   return sumpool2_launch(in, out, B, H, W, C, accumulate, (cudaStream_t)stream);
 }
-extern "C" int dmd_add(const float* a, float* out, long long n, int accumulate, void* stream) {
-  DMD_CHECK(a && out && n > 0 && n % 4 == 0, "add: bad arguments (n a multiple of 4)");
-  return add_launch(a, out, n / 4, accumulate, (cudaStream_t)stream);
-}
 extern "C" int dmd_dsilu_mul(const float* pre, const float* dh, float* out, long long n, void* stream) {
   DMD_CHECK(pre && dh && out && n > 0, "dsilu_mul: bad arguments");
   return dsilu_mul_launch(pre, dh, out, n, (cudaStream_t)stream);
@@ -833,9 +824,9 @@ constexpr float kGnEps = 1e-5f;  // blocks.py:13
 struct ConvW {          // one nn.Conv2d
   int w_idx, b_idx;     // indices into the state_dict pointer list
   int Cout, CoutPad, CinReal, Cin, taps, c0_real, c0_store;
-  int precise = 0;      // split-fp16: K = 3 * Cin
+  int precise = 0;      // split-fp16 in one launch: K = 3 * Cin
   int trs = 0;          // forward weights in the tap-row-stacked layout (3x3, non-split)
-  int three_pass = 0;   // split-fp16 as three launches (A_hi W_hi, A_lo W_hi, A_hi W_lo) when 3 * Cin weights exceed shared memory
+  int three_pass = 0;   // split-fp16 as three launches (A_hi W_hi, A_lo W_hi, A_hi W_lo): 3 * Cin weights would crowd out the slab ring
   size_t pk_off;        // byte offset into the packed-weight buffer
   size_t pk_lo_off = 0; // three_pass: the low-part pack
   // backward-data packs (transposed, tap-flipped; one per source of a channel concat), training only
@@ -864,7 +855,7 @@ struct Operand {
 };
 
 // backward op list (training).  Parameter-gradient destinations are OFFSETS into the caller's flat gradient buffer.
-enum BKind { B_PREP = 0, B_CONV, B_WGRAD, B_COLSUM, B_NORM1, B_NORM2, B_AFFINE, B_POOL, B_ADD, B_ATTN, B_MEMSET, B_SGEMM, B_FILMW,
+enum BKind { B_PREP = 0, B_CONV, B_WGRAD, B_COLSUM, B_NORM1, B_NORM2, B_AFFINE, B_POOL, B_ATTN, B_MEMSET, B_SGEMM, B_FILMW,
              B_LINEAR, B_DSILU, B_EMB };
 struct BOp {
   int kind = 0;
@@ -874,7 +865,7 @@ struct BOp {
   long long goff = -1, goff2 = -1;            // flat-gradient offsets (floats)
   NormBwdParams nb;
   int chunks = 0;                             // sgemm: split-K chunk count (<= 1: no split)
-  const float* src = nullptr; float* dst = nullptr; long long rows = 0; int C = 0, Creal = 0, H = 0, W = 0, acc = 0; long long total4 = 0;
+  const float* src = nullptr; float* dst = nullptr; long long rows = 0; int C = 0, Creal = 0, H = 0, W = 0, acc = 0;
   AttnBwdParams ab; long long goffs[6] = {-1, -1, -1, -1, -1, -1};
   void* ms_ptr = nullptr; size_t ms_bytes = 0;
   // sgemm: C = alpha * op(A) op(B); c_goff >= 0 -> C lives in the gradient buffer
@@ -933,23 +924,65 @@ struct SamplerGraph {
   cudaGraphExec_t exec = nullptr;
 };
 
+// What every model executor owns apart from its layers: the state_dict tensors (element counts, the caller's pointers and
+// offsets into the flat gradient buffer) and the packed-weight buffer (conv packs, then the FiLM table of all AdaGroupNorms).
+struct ModelCore {
+  int n_tensors = 0;
+  std::vector<long long> numel, goff;   // per state_dict tensor: element count and offset into the flat gradient buffer
+  long long grad_total = 0;
+  std::vector<const float*> ptrs;
+  uint8_t* packed = nullptr;
+  size_t packed_bytes = 0;
+  int cond_channels = 0, film_rows = 0;  // FiLM table: film_rows x cond_channels weights, then film_rows biases
+  size_t film_w_off = 0, film_b_off = 0;
+
+  const float* P(int idx) const { return ptrs.empty() ? nullptr : ptrs[idx]; }
+  // once every tensor is registered: 16-byte aligned gradient slices, and the FiLM table behind the pk bytes of conv packs
+  void finish(size_t pk) {
+    n_tensors = (int)numel.size();
+    goff.assign(n_tensors, 0);
+    grad_total = 0;
+    for (int i = 0; i < n_tensors; ++i) { goff[i] = grad_total; grad_total += (numel[i] + 3) & ~3ll; }
+    film_w_off = pk; pk += (size_t)film_rows * cond_channels * 4; pk = (pk + 255) & ~(size_t)255;
+    film_b_off = pk; pk += (size_t)film_rows * 4; pk = (pk + 255) & ~(size_t)255;
+    packed_bytes = pk;
+  }
+  // adopts the caller's tensors (`module`.state_dict() order); *moved: a tensor or the packed buffer is not where it was
+  int set_weights(const char* module, const float* const* ptrs_host, int n_ptrs, void* packed_buf, bool* moved) {
+    DMD_CHECK(ptrs_host && packed_buf, "set_weights: null argument");
+    DMD_CHECK(n_ptrs == n_tensors, "set_weights: expected %d tensors (%s.state_dict order), got %d", n_tensors, module, n_ptrs);
+    *moved = packed != (uint8_t*)packed_buf || ptrs.empty() || memcmp(ptrs.data(), ptrs_host, sizeof(float*) * n_ptrs) != 0;
+    ptrs.assign(ptrs_host, ptrs_host + n_ptrs);
+    packed = (uint8_t*)packed_buf;
+    return 0;
+  }
+  bool ready() const { return !ptrs.empty() && packed; }
+};
+
+long long grad_layout(const ModelCore* m, long long* offsets, long long* numels, int n) {
+  if (!m || n != m->n_tensors) { fail("grad_layout: expected %d entries", m ? m->n_tensors : 0); return -1; }
+  for (int i = 0; i < n; ++i) { if (offsets) offsets[i] = m->goff[i]; if (numels) numels[i] = m->numel[i]; }
+  return m->grad_total;
+}
+
+// one reward / termination workspace: the encoder plan (plan.B rows on the workspace at plan.base), then the LSTM / head buffers
+struct RewEndLayout {
+  Plan plan;
+  Tens feat{};  // encoder output: NHWC, last level, time-major rows
+  float *x_gates = nullptr, *y = nullptr, *hid = nullptr, *logits_tm = nullptr, *hc[2] = {nullptr, nullptr};
+};
+
 }  // namespace
 
 struct dmd_denoiser {
   dmd_denoiser_config cfg;
-  int n_tensors = 0;
+  ModelCore core;
   // state_dict indices
   int i_fourier = 0, i_actemb = 0, i_cp0w = 0, i_cp0b = 0, i_cp2w = 0, i_cp2b = 0, i_normout_w = 0, i_normout_b = 0;
   ConvW conv_in, conv_out;
   std::vector<std::vector<ResBlockW>> d_blocks, u_blocks;
   std::vector<ResBlockW> mid;
   std::vector<ConvW> downs, ups;  // index 0 unused (Identity)
-  int film_rows = 0;
-  size_t packed_bytes = 0, film_w_off = 0, film_b_off = 0;
-  std::vector<const float*> ptrs;
-  uint8_t* packed = nullptr;
-  std::vector<long long> numel, goff;   // per state_dict tensor: element count and offset into the flat gradient buffer
-  long long grad_total = 0;
   Plan plan;
   std::vector<SamplerGraph> graphs;     // one per distinct (buffers, ring head): a WorldModelEnv replays T of them round-robin
   unsigned long long graph_clock = 0;
@@ -960,38 +993,54 @@ struct dmd_denoiser {
   int need_B = 0, need_H = 0, need_W = 0; size_t need_bytes = 0;
 };
 
+// Reward / termination model (executor below dmd_lambda_returns): the encoder is built from the U-Net's ResBlocks
+struct dmd_rew_end {
+  dmd_rew_end_config cfg;
+  ModelCore core;
+  ConvW conv_in;
+  std::vector<std::vector<ResBlockW>> blocks;   // per level, then the two attention ResBlocks
+  std::vector<ConvW> downs;                     // index 0 unused
+  int i_actemb = 0, i_wih = 0, i_whh = 0, i_bih = 0, i_bhh = 0, i_h0w = 0, i_h0b = 0, i_h2w = 0;
+  int feat_c = 0, feat_hw = 0;
+  RewEndLayout lay;
+};
+
 namespace {
 
 struct Walker {  // assigns state_dict indices in module registration order and packed-buffer offsets
-  dmd_denoiser* h; int idx = 0; size_t pk = 0;
-  int next(long long n) { h->numel.push_back(n); return idx++; }
-  ConvW conv(int cout, int cin_real, int taps, int c0_real, int c0_store, int c1, int precise = 0, bool dgrad = true) {
+  ModelCore* m; size_t pk = 0;
+  int next(long long n) { m->numel.push_back(n); return (int)m->numel.size() - 1; }
+  size_t take(size_t bytes) { const size_t off = pk; pk = (pk + bytes + 255) & ~(size_t)255; return off; }
+  // split: split-fp16 forward (error ~2^-22), in one launch with K = 3 * Cin when those weights take at most 120 KB of shared
+  // memory, else in three launches that leave the slab ring its room
+  ConvW conv(int cout, int cin_real, int taps, int c0_real, int c0_store, int c1, bool split = false, bool dgrad = true) {
     ConvW c; c.w_idx = next((long long)cout * cin_real * taps); c.b_idx = next(cout);
     c.Cout = cout; c.CoutPad = round_up(cout, 16); c.CinReal = cin_real; c.taps = taps;
-    c.c0_real = c0_real; c.c0_store = c0_store; c.Cin = round_up(c0_store + c1, 16); c.precise = precise;
+    c.c0_real = c0_real; c.c0_store = c0_store; c.Cin = round_up(c0_store + c1, 16);
+    const size_t w1 = (size_t)taps * c.Cin * c.CoutPad * 2;
+    c.precise = split && 3 * w1 <= 120 * 1024;
+    c.three_pass = split && !c.precise;
     // tap-row-stacked weight layout: opt-in (DMD_CONV_TRS=1).  The conv kernel addresses each tap inside it, so the layout
     // changes the weight packing only, not the tensor-core work
-    c.trs = (taps == 9 && !precise && 3 * c.CoutPad <= 256 && tune_int("DMD_CONV_TRS", 0) != 0) ? 1 : 0;
-    c.pk_off = pk; pk += (size_t)taps * c.Cin * c.CoutPad * 2 * (precise ? 3 : 1); pk = (pk + 255) & ~(size_t)255;
+    c.trs = (taps == 9 && !split && 3 * c.CoutPad <= 256 && tune_int("DMD_CONV_TRS", 0) != 0) ? 1 : 0;
+    c.pk_off = take(w1 * (c.precise ? 3 : 1));
+    if (c.three_pass) c.pk_lo_off = take(w1);
     if (dgrad) {
       c.nsrcT = c1 ? 2 : 1;
       c.srcC[0] = c0_real; c.srcC[1] = c1; c.srcOff[0] = 0; c.srcOff[1] = c0_real;
-      for (int k = 0; k < c.nsrcT; ++k) {
-        c.pkT_off[k] = pk;
-        pk += (size_t)taps * round_up(cout, 16) * round_up(c.srcC[k], 16) * 2; pk = (pk + 255) & ~(size_t)255;
-      }
+      for (int k = 0; k < c.nsrcT; ++k) c.pkT_off[k] = take((size_t)taps * round_up(cout, 16) * round_up(c.srcC[k], 16) * 2);
     }
     return c;
   }
   FilmW film(int C) {
-    FilmW f; f.w_idx = next((long long)2 * C * h->cfg.cond_channels); f.b_idx = next(2 * C);
-    f.C = C; f.off = h->film_rows; h->film_rows += 2 * C; return f;
+    FilmW f; f.w_idx = next((long long)2 * C * m->cond_channels); f.b_idx = next(2 * C);
+    f.C = C; f.off = m->film_rows; m->film_rows += 2 * C; return f;
   }
   // c0/c1: channels of the two concatenated inputs (c1 = 0: single input)
   ResBlockW resblock(int c0, int c1, int cout, bool attn) {
     ResBlockW r; r.cin = c0 + c1; r.cout = cout;
     r.has_proj = (r.cin != cout);
-    if (r.has_proj) r.proj = conv(cout, r.cin, 1, c0, c0, c1, 1);  // raw residual stream -> split-fp16
+    if (r.has_proj) r.proj = conv(cout, r.cin, 1, c0, c0, c1, true);  // raw residual stream -> split-fp16
     r.n1 = film(r.cin);
     r.c1 = conv(cout, r.cin, 9, c0, c0, c1);
     r.n2 = film(cout);
@@ -1008,16 +1057,16 @@ struct Walker {  // assigns state_dict indices in module registration order and 
 int build_structure(dmd_denoiser* h) {
   const dmd_denoiser_config& c = h->cfg;
   const int L = c.num_levels;
-  Walker w{h};
+  h->core.cond_channels = c.cond_channels;
+  Walker w{&h->core};
   // InnerModel.__init__ registration order (inner_model.py:24-42): noise_emb, act_emb, cond_proj, conv_in, unet,
   // norm_out, conv_out.  UNet (blocks.py:183-220): d_blocks, u_blocks, mid_blocks, downsamples, upsamples.
   const long long CC = c.cond_channels;
-  h->numel.clear();
   h->i_fourier = w.next(CC / 2); h->i_actemb = w.next((long long)c.num_actions * (CC / c.num_steps_conditioning));
   h->i_cp0w = w.next(CC * CC); h->i_cp0b = w.next(CC); h->i_cp2w = w.next(CC * CC); h->i_cp2b = w.next(CC);
   const int cin_real = (c.num_steps_conditioning + 1) * c.img_channels;
   const int cin_store = round_up(cin_real, 16);
-  h->conv_in = w.conv(c.channels[0], cin_real, 9, cin_real, cin_store, 0, 1, false);  // its input needs no gradient
+  h->conv_in = w.conv(c.channels[0], cin_real, 9, cin_real, cin_store, 0, true, false);  // its input needs no gradient
   h->d_blocks.resize(L);
   for (int i = 0; i < L; ++i) {
     const int c1 = c.channels[i > 0 ? i - 1 : 0], c2 = c.channels[i];
@@ -1039,16 +1088,51 @@ int build_structure(dmd_denoiser* h) {
   for (int i = 1; i < L; ++i) h->downs[i] = w.conv(c.channels[i - 1], c.channels[i - 1], 9, c.channels[i - 1], c.channels[i - 1], 0);
   for (int m = 1; m < L; ++m) { const int ch = c.channels[L - 1 - m]; h->ups[m] = w.conv(ch, ch, 9, ch, ch, 0); }
   h->i_normout_w = w.next(c.channels[0]); h->i_normout_b = w.next(c.channels[0]);
-  h->conv_out = w.conv(c.img_channels, c.channels[0], 9, c.channels[0], c.channels[0], 0, 0);  // split-fp16 here costs 3x on an N=16 conv for 3.2e-4
-  h->n_tensors = w.idx;
-  h->goff.assign(h->n_tensors, 0);
-  h->grad_total = 0;
-  for (int i = 0; i < h->n_tensors; ++i) { h->goff[i] = h->grad_total; h->grad_total += (h->numel[i] + 3) & ~3ll; }  // 16-byte aligned slices
-  size_t pk = w.pk;
-  h->film_w_off = pk; pk += (size_t)h->film_rows * c.cond_channels * 4; pk = (pk + 255) & ~(size_t)255;
-  h->film_b_off = pk; pk += (size_t)h->film_rows * 4; pk = (pk + 255) & ~(size_t)255;
-  h->packed_bytes = pk;
+  h->conv_out = w.conv(c.img_channels, c.channels[0], 9, c.channels[0], c.channels[0], 0);  // split-fp16 here costs 3x on an N=16 conv for 3.2e-4
+  h->core.finish(w.pk);
   return 0;
+}
+
+// ---- descriptors shared by the plan builders and the actor-critic's immediate-mode launches
+// single-source operand of src [B][Hs][Ws][C]: raw (mode 0; ups = 2: zero insertion, the adjoint of a stride-2 conv) or
+// silu(GroupNorm(gamma, beta)) with the statistics `stats` (mode 2); dst_lo: optional low fp16 part
+dmd_prep_desc prep_desc(const float* src, int C, int B, int Hs, int Ws, int ups, int mode, const double* stats, const float* gamma,
+                        const float* beta, void* dst, void* dst_lo = nullptr) {
+  dmd_prep_desc d; memset(&d, 0, sizeof(d));
+  d.src0 = src; d.C0 = C; d.B = B; d.Hs = Hs; d.Ws = Ws; d.upsample = ups; d.mode = mode; d.silu = mode ? 1 : 0;
+  if (mode) { d.stats0 = stats; d.gs0 = gn_group_size(C); d.gamma = gamma; d.beta = beta; }
+  d.eps = kGnEps; d.dst0 = dst; d.dst_lo0 = dst_lo;
+  return d;
+}
+// backward-data for source k of conv cw: out (+)= conv(gy, W_k^T flipped) at H x W; wpk: the pack at cw.pkT_off[k]
+dmd_conv_desc dgrad_desc(const ConvW& cw, int k, const void* wpk, const void* gy, int B, int H, int W, float* out, bool accumulate) {
+  dmd_conv_desc d; memset(&d, 0, sizeof(d));
+  d.src0 = gy; d.C0 = round_up(cw.Cout, 16); d.B = B; d.H = H; d.W = W; d.taps = cw.taps; d.stride = 1;
+  d.wpk = wpk; d.Cout = cw.srcC[k]; d.CoutPad = round_up(cw.srcC[k], 16);
+  d.out = out; d.residual = accumulate ? out : nullptr;
+  return d;
+}
+// ConvW::three_pass: pass 0 = A_hi W_hi (+ bias, residual), pass 1 = A_lo W_hi, pass 2 = A_hi W_lo, the later two accumulating
+// into the output in place; the statistics come with the last.  d: the one-launch conv with the low operand parts in src*_lo
+dmd_conv_desc conv_pass(dmd_conv_desc d, int pass, const void* wpk_lo) {
+  const void *lo0 = d.src0_lo, *lo1 = d.src1_lo;
+  d.precise = 0; d.src0_lo = d.src1_lo = nullptr;
+  if (pass == 1) { d.src0 = lo0; d.src1 = lo1; }
+  if (pass == 2) d.wpk = wpk_lo;
+  if (pass > 0) { d.bias = nullptr; d.residual = d.out; }
+  if (pass < 2) d.out_stats = nullptr;
+  return d;
+}
+// silu(GroupNorm(gamma, beta)) backward of x [B][HW][C] (mode 2): per-channel sums in nsum ([2][B][kMaxCin], zeroed before
+// pass 1), gx (+)= the input gradient (+ addend)
+NormBwdParams gn_bwd_params(const float* x, const float* gy, const double* stats, int B, int HW, int C, int gs, const float* gamma,
+                            const float* beta, float* nsum, float* gx, const float* addend, bool accumulate) {
+  NormBwdParams nb; memset(&nb, 0, sizeof(nb));
+  nb.x = x; nb.gy = gy; nb.stats = stats; nb.B = B; nb.HW = HW; nb.C = C; nb.gs = gs; nb.mode = 2; nb.act = 1; nb.eps = kGnEps;
+  nb.gamma = gamma; nb.beta = beta;
+  nb.sumA = nsum; nb.sumB = nsum ? nsum + (size_t)B * kMaxCin : nullptr; nb.sum_stride = kMaxCin;
+  nb.gx = gx; nb.addend = addend; nb.accumulate = accumulate ? 1 : 0;
+  return nb;
 }
 
 struct Bump {
@@ -1058,7 +1142,7 @@ struct Bump {
 
 // -- plan construction: mirrors InnerModel.forward / UNet.forward / ResBlock.forward
 struct PlanBuilder {
-  dmd_denoiser* h; Plan* pl; Bump* bump; Bump* sbump; int err = 0;
+  const ModelCore* core; Plan* pl; Bump* bump; Bump* sbump; int err = 0;
 
   Tens tensor(int C, int H, int W, bool with_stats, bool with_grad = true) {
     Tens t; t.C = C; t.H = H; t.W = W; t.gs = gn_group_size(C);
@@ -1068,7 +1152,8 @@ struct PlanBuilder {
     return t;
   }
   void record(const Rec& r) { if (pl->train) pl->tape.push_back(r); }
-  const float* P(int idx) const { return h->ptrs.empty() ? nullptr : h->ptrs[idx]; }
+  const float* P(int idx) const { return core->P(idx); }
+  const void* pk(size_t off) const { return core->packed ? core->packed + off : (const void*)1; }
 
   uint8_t* scratch() {
     uint8_t* p = pl->scratch[pl->scratch_next];
@@ -1097,7 +1182,7 @@ struct PlanBuilder {
       d.stats0 = a.stats ? a.stats : (const double*)1; d.gs0 = a.gs;
       if (b) { d.stats1 = b->stats ? b->stats : (const double*)1; d.gs1 = b->gs; }
     }
-    if (o.mode == 1) { d.film = pl->film ? pl->film : (const float*)1; d.film_stride = h->film_rows; d.film_off = o.film->off; }
+    if (o.mode == 1) { d.film = pl->film ? pl->film : (const float*)1; d.film_stride = core->film_rows; d.film_off = o.film->off; }
     if (o.mode == 2) { d.gamma = P(o.gamma_idx) ? P(o.gamma_idx) : (const float*)1; d.beta = P(o.beta_idx) ? P(o.beta_idx) : (const float*)1; }
     d.eps = kGnEps;
     o.n0 = scratch(); d.dst0 = o.n0;
@@ -1120,21 +1205,26 @@ struct PlanBuilder {
     if (xproj) {  // skip projection of the block input, accumulated into this conv's output tile
       d.xsrc0 = xin->r0; d.xsrc0_lo = xin->rl0; d.xC0 = xin->C0;
       if (xin->C1) { d.xsrc1 = xin->r1; d.xsrc1_lo = xin->rl1; d.xC1 = xin->C1; }
-      d.wpk_x = h->packed ? h->packed + xproj->pk_off : (const void*)1; d.bias_x = P(xproj->b_idx);
+      d.wpk_x = pk(xproj->pk_off); d.bias_x = P(xproj->b_idx);
+      if (!xproj->precise) { fail("plan: a fused projection needs its split-fp16 weights in one pack"); err = 1; return; }
     }
+    const bool split = cw.precise || cw.three_pass;
     d.src0 = raw ? in.r0 : in.n0; d.src1 = in.C1 ? (raw ? in.r1 : in.n1) : nullptr;
     d.precise = cw.precise; d.wpk_layout = cw.trs;
-    if (cw.precise) { d.src0_lo = raw ? in.rl0 : in.nl0; d.src1_lo = in.C1 ? in.rl1 : nullptr; }
+    if (split) { d.src0_lo = raw ? in.rl0 : in.nl0; d.src1_lo = in.C1 ? in.rl1 : nullptr; }
     d.C0 = in.C0; d.C1 = in.C1; d.B = pl->B; d.H = in.H; d.W = in.W; d.taps = cw.taps; d.stride = stride;
-    d.wpk = h->packed ? h->packed + cw.pk_off : (const void*)1; d.bias = P(cw.b_idx);
+    d.wpk = pk(cw.pk_off); d.bias = P(cw.b_idx);
     d.Cout = cw.Cout; d.CoutPad = cw.CoutPad;
     d.residual = resid ? (resid->data ? resid->data : (const float*)1) : nullptr; d.out = out.data ? out.data : (float*)1;
     d.out_stats = out_stats ? (out.stats ? out.stats : (double*)1) : nullptr; d.out_gs = out.gs;
-    if (cw.precise && (!d.src0_lo || (in.C1 && !d.src1_lo))) { fail("plan: precise conv without low operand parts"); err = 1; return; }
+    if (split && (!d.src0_lo || (in.C1 && !d.src1_lo))) { fail("plan: precise conv without low operand parts"); err = 1; return; }
     if (in.C0 + in.C1 != cw.Cin) { fail("plan: operand channels %d+%d do not match the packed weights (%d)", in.C0, in.C1, cw.Cin); err = 1; return; }
-    Op op; op.kind = OP_CONV;
-    if (conv_fill(&d, &op.conv, &op.smem, &op.cols)) { err = 1; return; }
-    pl->ops.push_back(op);
+    for (int pass = 0; pass < (cw.three_pass ? 3 : 1); ++pass) {
+      const dmd_conv_desc dp = cw.three_pass ? conv_pass(d, pass, pk(cw.pk_lo_off)) : d;
+      Op op; op.kind = OP_CONV;
+      if (conv_fill(&dp, &op.conv, &op.smem, &op.cols)) { err = 1; return; }
+      pl->ops.push_back(op);
+    }
   }
 
   // ResBlock.forward (blocks.py:141-147)
@@ -1161,9 +1251,9 @@ struct PlanBuilder {
   }
 
   // RewEndEncoder.forward (rew_end_model.py:127-132): conv_in, then per level [Downsample] + ResBlocks, then two attention
-  // ResBlocks; the same blocks as the U-Net, conditioned on the action embedding.  Output: pl->feat (NHWC, last level).
-  int build_rew_end(const std::vector<std::vector<ResBlockW>>& blocks, const std::vector<ConvW>& downs, const ConvW& conv_in, Tens* feat) {
-    const dmd_denoiser_config& c = h->cfg;
+  // ResBlocks; the same blocks as the U-Net, conditioned on the action embedding.  Output: *feat (NHWC, last level).
+  int build_rew_end(const dmd_rew_end* h, Tens* feat) {
+    const dmd_rew_end_config& c = h->cfg;
     const int L = c.num_levels, B = pl->B, H = pl->H, W = pl->W;
     if (H % (1 << (L - 1)) || W % (1 << (L - 1))) return fail("rew_end: H=%d W=%d must be multiples of %d", H, W, 1 << (L - 1));
     int cmax = 16;
@@ -1171,20 +1261,20 @@ struct PlanBuilder {
     const size_t slot_bytes = (plc16_bytes(B, H, W, cmax) + 255) & ~(size_t)255;
     for (int i = 0; i < kScratchSlots; ++i) pl->scratch[i] = (uint8_t*)bump->take(slot_bytes);
     pl->scratch_next = 0;
-    pl->CP_in = conv_in.c0_store;
+    pl->CP_in = h->conv_in.c0_store;
     pl->xin = (float*)bump->take((size_t)B * H * W * pl->CP_in * 4);
     pl->cond = (float*)bump->take((size_t)B * c.cond_channels * 4);
-    pl->film = (float*)bump->take((size_t)B * h->film_rows * 4);
+    pl->film = (float*)bump->take((size_t)B * core->film_rows * 4);
     Tens xin{pl->xin, nullptr, pl->CP_in, H, W, 8};
     Tens x = tensor(c.channels[0], H, W, true);
-    { Operand in0 = prep(xin, nullptr, 0, 0, nullptr, 0, 0, false, false, true); conv(conv_in, in0, false, 1, nullptr, x, true); }
+    { Operand in0 = prep(xin, nullptr, 0, 0, nullptr, 0, 0, false, false, true); conv(h->conv_in, in0, false, 1, nullptr, x, true); }
     for (int i = 0; i <= L; ++i) {
       if (i > 0 && i < L) {
         Tens xd = tensor(c.channels[i - 1], x.H / 2, x.W / 2, true);
-        { Operand ind = prep(x, nullptr, 0, 0, nullptr, 0, 0, false, false); conv(downs[i], ind, false, 2, nullptr, xd, true); }
+        { Operand ind = prep(x, nullptr, 0, 0, nullptr, 0, 0, false, false); conv(h->downs[i], ind, false, 2, nullptr, xd, true); }
         x = xd;
       }
-      for (auto& rb : blocks[i]) x = resblock(rb, x, nullptr);
+      for (auto& rb : h->blocks[i]) x = resblock(rb, x, nullptr);
     }
     *feat = x;
     return err;
@@ -1197,7 +1287,7 @@ struct PlanBuilder {
     pl->ops.push_back(op);
   }
 
-  int build() {
+  int build(const dmd_denoiser* h) {
     const dmd_denoiser_config& c = h->cfg;
     const int L = c.num_levels, B = pl->B, H = pl->H, W = pl->W;
     const int div = 1 << (L - 1);
@@ -1218,7 +1308,7 @@ struct PlanBuilder {
     pl->cemb = (float*)bump->take((size_t)B * c.cond_channels * 4);
     pl->chid = (float*)bump->take((size_t)B * c.cond_channels * 4);
     pl->cond = (float*)bump->take((size_t)B * c.cond_channels * 4);
-    pl->film = (float*)bump->take((size_t)B * h->film_rows * 4);
+    pl->film = (float*)bump->take((size_t)B * core->film_rows * 4);
     Tens xin{pl->xin, nullptr, pl->CP_in, H, W, 8};
     Tens x = tensor(c.channels[0], H, W, !padded);
     {
@@ -1280,24 +1370,24 @@ struct PlanBuilder {
       const size_t K = kMaxSamplerEvals;
       pl->sig_all = (float*)bump->take(K * 4);
       pl->cemb_all = (float*)bump->take(K * B * c.cond_channels * 4); pl->chid_all = (float*)bump->take(K * B * c.cond_channels * 4);
-      pl->cond_all = (float*)bump->take(K * B * c.cond_channels * 4); pl->film_all = (float*)bump->take(K * B * h->film_rows * 4);
+      pl->cond_all = (float*)bump->take(K * B * c.cond_channels * 4); pl->film_all = (float*)bump->take(K * B * core->film_rows * 4);
     }
     return err;
   }
 };
 
-int make_plan(dmd_denoiser* h, Plan* pl, int B, int H, int W, uint8_t* base, size_t* total) {
+int make_plan(const dmd_denoiser* h, Plan* pl, int B, int H, int W, uint8_t* base, size_t* total) {
   pl->B = B; pl->H = H; pl->W = W; pl->ops.clear();
   // pass 1: stats region size (tiny) — run the builder on null bases
   Bump b0{nullptr}, s0{nullptr};
-  { Plan tmp; tmp.B = B; tmp.H = H; tmp.W = W; PlanBuilder pb{h, &tmp, &b0, &s0}; if (pb.build()) return 1; }
+  { Plan tmp; tmp.B = B; tmp.H = H; tmp.W = W; PlanBuilder pb{&h->core, &tmp, &b0, &s0}; if (pb.build(h)) return 1; }
   const size_t stats_bytes = (s0.off + 255) & ~(size_t)255;
   if (total) *total = stats_bytes + b0.off + 256;
   if (!base) return 0;
   Bump sb{base}, bb{base + stats_bytes};
   pl->base = base; pl->stats = (double*)base; pl->stats_bytes = stats_bytes;
-  PlanBuilder pb{h, pl, &bb, &sb};
-  if (pb.build()) return 1;
+  PlanBuilder pb{&h->core, pl, &bb, &sb};
+  if (pb.build(h)) return 1;
   pl->bytes = stats_bytes + bb.off;
   return 0;
 }
@@ -1307,64 +1397,55 @@ int make_plan(dmd_denoiser* h, Plan* pl, int B, int H, int W, uint8_t* base, siz
 // loss scale; "first writer assigns, later writers accumulate" is decided here at plan time (ginit), so no gradient
 // buffer needs a memset.  Forward conv inputs (the PLC16 operands) are not kept: the forward prep launch is replayed.
 struct BwdBuilder {
-  dmd_denoiser* h; Plan* pl; Bump* bump; int err = 0;
+  const dmd_denoiser* h; Plan* pl; Bump* bump; int err = 0;
   std::vector<char> ginit;
 
-  const float* P(int idx) const { return h->ptrs.empty() ? nullptr : h->ptrs[idx]; }
+  const float* P(int idx) const { return h->core.P(idx); }
+  long long G(int idx) const { return h->core.goff[idx]; }
   bool was_init(const Tens& t) { const bool w = ginit[t.gid] != 0; ginit[t.gid] = 1; return w; }
   void push(const BOp& b) { pl->bops.push_back(b); }
 
   void replay(const Operand& o) { BOp b; b.kind = B_PREP; b.prep = pl->ops[o.op].prep; b.prep_nsrc = pl->ops[o.op].prep_nsrc; push(b); }
   // NHWC fp32 gradient [B][Hs][Ws][C] -> PLC16 operand (ups = 2: zero insertion, the adjoint of a stride-2 conv)
   void gprep(const float* g, int C, int Hs, int Ws, int ups, uint8_t* dst) {
-    dmd_prep_desc d; memset(&d, 0, sizeof(d));
-    d.src0 = g ? g : (const float*)1; d.C0 = C; d.B = pl->B; d.Hs = Hs; d.Ws = Ws; d.upsample = ups; d.dst0 = dst ? dst : (void*)1; d.eps = kGnEps;
+    const dmd_prep_desc d = prep_desc(g, C, pl->B, Hs, Ws, ups, 0, nullptr, nullptr, nullptr, dst);
     BOp b; b.kind = B_PREP;
     if (prep_fill(&d, &b.prep, &b.prep_nsrc)) { err = 1; return; }
     push(b);
   }
   void colsum(const float* g, long long rows, int C, int Creal, int idx, int idx2 = -1) {
-    BOp b; b.kind = B_COLSUM; b.src = g; b.rows = rows; b.C = C; b.Creal = Creal; b.goff = h->goff[idx]; b.goff2 = idx2 >= 0 ? h->goff[idx2] : -1;
+    BOp b; b.kind = B_COLSUM; b.src = g; b.rows = rows; b.C = C; b.Creal = Creal; b.goff = G(idx); b.goff2 = idx2 >= 0 ? G(idx2) : -1;
     push(b);
   }
-  // backward-data for source k of conv cw: out (+)= conv(gy, W_k^T flipped)
   void dgrad(const ConvW& cw, int k, const uint8_t* gy, int H, int W, float* out, bool accumulate) {
-    dmd_conv_desc d; memset(&d, 0, sizeof(d));
-    d.src0 = gy ? gy : (const void*)1; d.C0 = round_up(cw.Cout, 16); d.B = pl->B; d.H = H; d.W = W; d.taps = cw.taps; d.stride = 1;
-    d.wpk = h->packed ? h->packed + cw.pkT_off[k] : (const void*)1;
-    d.Cout = cw.srcC[k]; d.CoutPad = round_up(cw.srcC[k], 16);
-    d.out = out ? out : (float*)1; d.residual = accumulate ? d.out : nullptr;
+    const dmd_conv_desc d = dgrad_desc(cw, k, h->core.packed + cw.pkT_off[k], gy, pl->B, H, W, out, accumulate);
     BOp b; b.kind = B_CONV;
     if (conv_fill(&d, &b.conv, &b.smem, &b.cols)) { err = 1; return; }
     push(b);
   }
   void wgrad(const ConvW& cw, const uint8_t* gy, const uint8_t* act, int Ca, int Cin, int ci_off, int H, int W) {
-    BOp b; b.kind = B_WGRAD; b.goff = h->goff[cw.w_idx];
+    BOp b; b.kind = B_WGRAD; b.goff = G(cw.w_idx);
     if (wgrad_fill(gy ? gy : (const void*)1, round_up(cw.Cout, 16), act ? act : (const void*)1, Ca, pl->B, H, W, cw.taps,
                    pl->partial ? pl->partial : (float*)1, cw.Cout, Cin, cw.CinReal, ci_off, pl->scale ? pl->scale + 1 : (const float*)1, 1, 0, &b.wg)) { err = 1; return; }
     push(b);
   }
   void norm_bwd(const Tens& x, const float* gy, int mode, const FilmW* film, int c_off, int ctot, int gamma_idx, int beta_idx,
                 float* gx, const float* addend, bool accumulate) {
-    NormBwdParams nb; memset(&nb, 0, sizeof(nb));
-    nb.x = x.data; nb.gy = gy; nb.stats = x.stats; nb.B = pl->B; nb.HW = x.H * x.W; nb.C = x.C; nb.gs = x.gs; nb.mode = mode; nb.act = 1;
-    nb.eps = kGnEps; nb.c_off = c_off;
-    BOp b1; b1.kind = B_NORM1;
-    if (mode == 1) {
-      nb.film = pl->film; nb.film_stride = h->film_rows; nb.film_off = film->off; nb.film_ctot = ctot;
+    const int R = h->core.film_rows;
+    NormBwdParams nb = gn_bwd_params(x.data, gy, x.stats, pl->B, x.H * x.W, x.C, x.gs, P(gamma_idx), P(beta_idx), pl->nsum, gx, addend, accumulate);
+    if (mode == 1) {   // AdaGroupNorm: FiLM rows in place of gamma / beta, their gradients in place of the per-channel sums
+      nb.mode = 1; nb.gamma = nb.beta = nullptr; nb.c_off = c_off;
+      nb.film = pl->film; nb.film_stride = R; nb.film_off = film->off; nb.film_ctot = ctot;
       nb.sumB = pl->dfilm ? pl->dfilm + film->off + c_off : nullptr;            // d scale
       nb.sumA = pl->dfilm ? pl->dfilm + film->off + ctot + c_off : nullptr;     // d shift
-      nb.sum_stride = h->film_rows;
+      nb.sum_stride = R;
     } else {
-      nb.gamma = P(gamma_idx); nb.beta = P(beta_idx);
-      nb.sumA = pl->nsum; nb.sumB = pl->nsum ? pl->nsum + (size_t)pl->B * kMaxCin : nullptr; nb.sum_stride = kMaxCin;
       BOp m; m.kind = B_MEMSET; m.ms_ptr = pl->nsum; m.ms_bytes = (size_t)2 * pl->B * kMaxCin * 4; push(m);
     }
-    nb.gx = gx; nb.addend = addend; nb.accumulate = accumulate ? 1 : 0;
-    b1.nb = nb;
+    BOp b1; b1.kind = B_NORM1; b1.nb = nb;
     push(b1);
     if (mode == 2) {
-      BOp a; a.kind = B_AFFINE; a.nb = nb; a.goff = h->goff[gamma_idx]; a.goff2 = h->goff[beta_idx]; push(a);
+      BOp a; a.kind = B_AFFINE; a.nb = nb; a.goff = G(gamma_idx); a.goff2 = G(beta_idx); push(a);
     }
     BOp b2 = b1; b2.kind = B_NORM2; push(b2);
   }
@@ -1380,7 +1461,7 @@ struct BwdBuilder {
       b.ab = AttnBwdParams{o.data, o.stats, P(rb.an_w), P(rb.an_b), P(rb.qkv_w), P(rb.qkv_b), P(rb.op_w), r.a.grad, o.grad,
                            nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, pl->scale ? pl->scale + 1 : nullptr, H * W, rb.cout, o.gs, kGnEps};
       const int ids[6] = {rb.an_w, rb.an_b, rb.qkv_w, rb.qkv_b, rb.op_w, rb.op_b};
-      for (int i = 0; i < 6; ++i) b.goffs[i] = h->goff[ids[i]];
+      for (int i = 0; i < 6; ++i) b.goffs[i] = h->core.goff[ids[i]];
       push(b);
       ginit[o.gid] = 1;
     }
@@ -1444,7 +1525,6 @@ struct BwdBuilder {
         wgrad(cw, pl->gyA, r.in1.n0, round_up(r.x.C, 16), r.x.C, 0, H, W);
         dgrad(cw, 0, pl->gyA, H, W, pl->tA, false);
         BOp b; b.kind = B_POOL; b.src = pl->tA; b.dst = r.x.grad; b.H = r.x.H; b.W = r.x.W; b.C = r.x.C; b.acc = was_init(r.x) ? 1 : 0;
-        b.total4 = (long long)B * r.x.H * r.x.W * r.x.C / 4;
         push(b);
       } else if (r.kind == R_DOWN) {  // Downsample (blocks.py:93-100): stride-2 conv == stride-1 conv sampled at even pixels
         const ConvW& cw = *r.cw;
@@ -1466,14 +1546,14 @@ struct BwdBuilder {
     }
     // ---- conditioning path (inner_model.py:45; blocks.py:39): FiLM linears, cond_proj MLP, action embedding
     const dmd_denoiser_config& c = h->cfg;
-    const int CC = c.cond_channels, R = h->film_rows;
+    const int CC = c.cond_channels, R = h->core.film_rows;
     { BOp b; b.kind = B_FILMW; push(b); }
     auto sgemm = [&](const float* A, long long sam, long long sak, const float* Bm, long long sbk, long long sbn, float* C, long long c_goff,
                      long long ldc, int M, int N, int K, int use_inv, int acc) {
       BOp b; b.kind = B_SGEMM; b.ga = A; b.sam = sam; b.sak = sak; b.gb = Bm; b.sbk = sbk; b.sbn = sbn; b.gc = C; b.c_goff = c_goff; b.ldc = ldc;
       b.M = M; b.N = N; b.K = K; b.use_inv = use_inv; b.acc = acc; push(b);
     };
-    const float* Wf = h->packed ? (const float*)(h->packed + h->film_w_off) : nullptr;
+    const float* Wf = h->core.packed ? (const float*)(h->core.packed + h->core.film_w_off) : nullptr;
     sgemm(pl->dfilm, R, 1, Wf, CC, 1, pl->dcond, -1, CC, B, CC, R, 0, 0);                       // dcond = dfilm Wf
     {   // K = R (7168 rows for the default net) over a handful of 64 x 64 output tiles: split K across the SMs
       int cmax = 16;
@@ -1482,29 +1562,29 @@ struct BwdBuilder {
       int splits = R / 256; if (splits > 32) splits = 32; if (splits > fit) splits = (int)fit;
       if (splits > 1) pl->bops.back().chunks = splits;
     }
-    sgemm(pl->dcond, 1, CC, pl->chid, CC, 1, nullptr, h->goff[h->i_cp2w], CC, CC, CC, B, 1, 1);  // dW2 += dcond^T h
+    sgemm(pl->dcond, 1, CC, pl->chid, CC, 1, nullptr, h->core.goff[h->i_cp2w], CC, CC, CC, B, 1, 1);  // dW2 += dcond^T h
     colsum(pl->dcond, B, CC, CC, h->i_cp2b);
     sgemm(pl->dcond, CC, 1, P(h->i_cp2w), CC, 1, pl->dh, -1, CC, B, CC, CC, 0, 0);               // dh = dcond W2
     { BOp b; b.kind = B_LINEAR; b.lin_in = pl->cemb; b.lin_w = P(h->i_cp0w); b.lin_b = P(h->i_cp0b); b.lin_out = pl->cpre; b.lin_K = CC; b.lin_F = CC; push(b); }
     { BOp b; b.kind = B_DSILU; b.src = pl->cpre; b.ga = pl->dh; b.dst = pl->dpre; b.rows = (long long)B * CC; push(b); }
-    sgemm(pl->dpre, 1, CC, pl->cemb, CC, 1, nullptr, h->goff[h->i_cp0w], CC, CC, CC, B, 1, 1);   // dW0 += dpre^T e
+    sgemm(pl->dpre, 1, CC, pl->cemb, CC, 1, nullptr, h->core.goff[h->i_cp0w], CC, CC, CC, B, 1, 1);   // dW0 += dpre^T e
     colsum(pl->dpre, B, CC, CC, h->i_cp0b);
     sgemm(pl->dpre, CC, 1, P(h->i_cp0w), CC, 1, pl->de, -1, CC, B, CC, CC, 0, 0);                // de = dpre W0
-    { BOp b; b.kind = B_EMB; b.src = pl->de; b.goff = h->goff[h->i_actemb]; push(b); }
+    { BOp b; b.kind = B_EMB; b.src = pl->de; b.goff = h->core.goff[h->i_actemb]; push(b); }
     return err;
   }
 };
 
 // training workspace = forward plan (with gradient buffers) + backward temporaries
-int make_train_plan(dmd_denoiser* h, Plan* pl, int B, int H, int W, uint8_t* base, size_t* total) {
+int make_train_plan(const dmd_denoiser* h, Plan* pl, int B, int H, int W, uint8_t* base, size_t* total) {
   pl->train = true; pl->n_grad_tensors = 0; pl->tape.clear();
   pl->B = B; pl->H = H; pl->W = W; pl->ops.clear(); pl->bops.clear();
   Bump b0{nullptr}, s0{nullptr};
-  { Plan tmp; tmp.train = true; tmp.B = B; tmp.H = H; tmp.W = W; PlanBuilder pb{h, &tmp, &b0, &s0}; if (pb.build()) return 1; }
+  { Plan tmp; tmp.train = true; tmp.B = B; tmp.H = H; tmp.W = W; PlanBuilder pb{&h->core, &tmp, &b0, &s0}; if (pb.build(h)) return 1; }
   const size_t stats_bytes = (s0.off + 255) & ~(size_t)255;
   Bump sb{base}, bb{base ? base + stats_bytes : nullptr};
   if (base) { pl->base = base; pl->stats = (double*)base; pl->stats_bytes = stats_bytes; }
-  if (base) { PlanBuilder pb{h, pl, &bb, &sb}; if (pb.build()) return 1; } else bb.off = b0.off;
+  if (base) { PlanBuilder pb{&h->core, pl, &bb, &sb}; if (pb.build(h)) return 1; } else bb.off = b0.off;
   // backward temporaries
   const dmd_denoiser_config& c = h->cfg;
   int cmax = 16;
@@ -1519,11 +1599,11 @@ int make_train_plan(dmd_denoiser* h, Plan* pl, int B, int H, int W, uint8_t* bas
   const int CC = c.cond_channels;
   pl->dcond = (float*)bb.take((size_t)B * CC * 4); pl->dh = (float*)bb.take((size_t)B * CC * 4); pl->cpre = (float*)bb.take((size_t)B * CC * 4);
   pl->dpre = (float*)bb.take((size_t)B * CC * 4); pl->de = (float*)bb.take((size_t)B * CC * 4);
-  pl->film_woff = (long long*)bb.take((size_t)h->film_rows * 8); pl->film_boff = (long long*)bb.take((size_t)h->film_rows * 8);
+  pl->film_woff = (long long*)bb.take((size_t)h->core.film_rows * 8); pl->film_boff = (long long*)bb.take((size_t)h->core.film_rows * 8);
   pl->scale = (float*)bb.take(256);
   // zeroed at the start of every backward: dfilm, affine-norm sums, amax
   uint8_t* z0 = (uint8_t*)bb.take(0);
-  pl->dfilm = (float*)bb.take((size_t)B * h->film_rows * 4);
+  pl->dfilm = (float*)bb.take((size_t)B * h->core.film_rows * 4);
   pl->nsum = (float*)bb.take((size_t)2 * B * kMaxCin * 4);
   pl->amax = (unsigned int*)bb.take(256);
   pl->zero_begin = z0; pl->zero_bytes = base ? (size_t)((uint8_t*)pl->amax + 256 - z0) : 0;
@@ -1533,9 +1613,9 @@ int make_train_plan(dmd_denoiser* h, Plan* pl, int B, int H, int W, uint8_t* bas
   BwdBuilder bw{h, pl, &bb};
   if (bw.build()) return 1;
   // flat-gradient offsets of every FiLM row (weights) / element (biases)
-  pl->film_woff_h.assign(h->film_rows, 0); pl->film_boff_h.assign(h->film_rows, 0);
+  pl->film_woff_h.assign(h->core.film_rows, 0); pl->film_boff_h.assign(h->core.film_rows, 0);
   auto fill_film = [&](const FilmW& f) {
-    for (int r = 0; r < 2 * f.C; ++r) { pl->film_woff_h[f.off + r] = h->goff[f.w_idx] + (long long)r * CC; pl->film_boff_h[f.off + r] = h->goff[f.b_idx] + r; }
+    for (int r = 0; r < 2 * f.C; ++r) { pl->film_woff_h[f.off + r] = h->core.goff[f.w_idx] + (long long)r * CC; pl->film_boff_h[f.off + r] = h->core.goff[f.b_idx] + r; }
   };
   auto fill_rb = [&](const ResBlockW& r) { fill_film(r.n1); fill_film(r.n2); };
   for (auto& lv : h->d_blocks) for (auto& r : lv) fill_rb(r);
@@ -1556,17 +1636,17 @@ int run_forward(dmd_denoiser* h, Plan& pl, const float* noisy, const float* sigm
   DMD_LAUNCH_OK();
   const float* film = pl.film;
   if (cond_k >= 0) {
-    film = pl.film_all + (size_t)cond_k * pl.B * h->film_rows;
+    film = pl.film_all + (size_t)cond_k * pl.B * h->core.film_rows;
   } else {
     const int total = pl.B * c.cond_channels;
-    cond_embed_kernel<<<(total + 255) / 256, 256, 0, st>>>(pl.cs, nullptr, c.sigma_data, c.sigma_offset_noise, act, h->ptrs[h->i_fourier],
-                                                           h->ptrs[h->i_actemb], pl.cemb, pl.B, pl.B, c.cond_channels, c.num_steps_conditioning,
+    cond_embed_kernel<<<(total + 255) / 256, 256, 0, st>>>(pl.cs, nullptr, c.sigma_data, c.sigma_offset_noise, act, h->core.ptrs[h->i_fourier],
+                                                           h->core.ptrs[h->i_actemb], pl.cemb, pl.B, pl.B, c.cond_channels, c.num_steps_conditioning,
                                                            c.num_actions, sv);
     DMD_LAUNCH_OK();
-    if (linear_launch(pl.cemb, h->ptrs[h->i_cp0w], h->ptrs[h->i_cp0b], pl.chid, pl.B, c.cond_channels, c.cond_channels, 1, st)) return 1;
-    if (linear_launch(pl.chid, h->ptrs[h->i_cp2w], h->ptrs[h->i_cp2b], pl.cond, pl.B, c.cond_channels, c.cond_channels, 0, st)) return 1;
-    if (linear_launch(pl.cond, (const float*)(h->packed + h->film_w_off), (const float*)(h->packed + h->film_b_off), pl.film,
-                      pl.B, c.cond_channels, h->film_rows, 0, st)) return 1;
+    if (linear_launch(pl.cemb, h->core.ptrs[h->i_cp0w], h->core.ptrs[h->i_cp0b], pl.chid, pl.B, c.cond_channels, c.cond_channels, 1, st)) return 1;
+    if (linear_launch(pl.chid, h->core.ptrs[h->i_cp2w], h->core.ptrs[h->i_cp2b], pl.cond, pl.B, c.cond_channels, c.cond_channels, 0, st)) return 1;
+    if (linear_launch(pl.cond, (const float*)(h->core.packed + h->core.film_w_off), (const float*)(h->core.packed + h->core.film_b_off), pl.film,
+                      pl.B, c.cond_channels, h->core.film_rows, 0, st)) return 1;
   }
   for (const Op& op : pl.ops) {
     if (op.kind == OP_CONV) { if (conv_launch(op.conv, op.smem, op.cols, st)) return 1; }
@@ -1590,7 +1670,7 @@ int run_wrap(dmd_denoiser* h, Plan& pl, const float* x, float* model_out, float*
 }
 
 int ensure_plan(dmd_denoiser* h, int B, int H, int W, void* ws, size_t ws_bytes) {
-  DMD_CHECK(!h->ptrs.empty() && h->packed, "denoiser: call dmd_denoiser_set_weights first");
+  DMD_CHECK(h->core.ready(), "denoiser: call dmd_denoiser_set_weights first");
   Plan& pl = h->plan;
   if (pl.B == B && pl.H == H && pl.W == W && pl.base == (uint8_t*)ws) return 0;
   // size and validate on a scratch plan: the cached plan is replaced only after every check has passed, and is
@@ -1623,45 +1703,46 @@ extern "C" void dmd_denoiser_destroy(dmd_denoiser* h) {
   if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
   delete h;
 }
-extern "C" int dmd_denoiser_num_tensors(const dmd_denoiser* h) { return h->n_tensors; }
-extern "C" size_t dmd_denoiser_packed_bytes(const dmd_denoiser* h) { return h->packed_bytes; }
+extern "C" int dmd_denoiser_num_tensors(const dmd_denoiser* h) { return h->core.n_tensors; }
+extern "C" size_t dmd_denoiser_packed_bytes(const dmd_denoiser* h) { return h->core.packed_bytes; }
 
-static int pack_one(dmd_denoiser* h, const ConvW& c, cudaStream_t st) {
-  if (dmd_pack_conv_weight(h->ptrs[c.w_idx], h->packed + c.pk_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, c.trs ? 3 : c.precise, st)) return 1;
+static int pack_one(const ModelCore& m, const ConvW& c, cudaStream_t st) {
+  const float* w = m.ptrs[c.w_idx];
+  if (dmd_pack_conv_weight(w, m.packed + c.pk_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, c.trs ? 3 : c.precise, st)) return 1;
+  if (c.three_pass && dmd_pack_conv_weight(w, m.packed + c.pk_lo_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, 2, st)) return 1;
   for (int k = 0; k < c.nsrcT; ++k)  // backward-data packs (transposed, flipped), one per concat source
-    if (dmd_pack_conv_weight_dgrad(h->ptrs[c.w_idx], h->packed + c.pkT_off[k], c.Cout, c.CinReal, c.srcOff[k], c.srcC[k], c.taps, st)) return 1;
+    if (dmd_pack_conv_weight_dgrad(w, m.packed + c.pkT_off[k], c.Cout, c.CinReal, c.srcOff[k], c.srcC[k], c.taps, st)) return 1;
   return 0;
 }
-static int pack_rb(dmd_denoiser* h, const ResBlockW& r, cudaStream_t st) {
-  const int CC = h->cfg.cond_channels;
-  if (r.has_proj && pack_one(h, r.proj, st)) return 1;
-  if (pack_one(h, r.c1, st) || pack_one(h, r.c2, st)) return 1;
+static int pack_rb(const ModelCore& m, const ResBlockW& r, cudaStream_t st) {
+  const int CC = m.cond_channels;
+  if (r.has_proj && pack_one(m, r.proj, st)) return 1;
+  if (pack_one(m, r.c1, st) || pack_one(m, r.c2, st)) return 1;
   for (const FilmW* f : {&r.n1, &r.n2}) {
-    DMD_CUDA(cudaMemcpyAsync(h->packed + h->film_w_off + (size_t)f->off * CC * 4, h->ptrs[f->w_idx], (size_t)2 * f->C * CC * 4, cudaMemcpyDeviceToDevice, st));
-    DMD_CUDA(cudaMemcpyAsync(h->packed + h->film_b_off + (size_t)f->off * 4, h->ptrs[f->b_idx], (size_t)2 * f->C * 4, cudaMemcpyDeviceToDevice, st));
+    DMD_CUDA(cudaMemcpyAsync(m.packed + m.film_w_off + (size_t)f->off * CC * 4, m.ptrs[f->w_idx], (size_t)2 * f->C * CC * 4, cudaMemcpyDeviceToDevice, st));
+    DMD_CUDA(cudaMemcpyAsync(m.packed + m.film_b_off + (size_t)f->off * 4, m.ptrs[f->b_idx], (size_t)2 * f->C * 4, cudaMemcpyDeviceToDevice, st));
   }
   return 0;
 }
 
 extern "C" int dmd_denoiser_set_weights(dmd_denoiser* h, const float* const* ptrs_host, int n_ptrs, void* packed, void* stream) {
-  DMD_CHECK(h && ptrs_host && packed, "set_weights: null argument");
-  DMD_CHECK(n_ptrs == h->n_tensors, "set_weights: expected %d tensors (InnerModel.state_dict order), got %d", h->n_tensors, n_ptrs);
+  DMD_CHECK(h, "set_weights: null argument");
   cudaStream_t st = (cudaStream_t)stream;
-  const bool moved = h->packed != (uint8_t*)packed || h->ptrs.empty() || memcmp(h->ptrs.data(), ptrs_host, sizeof(float*) * n_ptrs) != 0;
-  h->ptrs.assign(ptrs_host, ptrs_host + n_ptrs);
-  h->packed = (uint8_t*)packed;
+  bool moved = false;
+  if (h->core.set_weights("InnerModel", ptrs_host, n_ptrs, packed, &moved)) return 1;
   if (moved) { h->plan.B = 0; h->tplans.clear(); for (auto& g : h->graphs) g.valid = false; }
-  if (pack_one(h, h->conv_in, st) || pack_one(h, h->conv_out, st)) return 1;
-  for (auto& lv : h->d_blocks) for (auto& r : lv) if (pack_rb(h, r, st)) return 1;
-  for (auto& lv : h->u_blocks) for (auto& r : lv) if (pack_rb(h, r, st)) return 1;
-  for (auto& r : h->mid) if (pack_rb(h, r, st)) return 1;
-  for (int i = 1; i < h->cfg.num_levels; ++i) if (pack_one(h, h->downs[i], st) || pack_one(h, h->ups[i], st)) return 1;
+  const ModelCore& m = h->core;
+  if (pack_one(m, h->conv_in, st) || pack_one(m, h->conv_out, st)) return 1;
+  for (auto& lv : h->d_blocks) for (auto& r : lv) if (pack_rb(m, r, st)) return 1;
+  for (auto& lv : h->u_blocks) for (auto& r : lv) if (pack_rb(m, r, st)) return 1;
+  for (auto& r : h->mid) if (pack_rb(m, r, st)) return 1;
+  for (int i = 1; i < h->cfg.num_levels; ++i) if (pack_one(m, h->downs[i], st) || pack_one(m, h->ups[i], st)) return 1;
   return 0;
 }
 
 extern "C" size_t dmd_denoiser_workspace_bytes(const dmd_denoiser* h, int B, int H, int W) {
   Plan tmp; size_t need = 0;
-  if (make_plan(const_cast<dmd_denoiser*>(h), &tmp, B, H, W, nullptr, &need)) return 0;
+  if (make_plan(h, &tmp, B, H, W, nullptr, &need)) return 0;
   return need;
 }
 
@@ -1696,7 +1777,7 @@ Plan* find_train_plan(dmd_denoiser* h, int B, int H, int W, void* ws) {
 }
 
 int ensure_train_plan(dmd_denoiser* h, int B, int H, int W, void* ws, size_t ws_bytes, cudaStream_t st, Plan** out) {
-  DMD_CHECK(!h->ptrs.empty() && h->packed, "denoiser: call dmd_denoiser_set_weights first");
+  DMD_CHECK(h->core.ready(), "denoiser: call dmd_denoiser_set_weights first");
   if ((*out = find_train_plan(h, B, H, W, ws)) != nullptr) return 0;
   size_t need = 0;
   { Plan tmp; if (make_train_plan(h, &tmp, B, H, W, nullptr, &need)) return 1; }
@@ -1719,7 +1800,7 @@ int run_backward(dmd_denoiser* h, Plan& pl, const float* grad_out, float* grads,
   const dmd_denoiser_config& c = h->cfg;
   const int B = pl.B, HW = pl.H * pl.W, CC = c.cond_channels;
   const float* inv = pl.scale + 1;
-  DMD_CUDA(cudaMemsetAsync(grads, 0, (size_t)h->grad_total * 4, st));
+  DMD_CUDA(cudaMemsetAsync(grads, 0, (size_t)h->core.grad_total * 4, st));
   DMD_CUDA(cudaMemsetAsync(pl.zero_begin, 0, pl.zero_bytes, st));
   // loss scale from the incoming gradient, then the scaled NHWC gradient of the model output
   const long long n_out = (long long)B * c.img_channels * HW;
@@ -1738,7 +1819,6 @@ int run_backward(dmd_denoiser* h, Plan& pl, const float* grad_out, float* grads,
       case B_NORM2: if (norm_bwd_launch(b.nb, 2, st)) return 1; break;
       case B_AFFINE: if (affine_param_grad_launch(b.nb, grads + b.goff, grads + b.goff2, inv, st)) return 1; break;
       case B_POOL: if (sumpool2_launch(b.src, b.dst, B, b.H, b.W, b.C, b.acc, st)) return 1; break;
-      case B_ADD: if (add_launch(b.src, b.dst, b.total4, b.acc, st)) return 1; break;
       case B_ATTN: {
         AttnBwdParams ab = b.ab;
         ab.dgamma = grads + b.goffs[0]; ab.dbeta = grads + b.goffs[1]; ab.dwqkv = grads + b.goffs[2]; ab.dbqkv = grads + b.goffs[3];
@@ -1752,7 +1832,7 @@ int run_backward(dmd_denoiser* h, Plan& pl, const float* grad_out, float* grads,
                          b.use_inv ? inv : nullptr, b.acc, b.chunks, pl.tA, st)) return 1;
         break;
       case B_FILMW:
-        if (film_wgrad_launch(pl.dfilm, pl.cond, grads, pl.film_woff, pl.film_boff, B, h->film_rows, CC, inv, st)) return 1;
+        if (film_wgrad_launch(pl.dfilm, pl.cond, grads, pl.film_woff, pl.film_boff, B, h->core.film_rows, CC, inv, st)) return 1;
         break;
       case B_LINEAR: if (linear_launch(b.lin_in, b.lin_w, b.lin_b, b.lin_out, B, b.lin_K, b.lin_F, 0, st)) return 1; break;
       case B_DSILU: if (dsilu_mul_launch(b.src, b.ga, b.dst, b.rows, st)) return 1; break;
@@ -1769,13 +1849,11 @@ int run_backward(dmd_denoiser* h, Plan& pl, const float* grad_out, float* grads,
 
 extern "C" size_t dmd_denoiser_train_workspace_bytes(const dmd_denoiser* h, int B, int H, int W) {
   Plan tmp; size_t need = 0;
-  if (make_train_plan(const_cast<dmd_denoiser*>(h), &tmp, B, H, W, nullptr, &need)) return 0;
+  if (make_train_plan(h, &tmp, B, H, W, nullptr, &need)) return 0;
   return need;
 }
 extern "C" long long dmd_denoiser_grad_layout(const dmd_denoiser* h, long long* offsets, long long* numels, int n) {
-  if (!h || n != h->n_tensors) { fail("grad_layout: expected %d entries", h ? h->n_tensors : 0); return -1; }
-  for (int i = 0; i < n; ++i) { if (offsets) offsets[i] = h->goff[i]; if (numels) numels[i] = h->numel[i]; }
-  return h->grad_total;
+  return grad_layout(h ? &h->core : nullptr, offsets, numels, n);
 }
 
 extern "C" int dmd_inner_model_forward_train(dmd_denoiser* h, int B, int H, int W, const float* noisy_rescaled, const float* c_noise,
@@ -1796,7 +1874,7 @@ extern "C" int dmd_denoiser_backward(dmd_denoiser* h, int B, int H, int W, const
   Plan* plp = find_train_plan(h, B, H, W, workspace);
   DMD_CHECK(plp && plp->train, "denoiser_backward: no matching dmd_inner_model_forward_train on this workspace (B=%d H=%d W=%d)", B, H, W);
   Plan& pl = *plp;
-  DMD_CHECK(grads_numel >= h->grad_total, "denoiser_backward: gradient buffer too small (%lld < %lld floats)", grads_numel, h->grad_total);
+  DMD_CHECK(grads_numel >= h->core.grad_total, "denoiser_backward: gradient buffer too small (%lld < %lld floats)", grads_numel, h->core.grad_total);
   DMD_CHECK(((uintptr_t)grads & 15) == 0, "denoiser_backward: gradient buffer must be 16-byte aligned");
   return run_backward(h, pl, grad_out, grads, (cudaStream_t)stream);
 }
@@ -1835,13 +1913,13 @@ int sampler_body(dmd_denoiser* h, const dmd_sampler_config* sc, const SamplerIO&
     write_sigmas_kernel<<<1, 32, 0, st>>>(pl.sig_all, sl, K);
     DMD_LAUNCH_OK();
     const int rows = K * pl.B, CC = c.cond_channels;
-    cond_embed_kernel<<<(rows * CC + 255) / 256, 256, 0, st>>>(nullptr, pl.sig_all, c.sigma_data, c.sigma_offset_noise, io.act, h->ptrs[h->i_fourier],
-                                                               h->ptrs[h->i_actemb], pl.cemb_all, rows, pl.B, CC, c.num_steps_conditioning, c.num_actions, io.sv);
+    cond_embed_kernel<<<(rows * CC + 255) / 256, 256, 0, st>>>(nullptr, pl.sig_all, c.sigma_data, c.sigma_offset_noise, io.act, h->core.ptrs[h->i_fourier],
+                                                               h->core.ptrs[h->i_actemb], pl.cemb_all, rows, pl.B, CC, c.num_steps_conditioning, c.num_actions, io.sv);
     DMD_LAUNCH_OK();
-    if (linear_launch(pl.cemb_all, h->ptrs[h->i_cp0w], h->ptrs[h->i_cp0b], pl.chid_all, rows, CC, CC, 1, st)) return 1;
-    if (linear_launch(pl.chid_all, h->ptrs[h->i_cp2w], h->ptrs[h->i_cp2b], pl.cond_all, rows, CC, CC, 0, st)) return 1;
-    if (linear_launch(pl.cond_all, (const float*)(h->packed + h->film_w_off), (const float*)(h->packed + h->film_b_off), pl.film_all,
-                      rows, CC, h->film_rows, 0, st)) return 1;
+    if (linear_launch(pl.cemb_all, h->core.ptrs[h->i_cp0w], h->core.ptrs[h->i_cp0b], pl.chid_all, rows, CC, CC, 1, st)) return 1;
+    if (linear_launch(pl.chid_all, h->core.ptrs[h->i_cp2w], h->core.ptrs[h->i_cp2b], pl.cond_all, rows, CC, CC, 0, st)) return 1;
+    if (linear_launch(pl.cond_all, (const float*)(h->core.packed + h->core.film_w_off), (const float*)(h->core.packed + h->core.film_b_off), pl.film_all,
+                      rows, CC, h->core.film_rows, 0, st)) return 1;
   }
   int k = 0;
   auto forward = [&](const float* x, float sigma_value) -> int {
@@ -1953,43 +2031,22 @@ extern "C" int dmd_sampler_sample(dmd_denoiser* h, const dmd_sampler_config* sc,
 }
 
 // ---------------------------------------------------------------------------------------------- actor-critic executor
+// Immediate mode: its workspaces are pooled per autograd node (one per imagined step), so a cached plan per workspace would
+// multiply host state for launches that take microseconds to describe.  Forward convs of the encoder run in split-fp16 (error
+// ~2^-22): MaxPool2d (actor_critic.py:109) turns a 2^-11 operand rounding into a different arg-max in a few windows, which
+// moves the encoder GRADIENTS by several per cent against the fp32 reference (measured: 2.6e-2 whole-gradient error with fp16
+// operands, 1.8e-4 with an exact forward).  The encoder is 0.12 GFLOP, so the 3x tensor work is noise.
 struct dmd_actor_critic {
   dmd_actor_critic_config cfg;
-  int n_tensors = 0;
+  ModelCore core;
   struct Level { int cin, cout, down; int gn_w, gn_b; ConvW conv; int has_skip; ConvW skip; };
   ConvW conv0;
   std::vector<Level> levels;
   int i_wih = 0, i_whh = 0, i_bih = 0, i_bhh = 0, i_cw = 0, i_cb = 0, i_aw = 0, i_ab = 0;
   int feat_c = 0, feat_hw = 0;
-  size_t packed_bytes = 0;
-  std::vector<const float*> ptrs;
-  uint8_t* packed = nullptr;
-  std::vector<long long> numel, goff;   // flat gradient layout (state_dict order), as for the denoiser
-  long long grad_total = 0;
 };
 
 namespace {
-
-// Forward convs of the actor-critic encoder run in split-fp16 (error ~2^-22): MaxPool2d (actor_critic.py:109) turns a 2^-11
-// operand rounding into a different arg-max in a few windows, which moves the encoder GRADIENTS by several per cent against
-// the fp32 reference (measured: 2.6e-2 whole-gradient error with fp16 operands, 1.8e-4 with an exact forward).  The encoder
-// is 0.12 GFLOP, so the 3x tensor work is noise.  K = 3 * Cin per tap when that fits in shared memory, else three launches.
-ConvW ac_conv(dmd_actor_critic* h, int& idx, size_t& pk, int cout, int cin_real, int taps, int c0_store, bool dgrad) {
-  ConvW c; c.w_idx = idx++; c.b_idx = idx++;
-  h->numel.push_back((long long)cout * cin_real * taps); h->numel.push_back(cout);
-  c.Cout = cout; c.CoutPad = round_up(cout, 16); c.CinReal = cin_real; c.taps = taps;
-  c.c0_real = cin_real; c.c0_store = c0_store; c.Cin = round_up(c0_store, 16);
-  const size_t w1 = (size_t)taps * c.Cin * c.CoutPad * 2;
-  c.precise = (3 * w1 <= 120 * 1024) ? 1 : 0;
-  c.three_pass = c.precise ? 0 : 1;
-  c.pk_off = pk; pk += w1 * (c.precise ? 3 : 1); pk = (pk + 255) & ~(size_t)255;
-  if (c.three_pass) { c.pk_lo_off = pk; pk += w1; pk = (pk + 255) & ~(size_t)255; }
-  if (dgrad) {
-    c.nsrcT = 1; c.srcC[0] = cin_real; c.srcOff[0] = 0; c.pkT_off[0] = pk;
-    pk += (size_t)taps * round_up(cout, 16) * round_up(cin_real, 16) * 2; pk = (pk + 255) & ~(size_t)255;
-  }
-  return c;
-}
 
 struct AcBuffers {
   float* x0; void* opnd; void* opnd_lo; std::vector<float*> r, y, pooled; std::vector<double*> st_in, st_y; float *gates, *hx, *cx; double* stats; size_t stats_bytes; size_t total;
@@ -2037,52 +2094,39 @@ extern "C" dmd_actor_critic* dmd_actor_critic_create(const dmd_actor_critic_conf
   if (init_kernels()) return nullptr;
   dmd_actor_critic* h = new dmd_actor_critic();
   h->cfg = *cfg;
-  int idx = 0; size_t pk = 0;
+  Walker w{&h->core};
   // registration order (actor_critic.py:41-47,101-110): encoder.encoder.{0: Conv3x3, k: SmallResBlock(f.0.norm, f.2, skip_projection),
   // MaxPool...}, lstm.{weight_ih, weight_hh, bias_ih, bias_hh}, critic_linear, actor_linear
-  h->conv0 = ac_conv(h, idx, pk, cfg->channels[0], cfg->img_channels, 9, round_up(cfg->img_channels, 16), false);
+  h->conv0 = w.conv(cfg->channels[0], cfg->img_channels, 9, cfg->img_channels, round_up(cfg->img_channels, 16), 0, true, false);
   int S = cfg->img_size;
   for (int i = 0; i < cfg->num_levels; ++i) {
     dmd_actor_critic::Level lv;
     lv.cin = cfg->channels[i > 0 ? i - 1 : 0]; lv.cout = cfg->channels[i]; lv.down = cfg->down[i] ? 1 : 0;
-    lv.gn_w = idx++; lv.gn_b = idx++;
-    h->numel.push_back(lv.cin); h->numel.push_back(lv.cin);
-    lv.conv = ac_conv(h, idx, pk, lv.cout, lv.cin, 9, lv.cin, true);
+    lv.gn_w = w.next(lv.cin); lv.gn_b = w.next(lv.cin);
+    lv.conv = w.conv(lv.cout, lv.cin, 9, lv.cin, lv.cin, 0, true);
     lv.has_skip = lv.cin != lv.cout;
-    if (lv.has_skip) lv.skip = ac_conv(h, idx, pk, lv.cout, lv.cin, 1, lv.cin, true);
+    if (lv.has_skip) lv.skip = w.conv(lv.cout, lv.cin, 1, lv.cin, lv.cin, 0, true);
     h->levels.push_back(lv);
     if (lv.down) S /= 2;
   }
   h->feat_c = cfg->channels[cfg->num_levels - 1]; h->feat_hw = S * S;
-  h->i_wih = idx++; h->i_whh = idx++; h->i_bih = idx++; h->i_bhh = idx++;
-  h->i_cw = idx++; h->i_cb = idx++; h->i_aw = idx++; h->i_ab = idx++;
-  {
-    const long long D = cfg->lstm_dim, K = (long long)h->feat_c * h->feat_hw;
-    for (long long n : {4 * D * K, 4 * D * D, 4 * D, 4 * D, D, 1ll, (long long)cfg->num_actions * D, (long long)cfg->num_actions}) h->numel.push_back(n);
-  }
-  h->n_tensors = idx; h->packed_bytes = pk + 256;
-  h->goff.assign(idx, 0);
-  for (int i = 0; i < idx; ++i) { h->goff[i] = h->grad_total; h->grad_total += (h->numel[i] + 3) & ~3ll; }
+  const long long D = cfg->lstm_dim, K = (long long)h->feat_c * h->feat_hw;
+  h->i_wih = w.next(4 * D * K); h->i_whh = w.next(4 * D * D); h->i_bih = w.next(4 * D); h->i_bhh = w.next(4 * D);
+  h->i_cw = w.next(D); h->i_cb = w.next(1); h->i_aw = w.next((long long)cfg->num_actions * D); h->i_ab = w.next(cfg->num_actions);
+  h->core.finish(w.pk);
   return h;
 }
 extern "C" void dmd_actor_critic_destroy(dmd_actor_critic* h) { delete h; }
-extern "C" int dmd_actor_critic_num_tensors(const dmd_actor_critic* h) { return h->n_tensors; }
-extern "C" size_t dmd_actor_critic_packed_bytes(const dmd_actor_critic* h) { return h->packed_bytes; }
+extern "C" int dmd_actor_critic_num_tensors(const dmd_actor_critic* h) { return h->core.n_tensors; }
+extern "C" size_t dmd_actor_critic_packed_bytes(const dmd_actor_critic* h) { return h->core.packed_bytes; }
 
 extern "C" int dmd_actor_critic_set_weights(dmd_actor_critic* h, const float* const* ptrs_host, int n_ptrs, void* packed, void* stream) {
-  DMD_CHECK(h && ptrs_host && packed, "ac set_weights: null argument");
-  DMD_CHECK(n_ptrs == h->n_tensors, "ac set_weights: expected %d tensors (ActorCritic.state_dict order), got %d", h->n_tensors, n_ptrs);
-  h->ptrs.assign(ptrs_host, ptrs_host + n_ptrs);
-  h->packed = (uint8_t*)packed;
-  auto pack = [&](const ConvW& c) {
-    if (dmd_pack_conv_weight(h->ptrs[c.w_idx], h->packed + c.pk_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, c.precise, stream)) return 1;
-    if (c.three_pass && dmd_pack_conv_weight(h->ptrs[c.w_idx], h->packed + c.pk_lo_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, 2, stream)) return 1;
-    for (int k = 0; k < c.nsrcT; ++k)
-      if (dmd_pack_conv_weight_dgrad(h->ptrs[c.w_idx], h->packed + c.pkT_off[k], c.Cout, c.CinReal, c.srcOff[k], c.srcC[k], c.taps, stream)) return 1;
-    return 0;
-  };
-  if (pack(h->conv0)) return 1;
-  for (auto& lv : h->levels) { if (pack(lv.conv)) return 1; if (lv.has_skip && pack(lv.skip)) return 1; }
+  DMD_CHECK(h, "set_weights: null argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  bool moved = false;   // nothing is cached between calls
+  if (h->core.set_weights("ActorCritic", ptrs_host, n_ptrs, packed, &moved)) return 1;
+  if (pack_one(h->core, h->conv0, st)) return 1;
+  for (auto& lv : h->levels) if (pack_one(h->core, lv.conv, st) || (lv.has_skip && pack_one(h->core, lv.skip, st))) return 1;
   return 0;
 }
 
@@ -2094,39 +2138,29 @@ extern "C" int dmd_actor_critic_forward(dmd_actor_critic* h, int B, const float*
                                         float* logits, float* val, float* hx_out, float* cx_out, void* workspace,
                                         size_t workspace_bytes, void* stream) {
   DMD_CHECK(h && obs && hx_in && cx_in && logits && val && hx_out && cx_out && workspace, "ac forward: null argument");
-  DMD_CHECK(!h->ptrs.empty() && h->packed, "ac forward: call dmd_actor_critic_set_weights first");
+  DMD_CHECK(h->core.ready(), "ac forward: call dmd_actor_critic_set_weights first");
   DMD_CHECK(((uintptr_t)workspace & 255) == 0, "ac forward: workspace must be 256-byte aligned");
   const dmd_actor_critic_config& c = h->cfg;
+  const ModelCore& m = h->core;
   cudaStream_t st = (cudaStream_t)stream;
   AcBuffers b; ac_layout(h, B, (uint8_t*)workspace, &b);
   DMD_CHECK(workspace_bytes >= b.total, "ac forward: workspace too small (%zu < %zu)", workspace_bytes, b.total);
   DMD_CUDA(cudaMemsetAsync(b.stats, 0, b.stats_bytes, st));
   int S = c.img_size;
   if (dmd_nchw_to_nhwc(obs, b.x0, B, c.img_channels, h->conv0.c0_store, S * S, st)) return 1;
-  uint8_t* opnd = (uint8_t*)b.opnd;
-  uint8_t* opnd_lo = (uint8_t*)b.opnd_lo;
-  auto run_conv = [&](const ConvW& cw, const float* src, int Csrc, int hw, int pro, int gamma_idx, int beta_idx, const double* st_in,
+  // every conv reads the hi + lo parts of one operand buffer, written by the prep just before it
+  auto run_conv = [&](const ConvW& cw, const float* src, int Csrc, int hw, int mode, int gamma_idx, int beta_idx, const double* st_in,
                       const float* resid, float* out, double* st_out) -> int {
-    dmd_prep_desc pd; memset(&pd, 0, sizeof(pd));
-    pd.src0 = src; pd.C0 = Csrc; pd.B = B; pd.Hs = hw; pd.Ws = hw; pd.mode = pro; pd.silu = pro ? 1 : 0;
-    pd.stats0 = st_in; pd.gs0 = pro ? gn_group_size(Csrc) : 0;
-    if (pro) { pd.gamma = h->ptrs[gamma_idx]; pd.beta = h->ptrs[beta_idx]; }
-    pd.eps = kGnEps; pd.dst0 = opnd; pd.dst_lo0 = opnd_lo;   // hi + lo parts: the forward is split-fp16 (see ac_conv)
-    PrepParams pp; int nsrc;
-    if (prep_fill(&pd, &pp, &nsrc) || prep_launch(pp, nsrc, st)) return 1;
-    // passes: one launch with K = 3*Cin, or (A_hi W_hi) then (A_lo W_hi) and (A_hi W_lo) accumulated in place through `residual`
-    const int npass = cw.three_pass ? 3 : 1;
-    for (int pass = 0; pass < npass; ++pass) {
-      dmd_conv_desc d; memset(&d, 0, sizeof(d));
-      d.src0 = (pass == 1) ? opnd_lo : opnd; d.C0 = round_up(Csrc, 16); d.B = B; d.H = hw; d.W = hw; d.taps = cw.taps; d.stride = 1;
-      if (cw.precise) { d.precise = 1; d.src0_lo = opnd_lo; }
-      d.wpk = h->packed + (pass == 2 ? cw.pk_lo_off : cw.pk_off); d.bias = pass == 0 ? h->ptrs[cw.b_idx] : nullptr;
-      d.Cout = cw.Cout; d.CoutPad = cw.CoutPad;
-      d.residual = pass == 0 ? resid : out; d.out = out;
-      d.out_stats = pass == npass - 1 ? st_out : nullptr; d.out_gs = gn_group_size(cw.Cout);
-      ConvParams p; size_t smem; int cols;
-      if (conv_fill(&d, &p, &smem, &cols)) return 1;
-      if (conv_launch(p, smem, cols, st)) return 1;
+    dmd_prep_desc pd = prep_desc(src, Csrc, B, hw, hw, 0, mode, st_in, m.P(gamma_idx), m.P(beta_idx), b.opnd, b.opnd_lo);
+    if (dmd_prep_act(&pd, st)) return 1;
+    dmd_conv_desc d; memset(&d, 0, sizeof(d));
+    d.src0 = b.opnd; d.src0_lo = b.opnd_lo; d.precise = cw.precise; d.C0 = round_up(Csrc, 16);
+    d.B = B; d.H = hw; d.W = hw; d.taps = cw.taps; d.stride = 1;
+    d.wpk = m.packed + cw.pk_off; d.bias = m.ptrs[cw.b_idx]; d.Cout = cw.Cout; d.CoutPad = cw.CoutPad;
+    d.residual = resid; d.out = out; d.out_stats = st_out; d.out_gs = gn_group_size(cw.Cout);
+    for (int pass = 0; pass < (cw.three_pass ? 3 : 1); ++pass) {
+      dmd_conv_desc dp = cw.three_pass ? conv_pass(d, pass, m.packed + cw.pk_lo_off) : d;
+      if (dmd_conv2d_fprop(&dp, st)) return 1;
     }
     return 0;
   };
@@ -2148,11 +2182,11 @@ extern "C" int dmd_actor_critic_forward(dmd_actor_critic* h, int B, const float*
   }
   const float* feat = b.pooled[h->levels.size()];
   const int K = h->feat_c * h->feat_hw, D = c.lstm_dim;
-  if (linear_launch(feat, h->ptrs[h->i_wih], h->ptrs[h->i_bih], b.gates, B, K, 4 * D, 0, st, 0, h->feat_hw)) return 1;
-  if (linear_launch(hx_in, h->ptrs[h->i_whh], h->ptrs[h->i_bhh], b.gates, B, D, 4 * D, 0, st, 1, 0)) return 1;
+  if (linear_launch(feat, m.ptrs[h->i_wih], m.ptrs[h->i_bih], b.gates, B, K, 4 * D, 0, st, 0, h->feat_hw)) return 1;
+  if (linear_launch(hx_in, m.ptrs[h->i_whh], m.ptrs[h->i_bhh], b.gates, B, D, 4 * D, 0, st, 1, 0)) return 1;
   if (lstm_gates_launch(b.gates, cx_in, hx_out, cx_out, B, D, st)) return 1;
-  if (linear_launch(hx_out, h->ptrs[h->i_aw], h->ptrs[h->i_ab], logits, B, D, c.num_actions, 0, st)) return 1;
-  if (linear_launch(hx_out, h->ptrs[h->i_cw], h->ptrs[h->i_cb], val, B, D, 1, 0, st)) return 1;
+  if (linear_launch(hx_out, m.ptrs[h->i_aw], m.ptrs[h->i_ab], logits, B, D, c.num_actions, 0, st)) return 1;
+  if (linear_launch(hx_out, m.ptrs[h->i_cw], m.ptrs[h->i_cb], val, B, D, 1, 0, st)) return 1;
   return 0;
 }
 
@@ -2190,9 +2224,7 @@ extern "C" size_t dmd_actor_critic_backward_scratch_bytes(const dmd_actor_critic
   AcScratch s; if (ac_scratch_layout(h, B, nullptr, &s)) return 0; return s.total;
 }
 extern "C" long long dmd_actor_critic_grad_layout(const dmd_actor_critic* h, long long* offsets, long long* numels, int n) {
-  if (!h || n != h->n_tensors) { fail("ac grad_layout: expected %d entries", h ? h->n_tensors : 0); return -1; }
-  for (int i = 0; i < n; ++i) { if (offsets) offsets[i] = h->goff[i]; if (numels) numels[i] = h->numel[i]; }
-  return h->grad_total;
+  return grad_layout(h ? &h->core : nullptr, offsets, numels, n);
 }
 
 static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, const float* cx_in, const float* hx_out,
@@ -2217,16 +2249,17 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
                             float* grads, long long grads_numel, int accumulate, float* g_hx_in, float* g_cx_in, void* workspace,
                             void* scratch, size_t scratch_bytes, void* stream) {
   DMD_CHECK(h && hx_in && cx_in && hx_out && grads && g_hx_in && g_cx_in && workspace && scratch, "ac backward: null argument");
-  DMD_CHECK(!h->ptrs.empty() && h->packed, "ac backward: call dmd_actor_critic_set_weights first");
-  DMD_CHECK(grads_numel >= h->grad_total && ((uintptr_t)grads & 15) == 0, "ac backward: bad gradient buffer");
+  DMD_CHECK(h->core.ready(), "ac backward: call dmd_actor_critic_set_weights first");
+  DMD_CHECK(grads_numel >= h->core.grad_total && ((uintptr_t)grads & 15) == 0, "ac backward: bad gradient buffer");
   DMD_CHECK(((uintptr_t)scratch & 255) == 0, "ac backward: scratch must be 256-byte aligned");
   const dmd_actor_critic_config& c = h->cfg;
+  const ModelCore& m = h->core;
   cudaStream_t st = (cudaStream_t)stream;
   AcBuffers b; ac_layout(h, B, (uint8_t*)workspace, &b);
   AcScratch sc; if (ac_scratch_layout(h, B, (uint8_t*)scratch, &sc)) return 1;
   DMD_CHECK(scratch_bytes >= sc.total, "ac backward: scratch too small (%zu < %zu)", scratch_bytes, sc.total);
   const int D = c.lstm_dim, A = c.num_actions, K = h->feat_c * h->feat_hw;
-  auto G = [&](int idx) { return grads + h->goff[idx]; };
+  auto G = [&](int idx) { return grads + m.goff[idx]; };
   auto sgemm = [&](const float* Am, long long sam, long long sak, const float* Bm, long long sbk, long long sbn, float* C, long long ldc,
                    int M, int N, int Kd, int acc) -> int {
     return sgemm_launch(Am, sam, sak, Bm, sbk, sbn, C, ldc, M, N, Kd, nullptr, acc, 0, nullptr, st);
@@ -2234,10 +2267,10 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
   auto colsum = [&](const float* x, long long rows, int C, int Creal, float* out, float* out2, const float* inv) -> int {
     return colsum_launch(x, out, out2, inv, rows, C, Creal, st);
   };
-  if (!accumulate) DMD_CUDA(cudaMemsetAsync(grads, 0, (size_t)h->grad_total * 4, st));
+  if (!accumulate) DMD_CUDA(cudaMemsetAsync(grads, 0, (size_t)m.grad_total * 4, st));
   DMD_CUDA(cudaMemsetAsync(sc.amax, 0, 256, st));
   // ---- heads (actor_critic.py:73)
-  if (heads_bwd_launch(g_hx, g_logits, g_val, hx_out, h->ptrs[h->i_aw], h->ptrs[h->i_cw], sc.g_h, G(h->i_ab), G(h->i_cw), G(h->i_cb), B, D, A, st)) return 1;
+  if (heads_bwd_launch(g_hx, g_logits, g_val, hx_out, m.ptrs[h->i_aw], m.ptrs[h->i_cw], sc.g_h, G(h->i_ab), G(h->i_cw), G(h->i_cb), B, D, A, st)) return 1;
   if (g_logits && sgemm(g_logits, 1, A, hx_out, D, 1, G(h->i_aw), D, A, D, B, 1)) return 1;   // dWa += g_logits^T h'
   // ---- LSTMCell (actor_critic.py:72)
   if (lstm_cell_bwd_launch(b.gates, cx_in, sc.g_h, g_cx, sc.dgates, g_cx_in, B, D, st)) return 1;
@@ -2246,8 +2279,8 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
   if (sgemm(sc.dgates, 1, 4 * D, sc.x_flat, K, 1, G(h->i_wih), K, 4 * D, K, B, 1)) return 1;  // dWih += dgates^T x
   if (sgemm(sc.dgates, 1, 4 * D, hx_in, D, 1, G(h->i_whh), D, 4 * D, D, B, 1)) return 1;      // dWhh += dgates^T hx
   if (colsum(sc.dgates, B, 4 * D, 4 * D, G(h->i_bih), G(h->i_bhh), nullptr)) return 1;
-  if (sgemm(sc.dgates, 4 * D, 1, h->ptrs[h->i_whh], D, 1, g_hx_in, D, B, D, 4 * D, 0)) return 1;   // g_hx = dgates Whh
-  if (sgemm(sc.dgates, 4 * D, 1, h->ptrs[h->i_wih], K, 1, sc.g_xflat, K, B, K, 4 * D, 0)) return 1;  // g_x = dgates Wih
+  if (sgemm(sc.dgates, 4 * D, 1, m.ptrs[h->i_whh], D, 1, g_hx_in, D, B, D, 4 * D, 0)) return 1;   // g_hx = dgates Whh
+  if (sgemm(sc.dgates, 4 * D, 1, m.ptrs[h->i_wih], K, 1, sc.g_xflat, K, B, K, 4 * D, 0)) return 1;  // g_x = dgates Wih
   // ---- encoder (actor_critic.py:101-113): the feature gradient enters the fp16 tensor-core path with a loss scale
   float* g_cur = sc.g_a;    // gradient of pooled[i+1]; g_a / g_b ping-pong down the encoder
   auto other = [&](float* p) { return p == sc.g_a ? sc.g_b : sc.g_a; };
@@ -2259,29 +2292,10 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
     DMD_LAUNCH_OK();
   }
   const float* inv = sc.scale + 1;
-  auto prep = [&](const float* src, int Csrc, int hw, int mode, int gamma_idx, int beta_idx, const double* stats, uint8_t* dst) -> int {
-    dmd_prep_desc pd; memset(&pd, 0, sizeof(pd));
-    pd.src0 = src; pd.C0 = Csrc; pd.B = B; pd.Hs = hw; pd.Ws = hw; pd.mode = mode; pd.silu = mode ? 1 : 0;
-    pd.stats0 = stats; pd.gs0 = mode ? gn_group_size(Csrc) : 0;
-    if (mode) { pd.gamma = h->ptrs[gamma_idx]; pd.beta = h->ptrs[beta_idx]; }
-    pd.eps = kGnEps; pd.dst0 = dst;
-    PrepParams pp; int nsrc;
-    if (prep_fill(&pd, &pp, &nsrc)) return 1;
-    return prep_launch(pp, nsrc, st);
-  };
   auto wgrad = [&](const ConvW& cw, const uint8_t* gy, const uint8_t* act, int Ca, int hw) -> int {
     WgradLaunch L;
     if (wgrad_fill(gy, round_up(cw.Cout, 16), act, Ca, B, hw, hw, cw.taps, sc.partial, cw.Cout, cw.CinReal, cw.CinReal, 0, inv, 1, 0, &L)) return 1;
     return wgrad_launch(L, G(cw.w_idx), st);
-  };
-  auto dgrad = [&](const ConvW& cw, const uint8_t* gy, int hw, float* out, bool accumulate) -> int {
-    dmd_conv_desc d; memset(&d, 0, sizeof(d));
-    d.src0 = gy; d.C0 = round_up(cw.Cout, 16); d.B = B; d.H = hw; d.W = hw; d.taps = cw.taps; d.stride = 1;
-    d.wpk = h->packed + cw.pkT_off[0]; d.Cout = cw.srcC[0]; d.CoutPad = round_up(cw.srcC[0], 16);
-    d.out = out; d.residual = accumulate ? out : nullptr;
-    ConvParams p; size_t smem; int cols;
-    if (conv_fill(&d, &p, &smem, &cols)) return 1;
-    return conv_launch(p, smem, cols, st);
   };
   // spatial size of every level's input
   std::vector<int> size_in(h->levels.size() + 1);
@@ -2298,36 +2312,35 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
     }
     const long long pix = (long long)B * S * S;
     // SmallResBlock (blocks.py:116-123): y = skip(x) + conv3x3(silu(GroupNorm(x)))
-    if (prep(gy, lv.cout, S, 0, 0, 0, nullptr, sc.gy_op)) return 1;
+    dmd_prep_desc pd = prep_desc(gy, lv.cout, B, S, S, 0, 0, nullptr, nullptr, nullptr, sc.gy_op);
+    if (dmd_prep_act(&pd, st)) return 1;
     if (colsum(gy, pix, lv.cout, lv.cout, G(lv.conv.b_idx), lv.has_skip ? G(lv.skip.b_idx) : nullptr, inv)) return 1;
-    if (prep(b.pooled[i], lv.cin, S, 2, lv.gn_w, lv.gn_b, b.st_in[i], sc.x_op)) return 1;
+    pd = prep_desc(b.pooled[i], lv.cin, B, S, S, 0, 2, b.st_in[i], m.P(lv.gn_w), m.P(lv.gn_b), sc.x_op);
+    if (dmd_prep_act(&pd, st)) return 1;
     if (wgrad(lv.conv, sc.gy_op, sc.x_op, round_up(lv.cin, 16), S)) return 1;
-    if (dgrad(lv.conv, sc.gy_op, S, sc.tA, false)) return 1;
-    {
-      NormBwdParams nb; memset(&nb, 0, sizeof(nb));
-      nb.x = b.pooled[i]; nb.gy = sc.tA; nb.stats = b.st_in[i]; nb.B = B; nb.HW = S * S; nb.C = lv.cin; nb.gs = gn_group_size(lv.cin);
-      nb.mode = 2; nb.act = 1; nb.gamma = h->ptrs[lv.gn_w]; nb.beta = h->ptrs[lv.gn_b]; nb.eps = kGnEps;
-      nb.sumA = sc.nsum; nb.sumB = sc.nsum + (size_t)B * kMaxCin; nb.sum_stride = kMaxCin;
-      nb.gx = gx; nb.addend = lv.has_skip ? nullptr : gy; nb.accumulate = 0;
-      DMD_CUDA(cudaMemsetAsync(sc.nsum, 0, (size_t)2 * B * kMaxCin * 4, st));
-      if (norm_bwd_launch(nb, 1, st) || affine_param_grad_launch(nb, G(lv.gn_w), G(lv.gn_b), inv, st) || norm_bwd_launch(nb, 2, st)) return 1;
-    }
+    dmd_conv_desc cd = dgrad_desc(lv.conv, 0, m.packed + lv.conv.pkT_off[0], sc.gy_op, B, S, S, sc.tA, false);
+    if (dmd_conv2d_fprop(&cd, st)) return 1;
+    const NormBwdParams nb = gn_bwd_params(b.pooled[i], sc.tA, b.st_in[i], B, S * S, lv.cin, gn_group_size(lv.cin), m.P(lv.gn_w),
+                                           m.P(lv.gn_b), sc.nsum, gx, lv.has_skip ? nullptr : gy, false);
+    DMD_CUDA(cudaMemsetAsync(sc.nsum, 0, (size_t)2 * B * kMaxCin * 4, st));
+    if (norm_bwd_launch(nb, 1, st) || affine_param_grad_launch(nb, G(lv.gn_w), G(lv.gn_b), inv, st) || norm_bwd_launch(nb, 2, st)) return 1;
     if (lv.has_skip) {  // 1x1 skip projection on the raw input
-      if (prep(b.pooled[i], lv.cin, S, 0, 0, 0, nullptr, sc.x_op)) return 1;
+      pd = prep_desc(b.pooled[i], lv.cin, B, S, S, 0, 0, nullptr, nullptr, nullptr, sc.x_op);
+      if (dmd_prep_act(&pd, st)) return 1;
       if (wgrad(lv.skip, sc.gy_op, sc.x_op, round_up(lv.cin, 16), S)) return 1;
-      if (dgrad(lv.skip, sc.gy_op, S, gx, true)) return 1;
+      cd = dgrad_desc(lv.skip, 0, m.packed + lv.skip.pkT_off[0], sc.gy_op, B, S, S, gx, true);
+      if (dmd_conv2d_fprop(&cd, st)) return 1;
     }
     g_cur = gx;
   }
   {  // conv0 (Conv3x3(img_channels -> channels[0])): weight / bias gradients only
     const int S = c.img_size;
-    if (prep(g_cur, h->conv0.Cout, S, 0, 0, 0, nullptr, sc.gy_op)) return 1;
+    dmd_prep_desc pd = prep_desc(g_cur, h->conv0.Cout, B, S, S, 0, 0, nullptr, nullptr, nullptr, sc.gy_op);
+    if (dmd_prep_act(&pd, st)) return 1;
     if (colsum(g_cur, (long long)B * S * S, h->conv0.Cout, h->conv0.Cout, G(h->conv0.b_idx), nullptr, inv)) return 1;
-    if (prep(b.x0, h->conv0.c0_store, S, 0, 0, 0, nullptr, sc.x_op)) return 1;
-    WgradLaunch L;
-    if (wgrad_fill(sc.gy_op, round_up(h->conv0.Cout, 16), sc.x_op, h->conv0.c0_store, B, S, S, 9, sc.partial, h->conv0.Cout, h->conv0.CinReal,
-                   h->conv0.CinReal, 0, inv, 1, 0, &L)) return 1;
-    if (wgrad_launch(L, G(h->conv0.w_idx), st)) return 1;
+    pd = prep_desc(b.x0, h->conv0.c0_store, B, S, S, 0, 0, nullptr, nullptr, nullptr, sc.x_op);
+    if (dmd_prep_act(&pd, st)) return 1;
+    if (wgrad(h->conv0, sc.gy_op, sc.x_op, h->conv0.c0_store, S)) return 1;
   }
   return 0;
 }
@@ -2349,20 +2362,8 @@ extern "C" int dmd_lambda_returns(const float* rew, const int64_t* end, const in
 // sampler and the policy (world_model_env.py:97), and over the burn-in frames of every fresh episode (:120-129).
 //   encoder (conv_in + ResBlocks at C = 32 conditioned on the action embedding + two attention ResBlocks) -> (b t) features
 //   -> single-layer LSTM over time -> Linear / SiLU / Linear head -> 3 reward logits + 2 termination logits.
-// Rows are processed TIME-MAJOR (row = k * b + n) so that every LSTM step reads b contiguous feature rows.
-struct dmd_rew_end {
-  dmd_rew_end_config cfg;
-  dmd_denoiser core;     // parameter pointers / packed weights / FiLM table / plan of the encoder (reuses the U-Net block executor)
-  ConvW conv_in;
-  std::vector<std::vector<ResBlockW>> blocks;
-  std::vector<ConvW> downs;
-  int i_actemb = 0, i_wih = 0, i_whh = 0, i_bih = 0, i_bhh = 0, i_h0w = 0, i_h0b = 0, i_h2w = 0;
-  int feat_c = 0, feat_hw = 0;
-  Tens feat;
-  int planB = 0; void* plan_ws = nullptr;
-  float *x_gates = nullptr, *y = nullptr, *hid = nullptr, *logits_tm = nullptr, *hc[2] = {nullptr, nullptr};
-};
-
+// Rows are processed TIME-MAJOR (row = k * b + n) so that every LSTM step reads b contiguous feature rows.  The handle
+// (struct dmd_rew_end, next to dmd_denoiser) keeps the encoder plan of the last (rows, workspace) it ran.
 namespace {
 
 __global__ void pack_rew_end_input_kernel(const float* __restrict__ obs, const float* __restrict__ next_obs, const int64_t* __restrict__ act,
@@ -2396,25 +2397,26 @@ __global__ void split_logits_kernel(const float* __restrict__ tm, float* __restr
   end[(size_t)i * 2] = s[3]; end[(size_t)i * 2 + 1] = s[4];
 }
 
-int rew_end_layout(dmd_rew_end* h, int B, int H, int W, uint8_t* base, size_t* total) {
-  dmd_denoiser* core = &h->core;
-  Plan& pl = core->plan;
-  pl.train = false; pl.B = B; pl.H = H; pl.W = W; pl.ops.clear();
+// the encoder plan for B rows on the workspace at base (a first pass on null bases sizes the statistics region), then the LSTM /
+// head buffers behind it.  base == nullptr: sizes only (*total)
+int rew_end_layout(const dmd_rew_end* h, int B, uint8_t* base, RewEndLayout* o, size_t* total) {
+  const int S = h->cfg.img_size;
+  Plan& pl = o->plan;
+  pl.train = false; pl.B = B; pl.H = S; pl.W = S; pl.ops.clear();
   Bump b0{nullptr}, s0{nullptr};
-  Tens feat;
-  { Plan tmp; tmp.B = B; tmp.H = H; tmp.W = W; PlanBuilder pb{core, &tmp, &b0, &s0}; if (pb.build_rew_end(h->blocks, h->downs, h->conv_in, &feat)) return 1; }
+  { Plan tmp; tmp.B = B; tmp.H = S; tmp.W = S; PlanBuilder pb{&h->core, &tmp, &b0, &s0}; if (pb.build_rew_end(h, &o->feat)) return 1; }
   const size_t stats_bytes = (s0.off + 255) & ~(size_t)255;
   Bump sb{base}, bb{base ? base + stats_bytes : nullptr};
   if (base) {
     pl.base = base; pl.stats = (double*)base; pl.stats_bytes = stats_bytes;
-    PlanBuilder pb{core, &pl, &bb, &sb};
-    if (pb.build_rew_end(h->blocks, h->downs, h->conv_in, &h->feat)) return 1;
+    PlanBuilder pb{&h->core, &pl, &bb, &sb};
+    if (pb.build_rew_end(h, &o->feat)) return 1;
   } else bb.off = b0.off;
   const int D = h->cfg.lstm_dim;
-  h->x_gates = (float*)bb.take((size_t)B * 4 * D * 4);
-  h->y = (float*)bb.take((size_t)B * D * 4); h->hid = (float*)bb.take((size_t)B * D * 4);
-  h->logits_tm = (float*)bb.take((size_t)B * 5 * 4);
-  h->hc[0] = (float*)bb.take((size_t)B * D * 4); h->hc[1] = (float*)bb.take((size_t)B * D * 4);
+  o->x_gates = (float*)bb.take((size_t)B * 4 * D * 4);
+  o->y = (float*)bb.take((size_t)B * D * 4); o->hid = (float*)bb.take((size_t)B * D * 4);
+  o->logits_tm = (float*)bb.take((size_t)B * 5 * 4);
+  o->hc[0] = (float*)bb.take((size_t)B * D * 4); o->hc[1] = (float*)bb.take((size_t)B * D * 4);
   if (total) *total = stats_bytes + bb.off + 512;
   return 0;
 }
@@ -2430,17 +2432,12 @@ extern "C" dmd_rew_end* dmd_rew_end_create(const dmd_rew_end_config* cfg) {
   if (init_kernels()) return nullptr;
   dmd_rew_end* h = new dmd_rew_end();
   h->cfg = *cfg;
-  dmd_denoiser* core = &h->core;
-  memset(&core->cfg, 0, sizeof(core->cfg));
-  core->cfg.img_channels = cfg->img_channels; core->cfg.num_steps_conditioning = 1; core->cfg.cond_channels = cfg->cond_channels;
-  core->cfg.num_levels = cfg->num_levels; core->cfg.num_actions = cfg->num_actions;
-  for (int i = 0; i < cfg->num_levels; ++i) { core->cfg.depths[i] = cfg->depths[i]; core->cfg.channels[i] = cfg->channels[i]; core->cfg.attn_depths[i] = cfg->attn_depths[i]; }
+  h->core.cond_channels = cfg->cond_channels;
   // registration order (rew_end_model.py:27-41, :93-125): encoder.{conv_in, blocks[0..L], downsamples[1..L-1]}, act_emb, lstm, head
-  Walker w{core};
-  core->numel.clear();
+  Walker w{&h->core};
   const int L = cfg->num_levels;
   const int cin_real = 2 * cfg->img_channels;
-  h->conv_in = w.conv(cfg->channels[0], cin_real, 9, cin_real, round_up(cin_real, 16), 0, 1, false);
+  h->conv_in = w.conv(cfg->channels[0], cin_real, 9, cin_real, round_up(cin_real, 16), 0, true, false);
   h->blocks.resize(L + 1);
   for (int i = 0; i < L; ++i) {
     const int c1 = cfg->channels[i > 0 ? i - 1 : 0], c2 = cfg->channels[i];
@@ -2455,11 +2452,7 @@ extern "C" dmd_rew_end* dmd_rew_end_create(const dmd_rew_end_config* cfg) {
   h->i_actemb = w.next((long long)cfg->num_actions * cfg->cond_channels);
   h->i_wih = w.next(4 * D * K); h->i_whh = w.next(4 * D * D); h->i_bih = w.next(4 * D); h->i_bhh = w.next(4 * D);
   h->i_h0w = w.next(D * D); h->i_h0b = w.next(D); h->i_h2w = w.next(5 * D);
-  core->n_tensors = w.idx;
-  size_t pk = w.pk;
-  core->film_w_off = pk; pk += (size_t)core->film_rows * cfg->cond_channels * 4; pk = (pk + 255) & ~(size_t)255;
-  core->film_b_off = pk; pk += (size_t)core->film_rows * 4; pk = (pk + 255) & ~(size_t)255;
-  core->packed_bytes = pk;
+  h->core.finish(w.pk);
   return h;
 }
 extern "C" void dmd_rew_end_destroy(dmd_rew_end* h) { delete h; }
@@ -2467,23 +2460,21 @@ extern "C" int dmd_rew_end_num_tensors(const dmd_rew_end* h) { return h->core.n_
 extern "C" size_t dmd_rew_end_packed_bytes(const dmd_rew_end* h) { return h->core.packed_bytes; }
 
 extern "C" int dmd_rew_end_set_weights(dmd_rew_end* h, const float* const* ptrs_host, int n_ptrs, void* packed, void* stream) {
-  DMD_CHECK(h && ptrs_host && packed, "rew_end set_weights: null argument");
-  dmd_denoiser* core = &h->core;
-  DMD_CHECK(n_ptrs == core->n_tensors, "rew_end set_weights: expected %d tensors (RewEndModel.state_dict order), got %d", core->n_tensors, n_ptrs);
+  DMD_CHECK(h, "set_weights: null argument");
   cudaStream_t st = (cudaStream_t)stream;
-  core->ptrs.assign(ptrs_host, ptrs_host + n_ptrs);
-  core->packed = (uint8_t*)packed;
-  h->planB = 0;
-  if (pack_one(core, h->conv_in, st)) return 1;
-  for (auto& lv : h->blocks) for (auto& r : lv) if (pack_rb(core, r, st)) return 1;
-  for (int i = 1; i < h->cfg.num_levels; ++i) if (pack_one(core, h->downs[i], st)) return 1;
+  bool moved = false;
+  if (h->core.set_weights("RewEndModel", ptrs_host, n_ptrs, packed, &moved)) return 1;
+  if (moved) h->lay.plan.B = 0;   // the plan bakes parameter and packed-weight addresses in
+  const ModelCore& m = h->core;
+  if (pack_one(m, h->conv_in, st)) return 1;
+  for (auto& lv : h->blocks) for (auto& r : lv) if (pack_rb(m, r, st)) return 1;
+  for (int i = 1; i < h->cfg.num_levels; ++i) if (pack_one(m, h->downs[i], st)) return 1;
   return 0;
 }
 
-extern "C" size_t dmd_rew_end_workspace_bytes(dmd_rew_end* h, int rows) {
-  size_t total = 0;
-  h->planB = 0;
-  if (rew_end_layout(h, rows, h->cfg.img_size, h->cfg.img_size, nullptr, &total)) return 0;
+extern "C" size_t dmd_rew_end_workspace_bytes(const dmd_rew_end* h, int rows) {
+  RewEndLayout tmp; size_t total = 0;
+  if (rew_end_layout(h, rows, nullptr, &tmp, &total)) return 0;
   return total;
 }
 
@@ -2493,27 +2484,27 @@ extern "C" int dmd_rew_end_predict(dmd_rew_end* h, int b, int t, const float* ob
                                    const float* hx_in, const float* cx_in, float* logits_rew, float* logits_end, float* hx_out,
                                    float* cx_out, void* workspace, size_t workspace_bytes, void* stream) {
   DMD_CHECK(h && obs && next_obs && act && logits_rew && logits_end && hx_out && cx_out && workspace, "rew_end predict: null argument");
-  dmd_denoiser* core = &h->core;
-  DMD_CHECK(!core->ptrs.empty() && core->packed, "rew_end predict: call dmd_rew_end_set_weights first");
+  const ModelCore& m = h->core;
+  DMD_CHECK(m.ready(), "rew_end predict: call dmd_rew_end_set_weights first");
   DMD_CHECK(((uintptr_t)workspace & 255) == 0, "rew_end predict: workspace must be 256-byte aligned");
   const dmd_rew_end_config& c = h->cfg;
   cudaStream_t st = (cudaStream_t)stream;
   const int rows = b * t, S = c.img_size, HW = S * S, D = c.lstm_dim, CC = c.cond_channels;
-  if (h->planB != rows || h->plan_ws != workspace) {
+  RewEndLayout& o = h->lay;
+  Plan& pl = o.plan;
+  if (pl.B != rows || pl.base != (uint8_t*)workspace) {
+    // size and validate on a scratch layout; the cached one is invalidated (never left half-written) if the real build fails
     size_t need = 0;
-    h->planB = 0;
-    if (rew_end_layout(h, rows, S, S, nullptr, &need)) return 1;
+    { RewEndLayout tmp; if (rew_end_layout(h, rows, nullptr, &tmp, &need)) return 1; }
     DMD_CHECK(workspace_bytes >= need, "rew_end predict: workspace too small (%zu < %zu)", workspace_bytes, need);
-    if (rew_end_layout(h, rows, S, S, (uint8_t*)workspace, nullptr)) return 1;
-    h->planB = rows; h->plan_ws = workspace;
+    if (rew_end_layout(h, rows, (uint8_t*)workspace, &o, nullptr)) { pl.B = 0; pl.base = nullptr; pl.ops.clear(); return 1; }
   }
-  Plan& pl = core->plan;
   DMD_CUDA(cudaMemsetAsync(pl.stats, 0, pl.stats_bytes, st));
-  pack_rew_end_input_kernel<<<dim3((HW + 255) / 256, rows), 256, 0, st>>>(obs, next_obs, act, core->ptrs[h->i_actemb], pl.xin, pl.cond, b, t,
+  pack_rew_end_input_kernel<<<dim3((HW + 255) / 256, rows), 256, 0, st>>>(obs, next_obs, act, m.ptrs[h->i_actemb], pl.xin, pl.cond, b, t,
                                                                           c.img_channels, pl.CP_in, HW, CC, c.num_actions);
   DMD_LAUNCH_OK();
-  if (linear_launch(pl.cond, (const float*)(core->packed + core->film_w_off), (const float*)(core->packed + core->film_b_off), pl.film,
-                    rows, CC, core->film_rows, 0, st)) return 1;
+  if (linear_launch(pl.cond, (const float*)(m.packed + m.film_w_off), (const float*)(m.packed + m.film_b_off), pl.film,
+                    rows, CC, m.film_rows, 0, st)) return 1;
   for (const Op& op : pl.ops) {
     if (op.kind == OP_CONV) { if (conv_launch(op.conv, op.smem, op.cols, st)) return 1; }
     else if (op.kind == OP_PREP) { if (prep_launch(op.prep, op.prep_nsrc, st)) return 1; }
@@ -2522,21 +2513,21 @@ extern "C" int dmd_rew_end_predict(dmd_rew_end* h, int b, int t, const float* ob
   // LSTM over time (torch.nn.LSTM, gate order i f g o), rows of step k are the contiguous block [k*b, (k+1)*b)
   const int K = h->feat_c * h->feat_hw;
   const float* hprev = hx_in; const float* cprev = cx_in;
-  if (!hx_in) { DMD_CUDA(cudaMemsetAsync(h->hc[0], 0, (size_t)b * D * 4, st)); hprev = h->hc[0]; }
-  if (!cx_in) { DMD_CUDA(cudaMemsetAsync(h->hc[1], 0, (size_t)b * D * 4, st)); cprev = h->hc[1]; }
+  if (!hx_in) { DMD_CUDA(cudaMemsetAsync(o.hc[0], 0, (size_t)b * D * 4, st)); hprev = o.hc[0]; }
+  if (!cx_in) { DMD_CUDA(cudaMemsetAsync(o.hc[1], 0, (size_t)b * D * 4, st)); cprev = o.hc[1]; }
   for (int k = 0; k < t; ++k) {
-    const float* xk = h->feat.data + (size_t)k * b * K;
-    if (linear_launch(xk, core->ptrs[h->i_wih], core->ptrs[h->i_bih], h->x_gates, b, K, 4 * D, 0, st, 0, h->feat_hw)) return 1;
-    if (linear_launch(hprev, core->ptrs[h->i_whh], core->ptrs[h->i_bhh], h->x_gates, b, D, 4 * D, 0, st, 1, 0)) return 1;
-    float* hk = h->y + (size_t)k * b * D;   // y rows of step k (time-major); also the next step's h
-    if (lstm_gates_launch(h->x_gates, cprev, hk, cx_out, b, D, st)) return 1;
+    const float* xk = o.feat.data + (size_t)k * b * K;
+    if (linear_launch(xk, m.ptrs[h->i_wih], m.ptrs[h->i_bih], o.x_gates, b, K, 4 * D, 0, st, 0, h->feat_hw)) return 1;
+    if (linear_launch(hprev, m.ptrs[h->i_whh], m.ptrs[h->i_bhh], o.x_gates, b, D, 4 * D, 0, st, 1, 0)) return 1;
+    float* hk = o.y + (size_t)k * b * D;   // y rows of step k (time-major); also the next step's h
+    if (lstm_gates_launch(o.x_gates, cprev, hk, cx_out, b, D, st)) return 1;
     hprev = hk; cprev = cx_out;
   }
   DMD_CUDA(cudaMemcpyAsync(hx_out, hprev, (size_t)b * D * 4, cudaMemcpyDeviceToDevice, st));
   // head: Linear(D, D) + SiLU + Linear(D, 5, bias=False) over all (t b) rows
-  if (linear_launch(h->y, core->ptrs[h->i_h0w], core->ptrs[h->i_h0b], h->hid, rows, D, D, 1, st)) return 1;
-  if (linear_launch(h->hid, core->ptrs[h->i_h2w], nullptr, h->logits_tm, rows, D, 5, 0, st)) return 1;
-  split_logits_kernel<<<(rows + 127) / 128, 128, 0, st>>>(h->logits_tm, logits_rew, logits_end, b, t);
+  if (linear_launch(o.y, m.ptrs[h->i_h0w], m.ptrs[h->i_h0b], o.hid, rows, D, D, 1, st)) return 1;
+  if (linear_launch(o.hid, m.ptrs[h->i_h2w], nullptr, o.logits_tm, rows, D, 5, 0, st)) return 1;
+  split_logits_kernel<<<(rows + 127) / 128, 128, 0, st>>>(o.logits_tm, logits_rew, logits_end, b, t);
   DMD_LAUNCH_OK();
   return 0;
 }

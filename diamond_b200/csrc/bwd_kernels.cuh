@@ -269,15 +269,6 @@ __global__ void sumpool2_kernel(const float* __restrict__ in, float* __restrict_
   if (accumulate) { const float4 v = *dst; o.x += v.x; o.y += v.y; o.z += v.z; o.w += v.w; }
   *dst = o;
 }
-// out (+)= a    (identity residual path of a ResBlock / SmallResBlock, blocks.py:123,145)
-__global__ void add_kernel(const float* __restrict__ a, float* __restrict__ out, int accumulate, long long total4) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total4) return;
-  float4 v = __ldg(reinterpret_cast<const float4*>(a) + i);
-  float4* d = reinterpret_cast<float4*>(out) + i;
-  if (accumulate) { const float4 o = *d; v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w; }
-  *d = v;
-}
 // dpre = dh * silu'(pre)   (cond_proj SiLU, inner_model.py:33)
 __global__ void dsilu_mul_kernel(const float* __restrict__ pre, const float* __restrict__ dh, float* __restrict__ out, long long n) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;

@@ -1,5 +1,4 @@
 """ActorCritic (reference: src/models/actor_critic.py) with a native sm_90a forward for predict_act_value."""
-import ctypes as C
 import math
 from collections import namedtuple
 from dataclasses import dataclass
@@ -51,6 +50,9 @@ class ActorCriticEncoder(_NativeOnly):  # actor_critic.py:101-113 (parameter con
 
 
 class ActorCritic(NativeStateMixin, nn.Module):
+    _NATIVE_PREFIX = "dmd_actor_critic_"
+    _WS_POOL_CAP = 64   # one workspace per live autograd node of the imagined rollout (15 steps + burn-in calls)
+
     def __init__(self, cfg: ActorCriticConfig) -> None:
         super().__init__()
         self.cfg = cfg
@@ -69,18 +71,6 @@ class ActorCritic(NativeStateMixin, nn.Module):
         # True: the nodes of a backward pass accumulate their parameter gradients natively and `.grad` is set when the pass ends
         # (what `loss.backward()` needs).  False: every node returns its gradients to autograd (needed for torch.autograd.grad).
         self.accumulate_native_grads = True
-        self._h = None
-        self._h_dev = None
-        self._wkey = None
-        self._packed = None
-        self._ws = None
-
-    def __del__(self):
-        try:
-            if self._h is not None:
-                _lib.lib().dmd_actor_critic_destroy(self._h)
-        except Exception:
-            pass
 
     @property
     def device(self) -> torch.device:  # actor_critic.py:59-61
@@ -92,56 +82,14 @@ class ActorCritic(NativeStateMixin, nn.Module):
         self.loss_cfg = loss_cfg
 
     # ------------------------------------------------------------------ native plumbing
-    def _native(self):
-        lib = _lib.lib()
-        dev = self.device
-        if dev.type != "cuda":
-            raise RuntimeError("diamond_b200 runs on CUDA (sm_90a) only; move the model to a cuda device")
-        self.require_current_device(dev)
-        if self._h is None:
-            c = self.cfg
-            cc = _lib.ActorCriticConfigC()
-            cc.lstm_dim, cc.img_channels, cc.img_size, cc.num_levels = c.lstm_dim, c.img_channels, c.img_size, len(c.channels)
-            for i in range(len(c.channels)):
-                cc.channels[i], cc.down[i] = int(c.channels[i]), int(bool(c.down[i]))
-            cc.num_actions = int(c.num_actions)
-            h = lib.dmd_actor_critic_create(C.byref(cc))
-            if not h:
-                raise RuntimeError("diamond_b200: " + lib.dmd_last_error().decode())
-            self._h = h
-        tensors = self._state_tensors()
-        wkey = tuple((t.data_ptr(), t._version) for t in tensors)
-        if wkey != self._wkey:
-            n = lib.dmd_actor_critic_num_tensors(self._h)
-            if n != len(tensors):
-                raise RuntimeError(f"native actor-critic expects {n} tensors, module has {len(tensors)}")
-            if self._packed is None:
-                self._packed = torch.empty(lib.dmd_actor_critic_packed_bytes(self._h), dtype=torch.uint8, device=dev)
-            arr = (C.c_void_p * n)(*[t.data_ptr() for t in tensors])
-            _lib.check(lib.dmd_actor_critic_set_weights(self._h, arr, n, self._packed.data_ptr(), _lib.current_stream()))
-            self._wkey = wkey
-        return self._h
-
-    def grad_layout(self):
-        lib = _lib.lib()
-        h = self._native()
-        n = lib.dmd_actor_critic_num_tensors(h)
-        offs, nums = (C.c_longlong * n)(), (C.c_longlong * n)()
-        total = lib.dmd_actor_critic_grad_layout(h, offs, nums, n)
-        if total < 0:
-            raise RuntimeError("diamond_b200: " + lib.dmd_last_error().decode())
-        return list(offs), list(nums), int(total)
-
-    def _grad_views_layout(self):
-        """(offsets, numels) of every PARAMETER (in `parameters()` order) inside the flat gradient buffer, and its length.
-        Static for a module, so it is computed once (walking state_dict() costs ~0.2 ms, and there are ~60 backward nodes per update)."""
-        cached = self.__dict__.get("_gv_layout")
-        if cached is None:
-            offs, nums, total = self.grad_layout()
-            index = {k: i for i, k in enumerate(self.state_dict().keys())}
-            names = [k for k, _ in self.named_parameters()]
-            cached = self.__dict__["_gv_layout"] = ([offs[index[k]] for k in names], [nums[index[k]] for k in names], total)
-        return cached
+    def _native_config(self):
+        c = self.cfg
+        cc = _lib.ActorCriticConfigC()
+        cc.lstm_dim, cc.img_channels, cc.img_size, cc.num_levels = c.lstm_dim, c.img_channels, c.img_size, len(c.channels)
+        for i in range(len(c.channels)):
+            cc.channels[i], cc.down[i] = int(c.channels[i]), int(bool(c.down[i]))
+        cc.num_actions = int(c.num_actions)
+        return cc
 
     def _adopt_accumulated_grads(self) -> None:
         """End of a backward pass (autograd engine callback): the flat buffer the BPTT nodes accumulated into becomes `.grad`
@@ -159,18 +107,6 @@ class ActorCritic(NativeStateMixin, nn.Module):
             else:
                 p.grad.add_(g)
         self.last_flat_grad = flat
-
-    def _acquire_ws(self, nbytes: int, dev) -> Tensor:
-        pool = self.__dict__.setdefault("_ws_pool", [])
-        for i, ws in enumerate(pool):
-            if ws.numel() >= nbytes and ws.device == dev:
-                return pool.pop(i)
-        return torch.empty(nbytes, dtype=torch.uint8, device=dev)
-
-    def _release_ws(self, ws: Tensor) -> None:
-        pool = self.__dict__.setdefault("_ws_pool", [])
-        if len(pool) < 64:   # one workspace per live autograd node of the imagined rollout (15 steps + burn-in calls)
-            pool.append(ws)
 
     def _native_forward(self, obs: Tensor, hx: Tensor, cx: Tensor, ws: Tensor):
         lib = _lib.lib()
@@ -257,7 +193,7 @@ class _PredictActValueFn(torch.autograd.Function):
     def forward(ctx, module, obs, hx, cx, *params):
         lib = _lib.lib()
         h = module._native()
-        ws = module._acquire_ws(lib.dmd_actor_critic_workspace_bytes(h, obs.size(0)), obs.device)
+        ws = module._acquire_ws(lib.dmd_actor_critic_workspace_bytes(h, obs.size(0)))
         logits, val, hx_o, cx_o = module._native_forward(obs, hx.detach(), cx.detach(), ws)
         ctx.module, ctx.ws, ctx.b = module, ws, obs.size(0)
         ctx.save_for_backward(hx.detach(), cx.detach(), hx_o)
@@ -295,10 +231,10 @@ class _PredictActValueFn(torch.autograd.Function):
                 torch.autograd.Variable._execution_engine.queue_callback(module._adopt_accumulated_grads)
             else:
                 _lib.check(lib.dmd_actor_critic_backward_accumulate(*args, flat.data_ptr(), total, *tail))
-            module._release_ws(ctx.ws)
+            module._release_ws(ctx.ws, module._WS_POOL_CAP)
             return (None, None, g_hx_in, g_cx_in, *([None] * len(offs)))
         flat = torch.empty(total, dtype=torch.float32, device=dev)
         _lib.check(lib.dmd_actor_critic_backward(*args, flat.data_ptr(), total, *tail))
-        module._release_ws(ctx.ws)
+        module._release_ws(ctx.ws, module._WS_POOL_CAP)
         grads = [flat[o:o + n].view_as(p) for (o, n), p in zip(zip(offs, nums), module.parameters())]
         return (None, None, g_hx_in, g_cx_in, *grads)

@@ -5,7 +5,6 @@ over the burn-in frames of every fresh episode (:120-129).  Parameters live unde
 `Agent.load`, `configure_opt`'s isinstance split keep working); the arithmetic — encoder ResBlocks at C = 32 with FiLM on
 the action embedding, two attention blocks, LSTM over time, SiLU head — runs in `dmd_rew_end_predict`.
 Training of this model (`forward`, rew_end_model.py:57-90) is the next row (f2) and is not built."""
-import ctypes as C
 from dataclasses import dataclass
 from typing import List, Optional, Tuple
 
@@ -45,6 +44,8 @@ class RewEndEncoder(_NativeOnly):  # rew_end_model.py:93-125 (parameter containe
 
 
 class RewEndModel(NativeStateMixin, nn.Module):
+    _NATIVE_PREFIX = "dmd_rew_end_"
+
     def __init__(self, cfg: RewEndModelConfig) -> None:  # rew_end_model.py:27-41 (same registration order)
         super().__init__()
         self.cfg = cfg
@@ -54,57 +55,19 @@ class RewEndModel(NativeStateMixin, nn.Module):
         self.lstm = nn.LSTM(input_dim_lstm, cfg.lstm_dim, batch_first=True)
         self.head = nn.Sequential(nn.Linear(cfg.lstm_dim, cfg.lstm_dim), nn.SiLU(), nn.Linear(cfg.lstm_dim, 3 + 2, bias=False))
         init_lstm(self.lstm)
-        self._h = None
-        self._h_dev = None
-        self._wkey = None
-        self._packed = None
-        self._ws = None
-
-    def __del__(self):
-        try:
-            if self._h is not None:
-                _lib.lib().dmd_rew_end_destroy(self._h)
-        except Exception:
-            pass
 
     @property
     def device(self) -> torch.device:
         return self.act_emb.weight.device
 
-    def _native(self):
-        lib = _lib.lib()
-        dev = self.device
-        if dev.type != "cuda":
-            raise RuntimeError("diamond_b200 runs on CUDA (sm_90a) only; move the model to a cuda device")
-        self.require_current_device(dev)
-        if self._h is None or self._h_dev != dev.index:
-            if self._h is not None:
-                lib.dmd_rew_end_destroy(self._h)
-            c = self.cfg
-            cc = _lib.RewEndConfigC()
-            cc.lstm_dim, cc.img_channels, cc.img_size, cc.cond_channels, cc.num_levels = c.lstm_dim, c.img_channels, c.img_size, c.cond_channels, len(c.channels)
-            for i in range(len(c.channels)):
-                cc.depths[i], cc.channels[i], cc.attn_depths[i] = int(c.depths[i]), int(c.channels[i]), int(bool(c.attn_depths[i]))
-            cc.num_actions = int(c.num_actions)
-            h = lib.dmd_rew_end_create(C.byref(cc))
-            if not h:
-                raise RuntimeError("diamond_b200: " + lib.dmd_last_error().decode())
-            self._h, self._h_dev, self._wkey, self._packed, self._ws = h, dev.index, None, None, None
-        tensors = self._state_tensors()
-        wkey = tuple((t.data_ptr(), t._version) for t in tensors)
-        if wkey != self._wkey:
-            n = lib.dmd_rew_end_num_tensors(self._h)
-            if n != len(tensors):
-                raise RuntimeError(f"native rew_end model expects {n} tensors, module has {len(tensors)}")
-            for t in tensors:
-                if t.dtype != torch.float32 or not t.is_contiguous():
-                    raise RuntimeError("parameters must be contiguous fp32")
-            if self._packed is None:
-                self._packed = torch.empty(lib.dmd_rew_end_packed_bytes(self._h), dtype=torch.uint8, device=dev)
-            arr = (C.c_void_p * n)(*[t.data_ptr() for t in tensors])
-            _lib.check(lib.dmd_rew_end_set_weights(self._h, arr, n, self._packed.data_ptr(), _lib.current_stream()))
-            self._wkey = wkey
-        return self._h
+    def _native_config(self):
+        c = self.cfg
+        cc = _lib.RewEndConfigC()
+        cc.lstm_dim, cc.img_channels, cc.img_size, cc.cond_channels, cc.num_levels = c.lstm_dim, c.img_channels, c.img_size, c.cond_channels, len(c.channels)
+        for i in range(len(c.channels)):
+            cc.depths[i], cc.channels[i], cc.attn_depths[i] = int(c.depths[i]), int(c.channels[i]), int(bool(c.attn_depths[i]))
+        cc.num_actions = int(c.num_actions)
+        return cc
 
     @torch.no_grad()
     def predict_rew_end(self, obs: Tensor, act: Tensor, next_obs: Tensor,

@@ -336,12 +336,6 @@ def sumpool2(inp: Tensor, out: Tensor, accumulate: bool = False) -> Tensor:
     return out
 
 
-def add(a: Tensor, out: Tensor, accumulate: bool = True) -> Tensor:
-    _cuda(a, out)
-    _lib.check(_lib.lib().dmd_add(a.data_ptr(), out.data_ptr(), out.numel(), int(accumulate), _lib.current_stream()))
-    return out
-
-
 def dsilu_mul(pre: Tensor, dh: Tensor) -> Tensor:
     _cuda(pre, dh)
     out = torch.empty_like(pre)

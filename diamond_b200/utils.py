@@ -1,8 +1,12 @@
 """The two helpers of the reference's src/utils.py that the mirrored models need (init_lstm utils.py:184-196)."""
+import ctypes as C
 from typing import Any, Dict, Tuple
 
+import torch
 import torch.nn as nn
 from torch import Tensor
+
+from . import _lib
 
 LossAndLogs = Tuple[Tensor, Dict[str, Any]]
 
@@ -26,7 +30,93 @@ class NativeStateMixin:
     packed fp16 copies.  Walking state_dict() for that costs ~0.4 ms per call on the 235 tensors of the denoiser; the tensor
     list is therefore cached and dropped whenever `_apply` (to / cuda / float ...) may have replaced tensors.  In-place updates
     (optimizer steps, load_state_dict, p.data.copy_) keep the objects and bump `_version`, which the key sees; code that REPLACES
-    a Parameter object or writes through `.data.fill_` must call `refresh_weights()`."""
+    a Parameter object or writes through `.data.fill_` must call `refresh_weights()`.
+
+    A subclass names its C entry points by `_NATIVE_PREFIX` (`dmd_denoiser_`, ...) and provides `_native_config(*params)`
+    (the create-time config struct) and the `device` its parameters live on."""
+
+    _NATIVE_PREFIX = ""
+    _h = _h_key = _wkey = _packed = _ws = None
+
+    def __del__(self):
+        try:
+            if self._h is not None:
+                getattr(_lib.lib(), self._NATIVE_PREFIX + "destroy")(self._h)
+        except Exception:
+            pass
+
+    def _native_handle(self, *params):
+        """The native handle with up-to-date weights: (re)created when the device or the create-time `params` change,
+        re-packed when any parameter changed."""
+        lib, pre = _lib.lib(), self._NATIVE_PREFIX
+        dev = self.device
+        if dev.type != "cuda":
+            raise RuntimeError("diamond_b200 runs on CUDA (sm_90a) only; move the model to a cuda device")
+        self.require_current_device(dev)
+        key = (dev.index,) + params
+        if self._h is None or self._h_key != key:
+            if self._h is not None:
+                getattr(lib, pre + "destroy")(self._h)
+                self._h = None
+            h = getattr(lib, pre + "create")(C.byref(self._native_config(*params)))
+            if not h:
+                raise RuntimeError("diamond_b200: " + lib.dmd_last_error().decode())
+            self._h, self._h_key, self._wkey, self._packed = h, key, None, None
+        tensors = self._state_tensors()
+        wkey = tuple((t.data_ptr(), t._version) for t in tensors)
+        if wkey != self._wkey:
+            n = getattr(lib, pre + "num_tensors")(self._h)
+            if n != len(tensors):
+                raise RuntimeError(f"native {type(self).__name__} expects {n} tensors, module has {len(tensors)}")
+            for t in tensors:
+                if t.dtype != torch.float32 or not t.is_contiguous():
+                    raise RuntimeError("parameters must be contiguous fp32")
+            if self._packed is None:
+                self._packed = torch.empty(getattr(lib, pre + "packed_bytes")(self._h), dtype=torch.uint8, device=dev)
+            arr = (C.c_void_p * n)(*[t.data_ptr() for t in tensors])
+            _lib.check(getattr(lib, pre + "set_weights")(self._h, arr, n, self._packed.data_ptr(), _lib.current_stream()))
+            self._wkey = wkey
+        return self._h
+
+    def _native(self):
+        return self._native_handle()
+
+    def grad_layout(self):
+        """(offsets, numels, total) of the flat fp32 gradient buffer the native backward fills (state_dict order)."""
+        lib = _lib.lib()
+        h = self._native()
+        n = getattr(lib, self._NATIVE_PREFIX + "num_tensors")(h)
+        offs, nums = (C.c_longlong * n)(), (C.c_longlong * n)()
+        total = getattr(lib, self._NATIVE_PREFIX + "grad_layout")(h, offs, nums, n)
+        if total < 0:
+            raise RuntimeError("diamond_b200: " + lib.dmd_last_error().decode())
+        return list(offs), list(nums), int(total)
+
+    def _grad_views_layout(self):
+        """(offsets, numels) of every PARAMETER (in `parameters()` order) inside the flat gradient buffer, and its length.
+        Static for a module, so it is computed once (walking state_dict() costs ~0.2 ms, and a backward pass may run many nodes)."""
+        cached = self.__dict__.get("_gv_layout")
+        if cached is None:
+            offs, nums, total = self.grad_layout()
+            index = {k: i for i, k in enumerate(self.state_dict().keys())}
+            names = [k for k, _ in self.named_parameters()]
+            cached = self.__dict__["_gv_layout"] = ([offs[index[k]] for k in names], [nums[index[k]] for k in names], total)
+        return cached
+
+    def _acquire_ws(self, nbytes: int):
+        """A workspace that lives from a native forward to its backward (one per live autograd node), from a pool that is
+        reused across optimizer steps."""
+        dev = self.device
+        pool = self.__dict__.setdefault("_ws_pool", [])
+        for i, ws in enumerate(pool):
+            if ws.numel() >= nbytes and ws.device == dev:
+                return pool.pop(i)
+        return torch.empty(nbytes, dtype=torch.uint8, device=dev)
+
+    def _release_ws(self, ws, cap: int) -> None:
+        pool = self.__dict__.setdefault("_ws_pool", [])
+        if len(pool) < cap:
+            pool.append(ws)
 
     def _state_tensors(self):
         ts = self.__dict__.get("_state_tensor_cache")
@@ -46,8 +136,8 @@ class NativeStateMixin:
     # The native handle (`_h`, a raw pointer owned by __del__), the packed fp16 weights, workspaces and cached layouts belong
     # to ONE module object.  copy.deepcopy (EMA copies) and pickle (multiprocessing) go through __getstate__: the copy starts
     # without native state and builds its own on first use, so two objects never own -- and free -- the same handle.
-    _NATIVE_RESET = ("_h", "_h_key", "_h_dev", "_wkey", "_packed", "_ws")
-    _NATIVE_DROP = ("_state_tensor_cache", "_tws_pool", "_ws_pool", "_bwd_scratch", "_grad_acc", "_gv_layout", "last_flat_grad")
+    _NATIVE_RESET = ("_h", "_h_key", "_wkey", "_packed", "_ws")
+    _NATIVE_DROP = ("_state_tensor_cache", "_ws_pool", "_bwd_scratch", "_grad_acc", "_gv_layout", "last_flat_grad")
 
     def __getstate__(self):
         state = self.__dict__.copy()

@@ -246,8 +246,6 @@ int dmd_embedding_bwd(const float* de, const int64_t* act, float* dE, int B, int
 int dmd_colsum(const float* x, float* out, float* out2, const float* inv_scale, long long rows, int C, int Creal, void* stream);
 /* nearest-2x upsample adjoint: out [B][H][W][C] (+)= sum of the 2x2 blocks of in [B][2H][2W][C] */
 int dmd_sumpool2(const float* in, float* out, int B, int H, int W, int C, int accumulate, void* stream);
-/* out (+)= a, n floats (multiple of 4) */
-int dmd_add(const float* a, float* out, long long n, int accumulate, void* stream);
 /* out = dh * silu'(pre) */
 int dmd_dsilu_mul(const float* pre, const float* dh, float* out, long long n, void* stream);
 /* MaxPool2d(2) backward (actor_critic.py:109): y NHWC [B][H][W][C] pre-pool, gp [B][H/2][W/2][C] -> gy [B][H][W][C] (assigned) */
@@ -424,7 +422,7 @@ void dmd_rew_end_destroy(dmd_rew_end* h);
 int dmd_rew_end_num_tensors(const dmd_rew_end* h);           /* == len(RewEndModel.state_dict()) */
 size_t dmd_rew_end_packed_bytes(const dmd_rew_end* h);
 int dmd_rew_end_set_weights(dmd_rew_end* h, const float* const* ptrs_host, int n_ptrs, void* packed, void* stream);
-size_t dmd_rew_end_workspace_bytes(dmd_rew_end* h, int rows);  /* rows = b * t */
+size_t dmd_rew_end_workspace_bytes(const dmd_rew_end* h, int rows);  /* rows = b * t */
 /* obs / next_obs (b, t, C, S, S), act (b, t) int64, hx_in / cx_in (b, lstm_dim) or NULL (zero state).
  * logits_rew (b, t, 3), logits_end (b, t, 2), hx_out / cx_out (b, lstm_dim). */
 int dmd_rew_end_predict(dmd_rew_end* h, int b, int t, const float* obs, const float* next_obs, const int64_t* act,

@@ -80,6 +80,30 @@ def test_native_actor_critic_matches_reference_golden(golden_dir):
     assert torch.allclose(full.logits_act[1:3], part.logits_act, atol=1e-5)
 
 
+@pytest.mark.gpu
+def test_native_actor_critic_rejects_parameters_that_are_not_contiguous_fp32():
+    """The native layer reads every parameter through a raw fp32 pointer: a transposed or fp64 parameter is refused, as the
+    denoiser and the reward / termination model refuse it, and the same model runs once the parameter is restored."""
+    if not torch.cuda.is_available():
+        pytest.skip("needs CUDA")
+    from diamond_b200.models.actor_critic import ActorCritic, ActorCriticConfig
+
+    dev = torch.device("cuda:0")
+    cfg = O.ActorCriticCfg()
+    ac = ActorCritic(ActorCriticConfig(cfg.lstm_dim, cfg.img_channels, cfg.img_size, list(cfg.channels), list(cfg.down), cfg.num_actions))
+    ac = ac.to(dev).eval()
+    obs = torch.zeros(2, cfg.img_channels, cfg.img_size, cfg.img_size, device=dev)
+    hx = cx = torch.zeros(2, cfg.lstm_dim, device=dev)
+    for p, bad in ((ac.lstm.weight_hh, lambda d: d.t().contiguous().t()), (ac.critic_linear.bias, lambda d: d.double())):
+        good = p.data
+        p.data = bad(good)
+        with torch.no_grad(), pytest.raises(RuntimeError, match="contiguous fp32"):
+            ac.predict_act_value(obs, (hx, cx))
+        p.data = good
+        with torch.no_grad():
+            ac.predict_act_value(obs, (hx, cx))
+
+
 def test_accumulated_native_gradients_are_adopted_like_accumulate_grad():
     """Host half of the BPTT gradient path (CPU): the flat buffer the native backward nodes accumulated into becomes `.grad` of
     every trainable parameter as a VIEW (so one all-reduce on the buffer averages the model), frozen parameters are skipped, and

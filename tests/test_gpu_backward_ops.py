@@ -411,7 +411,7 @@ def test_embedding_bwd(b, same):
 @gpu
 @pytest.mark.parametrize("b,h,w,c", [(3, 5, 7, 16), (2, 4, 4, 64), (1, 32, 16, 32)])
 @pytest.mark.parametrize("acc", [False, True])
-def test_sumpool2_and_add(b, h, w, c, acc):
+def test_sumpool2(b, h, w, c, acc):
     dev = _dev()
     from diamond_b200 import ops
 
@@ -422,12 +422,8 @@ def test_sumpool2_and_add(b, h, w, c, acc):
     out = pre.to(dev).clone()
     ops.sumpool2(gin.to(dev), out, accumulate=acc)
     e = _acc_rel(out, pre.to(dev), ref.to(dev))
-    a = torch.randn(b, h, w, c, generator=g)
-    out2 = pre.to(dev).clone()
-    ops.add(a.to(dev), out2, accumulate=acc)
     print(f"sumpool2 B={b} {h}x{w} C={c} acc={acc}: {e:.2e}")
     assert e < TOL, e
-    assert torch.equal(out2.cpu(), (pre + a) if acc else a)
 
 
 @gpu

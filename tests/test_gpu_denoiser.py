@@ -174,6 +174,25 @@ def test_denoiser_vs_oracle_fresh_inputs_and_weight_update():
     assert _rel(model2.cpu(), ref) > 1e-3  # it really changed
 
 
+def test_conv_in_too_wide_for_one_split_launch_matches_the_oracle():
+    """7 conditioning frames of 8 channels: conv_in reads 64 channels into 64, and its split-fp16 weights (3 x 72 KB) exceed
+    the one-launch budget, so the plan runs it as three launches accumulating in place (A_hi W_hi, A_lo W_hi, A_hi W_lo)."""
+    dev = _dev()
+    from oracle import torch_oracle as O
+
+    inner = O.InnerCfg(img_channels=8, num_steps_conditioning=7, cond_channels=224, depths=[1, 1, 1], channels=[64] * 3, attn_depths=[0] * 3)
+    den, sd = _build(inner, 31, dev)
+    obs, act, x_noisy = O.synthetic_inputs(3, inner, 32, 32, 77)
+    b, t, ch, h, w = obs.shape
+    sig = torch.tensor([0.05, 1.0, 8.0])
+    with torch.no_grad():
+        ref = O.model_output(x_noisy, sig, obs.reshape(b, t * ch, h, w), act, sd, O.DenoiserCfg(inner=inner))
+    model, _ = den._native_forward(x_noisy.to(dev), sig.to(dev), obs.reshape(b, t * ch, h, w).to(dev), act.to(dev), True, False)
+    per = [_rel(model[i].cpu(), ref[i]) for i in range(b)]
+    print("per-sample rel err:", per)
+    assert max(per) < REL_TOL, per
+
+
 @pytest.mark.parametrize("b", [1, 32])
 def test_benchmarked_batch_sizes_match_the_oracle(b):
     """cfg 1 (B=1) and the bench.py workload (B=32: 1 057 tiles, every CTA's tile range straddles images) against the
