@@ -7,6 +7,7 @@ The fixtures pin oracle/torch_oracle.py (CPU tests) and the CUDA path (GPU tests
 Weights are NOT stored (17 MB); they are regenerated from the seed by torch_oracle.seeded_state_dict and guarded by a
 checksum stored in the fixture.
 """
+import hashlib
 import os
 import sys
 
@@ -252,6 +253,115 @@ def make_actor_critic_training():
     print("actor_critic_training loss", loss.item(), "grad norm", float(np.sqrt((norms**2).sum())), "size", os.path.getsize(path))
 
 
+def frames_from_u8(a) -> torch.Tensor:
+    """uint8 frames -> the float32 values on the 1/255 grid in [-1, 1] that the reference saw (episode.py:36-43)."""
+    return torch.from_numpy(np.asarray(a).astype(np.float32)).div(255).mul(2).sub(1)
+
+
+# actor_critic_burnin: (t, env, "end" | "trunc") of every death.  A death at t = 0, one env dying alone, two envs dying on the
+# same step, env 2 dying three times, every env truncated on one step, a death on the last step.
+BURNIN_T, BURNIN_B = 6, 6
+BURNIN_DEATHS = [(0, 2, "end"), (2, 0, "trunc"), (2, 4, "end"), (3, 2, "end")] + [(4, e, "trunc") for e in range(BURNIN_B)] + [(5, 5, "end")]
+
+
+class _BurninScriptedEnv(_ScriptedEnv):
+    """_ScriptedEnv that also returns `burnin_obs` (k, n, C, H, W) for its dead envs, as WorldModelEnv.step does
+    (world_model_env.py:84-87): the context frames of the new episodes their policy state is burnt in on."""
+
+    def __init__(self, obs_seq, rew, end, trunc, final_obs, burnin_obs, num_actions):
+        super().__init__(obs_seq, rew, end, trunc, final_obs, num_actions)
+        self.burnin_obs = burnin_obs
+
+    def step(self, act):
+        t = self.t
+        out = super().step(act)
+        if t in self.burnin_obs:
+            out[-1]["burnin_obs"] = self.burnin_obs[t]
+        return out
+
+
+def actor_critic_burnin_inputs():
+    """The frames, rewards and flags of actor_critic_burnin.npz, regenerated from their seed (numpy PCG64) rather than stored:
+    obs_seq [T+1, b, C, H, W], final / burn-in frames {t: [k, ...]} of the k envs that died at t, as uint8; rew, end, trunc
+    [T, b].  The fixture keeps a SHA-256 digest of the frames (`frames_sha256`)."""
+    rng = np.random.default_rng(94)
+    T, b, n_ctx = BURNIN_T, BURNIN_B, 3
+    img = (3, 64, 64)
+    obs_u8 = rng.integers(0, 256, size=(T + 1, b) + img, dtype=np.uint8)
+    rew = torch.from_numpy(rng.choice([-1.0, 0.0, 0.0, 2.0], size=(T, b)).astype(np.float32))
+    end = torch.zeros(T, b, dtype=torch.long); trunc = torch.zeros(T, b, dtype=torch.long)
+    for t, e, kind in BURNIN_DEATHS:
+        (end if kind == "end" else trunc)[t, e] = 1
+    final_u8, burnin_u8 = {}, {}
+    for t in range(T):
+        k = int(torch.logical_or(end[t].bool(), trunc[t].bool()).sum())
+        if k:
+            final_u8[t] = rng.integers(0, 256, size=(k,) + img, dtype=np.uint8)
+            burnin_u8[t] = rng.integers(0, 256, size=(k, n_ctx) + img, dtype=np.uint8)
+    return obs_u8, final_u8, burnin_u8, rew, end, trunc
+
+
+def _frames_digest(obs_u8, final_u8, burnin_u8) -> str:
+    h = hashlib.sha256(obs_u8.tobytes())
+    for t in sorted(final_u8):
+        h.update(final_u8[t].tobytes()); h.update(burnin_u8[t].tobytes())
+    return h.hexdigest()
+
+
+def load_actor_critic_burnin(g) -> dict:
+    """The rollout inputs of actor_critic_burnin.npz as tensors: obs_seq [T+1, b, C, H, W], rew / end / trunc [T, b],
+    final_obs / burnin_obs {t: frames of the envs that died at t}, act [b, T].  The frames are regenerated and checked
+    against the fixture's digest; the flags and rewards against its copies."""
+    obs_u8, final_u8, burnin_u8, rew, end, trunc = actor_critic_burnin_inputs()
+    assert _frames_digest(obs_u8, final_u8, burnin_u8) == str(g["frames_sha256"]), "regenerated frames differ from the fixture's"
+    assert np.array_equal(rew.numpy(), g["rew"]) and np.array_equal(end.numpy(), g["end"]) and np.array_equal(trunc.numpy(), g["trunc"])
+    return dict(obs_seq=frames_from_u8(obs_u8), rew=rew, end=end, trunc=trunc,
+                final_obs={t: frames_from_u8(v) for t, v in final_u8.items()},
+                burnin_obs={t: frames_from_u8(v) for t, v in burnin_u8.items()}, act=torch.from_numpy(g["act"]))
+
+
+def make_actor_critic_burnin():
+    """Reference ActorCritic.forward + backward through the reference's own make_env_loop over a scripted environment that
+    returns burn-in frames with every death (BURNIN_DEATHS): the dead envs' recurrent state is burnt in with gradient on
+    3 context frames (env_loop.py:53-56), so BPTT runs through burn-in nodes of 1, 2 and 6 rows.  The frames are regenerated
+    from their seed by actor_critic_burnin_inputs (1 MB of incompressible uint8 otherwise) and guarded by a digest."""
+    ns = ref_import.load()
+    AC = ns.actor_critic
+    cfg = O.ActorCriticCfg()
+    sd = O.seeded_actor_critic_state_dict(cfg, 557)
+    ac = AC.ActorCritic(AC.ActorCriticConfig(cfg.lstm_dim, cfg.img_channels, cfg.img_size, list(cfg.channels), list(cfg.down), cfg.num_actions))
+    ac.load_state_dict(sd)
+    lc = O.ActorCriticLossCfg(backup_every=BURNIN_T)
+    obs_u8, final_u8, burnin_u8, rew, end, trunc = actor_critic_burnin_inputs()
+    env = _BurninScriptedEnv(frames_from_u8(obs_u8), rew, end, trunc, {t: frames_from_u8(v) for t, v in final_u8.items()},
+                             {t: frames_from_u8(v) for t, v in burnin_u8.items()}, cfg.num_actions)
+    ac.setup_training(env, AC.ActorCriticLossConfig(lc.backup_every, lc.gamma, lc.lambda_, lc.weight_value_loss, lc.weight_entropy_loss))
+    torch.manual_seed(32)
+    captured = {}
+    real_loop = ac.env_loop
+
+    class _Tap:
+        def send(self, n):
+            out = real_loop.send(n)
+            captured["out"] = out
+            return out
+    ac.env_loop = _Tap()
+    loss, metrics = ac()
+    loss.backward()
+    _, act, _, _, _, logits, val, val_bootstrap, _ = captured["out"]
+    grads = [(k, p.grad) for k, p in ac.named_parameters()]
+    assert all(g is not None for _, g in grads)
+    keys, norms, samples = O.grad_summary(grads)
+    path = os.path.join(OUT, "actor_critic_burnin.npz")
+    np.savez_compressed(path, weights_checksum=np.float64(O.state_checksum(sd)), frames_sha256=np.array(_frames_digest(obs_u8, final_u8, burnin_u8)),
+                        rew=rew.numpy(), end=end.numpy(), trunc=trunc.numpy(),
+                        act=act.numpy(), logits=logits.detach().numpy(), val=val.detach().numpy(), val_bootstrap=val_bootstrap.numpy(),
+                        loss=np.float64(loss.item()), metric_keys=np.array(list(metrics.keys())),
+                        metric_vals=np.array([float(v) for v in metrics.values()], np.float64),
+                        grad_keys=np.array(keys), grad_norms=norms, grad_samples=samples)
+    print("actor_critic_burnin loss", loss.item(), "grad norm", float(np.sqrt((norms**2).sum())), "size", os.path.getsize(path))
+
+
 def make_rew_end():
     """Reference RewEndModel.predict_rew_end (SURVEY.md 8 f1): a 3-step burn-in call that returns the LSTM state, then two
     single-step calls carrying it -- the way WorldModelEnv uses it (world_model_env.py:96-105, :120-129)."""
@@ -292,3 +402,6 @@ if __name__ == "__main__":
     if "training" in which:
         make_denoiser_training()
         make_actor_critic_training()
+        make_actor_critic_burnin()
+    if "burnin" in which:   # only the burn-in fixture
+        make_actor_critic_burnin()
