@@ -9,6 +9,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -873,6 +874,8 @@ struct BOp {
   int M = 0, N = 0, K = 0, use_inv = 0;
   // linear recompute
   const float *lin_in = nullptr, *lin_w = nullptr, *lin_b = nullptr; float* lin_out = nullptr; int lin_K = 0, lin_F = 0;
+  // embedding: actions per row (the row's CC channels are T embeddings side by side) and the table's row count
+  int emb_T = 0, emb_actions = 0;
 };
 
 enum RecKind { R_CONVIN = 0, R_DOWN, R_UP, R_RES, R_OUT };
@@ -885,6 +888,8 @@ struct Rec {
 
 struct Plan {
   int B = 0, H = 0, W = 0;
+  int T = 1;   // time-major plans (reward / termination): B = T x segments rows
+  long long tmp_floats = 0;   // training: floats in each of tA / tB / tC
   uint8_t* base = nullptr;
   size_t bytes = 0;
   float *xin = nullptr, *cs = nullptr, *cemb = nullptr, *chid = nullptr, *cond = nullptr, *film = nullptr, *fout = nullptr;
@@ -908,6 +913,13 @@ struct Plan {
   long long *film_woff = nullptr, *film_boff = nullptr;   // device tables: flat-gradient offset of every FiLM row
   std::vector<long long> film_woff_h, film_boff_h;
   uint8_t* zero_begin = nullptr; size_t zero_bytes = 0;   // region cleared at the start of every backward (dfilm, sums, amax)
+  // reward / termination training: the encoder output and the LSTM / head tape, time-major rows (row = k * segments + n)
+  Tens feat{};
+  float *gates = nullptr;                                 // [T][b][4D] pre-activation gates of every step
+  float *cseq = nullptr, *hseq = nullptr;                 // [T+1][b][D] cell / hidden states; hseq[0] = h_in, hseq + b*D = y
+  float *hid = nullptr, *logits_tm = nullptr;             // [T*b][D] silu(head.0(y)), [T*b][5]
+  int64_t* act_tm = nullptr;                              // [T*b] actions
+  float *g_tm = nullptr, *g_hid = nullptr, *hpre = nullptr, *g_pre = nullptr, *g_y = nullptr, *dgates = nullptr, *gcs = nullptr;
   // sampler state (NCHW fp32): temporaries only -- the frame stack, the actions and the trajectory are used IN PLACE
   float *s_xc = nullptr, *s_x2 = nullptr, *s_d = nullptr;
   float *sig_all = nullptr, *cemb_all = nullptr, *chid_all = nullptr, *cond_all = nullptr, *film_all = nullptr;  // hoisted conditioning
@@ -935,6 +947,9 @@ struct ModelCore {
   size_t packed_bytes = 0;
   int cond_channels = 0, film_rows = 0;  // FiLM table: film_rows x cond_channels weights, then film_rows biases
   size_t film_w_off = 0, film_b_off = 0;
+  // training plans, one per live training workspace (an autoregressive Denoiser.forward holds several forwards before
+  // their backwards run); kept apart from the inference plan so that imagination and training can alternate
+  std::vector<std::unique_ptr<Plan>> tplans;
 
   const float* P(int idx) const { return ptrs.empty() ? nullptr : ptrs[idx]; }
   // once every tensor is registered: 16-byte aligned gradient slices, and the FiLM table behind the pk bytes of conv packs
@@ -987,9 +1002,6 @@ struct dmd_denoiser {
   std::vector<SamplerGraph> graphs;     // one per distinct (buffers, ring head): a WorldModelEnv replays T of them round-robin
   unsigned long long graph_clock = 0;
   cudaStream_t cap_stream = nullptr;
-  // training plans, one per live training workspace (an autoregressive Denoiser.forward holds several forwards before
-  // their backwards run); kept apart from `plan` so that imagination and training can alternate
-  std::vector<std::unique_ptr<Plan>> tplans;
   int need_B = 0, need_H = 0, need_W = 0; size_t need_bytes = 0;
 };
 
@@ -1267,11 +1279,17 @@ struct PlanBuilder {
     pl->film = (float*)bump->take((size_t)B * core->film_rows * 4);
     Tens xin{pl->xin, nullptr, pl->CP_in, H, W, 8};
     Tens x = tensor(c.channels[0], H, W, true);
-    { Operand in0 = prep(xin, nullptr, 0, 0, nullptr, 0, 0, false, false, true); conv(h->conv_in, in0, false, 1, nullptr, x, true); }
+    {
+      Operand in0 = prep(xin, nullptr, 0, 0, nullptr, 0, 0, false, false, true);
+      conv(h->conv_in, in0, false, 1, nullptr, x, true);
+      Rec rec; rec.kind = R_CONVIN; rec.cw = &h->conv_in; rec.x = xin; rec.o = x; rec.in1 = in0; record(rec);
+    }
     for (int i = 0; i <= L; ++i) {
       if (i > 0 && i < L) {
         Tens xd = tensor(c.channels[i - 1], x.H / 2, x.W / 2, true);
-        { Operand ind = prep(x, nullptr, 0, 0, nullptr, 0, 0, false, false); conv(h->downs[i], ind, false, 2, nullptr, xd, true); }
+        Operand ind = prep(x, nullptr, 0, 0, nullptr, 0, 0, false, false);
+        conv(h->downs[i], ind, false, 2, nullptr, xd, true);
+        Rec rec; rec.kind = R_DOWN; rec.cw = &h->downs[i]; rec.x = x; rec.o = xd; rec.in1 = ind; record(rec);
         x = xd;
       }
       for (auto& rb : h->blocks[i]) x = resblock(rb, x, nullptr);
@@ -1396,14 +1414,17 @@ int make_plan(const dmd_denoiser* h, Plan* pl, int B, int H, int W, uint8_t* bas
 // Walks the forward tape in reverse and emits the backward op list.  Every gradient tensor is fp32 NHWC and carries the
 // loss scale; "first writer assigns, later writers accumulate" is decided here at plan time (ginit), so no gradient
 // buffer needs a memset.  Forward conv inputs (the PLC16 operands) are not kept: the forward prep launch is replayed.
+// Both executors' encoders are made of the same records (R_RES, R_DOWN, R_UP, R_CONVIN), which walk() handles; each model
+// emits its own output head before the walk and its own conditioning path after it (film_tail is the part they share).
 struct BwdBuilder {
-  const dmd_denoiser* h; Plan* pl; Bump* bump; int err = 0;
+  const ModelCore* core; Plan* pl; int err = 0;
   std::vector<char> ginit;
 
-  const float* P(int idx) const { return h->core.P(idx); }
-  long long G(int idx) const { return h->core.goff[idx]; }
+  const float* P(int idx) const { return core->P(idx); }
+  long long G(int idx) const { return core->goff[idx]; }
   bool was_init(const Tens& t) { const bool w = ginit[t.gid] != 0; ginit[t.gid] = 1; return w; }
   void push(const BOp& b) { pl->bops.push_back(b); }
+  void begin() { ginit.assign(pl->n_grad_tensors, 0); pl->bops.clear(); }
 
   void replay(const Operand& o) { BOp b; b.kind = B_PREP; b.prep = pl->ops[o.op].prep; b.prep_nsrc = pl->ops[o.op].prep_nsrc; push(b); }
   // NHWC fp32 gradient [B][Hs][Ws][C] -> PLC16 operand (ups = 2: zero insertion, the adjoint of a stride-2 conv)
@@ -1418,7 +1439,7 @@ struct BwdBuilder {
     push(b);
   }
   void dgrad(const ConvW& cw, int k, const uint8_t* gy, int H, int W, float* out, bool accumulate) {
-    const dmd_conv_desc d = dgrad_desc(cw, k, h->core.packed + cw.pkT_off[k], gy, pl->B, H, W, out, accumulate);
+    const dmd_conv_desc d = dgrad_desc(cw, k, core->packed + cw.pkT_off[k], gy, pl->B, H, W, out, accumulate);
     BOp b; b.kind = B_CONV;
     if (conv_fill(&d, &b.conv, &b.smem, &b.cols)) { err = 1; return; }
     push(b);
@@ -1431,7 +1452,7 @@ struct BwdBuilder {
   }
   void norm_bwd(const Tens& x, const float* gy, int mode, const FilmW* film, int c_off, int ctot, int gamma_idx, int beta_idx,
                 float* gx, const float* addend, bool accumulate) {
-    const int R = h->core.film_rows;
+    const int R = core->film_rows;
     NormBwdParams nb = gn_bwd_params(x.data, gy, x.stats, pl->B, x.H * x.W, x.C, x.gs, P(gamma_idx), P(beta_idx), pl->nsum, gx, addend, accumulate);
     if (mode == 1) {   // AdaGroupNorm: FiLM rows in place of gamma / beta, their gradients in place of the per-channel sums
       nb.mode = 1; nb.gamma = nb.beta = nullptr; nb.c_off = c_off;
@@ -1461,7 +1482,7 @@ struct BwdBuilder {
       b.ab = AttnBwdParams{o.data, o.stats, P(rb.an_w), P(rb.an_b), P(rb.qkv_w), P(rb.qkv_b), P(rb.op_w), r.a.grad, o.grad,
                            nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, pl->scale ? pl->scale + 1 : nullptr, H * W, rb.cout, o.gs, kGnEps};
       const int ids[6] = {rb.an_w, rb.an_b, rb.qkv_w, rb.qkv_b, rb.op_w, rb.op_b};
-      for (int i = 0; i < 6; ++i) b.goffs[i] = h->core.goff[ids[i]];
+      for (int i = 0; i < 6; ++i) b.goffs[i] = G(ids[i]);
       push(b);
       ginit[o.gid] = 1;
     }
@@ -1498,23 +1519,12 @@ struct BwdBuilder {
     }
   }
 
-  int build() {
+  // records [0, end) of the tape, in reverse
+  int walk(int end) {
     const int B = pl->B;
-    ginit.assign(pl->n_grad_tensors, 0);
-    pl->bops.clear();
-    for (int i = (int)pl->tape.size() - 1; i >= 0; --i) {
+    for (int i = end - 1; i >= 0; --i) {
       const Rec& r = pl->tape[i];
-      if (r.kind == R_OUT) {
-        // conv_out(silu(norm_out(x))) (inner_model.py:48): gF is the scaled gradient of the model output, NHWC x 8 channels
-        const ConvW& cw = *r.cw;
-        const int H = r.x.H, W = r.x.W;
-        gprep(pl->gF, 8, H, W, 0, pl->gyA);
-        colsum(pl->gF, (long long)B * H * W, 8, cw.Cout, cw.b_idx);
-        replay(r.in1);
-        wgrad(cw, pl->gyA, r.in1.n0, round_up(r.x.C, 16), r.x.C, 0, H, W);
-        dgrad(cw, 0, pl->gyA, H, W, pl->tA, false);
-        norm_bwd(r.x, pl->tA, 2, nullptr, 0, r.x.C, h->i_normout_w, h->i_normout_b, r.x.grad, nullptr, was_init(r.x));
-      } else if (r.kind == R_RES) {
+      if (r.kind == R_RES) {
         resblock(r);
       } else if (r.kind == R_UP) {   // Upsample (blocks.py:103-110): nearest x2 then conv
         const ConvW& cw = *r.cw;
@@ -1534,94 +1544,137 @@ struct BwdBuilder {
         replay(r.in1);
         wgrad(cw, pl->gyA, r.in1.n0, round_up(r.x.C, 16), r.x.C, 0, H, W);
         dgrad(cw, 0, pl->gyA, H, W, r.x.grad, was_init(r.x));
-      } else {  // R_CONVIN: weight / bias gradients only (the network input needs none)
+      } else if (r.kind == R_CONVIN) {  // weight / bias gradients only (the network input needs none)
         const ConvW& cw = *r.cw;
         const int H = r.o.H, W = r.o.W;
         gprep(r.o.grad, cw.Cout, H, W, 0, pl->gyA);
         colsum(r.o.grad, (long long)B * H * W, cw.Cout, cw.Cout, cw.b_idx);
         replay(r.in1);
         wgrad(cw, pl->gyA, r.in1.n0, cw.c0_store, cw.c0_real, 0, H, W);
+      } else {
+        return fail("backward plan: record %d of kind %d belongs to a model's own head", i, r.kind);
       }
       if (err) return 1;
     }
-    // ---- conditioning path (inner_model.py:45; blocks.py:39): FiLM linears, cond_proj MLP, action embedding
-    const dmd_denoiser_config& c = h->cfg;
-    const int CC = c.cond_channels, R = h->core.film_rows;
+    return 0;
+  }
+
+  // C (+)= alpha * op(A) op(B); c_goff >= 0: C is that slice of the gradient buffer
+  void sgemm(const float* A, long long sam, long long sak, const float* Bm, long long sbk, long long sbn, float* C, long long c_goff,
+             long long ldc, int M, int N, int K, int use_inv, int acc) {
+    BOp b; b.kind = B_SGEMM; b.ga = A; b.sam = sam; b.sak = sak; b.gb = Bm; b.sbk = sbk; b.sbn = sbn; b.gc = C; b.c_goff = c_goff; b.ldc = ldc;
+    b.M = M; b.N = N; b.K = K; b.use_inv = use_inv; b.acc = acc; push(b);
+  }
+  // FiLM linears (blocks.py:39): their weight / bias gradients, then dcond = dfilm Wf, the gradient of their common input
+  void film_tail() {
+    const int B = pl->B, CC = core->cond_channels, R = core->film_rows;
     { BOp b; b.kind = B_FILMW; push(b); }
-    auto sgemm = [&](const float* A, long long sam, long long sak, const float* Bm, long long sbk, long long sbn, float* C, long long c_goff,
-                     long long ldc, int M, int N, int K, int use_inv, int acc) {
-      BOp b; b.kind = B_SGEMM; b.ga = A; b.sam = sam; b.sak = sak; b.gb = Bm; b.sbk = sbk; b.sbn = sbn; b.gc = C; b.c_goff = c_goff; b.ldc = ldc;
-      b.M = M; b.N = N; b.K = K; b.use_inv = use_inv; b.acc = acc; push(b);
-    };
-    const float* Wf = h->core.packed ? (const float*)(h->core.packed + h->core.film_w_off) : nullptr;
+    const float* Wf = core->packed ? (const float*)(core->packed + core->film_w_off) : nullptr;
     sgemm(pl->dfilm, R, 1, Wf, CC, 1, pl->dcond, -1, CC, B, CC, R, 0, 0);                       // dcond = dfilm Wf
     {   // K = R (7168 rows for the default net) over a handful of 64 x 64 output tiles: split K across the SMs
-      int cmax = 16;
-      for (int i = 0; i < c.num_levels; ++i) cmax = c.channels[i] > cmax ? c.channels[i] : cmax;
-      long long fit = (long long)pl->H * pl->W * cmax / CC;   // partials live in tA (B * H * W * cmax floats)
+      const long long fit = pl->tmp_floats / ((long long)B * CC);   // partials live in tA
       int splits = R / 256; if (splits > 32) splits = 32; if (splits > fit) splits = (int)fit;
       if (splits > 1) pl->bops.back().chunks = splits;
     }
-    sgemm(pl->dcond, 1, CC, pl->chid, CC, 1, nullptr, h->core.goff[h->i_cp2w], CC, CC, CC, B, 1, 1);  // dW2 += dcond^T h
-    colsum(pl->dcond, B, CC, CC, h->i_cp2b);
-    sgemm(pl->dcond, CC, 1, P(h->i_cp2w), CC, 1, pl->dh, -1, CC, B, CC, CC, 0, 0);               // dh = dcond W2
-    { BOp b; b.kind = B_LINEAR; b.lin_in = pl->cemb; b.lin_w = P(h->i_cp0w); b.lin_b = P(h->i_cp0b); b.lin_out = pl->cpre; b.lin_K = CC; b.lin_F = CC; push(b); }
-    { BOp b; b.kind = B_DSILU; b.src = pl->cpre; b.ga = pl->dh; b.dst = pl->dpre; b.rows = (long long)B * CC; push(b); }
-    sgemm(pl->dpre, 1, CC, pl->cemb, CC, 1, nullptr, h->core.goff[h->i_cp0w], CC, CC, CC, B, 1, 1);   // dW0 += dpre^T e
-    colsum(pl->dpre, B, CC, CC, h->i_cp0b);
-    sgemm(pl->dpre, CC, 1, P(h->i_cp0w), CC, 1, pl->de, -1, CC, B, CC, CC, 0, 0);                // de = dpre W0
-    { BOp b; b.kind = B_EMB; b.src = pl->de; b.goff = h->core.goff[h->i_actemb]; push(b); }
-    return err;
+  }
+  // nn.Embedding gradient of table `idx` from de [B][CC] (T embeddings of CC / T channels per row, actions pl->t_act [B][T])
+  void embedding(const float* de, int idx, int T, int num_actions) {
+    BOp b; b.kind = B_EMB; b.src = de; b.goff = G(idx); b.C = core->cond_channels; b.emb_T = T; b.emb_actions = num_actions; push(b);
   }
 };
 
-// training workspace = forward plan (with gradient buffers) + backward temporaries
-int make_train_plan(const dmd_denoiser* h, Plan* pl, int B, int H, int W, uint8_t* base, size_t* total) {
+// Denoiser backward op list: conv_out(silu(norm_out(x))) (inner_model.py:48), the U-Net, then the conditioning path
+// (inner_model.py:45): FiLM linears, cond_proj MLP, action embedding
+int build_denoiser_bwd(const dmd_denoiser* h, BwdBuilder& bw) {
+  Plan* pl = bw.pl;
+  const int B = pl->B;
+  bw.begin();
+  {   // the last record: gF is the scaled gradient of the model output, NHWC x 8 channels
+    const Rec& r = pl->tape.back();
+    if (r.kind != R_OUT) return fail("denoiser backward plan: the tape does not end with the output head");
+    const ConvW& cw = *r.cw;
+    const int H = r.x.H, W = r.x.W;
+    bw.gprep(pl->gF, 8, H, W, 0, pl->gyA);
+    bw.colsum(pl->gF, (long long)B * H * W, 8, cw.Cout, cw.b_idx);
+    bw.replay(r.in1);
+    bw.wgrad(cw, pl->gyA, r.in1.n0, round_up(r.x.C, 16), r.x.C, 0, H, W);
+    bw.dgrad(cw, 0, pl->gyA, H, W, pl->tA, false);
+    bw.norm_bwd(r.x, pl->tA, 2, nullptr, 0, r.x.C, h->i_normout_w, h->i_normout_b, r.x.grad, nullptr, bw.was_init(r.x));
+    if (bw.err) return 1;
+  }
+  if (bw.walk((int)pl->tape.size() - 1)) return 1;
+  bw.film_tail();
+  const int CC = h->cfg.cond_channels;
+  const long long* goff = h->core.goff.data();
+  bw.sgemm(pl->dcond, 1, CC, pl->chid, CC, 1, nullptr, goff[h->i_cp2w], CC, CC, CC, B, 1, 1);  // dW2 += dcond^T h
+  bw.colsum(pl->dcond, B, CC, CC, h->i_cp2b);
+  bw.sgemm(pl->dcond, CC, 1, bw.P(h->i_cp2w), CC, 1, pl->dh, -1, CC, B, CC, CC, 0, 0);          // dh = dcond W2
+  { BOp b; b.kind = B_LINEAR; b.lin_in = pl->cemb; b.lin_w = bw.P(h->i_cp0w); b.lin_b = bw.P(h->i_cp0b); b.lin_out = pl->cpre; b.lin_K = CC; b.lin_F = CC; bw.push(b); }
+  { BOp b; b.kind = B_DSILU; b.src = pl->cpre; b.ga = pl->dh; b.dst = pl->dpre; b.rows = (long long)B * CC; bw.push(b); }
+  bw.sgemm(pl->dpre, 1, CC, pl->cemb, CC, 1, nullptr, goff[h->i_cp0w], CC, CC, CC, B, 1, 1);   // dW0 += dpre^T e
+  bw.colsum(pl->dpre, B, CC, CC, h->i_cp0b);
+  bw.sgemm(pl->dpre, CC, 1, bw.P(h->i_cp0w), CC, 1, pl->de, -1, CC, B, CC, CC, 0, 0);           // de = dpre W0
+  bw.embedding(pl->de, h->i_actemb, h->cfg.num_steps_conditioning, h->cfg.num_actions);
+  return bw.err;
+}
+
+// training workspace = forward plan (with gradient buffers) + backward temporaries.  fwd builds the forward plan (taking
+// the model's own training buffers from pb.bump); bwd emits the backward op list.  cmax: the widest channel count of the
+// network; gF_ch: channels of the NHWC output-gradient buffer gF (0: none).
+using FwdPlanFn = std::function<int(PlanBuilder&)>;
+using BwdPlanFn = std::function<int(BwdBuilder&)>;
+int make_train_plan(const ModelCore& core, int cmax, int gF_ch, Plan* pl, int B, int H, int W, int T, uint8_t* base, size_t* total,
+                    const FwdPlanFn& fwd, const BwdPlanFn& bwd) {
   pl->train = true; pl->n_grad_tensors = 0; pl->tape.clear();
-  pl->B = B; pl->H = H; pl->W = W; pl->ops.clear(); pl->bops.clear();
+  pl->B = B; pl->H = H; pl->W = W; pl->T = T; pl->ops.clear(); pl->bops.clear();
   Bump b0{nullptr}, s0{nullptr};
-  { Plan tmp; tmp.train = true; tmp.B = B; tmp.H = H; tmp.W = W; PlanBuilder pb{&h->core, &tmp, &b0, &s0}; if (pb.build(h)) return 1; }
+  { Plan tmp; tmp.train = true; tmp.B = B; tmp.H = H; tmp.W = W; tmp.T = T; PlanBuilder pb{&core, &tmp, &b0, &s0}; if (fwd(pb)) return 1; }
   const size_t stats_bytes = (s0.off + 255) & ~(size_t)255;
   Bump sb{base}, bb{base ? base + stats_bytes : nullptr};
   if (base) { pl->base = base; pl->stats = (double*)base; pl->stats_bytes = stats_bytes; }
-  if (base) { PlanBuilder pb{&h->core, pl, &bb, &sb}; if (pb.build(h)) return 1; } else bb.off = b0.off;
+  if (base) { PlanBuilder pb{&core, pl, &bb, &sb}; if (fwd(pb)) return 1; } else bb.off = b0.off;
   // backward temporaries
-  const dmd_denoiser_config& c = h->cfg;
-  int cmax = 16;
-  for (int i = 0; i < c.num_levels; ++i) cmax = c.channels[i] > cmax ? c.channels[i] : cmax;
-  const size_t act_bytes = (size_t)B * H * W * cmax * 4;
+  pl->tmp_floats = (long long)B * H * W * cmax;
+  const size_t act_bytes = (size_t)pl->tmp_floats * 4;
   pl->tA = (float*)bb.take(act_bytes); pl->tB = (float*)bb.take(act_bytes); pl->tC = (float*)bb.take(act_bytes);
   const size_t op_bytes = plc16_bytes(B, H, W, cmax);
   pl->gyA = (uint8_t*)bb.take(op_bytes); pl->gyB = (uint8_t*)bb.take(op_bytes);
-  pl->gF = (float*)bb.take((size_t)B * H * W * 8 * 4);
+  pl->gF = (float*)bb.take((size_t)B * H * W * gF_ch * 4);
   if (init_kernels()) return 1;
   pl->partial = (float*)bb.take(wgrad_partial_bytes(g_num_sms));
-  const int CC = c.cond_channels;
+  const int CC = core.cond_channels;
   pl->dcond = (float*)bb.take((size_t)B * CC * 4); pl->dh = (float*)bb.take((size_t)B * CC * 4); pl->cpre = (float*)bb.take((size_t)B * CC * 4);
   pl->dpre = (float*)bb.take((size_t)B * CC * 4); pl->de = (float*)bb.take((size_t)B * CC * 4);
-  pl->film_woff = (long long*)bb.take((size_t)h->core.film_rows * 8); pl->film_boff = (long long*)bb.take((size_t)h->core.film_rows * 8);
+  pl->film_woff = (long long*)bb.take((size_t)core.film_rows * 8); pl->film_boff = (long long*)bb.take((size_t)core.film_rows * 8);
   pl->scale = (float*)bb.take(256);
   // zeroed at the start of every backward: dfilm, affine-norm sums, amax
   uint8_t* z0 = (uint8_t*)bb.take(0);
-  pl->dfilm = (float*)bb.take((size_t)B * h->core.film_rows * 4);
+  pl->dfilm = (float*)bb.take((size_t)B * core.film_rows * 4);
   pl->nsum = (float*)bb.take((size_t)2 * B * kMaxCin * 4);
   pl->amax = (unsigned int*)bb.take(256);
   pl->zero_begin = z0; pl->zero_bytes = base ? (size_t)((uint8_t*)pl->amax + 256 - z0) : 0;
   if (total) *total = stats_bytes + bb.off + 512;
   if (!base) return 0;
   pl->bytes = stats_bytes + bb.off;
-  BwdBuilder bw{h, pl, &bb};
-  if (bw.build()) return 1;
-  // flat-gradient offsets of every FiLM row (weights) / element (biases)
-  pl->film_woff_h.assign(h->core.film_rows, 0); pl->film_boff_h.assign(h->core.film_rows, 0);
+  BwdBuilder bw{&core, pl};
+  if (bwd(bw)) return 1;
+  // flat-gradient offsets of every FiLM row (weights) / element (biases); every ResBlock is on the tape
+  pl->film_woff_h.assign(core.film_rows, 0); pl->film_boff_h.assign(core.film_rows, 0);
   auto fill_film = [&](const FilmW& f) {
-    for (int r = 0; r < 2 * f.C; ++r) { pl->film_woff_h[f.off + r] = h->core.goff[f.w_idx] + (long long)r * CC; pl->film_boff_h[f.off + r] = h->core.goff[f.b_idx] + r; }
+    for (int r = 0; r < 2 * f.C; ++r) { pl->film_woff_h[f.off + r] = core.goff[f.w_idx] + (long long)r * CC; pl->film_boff_h[f.off + r] = core.goff[f.b_idx] + r; }
   };
-  auto fill_rb = [&](const ResBlockW& r) { fill_film(r.n1); fill_film(r.n2); };
-  for (auto& lv : h->d_blocks) for (auto& r : lv) fill_rb(r);
-  for (auto& lv : h->u_blocks) for (auto& r : lv) fill_rb(r);
-  for (auto& r : h->mid) fill_rb(r);
+  for (const Rec& r : pl->tape) if (r.kind == R_RES) { fill_film(r.rb->n1); fill_film(r.rb->n2); }
   return 0;
+}
+
+template <class Cfg> int widest_channels(const Cfg& c) {  // at least 16
+  int cmax = 16;
+  for (int i = 0; i < c.num_levels; ++i) cmax = c.channels[i] > cmax ? c.channels[i] : cmax;
+  return cmax;
+}
+int make_denoiser_train_plan(const dmd_denoiser* h, Plan* pl, int B, int H, int W, uint8_t* base, size_t* total) {
+  return make_train_plan(h->core, widest_channels(h->cfg), 8, pl, B, H, W, 1, base, total,
+                         [h](PlanBuilder& pb) { return pb.build(h); }, [h](BwdBuilder& bw) { return build_denoiser_bwd(h, bw); });
 }
 
 // cond_k >= 0: the conditioning of this evaluation was computed up front by sampler_conditioning (FiLM rows at film_all + k)
@@ -1730,7 +1783,7 @@ extern "C" int dmd_denoiser_set_weights(dmd_denoiser* h, const float* const* ptr
   cudaStream_t st = (cudaStream_t)stream;
   bool moved = false;
   if (h->core.set_weights("InnerModel", ptrs_host, n_ptrs, packed, &moved)) return 1;
-  if (moved) { h->plan.B = 0; h->tplans.clear(); for (auto& g : h->graphs) g.valid = false; }
+  if (moved) { h->plan.B = 0; h->core.tplans.clear(); for (auto& g : h->graphs) g.valid = false; }
   const ModelCore& m = h->core;
   if (pack_one(m, h->conv_in, st) || pack_one(m, h->conv_out, st)) return 1;
   for (auto& lv : h->d_blocks) for (auto& r : lv) if (pack_rb(m, r, st)) return 1;
@@ -1770,43 +1823,47 @@ extern "C" int dmd_inner_model_forward(dmd_denoiser* h, int B, int H, int W, con
 // ---------------------------------------------------------------------------------------------- training entry points
 namespace {
 
-Plan* find_train_plan(dmd_denoiser* h, int B, int H, int W, void* ws) {
-  for (auto& p : h->tplans)
-    if (p->B == B && p->H == H && p->W == W && p->base == (uint8_t*)ws) return p.get();
+Plan* find_train_plan(ModelCore& core, int B, int H, int W, int T, const void* ws) {
+  for (auto& p : core.tplans)
+    if (p->B == B && p->H == H && p->W == W && p->T == T && p->base == (const uint8_t*)ws) return p.get();
   return nullptr;
 }
 
-int ensure_train_plan(dmd_denoiser* h, int B, int H, int W, void* ws, size_t ws_bytes, cudaStream_t st, Plan** out) {
-  DMD_CHECK(h->core.ready(), "denoiser: call dmd_denoiser_set_weights first");
-  if ((*out = find_train_plan(h, B, H, W, ws)) != nullptr) return 0;
+// make(pl, base, total): make_train_plan of the model; who: the model's name in messages
+using MakeTrainPlanFn = std::function<int(Plan*, uint8_t*, size_t*)>;
+int ensure_train_plan(ModelCore& core, const char* who, int B, int H, int W, int T, void* ws, size_t ws_bytes, cudaStream_t st,
+                      const MakeTrainPlanFn& make, Plan** out) {
+  DMD_CHECK(core.ready(), "%s: call dmd_%s_set_weights first", who, who);
+  if ((*out = find_train_plan(core, B, H, W, T, ws)) != nullptr) return 0;
   size_t need = 0;
-  { Plan tmp; if (make_train_plan(h, &tmp, B, H, W, nullptr, &need)) return 1; }
-  DMD_CHECK(ws && ws_bytes >= need, "denoiser: training workspace too small (%zu < %zu)", ws_bytes, need);
-  DMD_CHECK(((uintptr_t)ws & 255) == 0, "denoiser: workspace must be 256-byte aligned");
+  { Plan tmp; if (make(&tmp, nullptr, &need)) return 1; }
+  DMD_CHECK(ws && ws_bytes >= need, "%s: training workspace too small (%zu < %zu)", who, ws_bytes, need);
+  DMD_CHECK(((uintptr_t)ws & 255) == 0, "%s: workspace must be 256-byte aligned", who);
   // a plan bound to the same workspace with another shape is stale; keep at most 8 plans
-  for (size_t i = 0; i < h->tplans.size();)
-    if (h->tplans[i]->base == (uint8_t*)ws) h->tplans.erase(h->tplans.begin() + i); else ++i;
-  if (h->tplans.size() >= 8) h->tplans.erase(h->tplans.begin());
+  auto& tp = core.tplans;
+  for (size_t i = 0; i < tp.size();)
+    if (tp[i]->base == (uint8_t*)ws) tp.erase(tp.begin() + i); else ++i;
+  if (tp.size() >= 8) tp.erase(tp.begin());
   std::unique_ptr<Plan> pl(new Plan());
-  if (make_train_plan(h, pl.get(), B, H, W, (uint8_t*)ws, nullptr)) return 1;
+  if (make(pl.get(), (uint8_t*)ws, nullptr)) return 1;
   DMD_CUDA(cudaMemcpyAsync(pl->film_woff, pl->film_woff_h.data(), pl->film_woff_h.size() * 8, cudaMemcpyHostToDevice, st));
   DMD_CUDA(cudaMemcpyAsync(pl->film_boff, pl->film_boff_h.data(), pl->film_boff_h.size() * 8, cudaMemcpyHostToDevice, st));
   *out = pl.get();
-  h->tplans.push_back(std::move(pl));
+  tp.push_back(std::move(pl));
   return 0;
 }
 
-int run_backward(dmd_denoiser* h, Plan& pl, const float* grad_out, float* grads, cudaStream_t st) {
-  const dmd_denoiser_config& c = h->cfg;
-  const int B = pl.B, HW = pl.H * pl.W, CC = c.cond_channels;
-  const float* inv = pl.scale + 1;
-  DMD_CUDA(cudaMemsetAsync(grads, 0, (size_t)h->core.grad_total * 4, st));
+// start of every backward: the flat gradient buffer and the accumulators of the plan (dfilm, affine-norm sums, amax) cleared
+int clear_backward(const ModelCore& core, Plan& pl, float* grads, cudaStream_t st) {
+  DMD_CUDA(cudaMemsetAsync(grads, 0, (size_t)core.grad_total * 4, st));
   DMD_CUDA(cudaMemsetAsync(pl.zero_begin, 0, pl.zero_bytes, st));
-  // loss scale from the incoming gradient, then the scaled NHWC gradient of the model output
-  const long long n_out = (long long)B * c.img_channels * HW;
-  if (loss_scale_launch(grad_out, n_out, pl.amax, pl.scale, st)) return 1;
-  nchw_to_nhwc_scaled_kernel<<<dim3((HW + 255) / 256, B), 256, 0, st>>>(grad_out, pl.gF, pl.scale, c.img_channels, 8, HW);
-  DMD_LAUNCH_OK();
+  return 0;
+}
+
+// the backward op list; the caller has cleared (clear_backward), set the loss scale and seeded the gradient the list starts from
+int run_backward(const ModelCore& core, Plan& pl, float* grads, cudaStream_t st) {
+  const int B = pl.B;
+  const float* inv = pl.scale + 1;
   for (const BOp& b : pl.bops) {
     switch (b.kind) {
       case B_PREP: if (prep_launch(b.prep, b.prep_nsrc, st)) return 1; break;
@@ -1832,12 +1889,12 @@ int run_backward(dmd_denoiser* h, Plan& pl, const float* grad_out, float* grads,
                          b.use_inv ? inv : nullptr, b.acc, b.chunks, pl.tA, st)) return 1;
         break;
       case B_FILMW:
-        if (film_wgrad_launch(pl.dfilm, pl.cond, grads, pl.film_woff, pl.film_boff, B, h->core.film_rows, CC, inv, st)) return 1;
+        if (film_wgrad_launch(pl.dfilm, pl.cond, grads, pl.film_woff, pl.film_boff, B, core.film_rows, core.cond_channels, inv, st)) return 1;
         break;
       case B_LINEAR: if (linear_launch(b.lin_in, b.lin_w, b.lin_b, b.lin_out, B, b.lin_K, b.lin_F, 0, st)) return 1; break;
       case B_DSILU: if (dsilu_mul_launch(b.src, b.ga, b.dst, b.rows, st)) return 1; break;
       case B_EMB:
-        if (embedding_bwd_launch(b.src, pl.t_act, grads + b.goff, B, CC, c.num_steps_conditioning, c.num_actions, inv, st)) return 1;
+        if (embedding_bwd_launch(b.src, pl.t_act, grads + b.goff, B, b.C, b.emb_T, b.emb_actions, inv, st)) return 1;
         break;
       default: return fail("backward: unknown op kind %d", b.kind);
     }
@@ -1849,7 +1906,7 @@ int run_backward(dmd_denoiser* h, Plan& pl, const float* grad_out, float* grads,
 
 extern "C" size_t dmd_denoiser_train_workspace_bytes(const dmd_denoiser* h, int B, int H, int W) {
   Plan tmp; size_t need = 0;
-  if (make_train_plan(h, &tmp, B, H, W, nullptr, &need)) return 0;
+  if (make_denoiser_train_plan(h, &tmp, B, H, W, nullptr, &need)) return 0;
   return need;
 }
 extern "C" long long dmd_denoiser_grad_layout(const dmd_denoiser* h, long long* offsets, long long* numels, int n) {
@@ -1862,7 +1919,8 @@ extern "C" int dmd_inner_model_forward_train(dmd_denoiser* h, int B, int H, int 
   DMD_CHECK(h && noisy_rescaled && c_noise && obs_rescaled && act && out, "inner_model_forward_train: null argument");
   cudaStream_t st = (cudaStream_t)stream;
   Plan* pl = nullptr;
-  if (ensure_train_plan(h, B, H, W, workspace, workspace_bytes, st, &pl)) return 1;
+  auto make = [h, B, H, W](Plan* p, uint8_t* base, size_t* total) { return make_denoiser_train_plan(h, p, B, H, W, base, total); };
+  if (ensure_train_plan(h->core, "denoiser", B, H, W, 1, workspace, workspace_bytes, st, make, &pl)) return 1;
   pl->t_act = act;
   if (run_forward(h, *pl, noisy_rescaled, c_noise, c_noise_is_scalar, obs_rescaled, act, st, 1)) return 1;
   return run_wrap(h, *pl, noisy_rescaled, out, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1.f, 0.f, st);
@@ -1871,12 +1929,19 @@ extern "C" int dmd_inner_model_forward_train(dmd_denoiser* h, int B, int H, int 
 extern "C" int dmd_denoiser_backward(dmd_denoiser* h, int B, int H, int W, const float* grad_out, float* grads, long long grads_numel,
                                      void* workspace, void* stream) {
   DMD_CHECK(h && grad_out && grads && workspace, "denoiser_backward: null argument");
-  Plan* plp = find_train_plan(h, B, H, W, workspace);
+  Plan* plp = find_train_plan(h->core, B, H, W, 1, workspace);
   DMD_CHECK(plp && plp->train, "denoiser_backward: no matching dmd_inner_model_forward_train on this workspace (B=%d H=%d W=%d)", B, H, W);
   Plan& pl = *plp;
   DMD_CHECK(grads_numel >= h->core.grad_total, "denoiser_backward: gradient buffer too small (%lld < %lld floats)", grads_numel, h->core.grad_total);
   DMD_CHECK(((uintptr_t)grads & 15) == 0, "denoiser_backward: gradient buffer must be 16-byte aligned");
-  return run_backward(h, pl, grad_out, grads, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int HW = H * W, C = h->cfg.img_channels;
+  if (clear_backward(h->core, pl, grads, st)) return 1;
+  // loss scale from the incoming gradient, then the scaled NHWC gradient of the model output
+  if (loss_scale_launch(grad_out, (long long)B * C * HW, pl.amax, pl.scale, st)) return 1;
+  nchw_to_nhwc_scaled_kernel<<<dim3((HW + 255) / 256, B), 256, 0, st>>>(grad_out, pl.gF, pl.scale, C, 8, HW);
+  DMD_LAUNCH_OK();
+  return run_backward(h->core, pl, grads, st);
 }
 
 // ---------------------------------------------------------------------------------------------- sampler
@@ -2367,14 +2432,15 @@ extern "C" int dmd_lambda_returns(const float* rew, const int64_t* end, const in
 namespace {
 
 __global__ void pack_rew_end_input_kernel(const float* __restrict__ obs, const float* __restrict__ next_obs, const int64_t* __restrict__ act,
-                                          const float* __restrict__ act_emb, float* __restrict__ xin, float* __restrict__ cond, int b, int t,
-                                          int C, int CP, int HW, int CC, int num_actions) {
-  // row r = k * b + n (time-major)  <-  obs[n][k], next_obs[n][k], act[n][k]
+                                          const float* __restrict__ act_emb, float* __restrict__ xin, float* __restrict__ cond,
+                                          int64_t* __restrict__ act_tm, int b, int t, int C, int CP, int HW, int CC, int num_actions) {
+  // row r = k * b + n (time-major)  <-  obs[n][k], next_obs[n][k], act[n][k]; act_tm (optional) [r] <- act[n][k]
   const int r = blockIdx.y, k = r / b, n = r - k * b;
   const size_t src = ((size_t)n * t + k) * C * HW;
   const int pix = blockIdx.x * blockDim.x + threadIdx.x;
   if (blockIdx.x == 0) {
     long long a = act[(size_t)n * t + k];
+    if (act_tm && threadIdx.x == 0) act_tm[r] = a;
     a = a < 0 ? 0 : (a >= num_actions ? num_actions - 1 : a);
     for (int j = threadIdx.x; j < CC; j += blockDim.x) cond[(size_t)r * CC + j] = act_emb[(size_t)a * CC + j];
   }
@@ -2395,6 +2461,15 @@ __global__ void split_logits_kernel(const float* __restrict__ tm, float* __restr
   const float* s = tm + ((size_t)k * b + n) * 5;
   rew[(size_t)i * 3] = s[0]; rew[(size_t)i * 3 + 1] = s[1]; rew[(size_t)i * 3 + 2] = s[2];
   end[(size_t)i * 2] = s[3]; end[(size_t)i * 2 + 1] = s[4];
+}
+// the adjoint of split_logits_kernel: g_rew [b][t][3], g_end [b][t][2] -> time-major [t*b][5]
+__global__ void merge_logits_kernel(const float* __restrict__ g_rew, const float* __restrict__ g_end, float* __restrict__ tm, int b, int t) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= b * t) return;
+  const int n = i / t, k = i - n * t;
+  float* d = tm + ((size_t)k * b + n) * 5;
+  d[0] = g_rew[(size_t)i * 3]; d[1] = g_rew[(size_t)i * 3 + 1]; d[2] = g_rew[(size_t)i * 3 + 2];
+  d[3] = g_end[(size_t)i * 2]; d[4] = g_end[(size_t)i * 2 + 1];
 }
 
 // the encoder plan for B rows on the workspace at base (a first pass on null bases sizes the statistics region), then the LSTM /
@@ -2418,6 +2493,89 @@ int rew_end_layout(const dmd_rew_end* h, int B, uint8_t* base, RewEndLayout* o, 
   o->logits_tm = (float*)bb.take((size_t)B * 5 * 4);
   o->hc[0] = (float*)bb.take((size_t)B * D * 4); o->hc[1] = (float*)bb.take((size_t)B * D * 4);
   if (total) *total = stats_bytes + bb.off + 512;
+  return 0;
+}
+
+// training workspace of b segments x t steps: the encoder plan with its gradients and backward temporaries
+// (make_train_plan), plus the LSTM / head tape and the temporaries of their backward
+int make_rew_end_train_plan(const dmd_rew_end* h, Plan* pl, int b, int t, uint8_t* base, size_t* total) {
+  const int S = h->cfg.img_size, D = h->cfg.lstm_dim;
+  auto fwd = [h, b, t, D](PlanBuilder& pb) {
+    Plan* p = pb.pl;
+    if (pb.build_rew_end(h, &p->feat)) return 1;
+    const size_t rows = (size_t)b * t, state = (rows + b) * D * 4;
+    Bump& m = *pb.bump;
+    p->gates = (float*)m.take(rows * 4 * D * 4); p->cseq = (float*)m.take(state); p->hseq = (float*)m.take(state);
+    p->hid = (float*)m.take(rows * D * 4); p->logits_tm = (float*)m.take(rows * 5 * 4); p->act_tm = (int64_t*)m.take(rows * 8);
+    p->g_tm = (float*)m.take(rows * 5 * 4); p->g_hid = (float*)m.take(rows * D * 4); p->hpre = (float*)m.take(rows * D * 4);
+    p->g_pre = (float*)m.take(rows * D * 4); p->g_y = (float*)m.take(rows * D * 4); p->dgates = (float*)m.take(rows * 4 * D * 4);
+    p->gcs = (float*)m.take((size_t)2 * b * D * 4);
+    return 0;
+  };
+  // the encoder's output gradient is seeded by the LSTM backward; the FiLM rows read act_emb(act) directly
+  // (rew_end_model.py:51, no conditioning MLP), so the conditioning path ends in the embedding
+  auto bwd = [h](BwdBuilder& bw) {
+    bw.begin();
+    bw.ginit[bw.pl->feat.gid] = 1;
+    if (bw.walk((int)bw.pl->tape.size())) return 1;
+    bw.film_tail();
+    bw.embedding(bw.pl->dcond, h->i_actemb, 1, h->cfg.num_actions);
+    return bw.err;
+  };
+  return make_train_plan(h->core, widest_channels(h->cfg), 0, pl, b * t, S, S, t, base, total, fwd, bwd);
+}
+
+// the encoder over the b * t time-major rows of pl: inputs, action embedding (act_tm, optional: a time-major copy of the
+// actions), all FiLM rows, then the plan's ops
+int rew_end_encode(const dmd_rew_end* h, Plan& pl, int b, int t, const float* obs, const float* next_obs, const int64_t* act,
+                   int64_t* act_tm, cudaStream_t st) {
+  const ModelCore& m = h->core;
+  const dmd_rew_end_config& c = h->cfg;
+  const int rows = b * t, HW = c.img_size * c.img_size;
+  DMD_CUDA(cudaMemsetAsync(pl.stats, 0, pl.stats_bytes, st));
+  pack_rew_end_input_kernel<<<dim3((HW + 255) / 256, rows), 256, 0, st>>>(obs, next_obs, act, m.ptrs[h->i_actemb], pl.xin, pl.cond, act_tm,
+                                                                          b, t, c.img_channels, pl.CP_in, HW, c.cond_channels, c.num_actions);
+  DMD_LAUNCH_OK();
+  if (linear_launch(pl.cond, (const float*)(m.packed + m.film_w_off), (const float*)(m.packed + m.film_b_off), pl.film,
+                    rows, c.cond_channels, m.film_rows, 0, st)) return 1;
+  for (const Op& op : pl.ops) {
+    if (op.kind == OP_CONV) { if (conv_launch(op.conv, op.smem, op.cols, st)) return 1; }
+    else if (op.kind == OP_PREP) { if (prep_launch(op.prep, op.prep_nsrc, st)) return 1; }
+    else { if (attn_launch(op.attn, pl.B, st)) return 1; }
+  }
+  return 0;
+}
+
+// LSTM over time (torch.nn.LSTM, gate order i f g o), rows of step k are the contiguous block [k*b, (k+1)*b).  gates: one
+// [b][4D] buffer for every step, or (keep_gates) [t][b][4D]; y [t][b][D] receives h_1 ... h_t; c_seq [t][b][D] receives
+// c_1 ... c_t, or (NULL) every step updates c_last in place
+int rew_end_lstm(const dmd_rew_end* h, int b, int t, const float* feat, float* gates, bool keep_gates, const float* h0, const float* c0,
+                 float* y, float* c_seq, float* c_last, cudaStream_t st) {
+  const ModelCore& m = h->core;
+  const int D = h->cfg.lstm_dim, K = h->feat_c * h->feat_hw;
+  const float* hprev = h0; const float* cprev = c0;
+  for (int k = 0; k < t; ++k) {
+    const float* xk = feat + (size_t)k * b * K;
+    float* gk = keep_gates ? gates + (size_t)k * b * 4 * D : gates;
+    if (linear_launch(xk, m.ptrs[h->i_wih], m.ptrs[h->i_bih], gk, b, K, 4 * D, 0, st, 0, h->feat_hw)) return 1;
+    if (linear_launch(hprev, m.ptrs[h->i_whh], m.ptrs[h->i_bhh], gk, b, D, 4 * D, 0, st, 1, 0)) return 1;
+    float* hk = y + (size_t)k * b * D;   // y rows of step k (time-major); also the next step's h
+    float* ck = c_seq ? c_seq + (size_t)k * b * D : c_last;
+    if (lstm_gates_launch(gk, cprev, hk, ck, b, D, st)) return 1;
+    hprev = hk; cprev = ck;
+  }
+  return 0;
+}
+
+// head: Linear(D, D) + SiLU + Linear(D, 5, bias=False) over all rows, then the split into (b, t, 3) and (b, t, 2)
+int rew_end_head(const dmd_rew_end* h, int b, int t, const float* y, float* hid, float* logits_tm, float* logits_rew, float* logits_end,
+                 cudaStream_t st) {
+  const ModelCore& m = h->core;
+  const int rows = b * t, D = h->cfg.lstm_dim;
+  if (linear_launch(y, m.ptrs[h->i_h0w], m.ptrs[h->i_h0b], hid, rows, D, D, 1, st)) return 1;
+  if (linear_launch(hid, m.ptrs[h->i_h2w], nullptr, logits_tm, rows, D, 5, 0, st)) return 1;
+  split_logits_kernel<<<(rows + 127) / 128, 128, 0, st>>>(logits_tm, logits_rew, logits_end, b, t);
+  DMD_LAUNCH_OK();
   return 0;
 }
 
@@ -2464,7 +2622,7 @@ extern "C" int dmd_rew_end_set_weights(dmd_rew_end* h, const float* const* ptrs_
   cudaStream_t st = (cudaStream_t)stream;
   bool moved = false;
   if (h->core.set_weights("RewEndModel", ptrs_host, n_ptrs, packed, &moved)) return 1;
-  if (moved) h->lay.plan.B = 0;   // the plan bakes parameter and packed-weight addresses in
+  if (moved) { h->lay.plan.B = 0; h->core.tplans.clear(); }   // plans bake parameter and packed-weight addresses in
   const ModelCore& m = h->core;
   if (pack_one(m, h->conv_in, st)) return 1;
   for (auto& lv : h->blocks) for (auto& r : lv) if (pack_rb(m, r, st)) return 1;
@@ -2489,7 +2647,7 @@ extern "C" int dmd_rew_end_predict(dmd_rew_end* h, int b, int t, const float* ob
   DMD_CHECK(((uintptr_t)workspace & 255) == 0, "rew_end predict: workspace must be 256-byte aligned");
   const dmd_rew_end_config& c = h->cfg;
   cudaStream_t st = (cudaStream_t)stream;
-  const int rows = b * t, S = c.img_size, HW = S * S, D = c.lstm_dim, CC = c.cond_channels;
+  const int rows = b * t, D = c.lstm_dim;
   RewEndLayout& o = h->lay;
   Plan& pl = o.plan;
   if (pl.B != rows || pl.base != (uint8_t*)workspace) {
@@ -2499,35 +2657,110 @@ extern "C" int dmd_rew_end_predict(dmd_rew_end* h, int b, int t, const float* ob
     DMD_CHECK(workspace_bytes >= need, "rew_end predict: workspace too small (%zu < %zu)", workspace_bytes, need);
     if (rew_end_layout(h, rows, (uint8_t*)workspace, &o, nullptr)) { pl.B = 0; pl.base = nullptr; pl.ops.clear(); return 1; }
   }
-  DMD_CUDA(cudaMemsetAsync(pl.stats, 0, pl.stats_bytes, st));
-  pack_rew_end_input_kernel<<<dim3((HW + 255) / 256, rows), 256, 0, st>>>(obs, next_obs, act, m.ptrs[h->i_actemb], pl.xin, pl.cond, b, t,
-                                                                          c.img_channels, pl.CP_in, HW, CC, c.num_actions);
-  DMD_LAUNCH_OK();
-  if (linear_launch(pl.cond, (const float*)(m.packed + m.film_w_off), (const float*)(m.packed + m.film_b_off), pl.film,
-                    rows, CC, m.film_rows, 0, st)) return 1;
-  for (const Op& op : pl.ops) {
-    if (op.kind == OP_CONV) { if (conv_launch(op.conv, op.smem, op.cols, st)) return 1; }
-    else if (op.kind == OP_PREP) { if (prep_launch(op.prep, op.prep_nsrc, st)) return 1; }
-    else { if (attn_launch(op.attn, pl.B, st)) return 1; }
-  }
-  // LSTM over time (torch.nn.LSTM, gate order i f g o), rows of step k are the contiguous block [k*b, (k+1)*b)
-  const int K = h->feat_c * h->feat_hw;
+  if (rew_end_encode(h, pl, b, t, obs, next_obs, act, nullptr, st)) return 1;
   const float* hprev = hx_in; const float* cprev = cx_in;
   if (!hx_in) { DMD_CUDA(cudaMemsetAsync(o.hc[0], 0, (size_t)b * D * 4, st)); hprev = o.hc[0]; }
   if (!cx_in) { DMD_CUDA(cudaMemsetAsync(o.hc[1], 0, (size_t)b * D * 4, st)); cprev = o.hc[1]; }
-  for (int k = 0; k < t; ++k) {
-    const float* xk = o.feat.data + (size_t)k * b * K;
-    if (linear_launch(xk, m.ptrs[h->i_wih], m.ptrs[h->i_bih], o.x_gates, b, K, 4 * D, 0, st, 0, h->feat_hw)) return 1;
-    if (linear_launch(hprev, m.ptrs[h->i_whh], m.ptrs[h->i_bhh], o.x_gates, b, D, 4 * D, 0, st, 1, 0)) return 1;
-    float* hk = o.y + (size_t)k * b * D;   // y rows of step k (time-major); also the next step's h
-    if (lstm_gates_launch(o.x_gates, cprev, hk, cx_out, b, D, st)) return 1;
-    hprev = hk; cprev = cx_out;
-  }
-  DMD_CUDA(cudaMemcpyAsync(hx_out, hprev, (size_t)b * D * 4, cudaMemcpyDeviceToDevice, st));
-  // head: Linear(D, D) + SiLU + Linear(D, 5, bias=False) over all (t b) rows
-  if (linear_launch(o.y, m.ptrs[h->i_h0w], m.ptrs[h->i_h0b], o.hid, rows, D, D, 1, st)) return 1;
-  if (linear_launch(o.hid, m.ptrs[h->i_h2w], nullptr, o.logits_tm, rows, D, 5, 0, st)) return 1;
-  split_logits_kernel<<<(rows + 127) / 128, 128, 0, st>>>(o.logits_tm, logits_rew, logits_end, b, t);
+  if (rew_end_lstm(h, b, t, o.feat.data, o.x_gates, false, hprev, cprev, o.y, nullptr, cx_out, st)) return 1;
+  DMD_CUDA(cudaMemcpyAsync(hx_out, o.y + (size_t)(t - 1) * b * D, (size_t)b * D * 4, cudaMemcpyDeviceToDevice, st));
+  return rew_end_head(h, b, t, o.y, o.hid, o.logits_tm, logits_rew, logits_end, st);
+}
+
+// ---------------------------------------------------------------------------------------------- reward / termination training
+// RewEndModel.forward (rew_end_model.py:57-90) under autograd: dmd_rew_end_forward_train is dmd_rew_end_predict that keeps the
+// encoder's activations, every LSTM step's gates and states and the head's hidden layer in a training workspace;
+// dmd_rew_end_backward runs the head and the LSTM (BPTT) backward, then the encoder's backward op list (BwdBuilder, shared
+// with the denoiser) and the FiLM / action-embedding tail.
+extern "C" size_t dmd_rew_end_train_workspace_bytes(const dmd_rew_end* h, int b, int t) {
+  if (!h || b <= 0 || t <= 0) { fail("rew_end_train_workspace_bytes: bad arguments"); return 0; }
+  Plan tmp; size_t need = 0;
+  if (make_rew_end_train_plan(h, &tmp, b, t, nullptr, &need)) return 0;
+  return need;
+}
+extern "C" long long dmd_rew_end_grad_layout(const dmd_rew_end* h, long long* offsets, long long* numels, int n) {
+  return grad_layout(h ? &h->core : nullptr, offsets, numels, n);
+}
+
+extern "C" int dmd_rew_end_forward_train(dmd_rew_end* h, int b, int t, const float* obs, const float* next_obs, const int64_t* act,
+                                         const float* hx_in, const float* cx_in, float* logits_rew, float* logits_end, float* hx_out,
+                                         float* cx_out, void* workspace, size_t workspace_bytes, void* stream) {
+  DMD_CHECK(h && obs && next_obs && act && logits_rew && logits_end && hx_out && cx_out && workspace, "rew_end forward_train: null argument");
+  DMD_CHECK(b > 0 && t > 0, "rew_end forward_train: bad shape b=%d t=%d", b, t);
+  const int S = h->cfg.img_size, D = h->cfg.lstm_dim;
+  cudaStream_t st = (cudaStream_t)stream;
+  Plan* pl = nullptr;
+  auto make = [h, b, t](Plan* p, uint8_t* base, size_t* total) { return make_rew_end_train_plan(h, p, b, t, base, total); };
+  if (ensure_train_plan(h->core, "rew_end", b * t, S, S, t, workspace, workspace_bytes, st, make, &pl)) return 1;
+  pl->t_act = pl->act_tm;
+  if (rew_end_encode(h, *pl, b, t, obs, next_obs, act, pl->act_tm, st)) return 1;
+  // hseq = [h_in; y], cseq = [c_in; c_1 ... c_t]
+  const size_t state = (size_t)b * D * 4;
+  if (hx_in) DMD_CUDA(cudaMemcpyAsync(pl->hseq, hx_in, state, cudaMemcpyDeviceToDevice, st)); else DMD_CUDA(cudaMemsetAsync(pl->hseq, 0, state, st));
+  if (cx_in) DMD_CUDA(cudaMemcpyAsync(pl->cseq, cx_in, state, cudaMemcpyDeviceToDevice, st)); else DMD_CUDA(cudaMemsetAsync(pl->cseq, 0, state, st));
+  float* y = pl->hseq + (size_t)b * D;
+  if (rew_end_lstm(h, b, t, pl->feat.data, pl->gates, true, pl->hseq, pl->cseq, y, pl->cseq + (size_t)b * D, nullptr, st)) return 1;
+  DMD_CUDA(cudaMemcpyAsync(hx_out, pl->hseq + (size_t)t * b * D, state, cudaMemcpyDeviceToDevice, st));
+  DMD_CUDA(cudaMemcpyAsync(cx_out, pl->cseq + (size_t)t * b * D, state, cudaMemcpyDeviceToDevice, st));
+  return rew_end_head(h, b, t, y, pl->hid, pl->logits_tm, logits_rew, logits_end, st);
+}
+
+extern "C" int dmd_rew_end_backward(dmd_rew_end* h, int b, int t, const float* g_logits_rew, const float* g_logits_end,
+                                    const float* g_hx_out, const float* g_cx_out, float* grads, long long grads_numel,
+                                    float* g_hx_in, float* g_cx_in, void* workspace, void* stream) {
+  DMD_CHECK(h && g_logits_rew && g_logits_end && grads && workspace, "rew_end backward: null argument");
+  const dmd_rew_end_config& c = h->cfg;
+  Plan* plp = (b > 0 && t > 0) ? find_train_plan(h->core, b * t, c.img_size, c.img_size, t, workspace) : nullptr;
+  DMD_CHECK(plp && plp->train, "rew_end backward: no matching dmd_rew_end_forward_train on this workspace (b=%d t=%d)", b, t);
+  const ModelCore& m = h->core;
+  DMD_CHECK(grads_numel >= m.grad_total, "rew_end backward: gradient buffer too small (%lld < %lld floats)", grads_numel, m.grad_total);
+  DMD_CHECK(((uintptr_t)grads & 15) == 0, "rew_end backward: gradient buffer must be 16-byte aligned");
+  Plan& pl = *plp;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int rows = b * t, D = c.lstm_dim, K = h->feat_c * h->feat_hw;
+  auto G = [&](int idx) { return grads + m.goff[idx]; };
+  auto sgemm = [&](const float* Am, long long sam, long long sak, const float* Bm, long long sbk, long long sbn, float* C, long long ldc,
+                   int M, int N, int Kd, int acc) -> int {
+    return sgemm_launch(Am, sam, sak, Bm, sbk, sbn, C, ldc, M, N, Kd, nullptr, acc, 0, nullptr, st);
+  };
+  if (clear_backward(m, pl, grads, st)) return 1;
+  // ---- head (rew_end_model.py:54): logits = W2 silu(W0 y + b0); these gradients are fp32 and unscaled
+  const float* y = pl.hseq + (size_t)b * D;
+  merge_logits_kernel<<<(rows + 127) / 128, 128, 0, st>>>(g_logits_rew, g_logits_end, pl.g_tm, b, t);
   DMD_LAUNCH_OK();
-  return 0;
+  if (sgemm(pl.g_tm, 1, 5, pl.hid, D, 1, G(h->i_h2w), D, 5, D, rows, 1)) return 1;                // dW2 += g^T hid
+  if (sgemm(pl.g_tm, 5, 1, m.ptrs[h->i_h2w], D, 1, pl.g_hid, D, rows, D, 5, 0)) return 1;          // g_hid = g W2
+  if (linear_launch(y, m.ptrs[h->i_h0w], m.ptrs[h->i_h0b], pl.hpre, rows, D, D, 0, st)) return 1;  // the forward's pre-activation
+  if (dsilu_mul_launch(pl.hpre, pl.g_hid, pl.g_pre, (long long)rows * D, st)) return 1;
+  if (sgemm(pl.g_pre, 1, D, y, D, 1, G(h->i_h0w), D, D, D, rows, 1)) return 1;                    // dW0 += g_pre^T y
+  if (colsum_launch(pl.g_pre, G(h->i_h0b), nullptr, nullptr, rows, D, D, st)) return 1;
+  if (sgemm(pl.g_pre, D, 1, m.ptrs[h->i_h0w], D, 1, pl.g_y, D, rows, D, D, 0)) return 1;          // g_y = g_pre W0
+  // ---- LSTM (rew_end_model.py:53), back through time: g_h of step k = g_y[k] (+ g_hx_out at the last step) + dgates_{k+1} W_hh
+  const float* Whh = m.ptrs[h->i_whh];
+  if (g_hx_out) {   // g_y[t-1] += g_hx_out (a one-way split-K reduce)
+    const long long n = (long long)b * D;
+    splitk_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(g_hx_out, 1, n, pl.g_y + (size_t)(t - 1) * b * D, nullptr, 1);
+    DMD_LAUNCH_OK();
+  }
+  for (int k = t - 1; k >= 0; --k) {
+    const size_t r0 = (size_t)k * b;
+    const float* g_c = k == t - 1 ? g_cx_out : pl.gcs + (size_t)((k + 1) & 1) * b * D;
+    float* g_c_in = (k == 0 && g_cx_in) ? g_cx_in : pl.gcs + (size_t)(k & 1) * b * D;
+    float* dg = pl.dgates + r0 * 4 * D;
+    if (lstm_cell_bwd_launch(pl.gates + r0 * 4 * D, pl.cseq + r0 * D, pl.g_y + r0 * D, g_c, dg, g_c_in, b, D, st)) return 1;
+    if (k > 0) { if (sgemm(dg, 4 * D, 1, Whh, D, 1, pl.g_y + (r0 - b) * D, D, b, D, 4 * D, 1)) return 1; }   // g_y[k-1] += dgates_k W_hh
+    else if (g_hx_in && sgemm(dg, 4 * D, 1, Whh, D, 1, g_hx_in, D, b, D, 4 * D, 0)) return 1;                  // g_hx_in = dgates_0 W_hh
+  }
+  // input / recurrent weights over all t*b rows at once; x: the NCHW flatten of the features (rew_end_model.py:52)
+  float* x_flat = pl.tB;
+  float* g_x = pl.tC;
+  if (dmd_nhwc_to_nchw(pl.feat.data, x_flat, rows, h->feat_c, h->feat_c, h->feat_hw, st)) return 1;
+  if (sgemm(pl.dgates, 1, 4 * D, x_flat, K, 1, G(h->i_wih), K, 4 * D, K, rows, 1)) return 1;     // dW_ih += dgates^T x
+  if (sgemm(pl.dgates, 1, 4 * D, pl.hseq, D, 1, G(h->i_whh), D, 4 * D, D, rows, 1)) return 1;    // dW_hh += dgates^T [h_in; y[:-1]]
+  if (colsum_launch(pl.dgates, G(h->i_bih), G(h->i_bhh), nullptr, rows, 4 * D, 4 * D, st)) return 1;
+  if (sgemm(pl.dgates, 4 * D, 1, m.ptrs[h->i_wih], K, 1, g_x, K, rows, K, 4 * D, 0)) return 1;   // g_x = dgates W_ih
+  // ---- encoder: the feature gradient enters the fp16 tensor-core path with a loss scale, NHWC in the last tensor's gradient
+  if (loss_scale_launch(g_x, (long long)rows * K, pl.amax, pl.scale, st)) return 1;
+  nchw_to_nhwc_scaled_kernel<<<dim3((h->feat_hw + 255) / 256, rows), 256, 0, st>>>(g_x, pl.feat.grad, pl.scale, h->feat_c, h->feat_c, h->feat_hw);
+  DMD_LAUNCH_OK();
+  return run_backward(m, pl, grads, st);
 }

@@ -1,16 +1,20 @@
-"""RewEndModel (reference: src/models/rew_end_model.py) with a native sm_90a `predict_rew_end` (SURVEY.md 8 f1).
+"""RewEndModel (reference: src/models/rew_end_model.py) with native sm_90a inference and training (SURVEY.md 8 f1, f2).
 
 The reward / termination model runs once per imagined step between the sampler and the policy (world_model_env.py:97) and
 over the burn-in frames of every fresh episode (:120-129).  Parameters live under the reference's names (state_dict keys,
 `Agent.load`, `configure_opt`'s isinstance split keep working); the arithmetic — encoder ResBlocks at C = 32 with FiLM on
 the action embedding, two attention blocks, LSTM over time, SiLU head — runs in `dmd_rew_end_predict`.
-Training of this model (`forward`, rew_end_model.py:57-90) is the next row (f2) and is not built."""
+Training (`forward`, rew_end_model.py:57-90) keeps the reference's host logic and loss in torch; with gradients enabled,
+`predict_rew_end` is one autograd node whose forward is `dmd_rew_end_forward_train` and whose backward is
+`dmd_rew_end_backward` (BPTT through the LSTM, the encoder on the denoiser's backward plan)."""
 from dataclasses import dataclass
 from typing import List, Optional, Tuple
 
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 from torch import Tensor
+from torch.autograd.function import once_differentiable
 
 from .. import _lib
 from ..utils import NativeStateMixin, init_lstm
@@ -69,10 +73,24 @@ class RewEndModel(NativeStateMixin, nn.Module):
         cc.num_actions = int(c.num_actions)
         return cc
 
-    @torch.no_grad()
+    # a training workspace holds one forward's activations until its backward has run
+    _WS_POOL_CAP = 2
+
     def predict_rew_end(self, obs: Tensor, act: Tensor, next_obs: Tensor,
                         hx_cx: Optional[Tuple[Tensor, Tensor]] = None) -> Tuple[Tensor, Tensor, Tuple[Tensor, Tensor]]:
         # rew_end_model.py:42-55.  hx_cx: each (1, b, lstm_dim) like torch.nn.LSTM
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            b = obs.size(0)
+            hx = cx = None
+            if hx_cx is not None:
+                hx, cx = hx_cx[0].reshape(b, -1), hx_cx[1].reshape(b, -1)
+            rew, end, hx_o, cx_o = _RewEndFn.apply(self, obs, act, next_obs, hx, cx, *self.parameters())
+            return rew, end, (hx_o.unsqueeze(0), cx_o.unsqueeze(0))
+        return self._predict(obs, act, next_obs, hx_cx)
+
+    @torch.no_grad()
+    def _predict(self, obs: Tensor, act: Tensor, next_obs: Tensor,
+                 hx_cx: Optional[Tuple[Tensor, Tensor]] = None) -> Tuple[Tensor, Tensor, Tuple[Tensor, Tensor]]:
         lib = _lib.lib()
         h = self._native()
         b, t, c, hh, ww = obs.shape
@@ -96,4 +114,93 @@ class RewEndModel(NativeStateMixin, nn.Module):
         return rew, end, (hx_o.unsqueeze(0), cx_o.unsqueeze(0))
 
     def forward(self, batch):  # rew_end_model.py:57-90
-        raise NotImplementedError("RewEndModel training (SURVEY.md 8 f2) is not built; predict_rew_end (f1) is native")
+        obs = batch.obs[:, :-1]
+        act = batch.act[:, :-1]
+        next_obs = batch.obs[:, 1:]
+        rew = batch.rew[:, :-1]
+        end = batch.end[:, :-1]
+        mask = batch.mask_padding[:, :-1]
+
+        # When dead, replace frame (gray padding) by true final obs; the write goes through the view into batch.obs
+        dead = end.bool().any(dim=1)
+        if dead.any():
+            final_obs = torch.stack([i["final_observation"] for i, d in zip(batch.info, dead) if d]).to(obs.device)
+            next_obs[dead, end[dead].argmax(dim=1)] = final_obs
+
+        logits_rew, logits_end, _ = self.predict_rew_end(obs, act, next_obs)
+        logits_rew = logits_rew[mask]
+        logits_end = logits_end[mask]
+        target_rew = rew[mask].sign().long().add(1)  # clipped to {-1, 0, 1}
+        target_end = end[mask]
+
+        loss_rew = F.cross_entropy(logits_rew, target_rew)
+        loss_end = F.cross_entropy(logits_end, target_end)
+        loss = loss_rew + loss_end
+
+        metrics = {
+            "loss_rew": loss_rew.detach(),
+            "loss_end": loss_end.detach(),
+            "loss_total": loss.detach(),
+            "confusion_matrix": {
+                "rew": confusion_matrix(logits_rew, target_rew, num_classes=3),
+                "end": confusion_matrix(logits_end, target_end, num_classes=2),
+            },
+        }
+        return loss, metrics
+
+
+def confusion_matrix(logits: Tensor, target: Tensor, num_classes: int) -> Tensor:
+    """torcheval.metrics.functional.multiclass_confusion_matrix for logits (N, num_classes): counts [true class, predicted
+    class] (row = target, column = argmax), int64.  This follows torcheval's documented convention; it has not been compared
+    with torcheval itself, which is not a dependency of this package."""
+    n = num_classes
+    return torch.bincount(target.long() * n + logits.detach().argmax(dim=1), minlength=n * n).view(n, n)
+
+
+class _RewEndFn(torch.autograd.Function):
+    """RewEndModel.predict_rew_end under autograd: forward = dmd_rew_end_forward_train (activations stay in the training
+    workspace), backward = dmd_rew_end_backward (all parameter gradients in one flat buffer, returned as views; the
+    gradients wrt a carried (hx, cx) when the caller's state requires them)."""
+
+    @staticmethod
+    def forward(ctx, module, obs, act, next_obs, hx, cx, *params):
+        lib = _lib.lib()
+        h = module._native()
+        b, t = obs.shape[:2]
+        D = module.cfg.lstm_dim
+        obs_, nxt_, act_ = obs.detach().float().contiguous(), next_obs.detach().float().contiguous(), act.long().contiguous()
+        hx_ = None if hx is None else hx.detach().float().contiguous()
+        cx_ = None if cx is None else cx.detach().float().contiguous()
+        rew = obs_.new_empty(b, t, 3)
+        end = obs_.new_empty(b, t, 2)
+        hx_o, cx_o = obs_.new_empty(b, D), obs_.new_empty(b, D)
+        need = lib.dmd_rew_end_train_workspace_bytes(h, b, t)
+        if need == 0:
+            raise RuntimeError("diamond_b200: " + lib.dmd_last_error().decode())
+        ws = module._acquire_ws(need)
+        _lib.check(lib.dmd_rew_end_forward_train(h, b, t, obs_.data_ptr(), nxt_.data_ptr(), act_.data_ptr(), _lib.ptr(hx_), _lib.ptr(cx_),
+                                                 rew.data_ptr(), end.data_ptr(), hx_o.data_ptr(), cx_o.data_ptr(), ws.data_ptr(),
+                                                 ws.numel(), _lib.current_stream()))
+        ctx.module, ctx.shape, ctx.ws = module, (b, t), ws
+        return rew, end, hx_o, cx_o
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_rew, g_end, g_hx, g_cx):
+        lib = _lib.lib()
+        module = ctx.module
+        h = module._native()
+        b, t = ctx.shape
+        offs, nums, total = module._grad_views_layout()
+        flat = torch.empty(total, dtype=torch.float32, device=g_rew.device)
+        g_rew, g_end = g_rew.float().contiguous(), g_end.float().contiguous()
+        g_hx = None if g_hx is None else g_hx.float().contiguous()
+        g_cx = None if g_cx is None else g_cx.float().contiguous()
+        g_hx_in = g_rew.new_empty(b, module.cfg.lstm_dim) if ctx.needs_input_grad[4] else None
+        g_cx_in = g_rew.new_empty(b, module.cfg.lstm_dim) if ctx.needs_input_grad[5] else None
+        _lib.check(lib.dmd_rew_end_backward(h, b, t, g_rew.data_ptr(), g_end.data_ptr(), _lib.ptr(g_hx), _lib.ptr(g_cx), flat.data_ptr(),
+                                            total, _lib.ptr(g_hx_in), _lib.ptr(g_cx_in), ctx.ws.data_ptr(), _lib.current_stream()))
+        grads = [flat[o:o + n].view_as(p) for o, n, p in zip(offs, nums, module.parameters())]
+        module._release_ws(ctx.ws, module._WS_POOL_CAP)
+        module.last_flat_grad = flat   # one contiguous buffer: what a data-parallel step all-reduces in a single collective
+        return (None, None, None, None, g_hx_in, g_cx_in, *grads)

@@ -429,6 +429,22 @@ int dmd_rew_end_predict(dmd_rew_end* h, int b, int t, const float* obs, const fl
                         const float* hx_in, const float* cx_in, float* logits_rew, float* logits_end, float* hx_out,
                         float* cx_out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Reward / termination training: RewEndModel.predict_rew_end under autograd (RewEndModel.forward,
+ * src/models/rew_end_model.py:57-90).  dmd_rew_end_forward_train = dmd_rew_end_predict that keeps every activation (encoder,
+ * the gates and states of every LSTM step, the head's hidden layer) in the training workspace of (b, t);
+ * dmd_rew_end_backward consumes them: given the gradients wrt (logits_rew, logits_end) and optionally (hx_out, cx_out)
+ * (NULL = zero) it writes the gradient of EVERY parameter into one flat fp32 buffer (layout: dmd_rew_end_grad_layout,
+ * state_dict order, fully written) and, when the pointers are not NULL, the gradients wrt (hx_in, cx_in).  The LSTM and head
+ * gradients are fp32; the encoder's run on the same wgmma backward as the denoiser's, under a power-of-two loss scale. */
+size_t dmd_rew_end_train_workspace_bytes(const dmd_rew_end* h, int b, int t);
+long long dmd_rew_end_grad_layout(const dmd_rew_end* h, long long* offsets, long long* numels, int n);
+int dmd_rew_end_forward_train(dmd_rew_end* h, int b, int t, const float* obs, const float* next_obs, const int64_t* act,
+                              const float* hx_in, const float* cx_in, float* logits_rew, float* logits_end, float* hx_out,
+                              float* cx_out, void* workspace, size_t workspace_bytes, void* stream);
+int dmd_rew_end_backward(dmd_rew_end* h, int b, int t, const float* g_logits_rew, const float* g_logits_end,
+                         const float* g_hx_out, const float* g_cx_out, float* grads, long long grads_numel,
+                         float* g_hx_in, float* g_cx_in, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
