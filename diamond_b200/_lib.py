@@ -99,6 +99,8 @@ SIGNATURES = {
     "dmd_conv2d_wgrad": (_i, [C.POINTER(WgradDesc), _vp]),
     "dmd_gn_stats": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "dmd_attn_fwd": (_i, [_vp] * 10 + [_i, _i, _i, _i, _f, _vp]),
+    "dmd_attn_scratch_bytes": (_sz, [_i, _i, _i]),
+    "dmd_attn_fwd_scratch": (_i, [_vp] * 10 + [_i, _i, _i, _i, _f, _vp, _sz, _vp]),
     "dmd_nchw_to_nhwc": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "dmd_nhwc_to_nchw": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "dmd_linear": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),

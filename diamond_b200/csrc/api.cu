@@ -477,10 +477,30 @@ extern "C" int dmd_gn_stats(const float* x, double* stats, int B, int HW, int C,
   return 0;
 }
 
+// scratch of the any-L attention path (q, k, v of every token); L = 64 runs in one launch without scratch
+static size_t attn_scratch_bytes(int B, int L, int C) { return L == kAttnL ? 0 : (size_t)B * L * 3 * C * sizeof(float); }
+
+// L = 64 (the 8x8 level of a 64x64 frame): one launch of attn_cluster_kernel / attn_kernel.  Any other L: attn_qkv_kernel, then
+// attn_stream_kernel, through p.scratch (attn_scratch_bytes)
 static int attn_launch(const AttnParams& p, int B, cudaStream_t st) {
-  DMD_CHECK((p.C == 64 || p.C == 32) && p.L == kAttnL && p.C % p.gs == 0 && p.gs % 8 == 0,
-            "attn: unsupported shape L=%d C=%d gs=%d (built for 8x8 = 64 tokens, C in {32, 64})", p.L, p.C, p.gs);
+  DMD_CHECK((p.C == 64 || p.C == 32) && p.L >= 1 && p.C % p.gs == 0 && p.gs % 8 == 0,
+            "attn: unsupported shape L=%d C=%d gs=%d (C in {32, 64}, groups of a multiple of 8 channels)", p.L, p.C, p.gs);
   if (init_kernels()) return 1;
+  if (p.L != kAttnL) {
+    DMD_CHECK(p.scratch && ((uintptr_t)p.scratch & 15) == 0, "attn: L=%d needs 16-byte aligned scratch of dmd_attn_scratch_bytes", p.L);
+    DMD_CHECK(B >= 1 && B <= 65535, "attn: B=%d out of range", B);
+    const dim3 grid((p.L + kAttnTile - 1) / kAttnTile, B);
+    AttnParams pa = p;
+    pa.ktrace = kt_slot("attn qkv", (int)(grid.x * grid.y), p.L);
+    if (p.C == 64) attn_qkv_kernel<64><<<grid, kAttnQkvThreads, 0, st>>>(pa);
+    else attn_qkv_kernel<32><<<grid, kAttnQkvThreads, 0, st>>>(pa);
+    DMD_LAUNCH_OK();
+    pa.ktrace = kt_slot("attn softmax", (int)(grid.x * grid.y), p.L);
+    if (p.C == 64) attn_stream_kernel<64><<<grid, kAttnSThreads, 0, st>>>(pa);
+    else attn_stream_kernel<32><<<grid, kAttnSThreads, 0, st>>>(pa);
+    DMD_LAUNCH_OK();
+    return 0;
+  }
   const size_t smem = sizeof(float) * ((size_t)p.L * (p.C + 1) * 2 + (size_t)p.L * (3 * p.C + 4));
   AttnParams pt = p;
   pt.ktrace = kt_slot("attn", B, p.C);
@@ -558,6 +578,19 @@ extern "C" int dmd_attn_fwd(const float* x, const double* stats_in, const float*
                             const float* wqkv, const float* bqkv, const float* wout, const float* bout, float* out,
                             double* out_stats, int B, int L, int C, int gs, float eps, void* stream) {
   AttnParams p{x, stats_in, gamma, beta, wqkv, bqkv, wout, bout, out, out_stats, L, C, gs, eps};
+  return attn_launch(p, B, (cudaStream_t)stream);
+}
+extern "C" size_t dmd_attn_scratch_bytes(int B, int L, int C) { return B > 0 && L > 0 && C > 0 ? attn_scratch_bytes(B, L, C) : 0; }
+extern "C" int dmd_attn_fwd_scratch(const float* x, const double* stats_in, const float* gamma, const float* beta,
+                                    const float* wqkv, const float* bqkv, const float* wout, const float* bout, float* out,
+                                    double* out_stats, int B, int L, int C, int gs, float eps, void* scratch, size_t scratch_bytes,
+                                    void* stream) {
+  DMD_CHECK(x && stats_in && gamma && beta && wqkv && bqkv && wout && bout && out && B > 0 && L > 0 && C > 0 && gs > 0,
+            "attn_fwd_scratch: bad arguments");
+  DMD_CHECK(scratch_bytes >= attn_scratch_bytes(B, L, C), "attn_fwd_scratch: scratch too small (%zu < %zu)", scratch_bytes,
+            attn_scratch_bytes(B, L, C));
+  AttnParams p{x, stats_in, gamma, beta, wqkv, bqkv, wout, bout, out, out_stats, L, C, gs, eps};
+  p.scratch = (float*)scratch;
   return attn_launch(p, B, (cudaStream_t)stream);
 }
 
@@ -1253,9 +1286,16 @@ struct PlanBuilder {
     Rec rec; rec.kind = R_RES; rec.rb = &rb; rec.x = x; rec.has_skip = skip != nullptr; if (skip) rec.skip = *skip;
     rec.t = t; rec.o = o; rec.in1 = in1; rec.in2 = in2;
     if (!rb.has_attn) { record(rec); return o; }
+    if (pl->train && H * W != kAttnL) {
+      fail("training: the attention backward (attn_bwd_kernel) is built for 8x8 = 64 tokens only; this plan has an attention block "
+           "over %dx%d = %d tokens (inference runs at any token count)", H, W, H * W);
+      err = 1;
+      return o;
+    }
     Tens a = tensor(rb.cout, H, W, true);
     Op op; op.kind = OP_ATTN;
     op.attn = AttnParams{o.data, o.stats, P(rb.an_w), P(rb.an_b), P(rb.qkv_w), P(rb.qkv_b), P(rb.op_w), P(rb.op_b), a.data, a.stats, H * W, rb.cout, o.gs, kGnEps};
+    if (H * W != kAttnL) op.attn.scratch = (float*)bump->take(attn_scratch_bytes(pl->B, H * W, rb.cout));
     pl->ops.push_back(op);
     rec.a = a;
     record(rec);

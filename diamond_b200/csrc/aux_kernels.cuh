@@ -259,6 +259,7 @@ struct AttnParams {
   int L, C, gs;
   float eps;
   long long* ktrace = nullptr;
+  float* scratch = nullptr;  // L != 64: q | k | v of every token, [B][3][C/8][L][8] (attn_qkv_kernel -> attn_stream_kernel)
 };
 
 constexpr int kAttnThreads = 512;
@@ -558,6 +559,200 @@ __global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(kAttnCThreads) attn_
         atomicAdd(p.ostats + ((size_t)n * G + g) * 2, (double)a);
         atomicAdd(p.ostats + ((size_t)n * G + g) * 2 + 1, (double)b);
       }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// SelfAttention2d over any token count L >= 1 (same math as attn_kernel, same parameter block plus p.scratch), in two launches
+// of grid (ceil(L / 32), B):
+//   attn_qkv_kernel   : 32 tokens per CTA: GroupNorm(x) from the producer's statistics, the qkv 1x1 projection into p.scratch,
+//                       head-major [B][3][C/8][L][8] (q, k, v), so that the keys of one head are contiguous
+//   attn_stream_kernel: 32 queries per CTA, all heads: K / V tiles of every head streamed through shared memory, the running
+//                       max, sum and y of each (head, query) in registers (keys past L masked), split over KS neighbouring
+//                       threads that share the running max and merge their sums with shuffles at the end; then
+//                       out_proj(y) + xn (xn recomputed from x and the statistics) and the output's GroupNorm partial sums.
+// 32 queries per CTA: at the 19x35 = 665 tokens of a 150x280 frame, 8 images give 168 CTAs for the 132 SMs.
+constexpr int kAttnTile = 32;        // tokens (queries) per CTA
+constexpr int kAttnQkvThreads = 256;
+constexpr int kAttnSThreads = 512;
+
+// (float) mean and rstd of every group of image n (as attn_kernel computes them), for the first C / gs threads
+__device__ __forceinline__ void attn_group_stats(const AttnParams& p, int n, float (*smr)[2]) {
+  const int G = p.C / p.gs;
+  if ((int)threadIdx.x < G) {
+    const double cnt = (double)p.L * p.gs;
+    const double mean = p.st_in[((size_t)n * G + threadIdx.x) * 2] / cnt;
+    double var = p.st_in[((size_t)n * G + threadIdx.x) * 2 + 1] / cnt - mean * mean;
+    var = var > 0.0 ? var : 0.0;
+    smr[threadIdx.x][0] = (float)mean;
+    smr[threadIdx.x][1] = (float)(1.0 / sqrt(var + (double)p.eps));
+  }
+}
+
+template <int C>
+__global__ void __launch_bounds__(kAttnQkvThreads) attn_qkv_kernel(const AttnParams p) {
+  constexpr int TQ = kAttnTile, C3 = 3 * C, XP = C + 1, HEADS = C / 8;
+  constexpr int NG = kAttnQkvThreads / TQ;   // 8 output groups
+  constexpr int NO = C3 / NG;                // 24 (C=64) or 12 (C=32) outputs per thread
+  __shared__ float xs[TQ * XP];
+  __shared__ float smr[8][2];
+  const int n = blockIdx.y, l0 = blockIdx.x * TQ, tid = threadIdx.x, L = p.L;
+  if (n == 0 && blockIdx.x == 0 && tid == 0) ktrace_stamp(p.ktrace);
+  attn_group_stats(p, n, smr);
+  __syncthreads();
+  const float* xg = p.x + (size_t)n * L * C;
+  for (int i = tid; i < TQ * C; i += kAttnQkvThreads) {
+    const int l = i / C, c = i - l * C;
+    const int g = c / p.gs;
+    xs[l * XP + c] = l0 + l < L ? (xg[(size_t)(l0 + l) * C + c] - smr[g][0]) * smr[g][1] * __ldg(p.gamma + c) + __ldg(p.beta + c) : 0.f;
+  }
+  __syncthreads();
+  // thread = (token l, output group og of NO outputs); a warp = 32 tokens of one og (weights broadcast)
+  const int l = tid % TQ, og = tid / TQ;
+  float acc[NO];
+#pragma unroll
+  for (int i = 0; i < NO; ++i) acc[i] = __ldg(p.bqkv + og * NO + i);
+  for (int c4 = 0; c4 < C / 4; ++c4) {
+    const float x0 = xs[l * XP + 4 * c4], x1 = xs[l * XP + 4 * c4 + 1], x2 = xs[l * XP + 4 * c4 + 2], x3 = xs[l * XP + 4 * c4 + 3];
+#pragma unroll
+    for (int i = 0; i < NO; ++i) {
+      const float4 w = __ldg(reinterpret_cast<const float4*>(p.wqkv + (size_t)(og * NO + i) * C) + c4);
+      acc[i] = fmaf(w.x, x0, acc[i]); acc[i] = fmaf(w.y, x1, acc[i]);
+      acc[i] = fmaf(w.z, x2, acc[i]); acc[i] = fmaf(w.w, x3, acc[i]);
+    }
+  }
+  if (l0 + l >= L) return;
+  float* dst = p.scratch + (size_t)n * C3 * L;
+#pragma unroll
+  for (int i = 0; i < NO; ++i) {
+    const int o = og * NO + i, part = o / C, c = o - part * C;   // row of the [3C][C] in-projection: q rows, then k, then v
+    dst[((size_t)(part * HEADS + (c >> 3)) * L + l0 + l) * 8 + (c & 7)] = acc[i];
+  }
+}
+
+template <int C>
+__global__ void __launch_bounds__(kAttnSThreads) attn_stream_kernel(const AttnParams p) {
+  constexpr int TQ = kAttnTile, XP = C + 1, HEADS = C / 8;
+  constexpr int KS = kAttnSThreads / (HEADS * TQ);   // threads per (head, query): 2 (C=64) or 4 (C=32)
+  constexpr int KPT = 32, TK = KS * KPT;             // keys per thread and per tile (64 or 128): 32 KB of K / V either way
+  __shared__ __align__(16) float kv[2 * HEADS * TK * 8];   // [k | v][head][TK][8]
+  __shared__ float ys[TQ * XP];
+  __shared__ float smr[8][2];
+  const int n = blockIdx.y, l0 = blockIdx.x * TQ, tid = threadIdx.x, L = p.L;
+  if (n == 0 && blockIdx.x == 0 && tid == 0) ktrace_stamp(p.ktrace);
+  attn_group_stats(p, n, smr);
+  const float* qkv = p.scratch + (size_t)n * 3 * C * L;
+  const int part = tid % KS, item = tid / KS;
+  const int h = item / TQ, ql = item - h * TQ;
+  float q[8];
+  {
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
+    if (l0 + ql < L) {
+      const float4* src = reinterpret_cast<const float4*>(qkv + ((size_t)h * L + l0 + ql) * 8);
+      a = __ldg(src); b = __ldg(src + 1);
+    }
+    q[0] = a.x; q[1] = a.y; q[2] = a.z; q[3] = a.w; q[4] = b.x; q[5] = b.y; q[6] = b.z; q[7] = b.w;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) q[e] *= 0.35355339059327373f;  // 1/sqrt(8)
+  }
+  float m = -INFINITY, den = 0.f;
+  float y[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  for (int j0 = 0; j0 < L; j0 += TK) {
+    __syncthreads();   // the previous tile has been consumed
+    for (int i = tid; i < 2 * HEADS * TK * 2; i += kAttnSThreads) {   // float4 units, two per key row; zeros past L
+      const int f4 = i & 1, r = i >> 1;
+      const int j = r % TK, hh = r / TK;                              // hh = k|v part * HEADS + head
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (j0 + j < L) v = __ldg(reinterpret_cast<const float4*>(qkv + ((size_t)(HEADS + hh) * L + j0 + j) * 8) + f4);
+      reinterpret_cast<float4*>(kv)[i] = v;
+    }
+    __syncthreads();
+    const float* ks = kv + h * TK * 8;
+    const float* vs = kv + (HEADS + h) * TK * 8;
+    float sc[KPT];
+    float mt = -INFINITY;
+#pragma unroll
+    for (int jj = 0; jj < KPT; ++jj) {
+      const int j = jj * KS + part;
+      const float4 k0 = *reinterpret_cast<const float4*>(ks + j * 8);
+      const float4 k1 = *reinterpret_cast<const float4*>(ks + j * 8 + 4);
+      float sj = q[0] * k0.x;
+      sj = fmaf(q[1], k0.y, sj); sj = fmaf(q[2], k0.z, sj); sj = fmaf(q[3], k0.w, sj);
+      sj = fmaf(q[4], k1.x, sj); sj = fmaf(q[5], k1.y, sj); sj = fmaf(q[6], k1.z, sj); sj = fmaf(q[7], k1.w, sj);
+      sc[jj] = j0 + j < L ? sj : -INFINITY;
+      mt = fmaxf(mt, sc[jj]);
+    }
+#pragma unroll
+    for (int s = 1; s < KS; s <<= 1) mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, s));
+    // every tile holds key j0 < L, so the new maximum is finite; on the first tile m = -inf and the correction is 0
+    const float mn = fmaxf(m, mt);
+    const float corr = expf(m - mn);
+    m = mn;
+    den *= corr;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) y[e] *= corr;
+#pragma unroll
+    for (int jj = 0; jj < KPT; ++jj) {
+      const int j = jj * KS + part;
+      const float pj = expf(sc[jj] - m);
+      den += pj;
+      const float4 v0 = *reinterpret_cast<const float4*>(vs + j * 8);
+      const float4 v1 = *reinterpret_cast<const float4*>(vs + j * 8 + 4);
+      y[0] = fmaf(pj, v0.x, y[0]); y[1] = fmaf(pj, v0.y, y[1]); y[2] = fmaf(pj, v0.z, y[2]); y[3] = fmaf(pj, v0.w, y[3]);
+      y[4] = fmaf(pj, v1.x, y[4]); y[5] = fmaf(pj, v1.y, y[5]); y[6] = fmaf(pj, v1.z, y[6]); y[7] = fmaf(pj, v1.w, y[7]);
+    }
+  }
+#pragma unroll
+  for (int s = 1; s < KS; s <<= 1) {
+    den += __shfl_xor_sync(0xffffffffu, den, s);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) y[e] += __shfl_xor_sync(0xffffffffu, y[e], s);
+  }
+  if (part == 0) {
+    const float inv = 1.0f / den;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) ys[ql * XP + h * 8 + e] = y[e] * inv;
+  }
+  __syncthreads();
+  // ---- out projection + residual on normed x; statistics.  thread = (token l, NO2 outputs); a warp = 32 tokens of one og
+  constexpr int NG = kAttnSThreads / TQ;   // 16
+  constexpr int NO2 = C / NG;              // 4 or 2 consecutive outputs: inside one GroupNorm group (gs % 8 == 0)
+  const int l = tid % TQ, og = tid / TQ;
+  float acc[NO2];
+#pragma unroll
+  for (int i = 0; i < NO2; ++i) acc[i] = __ldg(p.bout + og * NO2 + i);
+  for (int c4 = 0; c4 < C / 4; ++c4) {
+    const float y0 = ys[l * XP + 4 * c4], y1 = ys[l * XP + 4 * c4 + 1], y2 = ys[l * XP + 4 * c4 + 2], y3 = ys[l * XP + 4 * c4 + 3];
+#pragma unroll
+    for (int i = 0; i < NO2; ++i) {
+      const float4 w = __ldg(reinterpret_cast<const float4*>(p.wout + (size_t)(og * NO2 + i) * C) + c4);
+      acc[i] = fmaf(w.x, y0, acc[i]); acc[i] = fmaf(w.y, y1, acc[i]);
+      acc[i] = fmaf(w.z, y2, acc[i]); acc[i] = fmaf(w.w, y3, acc[i]);
+    }
+  }
+  float a = 0.f, b = 0.f;
+  if (l0 + l < L) {
+    const size_t row = ((size_t)n * L + l0 + l) * C + og * NO2;
+#pragma unroll
+    for (int i = 0; i < NO2; ++i) {
+      const int c = og * NO2 + i, g = c / p.gs;
+      const float xn = (p.x[row + i] - smr[g][0]) * smr[g][1] * __ldg(p.gamma + c) + __ldg(p.beta + c);
+      const float v = xn + acc[i];
+      p.out[row + i] = v;
+      a += v; b += v * v;
+    }
+  }
+  if (p.ostats) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      a += __shfl_xor_sync(0xffffffffu, a, off);
+      b += __shfl_xor_sync(0xffffffffu, b, off);
+    }
+    if ((tid & 31) == 0) {
+      const int G = C / p.gs, g = (og * NO2) / p.gs;
+      atomicAdd(p.ostats + ((size_t)n * G + g) * 2, (double)a);
+      atomicAdd(p.ostats + ((size_t)n * G + g) * 2 + 1, (double)b);
     }
   }
 }

@@ -164,10 +164,19 @@ int dmd_prep_plan(const dmd_prep_desc* d, int* blocks, int* pos_per_block, int* 
 /* GroupNorm partial sums of an NHWC tensor: stats[n][g] += (sum, sumsq) (blocks.py:28,43). */
 int dmd_gn_stats(const float* x, double* stats, int B, int HW, int C, int gs, void* stream);
 
-/* SelfAttention2d.forward (blocks.py:62-72), L = H*W <= 64 tokens, C <= 64, head_dim 8. */
+/* SelfAttention2d.forward (blocks.py:62-72), L = H*W = 64 tokens, C in {32, 64}, head_dim 8, groups of gs channels (gs a
+ * multiple of 8 dividing C): out = xn + out_proj(softmax(q k^T / sqrt(8)) v) with xn = GroupNorm(x) from the producer's
+ * statistics stats_in [B][C/gs][2]; out_stats (or NULL) [B][C/gs][2] += (sum, sumsq) of out. */
 int dmd_attn_fwd(const float* x, const double* stats_in, const float* gamma, const float* beta, const float* wqkv,
                  const float* bqkv, const float* wout, const float* bout, float* out, double* out_stats, int B, int L,
                  int C, int gs, float eps, void* stream);
+/* dmd_attn_fwd at any token count L >= 1 (the executors' attention op).  L = 64 runs the same single launch as dmd_attn_fwd
+ * and needs no scratch; any other L runs a qkv-projection kernel and a streaming-softmax kernel through `scratch`, device
+ * memory of at least dmd_attn_scratch_bytes(B, L, C) bytes, 16-byte aligned. */
+size_t dmd_attn_scratch_bytes(int B, int L, int C);
+int dmd_attn_fwd_scratch(const float* x, const double* stats_in, const float* gamma, const float* beta, const float* wqkv,
+                         const float* bqkv, const float* wout, const float* bout, float* out, double* out_stats, int B, int L,
+                         int C, int gs, float eps, void* scratch, size_t scratch_bytes, void* stream);
 
 int dmd_nchw_to_nhwc(const float* in, float* out, int B, int C, int CP, int HW, void* stream);
 int dmd_nhwc_to_nchw(const float* in, float* out, int B, int C, int CP, int HW, void* stream);
@@ -296,7 +305,9 @@ int dmd_denoiser_set_weights(dmd_denoiser* h, const float* const* ptrs_host, int
 
 /* H, W need not be multiples of 2^(levels-1): like UNet.forward (blocks.py:225-229,245) the executor zero-pads the conv_in
  * output at the bottom / right, runs the U-Net on the padded size and crops before norm_out / conv_out (inference entry
- * points; the training entry points reject such sizes).  The deepest level must hold 64 positions when it has attention. */
+ * points; the training entry points reject such sizes).  Attention runs over any token count at inference, and the workspace
+ * includes its scratch; the training entry points reject an attention block over other than 8x8 = 64 positions (the attention
+ * backward is built for 64 tokens only) before any launch. */
 size_t dmd_denoiser_workspace_bytes(const dmd_denoiser* h, int B, int H, int W);
 
 /* One Denoiser.denoise / compute_model_output call.  noisy (B,C,H,W), sigma (B) or (1), obs (B,T*C,H,W),
