@@ -80,6 +80,10 @@ class NormBwdDesc(C.Structure):  # dmd_norm_bwd_desc
 _ll = C.c_longlong
 
 
+class OptimTensor(C.Structure):  # dmd_optim_tensor
+    _fields_ = [("param", _vp), ("grad", _vp), ("exp_avg", _vp), ("exp_avg_sq", _vp), ("numel", _ll), ("weight_decay", C.c_double)]
+
+
 # name -> (restype, argtypes); this table is also what tests use to check that every symbol is exported
 SIGNATURES = {
     "dmd_version": (_i, []),
@@ -157,6 +161,9 @@ SIGNATURES = {
     "dmd_rew_end_forward_train": (_i, [_vp, _i, _i] + [_vp] * 9 + [_vp, _sz, _vp]),
     "dmd_rew_end_backward": (_i, [_vp, _i, _i] + [_vp] * 5 + [C.c_longlong, _vp, _vp, _vp, _vp]),
     "dmd_lambda_returns": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, C.c_double, C.c_double, _vp]),
+    "dmd_grad_norm_partial_bytes": (_sz, [C.POINTER(OptimTensor), _i]),
+    "dmd_grad_norm_clip": (_i, [C.POINTER(OptimTensor), _i, C.c_double, _i, _vp, _vp, _sz, _vp]),
+    "dmd_adamw_step": (_i, [C.POINTER(OptimTensor), _i, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, _vp]),
 }
 
 _lib: Optional[C.CDLL] = None

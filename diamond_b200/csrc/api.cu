@@ -18,6 +18,7 @@
 #include "conv_tc.cuh"
 #include "wgrad_tc.cuh"
 #include "bwd_kernels.cuh"
+#include "optim_kernels.cuh"
 
 using namespace dmd;
 
@@ -2803,4 +2804,125 @@ extern "C" int dmd_rew_end_backward(dmd_rew_end* h, int b, int t, const float* g
   nchw_to_nhwc_scaled_kernel<<<dim3((h->feat_hw + 255) / 256, rows), 256, 0, st>>>(g_x, pl.feat.grad, pl.scale, h->feat_c, h->feat_c, h->feat_hw);
   DMD_LAUNCH_OK();
   return run_backward(m, pl, grads, st);
+}
+
+// ---------------------------------------------------------------------------------------------- optimizer (optim_kernels.cuh)
+// clip_grad_norm_ + AdamW over a caller's tensor table (dmd_optim_tensor, host memory): the table is checked whole before any
+// CUDA call, then cut into launches of at most kOptMaxTensors non-empty tensors.
+
+static int optim_check_table(const dmd_optim_tensor* t, int n, bool adamw, const char* who) {
+  DMD_CHECK(t, "%s: null tensor table", who);
+  DMD_CHECK(((uintptr_t)t % alignof(dmd_optim_tensor)) == 0, "%s: misaligned tensor table (needs %d-byte alignment)", who,
+            (int)alignof(dmd_optim_tensor));
+  DMD_CHECK(n > 0, "%s: n = %d tensors (need n > 0)", who, n);
+  for (int i = 0; i < n; ++i) {
+    const dmd_optim_tensor& e = t[i];
+    DMD_CHECK(e.numel >= 0, "%s: tensor %d has negative numel %lld", who, i, e.numel);
+    DMD_CHECK(e.numel < (1ll << 40), "%s: tensor %d numel %lld too large", who, i, e.numel);
+    if (e.numel == 0) continue;
+    DMD_CHECK(e.grad, "%s: tensor %d has a null grad pointer", who, i);
+    DMD_CHECK(((uintptr_t)e.grad & 3) == 0, "%s: tensor %d grad pointer not 4-byte aligned", who, i);
+    if (!adamw) continue;
+    DMD_CHECK(e.param && e.exp_avg && e.exp_avg_sq, "%s: tensor %d has a null param / exp_avg / exp_avg_sq pointer", who, i);
+    DMD_CHECK((((uintptr_t)e.param | (uintptr_t)e.exp_avg | (uintptr_t)e.exp_avg_sq) & 3) == 0,
+              "%s: tensor %d param / exp_avg / exp_avg_sq pointer not 4-byte aligned", who, i);
+    DMD_CHECK(std::isfinite(e.weight_decay) && e.weight_decay >= 0, "%s: tensor %d weight_decay %g is not finite and >= 0", who, i,
+              e.weight_decay);
+  }
+  return 0;
+}
+
+// Splits the table into launches; for each, fills `tab` and calls launch(tab, blocks, first_block).  Returns total blocks.
+template <class F>
+static long long optim_for_each_launch(const dmd_optim_tensor* t, int n, bool adamw, double lr, OptTable& tab, F&& launch) {
+  long long total = 0;
+  int i = 0;
+  while (i < n) {
+    tab.count = 0;
+    int blocks = 0;
+    for (; i < n && tab.count < kOptMaxTensors; ++i) {
+      const dmd_optim_tensor& e = t[i];
+      if (e.numel == 0) continue;
+      const int k = tab.count++;
+      tab.p[k] = e.param; tab.g[k] = e.grad; tab.m[k] = e.exp_avg; tab.v[k] = e.exp_avg_sq;
+      tab.n[k] = e.numel;
+      tab.decay[k] = (adamw && e.weight_decay != 0) ? (float)(1.0 - lr * e.weight_decay) : 1.0f;
+      uintptr_t bits = (uintptr_t)e.grad;
+      if (adamw) bits |= (uintptr_t)e.param | (uintptr_t)e.exp_avg | (uintptr_t)e.exp_avg_sq;
+      tab.vec[k] = (bits & 15) == 0;
+      tab.block0[k] = blocks;
+      blocks += (int)((e.numel + kOptChunk - 1) / kOptChunk);
+    }
+    if (tab.count == 0) break;
+    if (launch(tab, blocks, total)) return -1;
+    total += blocks;
+  }
+  return total;
+}
+
+static long long optim_norm_blocks(const dmd_optim_tensor* t, int n) {
+  static thread_local OptTable tab;
+  return optim_for_each_launch(t, n, false, 0.0, tab, [](const OptTable&, int, long long) { return 0; });
+}
+
+extern "C" size_t dmd_grad_norm_partial_bytes(const dmd_optim_tensor* table_host, int n) {
+  if (optim_check_table(table_host, n, false, "dmd_grad_norm_partial_bytes")) return 0;
+  return (size_t)std::max(optim_norm_blocks(table_host, n), 1ll) * sizeof(double);
+}
+
+extern "C" int dmd_grad_norm_clip(const dmd_optim_tensor* table_host, int n, double max_norm, int clip, float* norm_coef,
+                                  void* partial, size_t partial_bytes, void* stream) {
+  if (optim_check_table(table_host, n, false, "dmd_grad_norm_clip")) return 1;
+  DMD_CHECK(!std::isnan(max_norm) && max_norm >= 0, "dmd_grad_norm_clip: max_norm %g is not >= 0", max_norm);
+  DMD_CHECK(norm_coef, "dmd_grad_norm_clip: null norm_coef");
+  DMD_CHECK(partial, "dmd_grad_norm_clip: null partial buffer");
+  DMD_CHECK(((uintptr_t)partial & 7) == 0, "dmd_grad_norm_clip: partial buffer not 8-byte aligned");
+  const long long blocks = optim_norm_blocks(table_host, n);
+  DMD_CHECK(partial_bytes >= (size_t)std::max(blocks, 1ll) * sizeof(double),
+            "dmd_grad_norm_clip: partial buffer too small (%zu < %zu bytes; dmd_grad_norm_partial_bytes)", partial_bytes,
+            (size_t)std::max(blocks, 1ll) * sizeof(double));
+  cudaStream_t st = (cudaStream_t)stream;
+  double* part = (double*)partial;
+  static thread_local OptTable tab;
+  auto norm = [&](const OptTable& tb, int nb, long long first) -> int {
+    grad_sqnorm_kernel<<<nb, kOptThreads, 0, st>>>(tb, part, (int)first);
+    DMD_LAUNCH_OK();
+    return 0;
+  };
+  if (optim_for_each_launch(table_host, n, false, 0.0, tab, norm) < 0) return 1;
+  grad_norm_finalize_kernel<<<1, kOptThreads, 0, st>>>(part, (int)blocks, (float)max_norm, norm_coef);
+  DMD_LAUNCH_OK();
+  if (!clip) return 0;
+  auto scale = [&](const OptTable& tb, int nb, long long) -> int {
+    grad_scale_kernel<<<nb, kOptThreads, 0, st>>>(tb, norm_coef + 1);
+    DMD_LAUNCH_OK();
+    return 0;
+  };
+  return optim_for_each_launch(table_host, n, false, 0.0, tab, scale) < 0 ? 1 : 0;
+}
+
+extern "C" int dmd_adamw_step(const dmd_optim_tensor* table_host, int n, double lr, double beta1, double beta2, double eps,
+                              double step, void* stream) {
+  if (optim_check_table(table_host, n, true, "dmd_adamw_step")) return 1;
+  DMD_CHECK(std::isfinite(lr) && lr >= 0, "dmd_adamw_step: lr %g is not finite and >= 0", lr);
+  DMD_CHECK(std::isfinite(eps) && eps >= 0, "dmd_adamw_step: eps %g is not finite and >= 0", eps);
+  DMD_CHECK(beta1 >= 0 && beta1 < 1 && beta2 >= 0 && beta2 < 1, "dmd_adamw_step: betas (%g, %g) not in [0, 1)", beta1, beta2);
+  DMD_CHECK(std::isfinite(step) && step >= 1, "dmd_adamw_step: step %g is not finite and >= 1", step);
+  // torch's Python-float arithmetic (adam.py, non-capturable branch), in double, then the fp32 values its kernels receive
+  const double bc1 = 1.0 - std::pow(beta1, step), bc2 = 1.0 - std::pow(beta2, step);
+  AdamWScalars s;
+  s.w1 = (float)(1.0 - beta1);
+  s.beta2 = (float)beta2;
+  s.omb2 = (float)(1.0 - beta2);
+  s.inv_bc2s = 1.0f / (float)std::pow(bc2, 0.5);
+  s.eps = (float)eps;
+  s.neg_step = (float)(-(lr / bc1));
+  cudaStream_t st = (cudaStream_t)stream;
+  static thread_local OptTable tab;
+  auto launch = [&](const OptTable& tb, int nb, long long) -> int {
+    adamw_kernel<<<nb, kOptThreads, 0, st>>>(tb, s);
+    DMD_LAUNCH_OK();
+    return 0;
+  };
+  return optim_for_each_launch(table_host, n, true, lr, tab, launch) < 0 ? 1 : 0;
 }

@@ -456,6 +456,33 @@ int dmd_rew_end_backward(dmd_rew_end* h, int b, int t, const float* g_logits_rew
                          const float* g_hx_out, const float* g_cx_out, float* grads, long long grads_numel,
                          float* g_hx_in, float* g_cx_in, void* workspace, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * Optimizer: torch.nn.utils.clip_grad_norm_ + torch.optim.AdamW (src/trainer.py:373-377, src/utils.py:164) over every
+ * tensor of a parameter list, one launch per kernel for up to 512 non-empty tensors (diamond_b200/optim.py).  The table is
+ * HOST memory, read at call time; every pointer in it is a device pointer to contiguous fp32 data.  Arguments are checked
+ * before any CUDA call.
+ * ------------------------------------------------------------------------------------------------------------- */
+typedef struct dmd_optim_tensor {
+  float* param;          /* AdamW only */
+  float* grad;
+  float* exp_avg;        /* AdamW only */
+  float* exp_avg_sq;     /* AdamW only */
+  long long numel;       /* >= 0; 0 = skipped */
+  double weight_decay;   /* AdamW only: the tensor's group value */
+} dmd_optim_tensor;
+/* Bytes of the fp64 per-block partial buffer dmd_grad_norm_clip needs for this table (0 on an invalid table). */
+size_t dmd_grad_norm_partial_bytes(const dmd_optim_tensor* table_host, int n);
+/* Squared 2-norm in fp64 per block, reduced in a fixed order (repeat runs are bit-identical); then norm_coef[0] = total_norm
+ * (fp32) and norm_coef[1] = min(1, max_norm / (total_norm + 1e-6)) computed as torch does (a NaN norm gives a NaN coefficient);
+ * with clip != 0 every grad is then multiplied by norm_coef[1] in place (not read or written when it is exactly 1).  No host
+ * synchronisation.  3 launches (norm, reduction, scale); clip = 0 leaves out the scale. */
+int dmd_grad_norm_clip(const dmd_optim_tensor* table_host, int n, double max_norm, int clip, float* norm_coef, void* partial,
+                       size_t partial_bytes, void* stream);
+/* One AdamW step of torch 2.11 (decoupled weight decay, amsgrad / maximize off) at step count `step` (>= 1, after the
+ * increment) for every tensor of the table; lr, betas, eps are the group's, weight decay the table entry's. */
+int dmd_adamw_step(const dmd_optim_tensor* table_host, int n, double lr, double beta1, double beta2, double eps, double step,
+                   void* stream);
+
 #ifdef __cplusplus
 }
 #endif
