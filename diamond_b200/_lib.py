@@ -80,6 +80,11 @@ class NormBwdDesc(C.Structure):  # dmd_norm_bwd_desc
 _ll = C.c_longlong
 
 
+class U8Frames(C.Structure):  # dmd_u8_frames
+    _fields_ = [("levels", _vp), ("batch_stride", _ll), ("frame_stride", _ll),
+                ("kinds", _vp), ("kind_batch_stride", _ll), ("kind_frame_stride", _ll), ("table", _vp)]
+
+
 class OptimTensor(C.Structure):  # dmd_optim_tensor
     _fields_ = [("param", _vp), ("grad", _vp), ("exp_avg", _vp), ("exp_avg_sq", _vp), ("numel", _ll), ("weight_decay", C.c_double)]
 
@@ -137,6 +142,8 @@ SIGNATURES = {
     "dmd_denoiser_grad_layout": (C.c_longlong, [_vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), _i]),
     "dmd_inner_model_forward_train": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dmd_denoiser_backward": (_i, [_vp, _i, _i, _i, _vp, _vp, C.c_longlong, _vp, _vp]),
+    "dmd_inner_model_forward_u8": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, C.POINTER(U8Frames), _vp, _vp, _vp, _sz, _vp]),
+    "dmd_inner_model_forward_train_u8": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, C.POINTER(U8Frames), _vp, _vp, _vp, _sz, _vp]),
     "dmd_sampler_sample": (_i, [_vp, C.POINTER(SamplerConfigC), _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _i, _vp]),
     "dmd_actor_critic_create": (_vp, [C.POINTER(ActorCriticConfigC)]),
     "dmd_actor_critic_destroy": (None, [_vp]),
@@ -160,6 +167,8 @@ SIGNATURES = {
     "dmd_rew_end_grad_layout": (C.c_longlong, [_vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), _i]),
     "dmd_rew_end_forward_train": (_i, [_vp, _i, _i] + [_vp] * 9 + [_vp, _sz, _vp]),
     "dmd_rew_end_backward": (_i, [_vp, _i, _i] + [_vp] * 5 + [C.c_longlong, _vp, _vp, _vp, _vp]),
+    "dmd_rew_end_predict_u8": (_i, [_vp, _i, _i, C.POINTER(U8Frames), C.POINTER(U8Frames)] + [_vp] * 7 + [_vp, _sz, _vp]),
+    "dmd_rew_end_forward_train_u8": (_i, [_vp, _i, _i, C.POINTER(U8Frames), C.POINTER(U8Frames)] + [_vp] * 7 + [_vp, _sz, _vp]),
     "dmd_lambda_returns": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, C.c_double, C.c_double, _vp]),
     "dmd_grad_norm_partial_bytes": (_sz, [C.POINTER(OptimTensor), _i]),
     "dmd_grad_norm_clip": (_i, [C.POINTER(OptimTensor), _i, C.c_double, _i, _vp, _vp, _sz, _vp]),

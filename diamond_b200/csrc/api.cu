@@ -51,6 +51,22 @@ static int fail(const char* fmt, ...) {
     if (e__ != cudaSuccess) return fail("kernel launch failed: %s (%s:%d)", cudaGetErrorString(e__), __FILE__, __LINE__); \
   } while (0)
 
+// the checks of a dmd_u8_frames argument, each named in its message; out: the kernels' copy
+static int u8_frames_arg(const char* who, const char* name, const dmd_u8_frames* f, U8Frames* out) {
+  DMD_CHECK(f, "%s: %s is NULL", who, name);
+  DMD_CHECK(f->levels, "%s: %s->levels is NULL", who, name);
+  DMD_CHECK(f->kinds, "%s: %s->kinds is NULL", who, name);
+  DMD_CHECK(f->table, "%s: %s->table is NULL", who, name);
+  DMD_CHECK(((uintptr_t)f->table & 3) == 0, "%s: %s->table is not 4-byte aligned", who, name);
+  DMD_CHECK(f->batch_stride >= 0 && f->frame_stride >= 0, "%s: %s->batch_stride / frame_stride must be >= 0 (got %lld, %lld)", who,
+            name, f->batch_stride, f->frame_stride);
+  DMD_CHECK(f->kind_batch_stride >= 0 && f->kind_frame_stride >= 0,
+            "%s: %s->kind_batch_stride / kind_frame_stride must be >= 0 (got %lld, %lld)", who, name, f->kind_batch_stride,
+            f->kind_frame_stride);
+  *out = U8Frames{f->levels, f->batch_stride, f->frame_stride, f->kinds, f->kind_batch_stride, f->kind_frame_stride, f->table};
+  return 0;
+}
+
 extern "C" int dmd_version(void) { return DMD_VERSION; }
 extern "C" const char* dmd_last_error(void) { return g_err.c_str(); }
 extern "C" long long dmd_launch_count(int reset) {
@@ -1719,14 +1735,21 @@ int make_denoiser_train_plan(const dmd_denoiser* h, Plan* pl, int B, int H, int 
 }
 
 // cond_k >= 0: the conditioning of this evaluation was computed up front by sampler_conditioning (FiLM rows at film_all + k)
+// u8 != null: the frame stack is read from uint8 frames (obs is not used)
 int run_forward(dmd_denoiser* h, Plan& pl, const float* noisy, const float* sigma, int sigma_is_scalar, const float* obs,
-                const int64_t* act, cudaStream_t st, int prescaled = 0, StackView sv = StackView{}, int cond_k = -1) {
+                const int64_t* act, cudaStream_t st, int prescaled = 0, StackView sv = StackView{}, int cond_k = -1,
+                const U8Frames* u8 = nullptr) {
   const dmd_denoiser_config& c = h->cfg;
   const int HW = pl.H * pl.W;
   DMD_CUDA(cudaMemsetAsync(pl.stats, 0, pl.stats_bytes, st));
-  pack_denoiser_input_kernel<<<dim3((HW + 255) / 256, pl.B), 256, 0, st>>>(
-      noisy, obs, sigma, sigma_is_scalar, pl.xin, pl.cs, c.num_steps_conditioning * c.img_channels, c.img_channels,
-      pl.CP_in, HW, c.sigma_data, c.sigma_offset_noise, prescaled, sv);
+  const dim3 grid((HW + 255) / 256, pl.B);
+  const int Cobs = c.num_steps_conditioning * c.img_channels;
+  if (u8)
+    pack_denoiser_input_kernel<<<grid, 256, 0, st>>>(noisy, *u8, sigma, sigma_is_scalar, pl.xin, pl.cs, Cobs, c.img_channels,
+                                                     pl.CP_in, HW, c.sigma_data, c.sigma_offset_noise, prescaled, sv);
+  else
+    pack_denoiser_input_kernel<<<grid, 256, 0, st>>>(noisy, obs, sigma, sigma_is_scalar, pl.xin, pl.cs, Cobs, c.img_channels,
+                                                     pl.CP_in, HW, c.sigma_data, c.sigma_offset_noise, prescaled, sv);
   DMD_LAUNCH_OK();
   const float* film = pl.film;
   if (cond_k >= 0) {
@@ -1861,6 +1884,28 @@ extern "C" int dmd_inner_model_forward(dmd_denoiser* h, int B, int H, int W, con
   return run_wrap(h, h->plan, noisy_rescaled, out, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1.f, 0.f, st);
 }
 
+// the arguments the two uint8 InnerModel entry points share, each named in its message
+static int inner_model_u8_args(const char* who, const dmd_denoiser* h, const float* noisy_rescaled, const float* c_noise,
+                               const dmd_u8_frames* obs, const int64_t* act, const float* out, U8Frames* u8) {
+  DMD_CHECK(h, "%s: handle is NULL", who);
+  DMD_CHECK(noisy_rescaled, "%s: noisy_rescaled is NULL", who);
+  DMD_CHECK(c_noise, "%s: c_noise is NULL", who);
+  DMD_CHECK(act, "%s: act is NULL", who);
+  DMD_CHECK(out, "%s: out is NULL", who);
+  return u8_frames_arg(who, "obs", obs, u8);
+}
+
+extern "C" int dmd_inner_model_forward_u8(dmd_denoiser* h, int B, int H, int W, const float* noisy_rescaled, const float* c_noise,
+                                          int c_noise_is_scalar, const dmd_u8_frames* obs, const int64_t* act, float* out,
+                                          void* workspace, size_t workspace_bytes, void* stream) {
+  U8Frames u8;
+  if (inner_model_u8_args("inner_model_forward_u8", h, noisy_rescaled, c_noise, obs, act, out, &u8)) return 1;
+  if (ensure_plan(h, B, H, W, workspace, workspace_bytes)) return 1;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (run_forward(h, h->plan, noisy_rescaled, c_noise, c_noise_is_scalar, nullptr, act, st, 1, StackView{}, -1, &u8)) return 1;
+  return run_wrap(h, h->plan, noisy_rescaled, out, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1.f, 0.f, st);
+}
+
 // ---------------------------------------------------------------------------------------------- training entry points
 namespace {
 
@@ -1964,6 +2009,20 @@ extern "C" int dmd_inner_model_forward_train(dmd_denoiser* h, int B, int H, int 
   if (ensure_train_plan(h->core, "denoiser", B, H, W, 1, workspace, workspace_bytes, st, make, &pl)) return 1;
   pl->t_act = act;
   if (run_forward(h, *pl, noisy_rescaled, c_noise, c_noise_is_scalar, obs_rescaled, act, st, 1)) return 1;
+  return run_wrap(h, *pl, noisy_rescaled, out, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1.f, 0.f, st);
+}
+
+extern "C" int dmd_inner_model_forward_train_u8(dmd_denoiser* h, int B, int H, int W, const float* noisy_rescaled, const float* c_noise,
+                                                int c_noise_is_scalar, const dmd_u8_frames* obs, const int64_t* act, float* out,
+                                                void* workspace, size_t workspace_bytes, void* stream) {
+  U8Frames u8;
+  if (inner_model_u8_args("inner_model_forward_train_u8", h, noisy_rescaled, c_noise, obs, act, out, &u8)) return 1;
+  cudaStream_t st = (cudaStream_t)stream;
+  Plan* pl = nullptr;
+  auto make = [h, B, H, W](Plan* p, uint8_t* base, size_t* total) { return make_denoiser_train_plan(h, p, B, H, W, base, total); };
+  if (ensure_train_plan(h->core, "denoiser", B, H, W, 1, workspace, workspace_bytes, st, make, &pl)) return 1;
+  pl->t_act = act;
+  if (run_forward(h, *pl, noisy_rescaled, c_noise, c_noise_is_scalar, nullptr, act, st, 1, StackView{}, -1, &u8)) return 1;
   return run_wrap(h, *pl, noisy_rescaled, out, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1.f, 0.f, st);
 }
 
@@ -2472,10 +2531,15 @@ extern "C" int dmd_lambda_returns(const float* rew, const int64_t* end, const in
 // (struct dmd_rew_end, next to dmd_denoiser) keeps the encoder plan of the last (rows, workspace) it ran.
 namespace {
 
-__global__ void pack_rew_end_input_kernel(const float* __restrict__ obs, const float* __restrict__ next_obs, const int64_t* __restrict__ act,
+// obs / next_obs: (b, t, C, HW) fp32 (Obs = const float*), or frames (n, k) of two U8Frames sources (Obs = U8Frames)
+template <class Obs>
+__global__ void pack_rew_end_input_kernel(const Obs obs, const Obs next_obs, const int64_t* __restrict__ act,
                                           const float* __restrict__ act_emb, float* __restrict__ xin, float* __restrict__ cond,
                                           int64_t* __restrict__ act_tm, int b, int t, int C, int CP, int HW, int CC, int num_actions) {
   // row r = k * b + n (time-major)  <-  obs[n][k], next_obs[n][k], act[n][k]; act_tm (optional) [r] <- act[n][k]
+  constexpr bool kU8 = std::is_same<Obs, U8Frames>::value;
+  [[maybe_unused]] const float* tab = nullptr;
+  if constexpr (kU8) tab = stage_decode_table(obs.table);   // both sources share one decode table (checked by the caller)
   const int r = blockIdx.y, k = r / b, n = r - k * b;
   const size_t src = ((size_t)n * t + k) * C * HW;
   const int pix = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2489,8 +2553,13 @@ __global__ void pack_rew_end_input_kernel(const float* __restrict__ obs, const f
   float* o = xin + ((size_t)r * HW + pix) * CP;
   for (int ch = 0; ch < CP; ++ch) {
     float v = 0.f;
-    if (ch < C) v = obs[src + (size_t)ch * HW + pix];
-    else if (ch < 2 * C) v = next_obs[src + (size_t)(ch - C) * HW + pix];
+    if constexpr (kU8) {
+      if (ch < C) v = u8_frame_value(obs, tab, n, k, (size_t)ch * HW + pix);
+      else if (ch < 2 * C) v = u8_frame_value(next_obs, tab, n, k, (size_t)(ch - C) * HW + pix);
+    } else {
+      if (ch < C) v = obs[src + (size_t)ch * HW + pix];
+      else if (ch < 2 * C) v = next_obs[src + (size_t)(ch - C) * HW + pix];
+    }
     o[ch] = v;
   }
 }
@@ -2567,15 +2636,20 @@ int make_rew_end_train_plan(const dmd_rew_end* h, Plan* pl, int b, int t, uint8_
 }
 
 // the encoder over the b * t time-major rows of pl: inputs, action embedding (act_tm, optional: a time-major copy of the
-// actions), all FiLM rows, then the plan's ops
+// actions), all FiLM rows, then the plan's ops.  u8 != null: u8[0] / u8[1] are the uint8 obs / next_obs (obs, next_obs unused)
 int rew_end_encode(const dmd_rew_end* h, Plan& pl, int b, int t, const float* obs, const float* next_obs, const int64_t* act,
-                   int64_t* act_tm, cudaStream_t st) {
+                   int64_t* act_tm, cudaStream_t st, const U8Frames* u8 = nullptr) {
   const ModelCore& m = h->core;
   const dmd_rew_end_config& c = h->cfg;
   const int rows = b * t, HW = c.img_size * c.img_size;
   DMD_CUDA(cudaMemsetAsync(pl.stats, 0, pl.stats_bytes, st));
-  pack_rew_end_input_kernel<<<dim3((HW + 255) / 256, rows), 256, 0, st>>>(obs, next_obs, act, m.ptrs[h->i_actemb], pl.xin, pl.cond, act_tm,
-                                                                          b, t, c.img_channels, pl.CP_in, HW, c.cond_channels, c.num_actions);
+  const dim3 grid((HW + 255) / 256, rows);
+  if (u8)
+    pack_rew_end_input_kernel<<<grid, 256, 0, st>>>(u8[0], u8[1], act, m.ptrs[h->i_actemb], pl.xin, pl.cond, act_tm,
+                                                    b, t, c.img_channels, pl.CP_in, HW, c.cond_channels, c.num_actions);
+  else
+    pack_rew_end_input_kernel<<<grid, 256, 0, st>>>(obs, next_obs, act, m.ptrs[h->i_actemb], pl.xin, pl.cond, act_tm,
+                                                    b, t, c.img_channels, pl.CP_in, HW, c.cond_channels, c.num_actions);
   DMD_LAUNCH_OK();
   if (linear_launch(pl.cond, (const float*)(m.packed + m.film_w_off), (const float*)(m.packed + m.film_b_off), pl.film,
                     rows, c.cond_channels, m.film_rows, 0, st)) return 1;
@@ -2679,10 +2753,10 @@ extern "C" size_t dmd_rew_end_workspace_bytes(const dmd_rew_end* h, int rows) {
 
 // obs / next_obs (b, t, C, S, S) fp32, act (b, t) int64, hx_in / cx_in (b, lstm_dim) or NULL (zeros).
 // Outputs: logits_rew (b, t, 3), logits_end (b, t, 2), hx_out / cx_out (b, lstm_dim).
-extern "C" int dmd_rew_end_predict(dmd_rew_end* h, int b, int t, const float* obs, const float* next_obs, const int64_t* act,
-                                   const float* hx_in, const float* cx_in, float* logits_rew, float* logits_end, float* hx_out,
-                                   float* cx_out, void* workspace, size_t workspace_bytes, void* stream) {
-  DMD_CHECK(h && obs && next_obs && act && logits_rew && logits_end && hx_out && cx_out && workspace, "rew_end predict: null argument");
+namespace {
+int rew_end_predict(dmd_rew_end* h, int b, int t, const float* obs, const float* next_obs, const U8Frames* u8, const int64_t* act,
+                    const float* hx_in, const float* cx_in, float* logits_rew, float* logits_end, float* hx_out,
+                    float* cx_out, void* workspace, size_t workspace_bytes, void* stream) {
   const ModelCore& m = h->core;
   DMD_CHECK(m.ready(), "rew_end predict: call dmd_rew_end_set_weights first");
   DMD_CHECK(((uintptr_t)workspace & 255) == 0, "rew_end predict: workspace must be 256-byte aligned");
@@ -2698,13 +2772,52 @@ extern "C" int dmd_rew_end_predict(dmd_rew_end* h, int b, int t, const float* ob
     DMD_CHECK(workspace_bytes >= need, "rew_end predict: workspace too small (%zu < %zu)", workspace_bytes, need);
     if (rew_end_layout(h, rows, (uint8_t*)workspace, &o, nullptr)) { pl.B = 0; pl.base = nullptr; pl.ops.clear(); return 1; }
   }
-  if (rew_end_encode(h, pl, b, t, obs, next_obs, act, nullptr, st)) return 1;
+  if (rew_end_encode(h, pl, b, t, obs, next_obs, act, nullptr, st, u8)) return 1;
   const float* hprev = hx_in; const float* cprev = cx_in;
   if (!hx_in) { DMD_CUDA(cudaMemsetAsync(o.hc[0], 0, (size_t)b * D * 4, st)); hprev = o.hc[0]; }
   if (!cx_in) { DMD_CUDA(cudaMemsetAsync(o.hc[1], 0, (size_t)b * D * 4, st)); cprev = o.hc[1]; }
   if (rew_end_lstm(h, b, t, o.feat.data, o.x_gates, false, hprev, cprev, o.y, nullptr, cx_out, st)) return 1;
   DMD_CUDA(cudaMemcpyAsync(hx_out, o.y + (size_t)(t - 1) * b * D, (size_t)b * D * 4, cudaMemcpyDeviceToDevice, st));
   return rew_end_head(h, b, t, o.y, o.hid, o.logits_tm, logits_rew, logits_end, st);
+}
+
+// the pointer arguments every reward / termination entry point shares, each named in its message
+int rew_end_args(const char* who, const dmd_rew_end* h, int b, int t, const int64_t* act, const float* logits_rew, const float* logits_end,
+                 const float* hx_out, const float* cx_out, const void* workspace) {
+  DMD_CHECK(h, "%s: handle is NULL", who);
+  DMD_CHECK(b > 0 && t > 0, "%s: bad shape b=%d t=%d", who, b, t);
+  DMD_CHECK(act, "%s: act is NULL", who);
+  DMD_CHECK(logits_rew && logits_end, "%s: logits_rew / logits_end is NULL", who);
+  DMD_CHECK(hx_out && cx_out, "%s: hx_out / cx_out is NULL", who);
+  DMD_CHECK(workspace, "%s: workspace is NULL", who);
+  return 0;
+}
+
+// both uint8 sources of a reward / termination call; they share one decode table
+int rew_end_u8_args(const char* who, const dmd_u8_frames* obs, const dmd_u8_frames* next_obs, U8Frames* out) {
+  if (u8_frames_arg(who, "obs", obs, &out[0]) || u8_frames_arg(who, "next_obs", next_obs, &out[1])) return 1;
+  DMD_CHECK(obs->table == next_obs->table, "%s: obs->table and next_obs->table differ (the sources share one decode table)", who);
+  return 0;
+}
+}  // namespace
+
+extern "C" int dmd_rew_end_predict(dmd_rew_end* h, int b, int t, const float* obs, const float* next_obs, const int64_t* act,
+                                   const float* hx_in, const float* cx_in, float* logits_rew, float* logits_end, float* hx_out,
+                                   float* cx_out, void* workspace, size_t workspace_bytes, void* stream) {
+  DMD_CHECK(h && obs && next_obs && act && logits_rew && logits_end && hx_out && cx_out && workspace, "rew_end predict: null argument");
+  return rew_end_predict(h, b, t, obs, next_obs, nullptr, act, hx_in, cx_in, logits_rew, logits_end, hx_out, cx_out, workspace,
+                         workspace_bytes, stream);
+}
+
+extern "C" int dmd_rew_end_predict_u8(dmd_rew_end* h, int b, int t, const dmd_u8_frames* obs, const dmd_u8_frames* next_obs,
+                                      const int64_t* act, const float* hx_in, const float* cx_in, float* logits_rew, float* logits_end,
+                                      float* hx_out, float* cx_out, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* who = "rew_end_predict_u8";
+  if (rew_end_args(who, h, b, t, act, logits_rew, logits_end, hx_out, cx_out, workspace)) return 1;
+  U8Frames u8[2];
+  if (rew_end_u8_args(who, obs, next_obs, u8)) return 1;
+  return rew_end_predict(h, b, t, nullptr, nullptr, u8, act, hx_in, cx_in, logits_rew, logits_end, hx_out, cx_out, workspace,
+                         workspace_bytes, stream);
 }
 
 // ---------------------------------------------------------------------------------------------- reward / termination training
@@ -2722,18 +2835,17 @@ extern "C" long long dmd_rew_end_grad_layout(const dmd_rew_end* h, long long* of
   return grad_layout(h ? &h->core : nullptr, offsets, numels, n);
 }
 
-extern "C" int dmd_rew_end_forward_train(dmd_rew_end* h, int b, int t, const float* obs, const float* next_obs, const int64_t* act,
-                                         const float* hx_in, const float* cx_in, float* logits_rew, float* logits_end, float* hx_out,
-                                         float* cx_out, void* workspace, size_t workspace_bytes, void* stream) {
-  DMD_CHECK(h && obs && next_obs && act && logits_rew && logits_end && hx_out && cx_out && workspace, "rew_end forward_train: null argument");
-  DMD_CHECK(b > 0 && t > 0, "rew_end forward_train: bad shape b=%d t=%d", b, t);
+namespace {
+int rew_end_forward_train(dmd_rew_end* h, int b, int t, const float* obs, const float* next_obs, const U8Frames* u8, const int64_t* act,
+                          const float* hx_in, const float* cx_in, float* logits_rew, float* logits_end, float* hx_out,
+                          float* cx_out, void* workspace, size_t workspace_bytes, void* stream) {
   const int S = h->cfg.img_size, D = h->cfg.lstm_dim;
   cudaStream_t st = (cudaStream_t)stream;
   Plan* pl = nullptr;
   auto make = [h, b, t](Plan* p, uint8_t* base, size_t* total) { return make_rew_end_train_plan(h, p, b, t, base, total); };
   if (ensure_train_plan(h->core, "rew_end", b * t, S, S, t, workspace, workspace_bytes, st, make, &pl)) return 1;
   pl->t_act = pl->act_tm;
-  if (rew_end_encode(h, *pl, b, t, obs, next_obs, act, pl->act_tm, st)) return 1;
+  if (rew_end_encode(h, *pl, b, t, obs, next_obs, act, pl->act_tm, st, u8)) return 1;
   // hseq = [h_in; y], cseq = [c_in; c_1 ... c_t]
   const size_t state = (size_t)b * D * 4;
   if (hx_in) DMD_CUDA(cudaMemcpyAsync(pl->hseq, hx_in, state, cudaMemcpyDeviceToDevice, st)); else DMD_CUDA(cudaMemsetAsync(pl->hseq, 0, state, st));
@@ -2743,6 +2855,28 @@ extern "C" int dmd_rew_end_forward_train(dmd_rew_end* h, int b, int t, const flo
   DMD_CUDA(cudaMemcpyAsync(hx_out, pl->hseq + (size_t)t * b * D, state, cudaMemcpyDeviceToDevice, st));
   DMD_CUDA(cudaMemcpyAsync(cx_out, pl->cseq + (size_t)t * b * D, state, cudaMemcpyDeviceToDevice, st));
   return rew_end_head(h, b, t, y, pl->hid, pl->logits_tm, logits_rew, logits_end, st);
+}
+}  // namespace
+
+extern "C" int dmd_rew_end_forward_train(dmd_rew_end* h, int b, int t, const float* obs, const float* next_obs, const int64_t* act,
+                                         const float* hx_in, const float* cx_in, float* logits_rew, float* logits_end, float* hx_out,
+                                         float* cx_out, void* workspace, size_t workspace_bytes, void* stream) {
+  DMD_CHECK(h && obs && next_obs && act && logits_rew && logits_end && hx_out && cx_out && workspace, "rew_end forward_train: null argument");
+  DMD_CHECK(b > 0 && t > 0, "rew_end forward_train: bad shape b=%d t=%d", b, t);
+  return rew_end_forward_train(h, b, t, obs, next_obs, nullptr, act, hx_in, cx_in, logits_rew, logits_end, hx_out, cx_out, workspace,
+                               workspace_bytes, stream);
+}
+
+extern "C" int dmd_rew_end_forward_train_u8(dmd_rew_end* h, int b, int t, const dmd_u8_frames* obs, const dmd_u8_frames* next_obs,
+                                            const int64_t* act, const float* hx_in, const float* cx_in, float* logits_rew,
+                                            float* logits_end, float* hx_out, float* cx_out, void* workspace, size_t workspace_bytes,
+                                            void* stream) {
+  const char* who = "rew_end_forward_train_u8";
+  if (rew_end_args(who, h, b, t, act, logits_rew, logits_end, hx_out, cx_out, workspace)) return 1;
+  U8Frames u8[2];
+  if (rew_end_u8_args(who, obs, next_obs, u8)) return 1;
+  return rew_end_forward_train(h, b, t, nullptr, nullptr, u8, act, hx_in, cx_in, logits_rew, logits_end, hx_out, cx_out, workspace,
+                               workspace_bytes, stream);
 }
 
 extern "C" int dmd_rew_end_backward(dmd_rew_end* h, int b, int t, const float* g_logits_rew, const float* g_logits_end,

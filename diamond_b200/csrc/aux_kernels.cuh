@@ -3,6 +3,7 @@
 // the uint8 quantiser reproduce the reference's fp32 arithmetic bit for bit where it matters (denoiser.py:66-84).
 #pragma once
 #include <cooperative_groups.h>
+#include <type_traits>
 #include "ptx.cuh"
 
 namespace dmd {
@@ -28,13 +29,42 @@ __device__ __forceinline__ float4 edm_conditioners(float sigma, float sigma_data
 // (world_model_env.py:74-75) becomes head = (head + 1) % T and no data moves.
 struct StackView { int ring_T; int head; long long frame_stride; long long batch_stride; long long act_slot_stride; long long act_batch_stride; };
 
+// Frames stored as one byte per value (dmd_u8_frames, include/diamond_b200.h).  Value (n, f, i) -- sample n, frame f, element
+// i = channel * H*W + pixel -- is table[kind * 256 + byte] with byte = levels[n * batch_stride + f * frame_stride + i] and
+// kind = kinds[n * kind_batch_stride + f * kind_frame_stride]: the table holds, per kind, the fp32 value an fp32 frame source
+// would hold for that byte (diamond_b200/frames.py builds it), so a decoded frame is bit-identical to the fp32 one.  A kind
+// outside [0, kFrameKinds) decodes as kind 0 (padding).
+constexpr int kFrameKinds = 3;
+struct U8Frames {
+  const uint8_t* levels; long long batch_stride; long long frame_stride;
+  const uint8_t* kinds; long long kind_batch_stride; long long kind_frame_stride;
+  const float* table;
+};
+// the decode table in shared memory; every thread of the block must call it (it synchronises)
+__device__ __forceinline__ const float* stage_decode_table(const float* __restrict__ table) {
+  __shared__ float tab[kFrameKinds * 256];
+  for (int i = threadIdx.x; i < kFrameKinds * 256; i += blockDim.x) tab[i] = table[i];
+  __syncthreads();
+  return tab;
+}
+__device__ __forceinline__ float u8_frame_value(const U8Frames& s, const float* tab, long long n, long long f, size_t i) {
+  unsigned kind = s.kinds[(size_t)n * s.kind_batch_stride + (size_t)f * s.kind_frame_stride];
+  if (kind >= (unsigned)kFrameKinds) kind = 0;
+  return tab[kind * 256 + s.levels[(size_t)n * s.batch_stride + (size_t)f * s.frame_stride + i]];
+}
+
 // Pack the conv_in input (inner_model.py:46 cat((obs, noisy)) after denoiser.py:75-76 rescaling) as NHWC with the
-// channel count rounded up to CP (multiple of 8; zero filled).   obs: (B, Cobs, H, W)  noisy: (B, Cimg, H, W) NCHW.
+// channel count rounded up to CP (multiple of 8; zero filled).   obs: (B, Cobs, H, W) fp32 (Obs = const float*), or the
+// Cobs / Cimg frames of a U8Frames source (Obs = U8Frames; sv is not used);  noisy: (B, Cimg, H, W) NCHW.
 // Also writes cs[n] (4 floats).  grid: (ceil(H*W/256), B)
-__global__ void pack_denoiser_input_kernel(const float* __restrict__ noisy, const float* __restrict__ obs,
+template <class Obs>
+__global__ void pack_denoiser_input_kernel(const float* __restrict__ noisy, const Obs obs,
                                            const float* __restrict__ sigma, int sigma_is_scalar, float* __restrict__ xin,
                                            float* __restrict__ cs, int Cobs, int Cimg, int CP, int HW, float sigma_data,
                                            float sigma_offset, int prescaled, StackView sv) {
+  constexpr bool kU8 = std::is_same<Obs, U8Frames>::value;
+  [[maybe_unused]] const float* tab = nullptr;
+  if constexpr (kU8) tab = stage_decode_table(obs.table);
   const int n = blockIdx.y;
   const float sg = sigma[sigma_is_scalar ? 0 : n];
   // prescaled: caller already applied denoiser.py:75-76 and `sigma` holds c_noise (InnerModel.forward surface)
@@ -46,7 +76,10 @@ __global__ void pack_denoiser_input_kernel(const float* __restrict__ noisy, cons
   for (int ch = 0; ch < CP; ++ch) {
     float v = 0.f;
     if (ch < Cobs) {
-      if (sv.ring_T > 0) {
+      if constexpr (kU8) {
+        const int f = ch / Cimg, cc = ch - f * Cimg;
+        v = u8_frame_value(obs, tab, n, f, (size_t)cc * HW + pix);
+      } else if (sv.ring_T > 0) {
         const int f = ch / Cimg, cc = ch - f * Cimg;
         int pf = sv.head + f; if (pf >= sv.ring_T) pf -= sv.ring_T;
         v = obs[(size_t)pf * sv.frame_stride + (size_t)n * sv.batch_stride + (size_t)cc * HW + pix];

@@ -17,6 +17,7 @@ import torch
 from torch import Tensor
 from torch.distributions.categorical import Categorical
 
+from .. import frames as frames_u8
 from ..models.diffusion import Denoiser, DiffusionSampler, DiffusionSamplerConfig
 
 ResetOutput = Tuple[torch.FloatTensor, Dict[str, Any]]
@@ -34,25 +35,37 @@ class _InitialConditionPool:
     """Fresh episodes for dead environments (world_model_env.py:107-139): real segments are preloaded
     `num_batches_to_preload` batches at a time, the reward/termination LSTM is burnt in on each batch, and requests for `k`
     initial conditions are served in order; what is left when a request does not fit is dropped and the pool is refilled
-    (the reference's generator does exactly this)."""
+    (the reference's generator does exactly this).
+
+    A loader of uint8 batches (Episode.save's levels) keeps the pool in uint8 with one kind per frame (frames.py; a batch
+    without `mask_padding` has real frames only), a quarter of the fp32 pool's memory; the burn-in reads it in place and
+    `take` decodes only the stacks it hands out, to the fp32 values a float loader's pool would hold."""
 
     def __init__(self, env: "WorldModelEnv", data_loader, num_batches: int) -> None:
         self.env, self.num_batches = env, num_batches
         self.batches = iter(data_loader)
-        self.obs = self.act = self.hx = self.cx = None
+        self.obs = self.act = self.hx = self.cx = self.kinds = None
         self.cursor = 0
 
     def _refill(self) -> None:
         env = self.env
-        obs_, act_, hx_, cx_ = [], [], [], []
+        obs_, act_, hx_, cx_, kinds_ = [], [], [], [], []
         for _ in range(self.num_batches):
             batch = next(self.batches)
             obs, act = batch.obs.to(env.device), batch.act.to(env.device)
+            kinds = None
+            if obs.dtype == torch.uint8:
+                kinds = frames_u8.kinds_from_mask(getattr(batch, "mask_padding", None), obs.shape[:2], env.device)
+                kinds_.append(kinds)
+            u8 = {} if kinds is None else {"kinds": (kinds[:, :-1], kinds[:, 1:])}
             with torch.no_grad():
-                *_, (hx, cx) = env.rew_end_model.predict_rew_end(obs[:, :-1], act[:, :-1], obs[:, 1:])
+                *_, (hx, cx) = env.rew_end_model.predict_rew_end(obs[:, :-1], act[:, :-1], obs[:, 1:], **u8)
             assert hx.size(0) == cx.size(0) == 1
             obs_.append(obs); act_.append(act); hx_.append(hx[0]); cx_.append(cx[0])
         self.obs, self.act, self.hx, self.cx = (torch.cat(v) for v in (obs_, act_, hx_, cx_))
+        if kinds_ and len(kinds_) != len(obs_):
+            raise ValueError("WorldModelEnv: the data loader mixes uint8 and float batches")
+        self.kinds = torch.cat(kinds_) if kinds_ else None
         self.cursor = 0
 
     def take(self, k: int):
@@ -62,7 +75,8 @@ class _InitialConditionPool:
                 self._refill()
         sl = slice(self.cursor, self.cursor + k)
         self.cursor += k
-        return self.obs[sl], self.act[sl], (self.hx[sl].unsqueeze(0), self.cx[sl].unsqueeze(0))
+        obs = self.obs[sl] if self.kinds is None else frames_u8.decode(self.obs[sl], self.kinds[sl])
+        return obs, self.act[sl], (self.hx[sl].unsqueeze(0), self.cx[sl].unsqueeze(0))
 
 
 class WorldModelEnv:
@@ -111,7 +125,7 @@ class WorldModelEnv:
     def reset(self, **kwargs) -> ResetOutput:  # world_model_env.py:45-53
         obs, act, (hx, cx) = self._pool.take(self.num_envs)
         b, t = obs.shape[:2]
-        self._frames = obs.new_empty(t, b, *obs.shape[2:])
+        self._frames = torch.empty(t, b, *obs.shape[2:], dtype=torch.float32, device=obs.device)
         self._acts = act.new_empty(t, b)
         self._head = 0
         self._write_stacks(slice(None), obs, act)

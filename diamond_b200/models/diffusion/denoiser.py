@@ -17,6 +17,7 @@ from torch import Tensor
 import torch.nn as nn
 
 from ... import _lib
+from ... import frames as frames_u8
 from .inner_model import InnerModel, InnerModelConfig
 
 LossAndLogs = Tuple[Tensor, Dict[str, Any]]
@@ -81,7 +82,7 @@ class EdmCoefficients:
 def quantise_frame(x: Tensor) -> Tensor:
     """[-1, 1] -> the 256-level grid and back, TRUNCATING like a uint8 cast (denoiser.py:83); the native inference path does
     the same inside `wrap_update_kernel`."""
-    levels = x.clamp(-1, 1).add(1).div(2).mul(255).byte()
+    levels = frames_u8.quantise_levels(x)
     return levels.div(255).mul(2).sub(1)
 
 
@@ -165,9 +166,14 @@ class Denoiser(nn.Module):
         `batch.obs` is (B, T, C, H, W) with T = n_cond + steps.  Step i noises frame n_cond + i, predicts it from frames
         [i, n_cond + i) and their actions, and regresses the EDM target (x - c_skip * noisy) / c_out on the unpadded samples;
         the quantised prediction then REPLACES that frame, so later steps are conditioned on the model's own output.
-        Random draws per step, in order: sigma, offset noise, white noise."""
+        Random draws per step, in order: sigma, offset noise, white noise.
+
+        A uint8 `batch.obs` (Episode.save's levels, padding where `batch.mask_padding` is False) computes the same loss and
+        gradients as its fp32 decoding; see `_forward_u8`."""
         if self.sample_sigma_training is None:
             raise RuntimeError("call setup_training(SigmaDistributionConfig) first")
+        if batch.obs.dtype == torch.uint8:
+            return self._forward_u8(batch)
         n_cond = self.cfg.inner_model.num_steps_conditioning
         frames = batch.obs.clone()
         b, t_total, c, h, w = frames.shape
@@ -185,5 +191,35 @@ class Denoiser(nn.Module):
             regression_target = (clean - cs.c_skip * noisy) / cs.c_out
             step_losses.append(torch.nn.functional.mse_loss(out[real], regression_target[real]))
             frames[:, tgt] = self.wrap_model_output(noisy, out, cs)
+        loss = sum(step_losses) / steps
+        return loss, {"loss_denoising": loss.detach()}
+
+    def _forward_u8(self, batch) -> LossAndLogs:
+        """`forward` on a uint8 batch.  The working copy of the frames stays uint8, with one kind per frame (frames.py): the
+        loaded frames decode as Episode.load does, padding as 0.0, and each write-back stores the quantiser's levels with
+        the kind of a GPU decode.  Only the target frame is decoded in torch (for the noise and the regression target); the
+        native pack kernel reads the context frames [i, n_cond + i) in place through the table of obs / sigma_data."""
+        n_cond = self.cfg.inner_model.num_steps_conditioning
+        frames = batch.obs.clone()
+        b, t_total = frames.shape[:2]
+        kinds = frames_u8.kinds_from_mask(batch.mask_padding, (b, t_total), frames.device)
+        table = frames_u8.decode_table(frames.device)
+        ctx_table = frames_u8.context_table(frames.device, self.cfg.sigma_data)
+        steps = t_total - n_cond
+        step_losses = []
+        for i in range(steps):
+            tgt = n_cond + i
+            clean = frames_u8.decode(frames[:, tgt], kinds[:, tgt], table)
+            sigma = self.sample_sigma_training(b, self.device)
+            noisy = self.apply_noise(clean, sigma, self.cfg.sigma_offset_noise)
+            cs = self._coefficients(sigma).broadcast()
+            context = frames_u8.U8FrameStack(frames[:, i:tgt], kinds[:, i:tgt], ctx_table)
+            out = self.inner_model(noisy * cs.c_in, cs.c_noise, context, batch.act[:, i:tgt])
+            real = batch.mask_padding[:, tgt]
+            regression_target = (clean - cs.c_skip * noisy) / cs.c_out
+            step_losses.append(torch.nn.functional.mse_loss(out[real], regression_target[real]))
+            with torch.no_grad():
+                frames[:, tgt] = frames_u8.quantise_levels(cs.c_skip * noisy + cs.c_out * out)
+            kinds[:, tgt] = frames_u8.KIND_GPU
         loss = sum(step_losses) / steps
         return loss, {"loss_denoising": loss.detach()}

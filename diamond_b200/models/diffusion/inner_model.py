@@ -1,4 +1,6 @@
-"""InnerModel (reference: src/models/diffusion/inner_model.py) bound to the native denoiser executor."""
+"""InnerModel (reference: src/models/diffusion/inner_model.py) bound to the native denoiser executor.  `obs` is an fp32
+frame stack (B, T*C, H, W), or a `frames.U8FrameStack` whose table already holds obs / sigma_data."""
+import ctypes as C
 from dataclasses import dataclass
 from typing import List, Optional
 
@@ -7,6 +9,7 @@ from torch import Tensor
 import torch.nn as nn
 
 from ... import _lib
+from ...frames import U8FrameStack
 from ...utils import NativeStateMixin
 from ..blocks import FourierFeatures, GroupNorm, UNet, conv3x3
 
@@ -76,6 +79,11 @@ class InnerModel(NativeStateMixin, nn.Module):
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         return self._ws
 
+    def check_frame_stack(self, obs: U8FrameStack, b: int, h: int, w: int) -> None:
+        want = (b, self.cfg.num_steps_conditioning, self.cfg.img_channels, h, w)
+        if tuple(obs.shape) != want:
+            raise ValueError(f"InnerModel: uint8 frame stack of shape {tuple(obs.shape)}, expected {want}")
+
     # ------------------------------------------------------------------ reference surface
     def forward(self, noisy_next_obs: Tensor, c_noise: Tensor, obs: Tensor, act: Tensor) -> Tensor:  # inner_model.py:44-49
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
@@ -85,12 +93,19 @@ class InnerModel(NativeStateMixin, nn.Module):
         lib = _lib.lib()
         h = self.native()
         b, _, hh, ww = noisy_next_obs.shape
-        noisy, obs_ = noisy_next_obs.float().contiguous(), obs.float().contiguous()
+        noisy = noisy_next_obs.float().contiguous()
         cn = c_noise.float().contiguous().reshape(-1)
         act_ = act.long().contiguous()
         out = torch.empty_like(noisy)
         need = lib.dmd_denoiser_workspace_bytes(h, b, hh, ww)
         ws = self.workspace(need)
+        if isinstance(obs, U8FrameStack):
+            self.check_frame_stack(obs, b, hh, ww)
+            _lib.check(lib.dmd_inner_model_forward_u8(h, b, hh, ww, noisy.data_ptr(), cn.data_ptr(), int(cn.numel() == 1),
+                                                      C.byref(obs.c_struct()), act_.data_ptr(), out.data_ptr(), ws.data_ptr(),
+                                                      ws.numel(), _lib.current_stream()))
+            return out
+        obs_ = obs.float().contiguous()
         _lib.check(lib.dmd_inner_model_forward(h, b, hh, ww, noisy.data_ptr(), cn.data_ptr(), int(cn.numel() == 1),
                                                obs_.data_ptr(), act_.data_ptr(), out.data_ptr(), ws.data_ptr(), ws.numel(),
                                                _lib.current_stream()))
@@ -106,14 +121,23 @@ class _InnerModelFn(torch.autograd.Function):
         lib = _lib.lib()
         h = module.native()
         b, _, hh, ww = noisy.shape
-        noisy_, obs_ = noisy.detach().float().contiguous(), obs.detach().float().contiguous()
+        if isinstance(obs, U8FrameStack):
+            module.check_frame_stack(obs, b, hh, ww)
+        noisy_ = noisy.detach().float().contiguous()
         cn = c_noise.detach().float().contiguous().reshape(-1)
         act_ = act.long().contiguous()
         out = torch.empty_like(noisy_)
         ws = module._acquire_ws(lib.dmd_denoiser_train_workspace_bytes(h, b, hh, ww))
-        _lib.check(lib.dmd_inner_model_forward_train(h, b, hh, ww, noisy_.data_ptr(), cn.data_ptr(), int(cn.numel() == 1),
-                                                     obs_.data_ptr(), act_.data_ptr(), out.data_ptr(), ws.data_ptr(), ws.numel(),
-                                                     _lib.current_stream()))
+        if isinstance(obs, U8FrameStack):   # uint8 frame stack, read in place (its tensors are kept like obs_)
+            obs_ = obs
+            _lib.check(lib.dmd_inner_model_forward_train_u8(h, b, hh, ww, noisy_.data_ptr(), cn.data_ptr(), int(cn.numel() == 1),
+                                                            C.byref(obs.c_struct()), act_.data_ptr(), out.data_ptr(), ws.data_ptr(),
+                                                            ws.numel(), _lib.current_stream()))
+        else:
+            obs_ = obs.detach().float().contiguous()
+            _lib.check(lib.dmd_inner_model_forward_train(h, b, hh, ww, noisy_.data_ptr(), cn.data_ptr(), int(cn.numel() == 1),
+                                                         obs_.data_ptr(), act_.data_ptr(), out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                         _lib.current_stream()))
         ctx.module, ctx.shape, ctx.ws, ctx.keep = module, (b, hh, ww), ws, (noisy_, obs_, cn, act_)
         return out
 

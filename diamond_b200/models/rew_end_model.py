@@ -6,7 +6,10 @@ over the burn-in frames of every fresh episode (:120-129).  Parameters live unde
 the action embedding, two attention blocks, LSTM over time, SiLU head — runs in `dmd_rew_end_predict`.
 Training (`forward`, rew_end_model.py:57-90) keeps the reference's host logic and loss in torch; with gradients enabled,
 `predict_rew_end` is one autograd node whose forward is `dmd_rew_end_forward_train` and whose backward is
-`dmd_rew_end_backward` (BPTT through the LSTM, the encoder on the denoiser's backward plan)."""
+`dmd_rew_end_backward` (BPTT through the LSTM, the encoder on the denoiser's backward plan).
+uint8 frames (Episode.save's levels) go through the `_u8` entry points, with one kind per frame (frames.py): obs / next_obs
+are then uint8 (b, t, C, S, S) and `kinds` = (obs kinds, next_obs kinds), each (b, t) uint8."""
+import ctypes as C
 from dataclasses import dataclass
 from typing import List, Optional, Tuple
 
@@ -17,6 +20,7 @@ from torch import Tensor
 from torch.autograd.function import once_differentiable
 
 from .. import _lib
+from .. import frames as frames_u8
 from ..utils import NativeStateMixin, init_lstm
 from .blocks import Downsample, ResBlocks, _NativeOnly, conv3x3
 
@@ -76,26 +80,40 @@ class RewEndModel(NativeStateMixin, nn.Module):
     # a training workspace holds one forward's activations until its backward has run
     _WS_POOL_CAP = 2
 
-    def predict_rew_end(self, obs: Tensor, act: Tensor, next_obs: Tensor,
-                        hx_cx: Optional[Tuple[Tensor, Tensor]] = None) -> Tuple[Tensor, Tensor, Tuple[Tensor, Tensor]]:
+    def predict_rew_end(self, obs: Tensor, act: Tensor, next_obs: Tensor, hx_cx: Optional[Tuple[Tensor, Tensor]] = None,
+                        kinds: Optional[Tuple[Tensor, Tensor]] = None) -> Tuple[Tensor, Tensor, Tuple[Tensor, Tensor]]:
         # rew_end_model.py:42-55.  hx_cx: each (1, b, lstm_dim) like torch.nn.LSTM
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             b = obs.size(0)
             hx = cx = None
             if hx_cx is not None:
                 hx, cx = hx_cx[0].reshape(b, -1), hx_cx[1].reshape(b, -1)
-            rew, end, hx_o, cx_o = _RewEndFn.apply(self, obs, act, next_obs, hx, cx, *self.parameters())
+            src = self._u8_sources(obs, next_obs, kinds)
+            rew, end, hx_o, cx_o = _RewEndFn.apply(self, obs, act, next_obs, hx, cx, src, *self.parameters())
             return rew, end, (hx_o.unsqueeze(0), cx_o.unsqueeze(0))
-        return self._predict(obs, act, next_obs, hx_cx)
+        return self._predict(obs, act, next_obs, hx_cx, kinds)
+
+    def _u8_sources(self, obs: Tensor, next_obs: Tensor, kinds: Optional[Tuple[Tensor, Tensor]]):
+        """None for fp32 frames; for uint8 frames the two U8FrameStacks the `_u8` entry points read (one decode table)."""
+        if obs.dtype != torch.uint8 and next_obs.dtype != torch.uint8:
+            return None
+        if obs.dtype != next_obs.dtype or kinds is None:
+            raise ValueError("RewEndModel: uint8 obs and next_obs go together, with kinds = (obs kinds, next_obs kinds)")
+        want = (obs.size(0), obs.size(1), self.cfg.img_channels, self.cfg.img_size, self.cfg.img_size)
+        if tuple(obs.shape) != want or tuple(next_obs.shape) != want:
+            raise ValueError(f"RewEndModel: uint8 obs / next_obs of shapes {tuple(obs.shape)} / {tuple(next_obs.shape)}, expected {want}")
+        table = frames_u8.decode_table(obs.device)
+        return frames_u8.U8FrameStack(obs, kinds[0], table), frames_u8.U8FrameStack(next_obs, kinds[1], table)
 
     @torch.no_grad()
-    def _predict(self, obs: Tensor, act: Tensor, next_obs: Tensor,
-                 hx_cx: Optional[Tuple[Tensor, Tensor]] = None) -> Tuple[Tensor, Tensor, Tuple[Tensor, Tensor]]:
+    def _predict(self, obs: Tensor, act: Tensor, next_obs: Tensor, hx_cx: Optional[Tuple[Tensor, Tensor]] = None,
+                 kinds: Optional[Tuple[Tensor, Tensor]] = None) -> Tuple[Tensor, Tensor, Tuple[Tensor, Tensor]]:
         lib = _lib.lib()
         h = self._native()
         b, t, c, hh, ww = obs.shape
         dev = obs.device
-        obs_, nxt_, act_ = obs.float().contiguous(), next_obs.float().contiguous(), act.long().contiguous()
+        src = self._u8_sources(obs, next_obs, kinds)
+        act_ = act.long().contiguous()
         hx = cx = None
         if hx_cx is not None:
             hx, cx = hx_cx[0].reshape(b, -1).float().contiguous(), hx_cx[1].reshape(b, -1).float().contiguous()
@@ -108,6 +126,12 @@ class RewEndModel(NativeStateMixin, nn.Module):
             raise RuntimeError("diamond_b200: " + lib.dmd_last_error().decode())
         if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
             self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        if src is not None:
+            _lib.check(lib.dmd_rew_end_predict_u8(h, b, t, C.byref(src[0].c_struct()), C.byref(src[1].c_struct()), act_.data_ptr(),
+                                                  _lib.ptr(hx), _lib.ptr(cx), rew.data_ptr(), end.data_ptr(), hx_o.data_ptr(),
+                                                  cx_o.data_ptr(), self._ws.data_ptr(), self._ws.numel(), _lib.current_stream()))
+            return rew, end, (hx_o.unsqueeze(0), cx_o.unsqueeze(0))
+        obs_, nxt_ = obs.float().contiguous(), next_obs.float().contiguous()
         _lib.check(lib.dmd_rew_end_predict(h, b, t, obs_.data_ptr(), nxt_.data_ptr(), act_.data_ptr(), _lib.ptr(hx), _lib.ptr(cx),
                                            rew.data_ptr(), end.data_ptr(), hx_o.data_ptr(), cx_o.data_ptr(), self._ws.data_ptr(),
                                            self._ws.numel(), _lib.current_stream()))
@@ -123,11 +147,24 @@ class RewEndModel(NativeStateMixin, nn.Module):
 
         # When dead, replace frame (gray padding) by true final obs; the write goes through the view into batch.obs
         dead = end.bool().any(dim=1)
-        if dead.any():
+        kinds = None
+        if batch.obs.dtype == torch.uint8:
+            # uint8 batch: one kind per frame; a float final observation is encoded (a frame off the level grid raises), a
+            # uint8 one is taken as the bytes a real env decodes on the GPU (src/envs/env.py:89)
+            all_kinds = frames_u8.kinds_from_mask(batch.mask_padding, batch.obs.shape[:2], batch.obs.device)
+            if dead.any():
+                finals = [i["final_observation"] for i, d in zip(batch.info, dead) if d]
+                levels, fk = zip(*[(f, torch.tensor(frames_u8.KIND_GPU, dtype=torch.uint8, device=f.device))
+                                   if f.dtype == torch.uint8 else frames_u8.encode(f) for f in finals])
+                slot = end[dead].argmax(dim=1)
+                next_obs[dead, slot] = torch.stack(levels).to(obs.device)
+                all_kinds[:, 1:][dead, slot] = torch.stack([k.to(obs.device) for k in fk])
+            kinds = (all_kinds[:, :-1], all_kinds[:, 1:])
+        elif dead.any():
             final_obs = torch.stack([i["final_observation"] for i, d in zip(batch.info, dead) if d]).to(obs.device)
             next_obs[dead, end[dead].argmax(dim=1)] = final_obs
 
-        logits_rew, logits_end, _ = self.predict_rew_end(obs, act, next_obs)
+        logits_rew, logits_end, _ = self.predict_rew_end(obs, act, next_obs, **({} if kinds is None else {"kinds": kinds}))
         logits_rew = logits_rew[mask]
         logits_end = logits_end[mask]
         target_rew = rew[mask].sign().long().add(1)  # clipped to {-1, 0, 1}
@@ -163,24 +200,31 @@ class _RewEndFn(torch.autograd.Function):
     gradients wrt a carried (hx, cx) when the caller's state requires them)."""
 
     @staticmethod
-    def forward(ctx, module, obs, act, next_obs, hx, cx, *params):
+    def forward(ctx, module, obs, act, next_obs, hx, cx, src, *params):
         lib = _lib.lib()
         h = module._native()
         b, t = obs.shape[:2]
         D = module.cfg.lstm_dim
-        obs_, nxt_, act_ = obs.detach().float().contiguous(), next_obs.detach().float().contiguous(), act.long().contiguous()
+        act_ = act.long().contiguous()
         hx_ = None if hx is None else hx.detach().float().contiguous()
         cx_ = None if cx is None else cx.detach().float().contiguous()
-        rew = obs_.new_empty(b, t, 3)
-        end = obs_.new_empty(b, t, 2)
-        hx_o, cx_o = obs_.new_empty(b, D), obs_.new_empty(b, D)
+        f32 = dict(dtype=torch.float32, device=obs.device)
+        rew = torch.empty(b, t, 3, **f32)
+        end = torch.empty(b, t, 2, **f32)
+        hx_o, cx_o = torch.empty(b, D, **f32), torch.empty(b, D, **f32)
         need = lib.dmd_rew_end_train_workspace_bytes(h, b, t)
         if need == 0:
             raise RuntimeError("diamond_b200: " + lib.dmd_last_error().decode())
         ws = module._acquire_ws(need)
-        _lib.check(lib.dmd_rew_end_forward_train(h, b, t, obs_.data_ptr(), nxt_.data_ptr(), act_.data_ptr(), _lib.ptr(hx_), _lib.ptr(cx_),
-                                                 rew.data_ptr(), end.data_ptr(), hx_o.data_ptr(), cx_o.data_ptr(), ws.data_ptr(),
-                                                 ws.numel(), _lib.current_stream()))
+        if src is not None:
+            _lib.check(lib.dmd_rew_end_forward_train_u8(h, b, t, C.byref(src[0].c_struct()), C.byref(src[1].c_struct()), act_.data_ptr(),
+                                                        _lib.ptr(hx_), _lib.ptr(cx_), rew.data_ptr(), end.data_ptr(), hx_o.data_ptr(),
+                                                        cx_o.data_ptr(), ws.data_ptr(), ws.numel(), _lib.current_stream()))
+        else:
+            obs_, nxt_ = obs.detach().float().contiguous(), next_obs.detach().float().contiguous()
+            _lib.check(lib.dmd_rew_end_forward_train(h, b, t, obs_.data_ptr(), nxt_.data_ptr(), act_.data_ptr(), _lib.ptr(hx_), _lib.ptr(cx_),
+                                                     rew.data_ptr(), end.data_ptr(), hx_o.data_ptr(), cx_o.data_ptr(), ws.data_ptr(),
+                                                     ws.numel(), _lib.current_stream()))
         ctx.module, ctx.shape, ctx.ws = module, (b, t), ws
         return rew, end, hx_o, cx_o
 
@@ -203,4 +247,4 @@ class _RewEndFn(torch.autograd.Function):
         grads = [flat[o:o + n].view_as(p) for o, n, p in zip(offs, nums, module.parameters())]
         module._release_ws(ctx.ws, module._WS_POOL_CAP)
         module.last_flat_grad = flat   # one contiguous buffer: what a data-parallel step all-reduces in a single collective
-        return (None, None, None, None, g_hx_in, g_cx_in, *grads)
+        return (None, None, None, None, g_hx_in, g_cx_in, None, *grads)

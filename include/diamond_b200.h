@@ -292,6 +292,25 @@ typedef struct dmd_denoiser_config {
 
 typedef struct dmd_denoiser dmd_denoiser;
 
+/* Frames stored as one byte per value (Episode.save's levels, src/data/episode.py:47), read in place through strides.
+ * Frame (n, f) of the source -- sample n, frame f -- is C*H*W contiguous bytes at levels + n * batch_stride + f * frame_stride
+ * (strides in bytes), and has one kind byte at kinds[n * kind_batch_stride + f * kind_frame_stride].  Value i of the frame is
+ * table[kind * 256 + byte]: table (DMD_FRAME_KINDS x 256 fp32, device memory) holds, per kind, the value the fp32 entry point
+ * would have read for that byte, so the two entry points compute the same thing (diamond_b200/frames.py builds the tables).
+ * Kinds: 0 padding (0.0 whatever the byte), 1 decoded on the CPU (Episode.load, src/data/episode.py:39), 2 decoded on the
+ * GPU by torch (the denoiser's quantiser write-back, a real env's final observation).  A kind >= DMD_FRAME_KINDS reads as 0.
+ * A (B, T, C, H, W) uint8 tensor with its (B, T) kinds gives frames [i, i + n) as levels + i * C*H*W, kinds + i. */
+#define DMD_FRAME_KINDS 3
+typedef struct dmd_u8_frames {
+  const uint8_t* levels;
+  long long batch_stride;
+  long long frame_stride;
+  const uint8_t* kinds;
+  long long kind_batch_stride;
+  long long kind_frame_stride;
+  const float* table;
+} dmd_u8_frames;
+
 dmd_denoiser* dmd_denoiser_create(const dmd_denoiser_config* cfg);
 void dmd_denoiser_destroy(dmd_denoiser* h);
 
@@ -337,6 +356,17 @@ int dmd_inner_model_forward_train(dmd_denoiser* h, int B, int H, int W, const fl
                                   void* workspace, size_t workspace_bytes, void* stream);
 int dmd_denoiser_backward(dmd_denoiser* h, int B, int H, int W, const float* grad_out, float* grads, long long grads_numel,
                           void* workspace, void* stream);
+
+/* dmd_inner_model_forward / dmd_inner_model_forward_train with the frame stack read from uint8 frames: obs holds the
+ * num_steps_conditioning frames of each sample, f = 0 oldest, and its table the rescaled values obs / sigma_data (what
+ * obs_rescaled would hold).  dmd_denoiser_backward is the same after either forward.  Every argument is checked before
+ * any launch. */
+int dmd_inner_model_forward_u8(dmd_denoiser* h, int B, int H, int W, const float* noisy_rescaled, const float* c_noise,
+                               int c_noise_is_scalar, const dmd_u8_frames* obs, const int64_t* act, float* out,
+                               void* workspace, size_t workspace_bytes, void* stream);
+int dmd_inner_model_forward_train_u8(dmd_denoiser* h, int B, int H, int W, const float* noisy_rescaled, const float* c_noise,
+                                     int c_noise_is_scalar, const dmd_u8_frames* obs, const int64_t* act, float* out,
+                                     void* workspace, size_t workspace_bytes, void* stream);
 
 typedef struct dmd_sampler_config {
   int num_sigmas;               /* len(self.sigmas) = num_steps_denoising + 1, last one 0 */
@@ -455,6 +485,16 @@ int dmd_rew_end_forward_train(dmd_rew_end* h, int b, int t, const float* obs, co
 int dmd_rew_end_backward(dmd_rew_end* h, int b, int t, const float* g_logits_rew, const float* g_logits_end,
                          const float* g_hx_out, const float* g_cx_out, float* grads, long long grads_numel,
                          float* g_hx_in, float* g_cx_in, void* workspace, void* stream);
+/* dmd_rew_end_predict / dmd_rew_end_forward_train with obs / next_obs read from uint8 frames (frame (n, k) = step k of
+ * segment n); both sources share one decode table (values as the fp32 entry points read them).  dmd_rew_end_backward is the
+ * same after either forward.  Every argument is checked before any launch. */
+int dmd_rew_end_predict_u8(dmd_rew_end* h, int b, int t, const dmd_u8_frames* obs, const dmd_u8_frames* next_obs,
+                           const int64_t* act, const float* hx_in, const float* cx_in, float* logits_rew, float* logits_end,
+                           float* hx_out, float* cx_out, void* workspace, size_t workspace_bytes, void* stream);
+int dmd_rew_end_forward_train_u8(dmd_rew_end* h, int b, int t, const dmd_u8_frames* obs, const dmd_u8_frames* next_obs,
+                                 const int64_t* act, const float* hx_in, const float* cx_in, float* logits_rew,
+                                 float* logits_end, float* hx_out, float* cx_out, void* workspace, size_t workspace_bytes,
+                                 void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Optimizer: torch.nn.utils.clip_grad_norm_ + torch.optim.AdamW (src/trainer.py:373-377, src/utils.py:164) over every
