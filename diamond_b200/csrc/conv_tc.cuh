@@ -134,128 +134,176 @@ struct RegEpilogue {
     n_cur = -1;
   }
 
-  // whole warp, converged
+  // whole warp, converged.  kG: groups that can hold a nonzero sum (at most kMaxOutGroups).  The butterflies of all groups are
+  // independent, so they run round by round side by side instead of one group's five dependent rounds after another's; each
+  // value still goes through the same five additions in the same order.
+  template <int kG = kMaxOutGroups>
   __device__ __forceinline__ void flush_stats(const ConvParams& p, int img0, int nslots) {
 #pragma unroll
     for (int k = 0; k < kStatSlots; ++k) {
+      if (k < nslots) {
+        float a[kG], b[kG];
 #pragma unroll
-      for (int g = 0; g < kMaxOutGroups; ++g) {
-        if (k < nslots && g < G) {
-          float a = s[k][g], b = ss[k][g];
+        for (int g = 0; g < kG; ++g) { a[g] = s[k][g]; b[g] = ss[k][g]; }
 #pragma unroll
-          for (int m = 16; m > 0; m >>= 1) {
-            a += __shfl_xor_sync(0xffffffffu, a, m);
-            b += __shfl_xor_sync(0xffffffffu, b, m);
+        for (int m = 16; m > 0; m >>= 1)
+#pragma unroll
+          for (int g = 0; g < kG; ++g) {
+            a[g] += __shfl_xor_sync(0xffffffffu, a[g], m);
+            b[g] += __shfl_xor_sync(0xffffffffu, b[g], m);
           }
-          if (lane == 0 && img0 + k < p.B && (a != 0.f || b != 0.f)) {
-            double* dst = p.ostats + ((size_t)(img0 + k) * G + g) * 2;
-            atomicAdd(dst, (double)a);
-            atomicAdd(dst + 1, (double)b);
-          }
+        if (lane == 0 && img0 + k < p.B) {
+#pragma unroll
+          for (int g = 0; g < kG; ++g)
+            if (g < G && (a[g] != 0.f || b[g] != 0.f)) {
+              double* dst = p.ostats + ((size_t)(img0 + k) * G + g) * 2;
+              atomicAdd(dst, (double)a[g]);
+              atomicAdd(dst + 1, (double)b[g]);
+            }
         }
-        s[k][g] = ss[k][g] = 0.f;
       }
+#pragma unroll
+      for (int g = 0; g < kMaxOutGroups; ++g) s[k][g] = ss[k][g] = 0.f;
     }
   }
 
   // the tile starting at padded-linear position q0; acc: this thread's wgmma accumulator fragment.  kLgs: 0 without
   // statistics, else log2 of the 8-column blocks per output group (ogs 16/32/64/128 -> 1..4), so that block j's group j >> kLgs
-  // is known at compile time and each block adds straight into its group's sums.
-  template <int kLgs>
+  // is known at compile time and each block adds straight into its group's sums.  kFull: Cout == N and stride 1 (every
+  // stride-1 layer whose Cout is the accumulator width), so every column is stored with an 8-byte access and the column
+  // tests and the subsampling compile away; the straight-line code that remains has no branch per column block.
+  template <int kLgs, bool kFull>
   __device__ __forceinline__ void tile(const ConvParams& p, const float* sbias, const float (&acc)[N / 2], int q0) {
     constexpr bool kStats = kLgs > 0;
     constexpr int kGroups = (N / 8) >> kLgs > 0 ? ((N / 8) >> kLgs < kMaxOutGroups ? (N / 8) >> kLgs : kMaxOutGroups) : 1;
     const int n_lo = (int)p.dPH.div(p.dPW.div((uint32_t)q0));
     const int q_last = min(q0 + kTileM, p.Q) - 1;
     const bool single_image = (int)p.dPH.div(p.dPW.div((uint32_t)q_last)) == n_lo;
-    if (kStats && n_cur >= 0 && (!single_image || n_lo != n_cur)) { flush_stats(p, n_cur, 1); n_cur = -1; }
+    if (kStats && n_cur >= 0 && (!single_image || n_lo != n_cur)) { flush_stats<kGroups>(p, n_cur, 1); n_cur = -1; }
     const int c0 = 2 * (lane & 3);
-    const bool vec = (p.Cout & 1) == 0;   // 8-byte accesses (every layer but conv_out / the 15-channel dgrad)
+    const bool vec = kFull || (p.Cout & 1) == 0;   // 8-byte accesses (every layer but conv_out / the 15-channel dgrad)
+    const bool resid = p.resid != nullptr;
+    // Every load of a batch (bias from shared memory, residual from global memory) is issued before the batch's first store.
+    // The compiler cannot prove that a store to `out` leaves a later load's address alone, so loads placed after stores would
+    // each wait out their whole latency in turn.  Up to N = 64 a batch is both rows, all columns: one residual latency per
+    // tile instead of one per row, and the bias of a column is read once for both rows.  At N = 128 a batch is 8 column
+    // blocks of one row, which bounds the extra registers (that instantiation already uses all 168 a thread can have).
+    constexpr int kBatch = N / 8 < 8 ? N / 8 : 8;
+    constexpr int kRows = N / 8 <= 8 ? 2 : 1;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int q = q0 + r0 + 8 * h;
-      int opix = -1, slot = 0;
-      if (q < p.Q) {
-        const uint32_t R = p.dPW.div((uint32_t)q);
-        const int x = q - (int)R * p.PW;
-        const int n = (int)p.dPH.div(R);
-        const int y = (int)R - n * p.PH;
-        bool valid = (x < p.W) && (y < p.H);
-        int yo = y, xo = x, Ho = p.H, Wo = p.W;
-        if (p.stride == 2) {
-          valid = valid && ((x & 1) == 0) && ((y & 1) == 0);
-          yo = y >> 1; xo = x >> 1; Ho = p.H >> 1; Wo = p.W >> 1;
+    for (int h0 = 0; h0 < 2; h0 += kRows) {
+      // the output pixel of each row of the batch (-1: a pad position or past the end), and its image slot
+      int opix[kRows], slot[kRows];
+#pragma unroll
+      for (int r = 0; r < kRows; ++r) {
+        const int q = q0 + r0 + 8 * (h0 + r);
+        opix[r] = -1; slot[r] = 0;
+        if (q < p.Q) {
+          const uint32_t R = p.dPW.div((uint32_t)q);
+          const int x = q - (int)R * p.PW;
+          const int n = (int)p.dPH.div(R);
+          const int y = (int)R - n * p.PH;
+          bool valid = (x < p.W) && (y < p.H);
+          int yo = y, xo = x, Ho = p.H, Wo = p.W;
+          if (!kFull && p.stride == 2) {
+            valid = valid && ((x & 1) == 0) && ((y & 1) == 0);
+            yo = y >> 1; xo = x >> 1; Ho = p.H >> 1; Wo = p.W >> 1;
+          }
+          if (valid) { opix[r] = (n * Ho + yo) * Wo + xo; slot[r] = n - n_lo; }
         }
-        if (valid) { opix = (n * Ho + yo) * Wo + xo; slot = n - n_lo; }
       }
-      if (opix < 0) continue;
-      float* op = p.out + (size_t)opix * p.Cout;
-      const float* rp = p.resid != nullptr ? p.resid + (size_t)opix * p.Cout : nullptr;
-      float gs[kMaxOutGroups], gss[kMaxOutGroups];
+      if (kRows == 1 && opix[0] < 0) continue;   // a one-row batch on a pad position: nothing to load, store or count
+      float gs[kRows][kMaxOutGroups], gss[kRows][kMaxOutGroups];   // group sums of each row of the batch
 #pragma unroll
-      for (int g = 0; g < kMaxOutGroups; ++g) gs[g] = gss[g] = 0.f;
-      // Every load of a batch of columns (bias from shared memory, residual from global memory) is issued before the batch's
-      // first store.  The compiler cannot prove that a store to `out` leaves the next load's address alone, so loads placed
-      // after stores would each wait out their whole latency in turn.  A batch is at most 8 column blocks, which bounds the
-      // extra registers at N = 128.
-      constexpr int kBatch = N / 8 < 8 ? N / 8 : 8;
+      for (int r = 0; r < kRows; ++r)
+#pragma unroll
+        for (int g = 0; g < kMaxOutGroups; ++g) gs[r][g] = gss[r][g] = 0.f;
 #pragma unroll
       for (int jb = 0; jb < N / 8; jb += kBatch) {
-        float2 bv[kBatch], rv[kBatch];
+        float2 bv[kBatch], rv[kRows][kBatch];
 #pragma unroll
         for (int u = 0; u < kBatch; ++u) {
           const int col = 8 * (jb + u) + c0;
-          bv[u] = rv[u] = make_float2(0.f, 0.f);
-          if (col < p.Cout) {
-            bv[u] = make_float2(sbias[col], sbias[col + 1]);
-            if (rp) {
-              if (vec) rv[u] = __ldg(reinterpret_cast<const float2*>(rp + col));
+          bv[u] = (kFull || col < p.Cout) ? *reinterpret_cast<const float2*>(sbias + col) : make_float2(0.f, 0.f);
+#pragma unroll
+          for (int r = 0; r < kRows; ++r) {
+            const int h = h0 + r;
+            rv[r][u] = make_float2(0.f, 0.f);
+            if (resid && opix[r] >= 0 && (kFull || col < p.Cout)) {
+              const float* rp = p.resid + (size_t)opix[r] * p.Cout;
+              if (vec) rv[r][u] = __ldg(reinterpret_cast<const float2*>(rp + col));
               else {
-                rv[u].x = __ldg(rp + col);
-                if (col + 1 < p.Cout) rv[u].y = __ldg(rp + col + 1);
+                rv[r][u].x = __ldg(rp + col);
+                if (col + 1 < p.Cout) rv[r][u].y = __ldg(rp + col + 1);
               }
             }
           }
         }
 #pragma unroll
-        for (int u = 0; u < kBatch; ++u) {
-          const int j = jb + u;
-          const int col = 8 * j + c0;
-          if (col < p.Cout) {
-            float2 o = make_float2(acc[4 * j + 2 * h] + bv[u].x, acc[4 * j + 2 * h + 1] + bv[u].y);
-            if (vec) {
-              if (rp) { o.x += rv[u].x; o.y += rv[u].y; }
-              *reinterpret_cast<float2*>(op + col) = o;
-            } else {
-              if (rp) o.x += rv[u].x;
-              op[col] = o.x;
-              if (col + 1 < p.Cout) { if (rp) o.y += rv[u].y; op[col + 1] = o.y; } else o.y = 0.f;
-            }
-            if (kStats) {
-              gs[j >> kLgs] += o.x + o.y;
-              gss[j >> kLgs] += fmaf(o.x, o.x, o.y * o.y);
+        for (int r = 0; r < kRows; ++r) {
+          const int h = h0 + r;
+          if (opix[r] < 0) continue;
+          float* op = p.out + (size_t)opix[r] * p.Cout;
+#pragma unroll
+          for (int u = 0; u < kBatch; ++u) {
+            const int j = jb + u;
+            const int col = 8 * j + c0;
+            if (kFull || col < p.Cout) {
+              float2 o = make_float2(acc[4 * j + 2 * h] + bv[u].x, acc[4 * j + 2 * h + 1] + bv[u].y);
+              if (vec) {
+                if (resid) { o.x += rv[r][u].x; o.y += rv[r][u].y; }
+                *reinterpret_cast<float2*>(op + col) = o;
+              } else {
+                if (resid) o.x += rv[r][u].x;
+                op[col] = o.x;
+                if (col + 1 < p.Cout) { if (resid) o.y += rv[r][u].y; op[col + 1] = o.y; } else o.y = 0.f;
+              }
+              if (kStats) {
+                gs[r][j >> kLgs] += o.x + o.y;
+                gss[r][j >> kLgs] += fmaf(o.x, o.x, o.y * o.y);
+              }
             }
           }
         }
       }
       if (kStats) {
-        // Groups and slots that a value does not belong to are skipped rather than given +0.0: every sum starts at +0.0 and
-        // so is never -0.0, which makes adding +0.0 an identity, and the sums keep the bits of the select-and-add form.
-        if (single_image) {   // warp-uniform: every row of the tile is in image n_lo
+        // Row h's group sums enter the image sums after the row is complete, row 0 before row 1.  Groups and slots that a
+        // value does not belong to are skipped rather than given +0.0: every sum starts at +0.0 and so is never -0.0, which
+        // makes adding +0.0 an identity, and the sums keep the bits of the select-and-add form.
 #pragma unroll
-          for (int g = 0; g < kGroups; ++g) { s[0][g] += gs[g]; ss[0][g] += gss[g]; }
-        } else {
+        for (int r = 0; r < kRows; ++r) {
+          const int h = h0 + r;
+          if (opix[r] < 0) continue;
+          if (single_image) {   // warp-uniform: every row of the tile is in image n_lo
 #pragma unroll
-          for (int k = 0; k < kStatSlots; ++k)
+            for (int g = 0; g < kGroups; ++g) { s[0][g] += gs[r][g]; ss[0][g] += gss[r][g]; }
+          } else {
 #pragma unroll
-            for (int g = 0; g < kGroups; ++g) { s[k][g] += (slot == k) ? gs[g] : 0.f; ss[k][g] += (slot == k) ? gss[g] : 0.f; }
+            for (int k = 0; k < kStatSlots; ++k)
+#pragma unroll
+              for (int g = 0; g < kGroups; ++g) {
+                s[k][g] += (slot[r] == k) ? gs[r][g] : 0.f;
+                ss[k][g] += (slot[r] == k) ? gss[r][g] : 0.f;
+              }
+          }
         }
       }
     }
     if (kStats) {
       if (single_image) n_cur = n_lo;            // keep running across the single-image tiles of this CTA
-      else { flush_stats(p, n_lo, kStatSlots); n_cur = -1; }
+      else { flush_stats<kGroups>(p, n_lo, kStatSlots); n_cur = -1; }
     }
+  }
+
+  // tile() with the statistics' group size as a template argument (only the sizes an N-column accumulator can hold are
+  // instantiated); lgs = log2 of the 8-column blocks per output group, 0 without statistics
+  template <bool kFull>
+  __device__ __forceinline__ void tile_any(const ConvParams& p, int lgs, const float* sbias, const float (&acc)[N / 2], int q0) {
+    if (lgs == 0) tile<0, kFull>(p, sbias, acc, q0);
+    else if (lgs == 1 || N == 16) tile<1, kFull>(p, sbias, acc, q0);
+    else if (lgs == 2 || N == 32) tile<2, kFull>(p, sbias, acc, q0);
+    else if (lgs == 3 || N == 64) tile<3, kFull>(p, sbias, acc, q0);
+    else tile<4, kFull>(p, sbias, acc, q0);
   }
 
   __device__ __forceinline__ void finish(const ConvParams& p) {
@@ -343,6 +391,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_tc_kernel(const ConvPara
     RegEpilogue<N> epi;
     epi.init(p, m0 + 16 * (warp & 3) + (lane >> 2), lane);
     const int lgs = p.ostats ? 31 - __clz(p.ogs >> 3) : 0;   // 8-column block j lies in output group j >> lgs
+    const bool full_cols = p.Cout == N && p.stride == 1;      // the epilogue without column tests (RegEpilogue::tile)
     if (my_tiles > 0) mbar_wait(wbar, 0);
     // Descriptor words: per wgmma only the 14-bit start-address fields change (A: ring stage + tap shift, B: tap + slab), all in
     // 16-byte units.  K-major operands: LBO = stride of the 8-channel chunks, SBO = 128 B (eight 16-byte rows).
@@ -404,13 +453,9 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_tc_kernel(const ConvPara
       wgmma_wait<0>();
       wgmma_fence_operands(acc);
       if (done > 0 && lane == 0) mbar_arrive(empty + prev);
-      // statistics' group size -> template argument (only the sizes an N-column accumulator can hold are instantiated)
       const int q0 = (tile_begin + it) * kTileM;
-      if (lgs == 0) epi.template tile<0>(p, sbias, acc, q0);
-      else if (lgs == 1 || N == 16) epi.template tile<1>(p, sbias, acc, q0);
-      else if (lgs == 2 || N == 32) epi.template tile<2>(p, sbias, acc, q0);
-      else if (lgs == 3 || N == 64) epi.template tile<3>(p, sbias, acc, q0);
-      else epi.template tile<4>(p, sbias, acc, q0);
+      if (full_cols) epi.template tile_any<true>(p, lgs, sbias, acc, q0);
+      else epi.template tile_any<false>(p, lgs, sbias, acc, q0);
     }
     epi.finish(p);
   }
