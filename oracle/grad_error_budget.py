@@ -26,53 +26,8 @@ import torch.nn.functional as F
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import torch_oracle as O  # noqa: E402
+from oracle.fp16_emulation import QConv, _SCALE, _real_conv2d  # noqa: E402
 from oracle.make_golden import CASES, TRAIN_CASES  # noqa: E402
-
-_real_conv2d = F.conv2d
-
-
-def _h(t):
-    return t.half().float()
-
-
-# the loss-scale scheme: None = a per-tensor scale (max near 2^12); an int E = one scale per backward call, set by conv_out
-_SCALE = {"exp": None, "S": None}
-
-
-def _pow2_scale(m, e):
-    """2^(e - k) for m = f 2^k, f in [0.5, 1): loss_scale_kernel's choice, max |S g| in [2^(e-1), 2^e)."""
-    return 1.0 if m == 0.0 else 2.0 ** (e - math.frexp(m)[1])
-
-
-def _scaled_h(g):
-    """fp16 rounding of a gradient tensor under the loss scale of _SCALE."""
-    s = _SCALE["S"] if _SCALE["exp"] is not None else _pow2_scale(float(g.abs().max()), 12)
-    return _h(g * s) / s
-
-
-class QConv(torch.autograd.Function):
-    """conv2d whose forward / dgrad / wgrad operands are rounded per `mode` = (fwd, dgrad, wgrad), each in {0: exact, 1: fp16}."""
-
-    @staticmethod
-    def forward(ctx, x, w, b, stride, padding, mode, is_out=False):
-        ctx.save_for_backward(x, w)
-        ctx.cfg = (stride, padding, mode, b is not None)
-        ctx.is_out = is_out
-        xq, wq = (_h(x), _h(w)) if mode[0] else (x, w)
-        return _real_conv2d(xq, wq, b, stride=stride, padding=padding)
-
-    @staticmethod
-    def backward(ctx, gy):
-        x, w = ctx.saved_tensors
-        stride, padding, mode, has_b = ctx.cfg
-        if ctx.is_out and _SCALE["exp"] is not None:   # conv_out: its dL/dy is the gradient of the model output
-            _SCALE["S"] = _pow2_scale(float(gy.abs().max()), _SCALE["exp"])
-        gd = _scaled_h(gy) if mode[1] else gy
-        gx = torch.nn.grad.conv2d_input(x.shape, _h(w) if mode[1] else w, gd, stride=stride, padding=padding)
-        gwy = _scaled_h(gy) if mode[2] else gy
-        gw = torch.nn.grad.conv2d_weight(_h(x) if mode[2] else x, w.shape, gwy, stride=stride, padding=padding)
-        gb = gy.sum(dim=(0, 2, 3)) if has_b else None
-        return gx, gw, gb, None, None, None, None
 
 
 def run(case_name, mode_main, mode_stream, exp=None, gain=1.0):

@@ -94,7 +94,21 @@ def _seeded_batch(b, T, seed):
     return RT.frames(obs_u8), act, rew, end, mask, final_obs
 
 
+# native logits lie within this many ensemble spreads of the fp16-operand emulation: 1.5 x (5.75e-4, 4.13e-4) is tighter than the
+# old 1e-3 against the reference, and still admits a regrouping of the GroupNorm partial sums
+SPREAD_MULTIPLE = 1.5
+
+
 def test_rew_end_training_step_matches_reference():
+    """The logits are bounded by what the native operand rounding produces (oracle/fp16_emulation.py, derived on the CPU in
+    tests/test_oracle_rew_end_training.py::test_rew_end_logits_bound_from_fp16_emulation): against the reference's fp32 logits
+    within 1.5 x the worst distance of the fp16-operand emulation ensemble (1.66e-3 rew, 1.19e-3 end), and against the
+    unperturbed emulation within SPREAD_MULTIPLE x the ensemble's spread (5.75e-4 rew, 4.13e-4 end).  Measured on an H100
+    80GB HBM3 (700 W power limit): 9.73e-4 / 6.44e-4 from the reference, 5.52e-4 / 3.38e-4 from the emulation; with the
+    all-padding tail tile dropped from the conv schedule (a regrouping of the fp32 GroupNorm partial sums) 1.08e-3 / 6.95e-4
+    and 5.92e-4 / 3.50e-4, inside both bounds."""
+    from oracle import fp16_emulation as E
+
     dev = _dev()
     (obs, act, rew, end, mask, final_obs), g = RT.load_golden()
     cfg = O.RewEndCfg()
@@ -103,8 +117,15 @@ def test_rew_end_training_step_matches_reference():
     loss, metrics, (lr, le) = _native_step(model, batch)
     e_loss = abs(loss.item() - float(g["loss"])) / abs(float(g["loss"]))
     e_rew, e_end = _rel(lr, torch.from_numpy(g["logits_rew"])), _rel(le, torch.from_numpy(g["logits_end"]))
-    print(f"rew_end golden: loss {loss.item():.6f} reference {float(g['loss']):.6f} (rel {e_loss:.2e}); logits rel {e_rew:.2e} {e_end:.2e}")
-    assert e_loss < 1e-3 and e_rew < 1e-3 and e_end < 1e-3
+    torch.set_num_threads(16)
+    bound, spread, emu = E.rew_end_logits_bounds()
+    d_rew, d_end = _rel(lr, emu[0]), _rel(le, emu[1])
+    print(f"rew_end golden: loss {loss.item():.6f} reference {float(g['loss']):.6f} (rel {e_loss:.2e}); logits rel {e_rew:.2e} {e_end:.2e} "
+          f"(bound {bound['rew']:.2e} {bound['end']:.2e}); from the emulation {d_rew:.2e} {d_end:.2e} "
+          f"(spread {spread['rew']:.2e} {spread['end']:.2e})")
+    assert e_loss < 1e-3
+    assert e_rew <= bound["rew"] and e_end <= bound["end"], (e_rew, e_end, bound)
+    assert d_rew <= SPREAD_MULTIPLE * spread["rew"] and d_end <= SPREAD_MULTIPLE * spread["end"], (d_rew, d_end, spread)
     assert torch.equal(batch.obs.cpu(), RT.frames(g["obs_substituted_u8"]))
     named = [(k, p.grad.cpu()) for k, p in model.named_parameters()]
     keys, norms, _ = O.grad_summary(named)

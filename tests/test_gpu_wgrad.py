@@ -87,6 +87,33 @@ def test_wgrad_matches_autograd(b, h, w, cin, cout, taps, stride):
     assert e32 < 2e-3, e32
 
 
+@pytest.mark.parametrize("b,h,w", [(32, 64, 64), (512, 8, 8), (16, 152, 280)], ids=["32x64x64", "512x8x8", "16x152x280"])
+def test_wgrad_many_tiles_per_cta(b, h, w):
+    """The persistent schedule at several tiles per CTA (the grid is min(tiles, SMs)): every CTA's partial sum covers a range
+    of tiles, images straddle tiles (8x8) and the rows are wide (the 280-column CSGO frame).  Against the fp16-operand float64
+    reference with the 2e-5 relative-RMS bound of test_wgrad_matches_autograd (measured, not derived), and two launches are
+    bit-identical (the partials are reduced in a fixed order)."""
+    dev = _dev()
+    from diamond_b200 import ops
+
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    tiles = -(-b * (h + 1) * (w + 1) // 128)
+    assert tiles >= 2 * sms, (tiles, sms)      # every CTA runs two tiles or more
+    g = torch.Generator(device=dev).manual_seed(b + h + w)
+    x = torch.randn(b, 64, h, w, device=dev, generator=g)
+    gy = torch.randn(b, 64, h, w, device=dev, generator=g)
+    x_op = ops.prep_act(ops.nchw_to_nhwc(x))[0]
+    g_op = ops.prep_act(ops.nchw_to_nhwc(gy))[0]
+    dw = ops.conv2d_wgrad(g_op, 64, x_op, 64, b, h, w, 64, 64, 9)
+    dw2 = ops.conv2d_wgrad(g_op, 64, x_op, 64, b, h, w, 64, 64, 9)
+    torch.cuda.synchronize()
+    ref = torch.nn.grad.conv2d_weight(_h(x).double(), (64, 64, 3, 3), _h(gy).double(), padding=1)
+    e16 = _rel(dw.reshape(64, 64, 3, 3).double(), ref)
+    print(f"wgrad B={b} {h}x{w}: {tiles} tiles on {sms} SMs, err vs fp16-operand ref {e16:.2e}")
+    assert e16 < 2e-5, e16
+    assert torch.equal(dw, dw2)
+
+
 def test_wgrad_concat_halves_scale_and_accumulate():
     """A channel-concat conv (blocks.py:174) takes its weight gradient as two launches writing disjoint Cin ranges; inv_scale
     undoes the loss scale; accumulate adds to an existing gradient; two runs are bit-identical (fixed-order reduction)."""
