@@ -960,8 +960,7 @@ struct Plan {
   float *dfilm = nullptr, *nsum = nullptr, *partial = nullptr, *scale = nullptr;
   float *dcond = nullptr, *dh = nullptr, *cpre = nullptr, *dpre = nullptr, *de = nullptr;
   unsigned int* amax = nullptr;
-  long long *film_woff = nullptr, *film_boff = nullptr;   // device tables: flat-gradient offset of every FiLM row
-  std::vector<long long> film_woff_h, film_boff_h;
+  const long long *film_woff = nullptr, *film_boff = nullptr;   // the model's FiLM gradient offsets (in its packed buffer)
   uint8_t* zero_begin = nullptr; size_t zero_bytes = 0;   // region cleared at the start of every backward (dfilm, sums, amax)
   // reward / termination training: the encoder output and the LSTM / head tape, time-major rows (row = k * segments + n)
   Tens feat{};
@@ -997,6 +996,12 @@ struct ModelCore {
   size_t packed_bytes = 0;
   int cond_channels = 0, film_rows = 0;  // FiLM table: film_rows x cond_channels weights, then film_rows biases
   size_t film_w_off = 0, film_b_off = 0;
+  // flat-gradient offset of every FiLM row (weights) / element (biases), the index tables of film_wgrad_kernel.  Model
+  // constants, so they live in the packed buffer behind the FiLM table (written by set_weights) and not in a training
+  // workspace, whose contents the caller may change between steps
+  std::vector<FilmW> films;
+  std::vector<long long> film_woff_h, film_boff_h;
+  size_t film_woff_off = 0, film_boff_off = 0;
   // training plans, one per live training workspace (an autoregressive Denoiser.forward holds several forwards before
   // their backwards run); kept apart from the inference plan so that imagination and training can alternate
   std::vector<std::unique_ptr<Plan>> tplans;
@@ -1010,7 +1015,18 @@ struct ModelCore {
     for (int i = 0; i < n_tensors; ++i) { goff[i] = grad_total; grad_total += (numel[i] + 3) & ~3ll; }
     film_w_off = pk; pk += (size_t)film_rows * cond_channels * 4; pk = (pk + 255) & ~(size_t)255;
     film_b_off = pk; pk += (size_t)film_rows * 4; pk = (pk + 255) & ~(size_t)255;
+    film_woff_h.assign(film_rows, 0); film_boff_h.assign(film_rows, 0);
+    for (const FilmW& f : films)
+      for (int r = 0; r < 2 * f.C; ++r) { film_woff_h[f.off + r] = goff[f.w_idx] + (long long)r * cond_channels; film_boff_h[f.off + r] = goff[f.b_idx] + r; }
+    film_woff_off = pk; pk += (size_t)film_rows * 8; pk = (pk + 255) & ~(size_t)255;
+    film_boff_off = pk; pk += (size_t)film_rows * 8; pk = (pk + 255) & ~(size_t)255;
     packed_bytes = pk;
+  }
+  int upload_film_offsets(cudaStream_t st) const {
+    if (film_rows == 0) return 0;
+    DMD_CUDA(cudaMemcpyAsync(packed + film_woff_off, film_woff_h.data(), (size_t)film_rows * 8, cudaMemcpyHostToDevice, st));
+    DMD_CUDA(cudaMemcpyAsync(packed + film_boff_off, film_boff_h.data(), (size_t)film_rows * 8, cudaMemcpyHostToDevice, st));
+    return 0;
   }
   // adopts the caller's tensors (`module`.state_dict() order); *moved: a tensor or the packed buffer is not where it was
   int set_weights(const char* module, const float* const* ptrs_host, int n_ptrs, void* packed_buf, bool* moved) {
@@ -1096,7 +1112,7 @@ struct Walker {  // assigns state_dict indices in module registration order and 
   }
   FilmW film(int C) {
     FilmW f; f.w_idx = next((long long)2 * C * m->cond_channels); f.b_idx = next(2 * C);
-    f.C = C; f.off = m->film_rows; m->film_rows += 2 * C; return f;
+    f.C = C; f.off = m->film_rows; m->film_rows += 2 * C; m->films.push_back(f); return f;
   }
   // c0/c1: channels of the two concatenated inputs (c1 = 0: single input)
   ResBlockW resblock(int c0, int c1, int cout, bool attn) {
@@ -1702,7 +1718,6 @@ int make_train_plan(const ModelCore& core, int cmax, int gF_ch, Plan* pl, int B,
   const int CC = core.cond_channels;
   pl->dcond = (float*)bb.take((size_t)B * CC * 4); pl->dh = (float*)bb.take((size_t)B * CC * 4); pl->cpre = (float*)bb.take((size_t)B * CC * 4);
   pl->dpre = (float*)bb.take((size_t)B * CC * 4); pl->de = (float*)bb.take((size_t)B * CC * 4);
-  pl->film_woff = (long long*)bb.take((size_t)core.film_rows * 8); pl->film_boff = (long long*)bb.take((size_t)core.film_rows * 8);
   pl->scale = (float*)bb.take(256);
   // zeroed at the start of every backward: dfilm, affine-norm sums, amax
   uint8_t* z0 = (uint8_t*)bb.take(0);
@@ -1715,12 +1730,7 @@ int make_train_plan(const ModelCore& core, int cmax, int gF_ch, Plan* pl, int B,
   pl->bytes = stats_bytes + bb.off;
   BwdBuilder bw{&core, pl};
   if (bwd(bw)) return 1;
-  // flat-gradient offsets of every FiLM row (weights) / element (biases); every ResBlock is on the tape
-  pl->film_woff_h.assign(core.film_rows, 0); pl->film_boff_h.assign(core.film_rows, 0);
-  auto fill_film = [&](const FilmW& f) {
-    for (int r = 0; r < 2 * f.C; ++r) { pl->film_woff_h[f.off + r] = core.goff[f.w_idx] + (long long)r * CC; pl->film_boff_h[f.off + r] = core.goff[f.b_idx] + r; }
-  };
-  for (const Rec& r : pl->tape) if (r.kind == R_RES) { fill_film(r.rb->n1); fill_film(r.rb->n2); }
+  pl->film_woff = (const long long*)(core.packed + core.film_woff_off); pl->film_boff = (const long long*)(core.packed + core.film_boff_off);
   return 0;
 }
 
@@ -1849,7 +1859,7 @@ extern "C" int dmd_denoiser_set_weights(dmd_denoiser* h, const float* const* ptr
   if (h->core.set_weights("InnerModel", ptrs_host, n_ptrs, packed, &moved)) return 1;
   if (moved) { h->plan.B = 0; h->core.tplans.clear(); for (auto& g : h->graphs) g.valid = false; }
   const ModelCore& m = h->core;
-  if (pack_one(m, h->conv_in, st) || pack_one(m, h->conv_out, st)) return 1;
+  if (m.upload_film_offsets(st) || pack_one(m, h->conv_in, st) || pack_one(m, h->conv_out, st)) return 1;
   for (auto& lv : h->d_blocks) for (auto& r : lv) if (pack_rb(m, r, st)) return 1;
   for (auto& lv : h->u_blocks) for (auto& r : lv) if (pack_rb(m, r, st)) return 1;
   for (auto& r : h->mid) if (pack_rb(m, r, st)) return 1;
@@ -1917,7 +1927,7 @@ Plan* find_train_plan(ModelCore& core, int B, int H, int W, int T, const void* w
 
 // make(pl, base, total): make_train_plan of the model; who: the model's name in messages
 using MakeTrainPlanFn = std::function<int(Plan*, uint8_t*, size_t*)>;
-int ensure_train_plan(ModelCore& core, const char* who, int B, int H, int W, int T, void* ws, size_t ws_bytes, cudaStream_t st,
+int ensure_train_plan(ModelCore& core, const char* who, int B, int H, int W, int T, void* ws, size_t ws_bytes,
                       const MakeTrainPlanFn& make, Plan** out) {
   DMD_CHECK(core.ready(), "%s: call dmd_%s_set_weights first", who, who);
   if ((*out = find_train_plan(core, B, H, W, T, ws)) != nullptr) return 0;
@@ -1932,8 +1942,6 @@ int ensure_train_plan(ModelCore& core, const char* who, int B, int H, int W, int
   if (tp.size() >= 8) tp.erase(tp.begin());
   std::unique_ptr<Plan> pl(new Plan());
   if (make(pl.get(), (uint8_t*)ws, nullptr)) return 1;
-  DMD_CUDA(cudaMemcpyAsync(pl->film_woff, pl->film_woff_h.data(), pl->film_woff_h.size() * 8, cudaMemcpyHostToDevice, st));
-  DMD_CUDA(cudaMemcpyAsync(pl->film_boff, pl->film_boff_h.data(), pl->film_boff_h.size() * 8, cudaMemcpyHostToDevice, st));
   *out = pl.get();
   tp.push_back(std::move(pl));
   return 0;
@@ -2006,7 +2014,7 @@ extern "C" int dmd_inner_model_forward_train(dmd_denoiser* h, int B, int H, int 
   cudaStream_t st = (cudaStream_t)stream;
   Plan* pl = nullptr;
   auto make = [h, B, H, W](Plan* p, uint8_t* base, size_t* total) { return make_denoiser_train_plan(h, p, B, H, W, base, total); };
-  if (ensure_train_plan(h->core, "denoiser", B, H, W, 1, workspace, workspace_bytes, st, make, &pl)) return 1;
+  if (ensure_train_plan(h->core, "denoiser", B, H, W, 1, workspace, workspace_bytes, make, &pl)) return 1;
   pl->t_act = act;
   if (run_forward(h, *pl, noisy_rescaled, c_noise, c_noise_is_scalar, obs_rescaled, act, st, 1)) return 1;
   return run_wrap(h, *pl, noisy_rescaled, out, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1.f, 0.f, st);
@@ -2020,7 +2028,7 @@ extern "C" int dmd_inner_model_forward_train_u8(dmd_denoiser* h, int B, int H, i
   cudaStream_t st = (cudaStream_t)stream;
   Plan* pl = nullptr;
   auto make = [h, B, H, W](Plan* p, uint8_t* base, size_t* total) { return make_denoiser_train_plan(h, p, B, H, W, base, total); };
-  if (ensure_train_plan(h->core, "denoiser", B, H, W, 1, workspace, workspace_bytes, st, make, &pl)) return 1;
+  if (ensure_train_plan(h->core, "denoiser", B, H, W, 1, workspace, workspace_bytes, make, &pl)) return 1;
   pl->t_act = act;
   if (run_forward(h, *pl, noisy_rescaled, c_noise, c_noise_is_scalar, nullptr, act, st, 1, StackView{}, -1, &u8)) return 1;
   return run_wrap(h, *pl, noisy_rescaled, out, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1.f, 0.f, st);
@@ -2739,7 +2747,7 @@ extern "C" int dmd_rew_end_set_weights(dmd_rew_end* h, const float* const* ptrs_
   if (h->core.set_weights("RewEndModel", ptrs_host, n_ptrs, packed, &moved)) return 1;
   if (moved) { h->lay.plan.B = 0; h->core.tplans.clear(); }   // plans bake parameter and packed-weight addresses in
   const ModelCore& m = h->core;
-  if (pack_one(m, h->conv_in, st)) return 1;
+  if (m.upload_film_offsets(st) || pack_one(m, h->conv_in, st)) return 1;
   for (auto& lv : h->blocks) for (auto& r : lv) if (pack_rb(m, r, st)) return 1;
   for (int i = 1; i < h->cfg.num_levels; ++i) if (pack_one(m, h->downs[i], st)) return 1;
   return 0;
@@ -2843,7 +2851,7 @@ int rew_end_forward_train(dmd_rew_end* h, int b, int t, const float* obs, const 
   cudaStream_t st = (cudaStream_t)stream;
   Plan* pl = nullptr;
   auto make = [h, b, t](Plan* p, uint8_t* base, size_t* total) { return make_rew_end_train_plan(h, p, b, t, base, total); };
-  if (ensure_train_plan(h->core, "rew_end", b * t, S, S, t, workspace, workspace_bytes, st, make, &pl)) return 1;
+  if (ensure_train_plan(h->core, "rew_end", b * t, S, S, t, workspace, workspace_bytes, make, &pl)) return 1;
   pl->t_act = pl->act_tm;
   if (rew_end_encode(h, *pl, b, t, obs, next_obs, act, pl->act_tm, st, u8)) return 1;
   // hseq = [h_in; y], cseq = [c_in; c_1 ... c_t]

@@ -10,6 +10,24 @@
  *     allocate on the hot path (the caller owns every buffer, including the workspace)
  *   - return value 0 = ok; nonzero = error, message via dmd_last_error() (thread-local)
  *   - one host thread per GPU (the reference is one process per rank, src/main.py:26)
+ *
+ * Workspace contract (what the caller may do with its buffers between calls; tests/test_gpu_poisoned_buffers.py checks it)
+ *   Scratch -- contents undefined on entry and after the call; every byte a call reads it has written first in the same call,
+ *   so the caller may reuse the memory for anything in between:
+ *     - the inference workspaces of dmd_denoiser_forward, dmd_inner_model_forward[_u8], dmd_sampler_sample (also between
+ *       replays of its graph), dmd_actor_critic_forward when no backward follows, dmd_rew_end_predict[_u8];
+ *     - a training workspace before its *_forward_train and after its *_backward (so between optimizer steps);
+ *     - the `scratch` of dmd_actor_critic_backward[_accumulate], the `partial` buffers of dmd_conv2d_wgrad, dmd_sgemm and
+ *       dmd_grad_norm_clip;
+ *     - every output: logits, states, model outputs, out_x, trajectory slots >= 1, the flat gradient buffer of
+ *       dmd_denoiser_backward / dmd_rew_end_backward / dmd_actor_critic_backward (fully written), g_*_in, norm_coef.
+ *   Kept -- must not be touched by the caller while the library relies on it:
+ *     - a training workspace from dmd_inner_model_forward_train[_u8] / dmd_rew_end_forward_train[_u8] to its backward, and an
+ *       actor-critic workspace from dmd_actor_critic_forward to its backward (it holds the activations);
+ *     - the flat gradient buffer of dmd_actor_critic_backward_accumulate (it is added to);
+ *     - the packed-weight buffers (conv packs, FiLM table and the FiLM gradient offsets, written by *_set_weights), the
+ *       optimizer state (param, exp_avg, exp_avg_sq), and the frame / action rings a sampler reads (ring_head >= 0);
+ *     - every input, including trajectory slot 0 and the churn noise `eps`.
  */
 #ifndef DIAMOND_B200_H_
 #define DIAMOND_B200_H_
