@@ -24,8 +24,8 @@ class ConvDesc(C.Structure):
     _fields_ = [
         ("src0", _vp), ("src1", _vp), ("C0", _i), ("C1", _i), ("B", _i), ("H", _i), ("W", _i), ("taps", _i), ("stride", _i),
         ("wpk", _vp), ("bias", _vp), ("Cout", _i), ("CoutPad", _i),
-        ("residual", _vp), ("out", _vp), ("out_stats", _vp), ("out_gs", _i), ("debug", _i), ("debug_buf", _vp),
-        ("precise", _i), ("wpk_layout", _i), ("src0_lo", _vp), ("src1_lo", _vp),
+        ("residual", _vp), ("out", _vp), ("out_stats", _vp), ("out_gs", _i),
+        ("precise", _i), ("src0_lo", _vp), ("src1_lo", _vp),
         ("xsrc0", _vp), ("xsrc1", _vp), ("xsrc0_lo", _vp), ("xsrc1_lo", _vp), ("xC0", _i), ("xC1", _i), ("wpk_x", _vp), ("bias_x", _vp),
     ]
 
@@ -62,7 +62,7 @@ class SamplerConfigC(C.Structure):
 class WgradDesc(C.Structure):  # dmd_wgrad_desc
     _fields_ = [("grad", _vp), ("act", _vp), ("Cg", _i), ("Ca", _i), ("B", _i), ("H", _i), ("W", _i), ("taps", _i),
                 ("dW", _vp), ("Cout", _i), ("Cin", _i), ("CinTot", _i), ("ci_off", _i), ("inv_scale", _vp),
-                ("accumulate", _i), ("partial", _vp), ("partial_bytes", _sz), ("debug", _i)]
+                ("accumulate", _i), ("partial", _vp), ("partial_bytes", _sz)]
 
 
 class ConvPlanInfo(C.Structure):  # dmd_conv_plan_info

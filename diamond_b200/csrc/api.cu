@@ -123,23 +123,9 @@ static size_t plc16_bytes(int B, int H, int W, int C) {
 }
 extern "C" size_t dmd_plc16_bytes(int B, int H, int W, int C) { return plc16_bytes(B, H, W, C); }
 
-// Tuning knobs (read once per name): integers from the environment, for sweeps on the GPU box without a rebuild.
-static int tune_int(const char* name, int dflt) {
-  static std::mutex mu;
-  static std::map<std::string, int> cache;
-  std::lock_guard<std::mutex> lk(mu);
-  auto it = cache.find(name);
-  if (it != cache.end()) return it->second;
-  const char* v = getenv(name);
-  const int r = (v && *v) ? atoi(v) : dflt;
-  cache[name] = r;
-  return r;
-}
-
 static int conv_fill(const dmd_conv_desc* d, ConvParams* p, size_t* smem, int* acc_cols) {
   DMD_CHECK(d->src0 && d->out && d->wpk, "conv: null src0/out/wpk");
   DMD_CHECK(d->taps == 9 || d->taps == 1, "conv: taps must be 1 or 9 (got %d)", d->taps);
-  DMD_CHECK(d->debug == 0 && d->debug_buf == nullptr, "conv: debug / debug_buf must be 0 / NULL (the kernel has no bring-up switches)");
   DMD_CHECK(d->stride == 1 || d->stride == 2, "conv: stride must be 1 or 2");
   DMD_CHECK(d->C0 > 0 && d->C0 % 16 == 0 && d->C1 % 16 == 0 && d->C0 + d->C1 <= kMaxCin, "conv: operand channels must be multiples of 16, total <= %d (C0=%d C1=%d)", kMaxCin, d->C0, d->C1);
   DMD_CHECK((d->C1 == 0) == (d->src1 == nullptr), "conv: src1/C1 mismatch");
@@ -183,9 +169,6 @@ static int conv_fill(const dmd_conv_desc* d, ConvParams* p, size_t* smem, int* a
   const Plc g = plc_geometry(d->B, d->H, d->W);
   p->PW = g.PW; p->PH = g.PH; p->Q = g.Q; p->G = g.G; p->plane_bytes = (unsigned long long)g.Qalloc * 16;
   DMD_CHECK((long long)g.Q * (g.PW > g.PH ? g.PW : g.PH) < (1ll << 32), "conv: problem too large for 32-bit position math");
-  // tap-row-stacked weights: dmd_pack_conv_weight(precise = 3); the kernel addresses tap (dy, dx) inside kernel row dy
-  p->trs = d->wpk_layout == 1 ? 1 : 0;
-  if (p->trs) DMD_CHECK(d->taps == 9 && !d->precise && 3 * d->CoutPad <= 256, "conv: row-stacked weights need a 3x3, non-split conv with CoutPad <= 80");
   const int halo = d->taps == 9 ? g.PW + 1 : 0;
   p->P = kTileM + 2 * halo; p->Palloc = p->P | 1;
   if (d->out_stats) {
@@ -241,8 +224,6 @@ static int init_kernels() {
     DMD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(attn_cluster_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(attn_cluster_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(attn_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(attn_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(linear_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
@@ -267,7 +248,7 @@ static int launch_pdl(Kernel kernel, dim3 grid, dim3 block, size_t smem, cudaStr
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = tune_int("DMD_NO_PDL", 0) ? 0 : 1;   // bring-up switch: plain stream-ordered launches
+  cfg.attrs = attr; cfg.numAttrs = 1;
   DMD_CUDA(cudaLaunchKernelEx(&cfg, kernel, p));
   DMD_LAUNCH_OK();
   return 0;
@@ -319,7 +300,7 @@ static int prep_fill(const dmd_prep_desc* d, PrepParams* p, int* nsrc) {
   DMD_CHECK(g.PH * g.PW >= 32, "prep: image too small");
   // a block touches at most 2 images; low-resolution levels get smaller blocks so that the grid still covers the SMs
   int ppb = g.PH * g.PW >= 256 ? 256 : (g.PH * g.PW / 32) * 32;
-  while (ppb > 64 && (g.Qalloc + ppb - 1) / ppb < tune_int("DMD_PREP_MIN_BLOCKS", 2 * kPlanSms)) ppb >>= 1;
+  while (ppb > 64 && (g.Qalloc + ppb - 1) / ppb < 2 * kPlanSms) ppb >>= 1;
   ppb = (ppb / 32) * 32;
   p->pos_per_block = ppb;
   // both kernels keep (mean, rstd) of at most 4 groups per image slot in shared memory, for every source
@@ -341,7 +322,7 @@ static int prep_launch(const PrepParams& p0, int nsrc, cudaStream_t st) {
   const dim3 grid((p.Qalloc + p.pos_per_block - 1) / p.pos_per_block, 1, nsrc);
   // the hot cases (norm + SiLU, no upsample, no low part of the normalised operand; raw + raw-low on every source or on none)
   // run on the lean kernel; everything else on the generic one
-  bool fast = tune_int("DMD_PREP_FAST", 1) != 0 && p.mode != 0 && p.act && p.ups == 0;
+  bool fast = p.mode != 0 && p.act && p.ups == 0;
   const bool raw = p.s[0].dst_raw != nullptr;
   for (int k = 0; k < nsrc && fast; ++k) {
     const PrepSrc& S = p.s[k];
@@ -399,7 +380,7 @@ struct WgradLaunch { WgradParams wp; WgradReduceParams rp; size_t smem; int grid
 static size_t wgrad_partial_bytes(int num_sms) { return (size_t)num_sms * kWgTaps * 64 * 64 * sizeof(float); }
 
 static int wgrad_fill(const void* grad, int Cg, const void* act, int Ca, int B, int H, int W, int taps, float* partial,
-                      int Cout, int Cin, int CinTot, int ci_off, const float* inv_scale, int accumulate, int debug, WgradLaunch* L) {
+                      int Cout, int Cin, int CinTot, int ci_off, const float* inv_scale, int accumulate, WgradLaunch* L) {
   DMD_CHECK(grad && act && partial, "wgrad: null operand / partial buffer");
   DMD_CHECK(taps == 9 || taps == 1, "wgrad: taps must be 1 or 9");
   DMD_CHECK(Cg % 8 == 0 && Cg > 0 && Cg <= 64, "wgrad: gradient operand channels must be a multiple of 8, <= 64 (got %d)", Cg);
@@ -422,7 +403,7 @@ static int wgrad_fill(const void* grad, int Cg, const void* act, int Ca, int B, 
   if (stages > kWgStagesMax) stages = kWgStagesMax;
   DMD_CHECK(stages >= 2, "wgrad: image too wide for the shared-memory stage (W=%d)", W);
   wp.stages = stages;
-  wp.partial = partial; wp.dbg = debug;
+  wp.partial = partial;
   L->smem = wgrad_smem(wp.nB, wp.halo, stages).total;
   L->grid = wp.num_tiles < g_num_sms ? wp.num_tiles : g_num_sms;
   WgradReduceParams& rp = L->rp;
@@ -454,7 +435,7 @@ extern "C" int dmd_conv2d_wgrad(const dmd_wgrad_desc* d, void* stream) {
   DMD_CHECK(d->partial_bytes >= wgrad_partial_bytes(g_num_sms), "wgrad: partial buffer too small (%zu < %zu)", d->partial_bytes, wgrad_partial_bytes(g_num_sms));
   WgradLaunch L;
   if (wgrad_fill(d->grad, d->Cg, d->act, d->Ca, d->B, d->H, d->W, d->taps, (float*)d->partial, d->Cout, d->Cin, d->CinTot, d->ci_off,
-                 d->inv_scale, d->accumulate, d->debug, &L)) return 1;
+                 d->inv_scale, d->accumulate, &L)) return 1;
   return wgrad_launch(L, d->dW, (cudaStream_t)stream);
 }
 extern "C" int dmd_pack_conv_weight_dgrad(const float* w, void* wpk, int CoutF, int CinTotF, int ci_off, int CinK, int taps, void* stream) {
@@ -469,14 +450,7 @@ extern "C" int dmd_pack_conv_weight_dgrad(const float* w, void* wpk, int CoutF, 
 extern "C" int dmd_pack_conv_weight(const float* w, void* wpk, int Cout, int CoutPad, int CinReal, int Cin, int taps,
                                     int c0_real, int c0_store, int precise, void* stream) {
   DMD_CHECK(w && wpk, "pack: null pointer");
-  if (precise == 3) {   // tap-row-stacked layout [dy][Cin/8][3 * CoutPad][8]: column dx * CoutPad + co of kernel row dy
-    DMD_CHECK(taps == 9, "pack: the row-stacked layout is for 3x3 kernels");
-    const int total3 = 9 * Cin * CoutPad;
-    pack_conv_weight_trs_kernel<<<(total3 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(w, (__half*)wpk, Cout, CoutPad, CinReal, Cin, c0_real, c0_store);
-    DMD_LAUNCH_OK();
-    return 0;
-  }
-  DMD_CHECK(precise >= 0 && precise <= 2, "pack: precise must be 0, 1 (split [W_hi | W_hi | W_lo]), 2 (low parts only) or 3 (row-stacked)");
+  DMD_CHECK(precise >= 0 && precise <= 2, "pack: precise must be 0, 1 (split [W_hi | W_hi | W_lo]) or 2 (low parts only)");
   const int total = taps * Cin * CoutPad * (precise == 1 ? 3 : 1);
   pack_conv_weight_kernel<<<(total + 255) / 256, 256, 0, (cudaStream_t)stream>>>(w, (__half*)wpk, Cout, CoutPad, CinReal, Cin, taps, c0_real, c0_store, precise);
   DMD_LAUNCH_OK();
@@ -497,11 +471,13 @@ extern "C" int dmd_gn_stats(const float* x, double* stats, int B, int HW, int C,
 // scratch of the any-L attention path (q, k, v of every token); L = 64 runs in one launch without scratch
 static size_t attn_scratch_bytes(int B, int L, int C) { return L == kAttnL ? 0 : (size_t)B * L * 3 * C * sizeof(float); }
 
-// L = 64 (the 8x8 level of a 64x64 frame): one launch of attn_cluster_kernel / attn_kernel.  Any other L: attn_qkv_kernel, then
+// L = 64 (the 8x8 level of a 64x64 frame): one launch of attn_cluster_kernel.  Any other L: attn_qkv_kernel, then
 // attn_stream_kernel, through p.scratch (attn_scratch_bytes)
 static int attn_launch(const AttnParams& p, int B, cudaStream_t st) {
   DMD_CHECK((p.C == 64 || p.C == 32) && p.L >= 1 && p.C % p.gs == 0 && p.gs % 8 == 0,
             "attn: unsupported shape L=%d C=%d gs=%d (C in {32, 64}, groups of a multiple of 8 channels)", p.L, p.C, p.gs);
+  // attn_cluster_kernel adds the output statistics of each CTA's C/4 channels to one GroupNorm group
+  DMD_CHECK(p.L != kAttnL || p.gs % (p.C / 4) == 0, "attn: L=%d needs gs a multiple of C/4 (C=%d gs=%d)", kAttnL, p.C, p.gs);
   if (init_kernels()) return 1;
   if (p.L != kAttnL) {
     DMD_CHECK(p.scratch && ((uintptr_t)p.scratch & 15) == 0, "attn: L=%d needs 16-byte aligned scratch of dmd_attn_scratch_bytes", p.L);
@@ -518,20 +494,13 @@ static int attn_launch(const AttnParams& p, int B, cudaStream_t st) {
     DMD_LAUNCH_OK();
     return 0;
   }
-  const size_t smem = sizeof(float) * ((size_t)p.L * (p.C + 1) * 2 + (size_t)p.L * (3 * p.C + 4));
   AttnParams pt = p;
   pt.ktrace = kt_slot("attn", B, p.C);
-  if (tune_int("DMD_ATTN_CLUSTER", 1) != 0 && p.gs % (p.C / 4) == 0) {
-    // four CTAs per image (thread-block cluster), distributed shared memory for the head outputs
-    const int CH = p.C / 4;
-    const size_t csmem = sizeof(float) * ((size_t)p.L * (p.C + 1) * 2 + (size_t)p.L * (3 * CH + 4) + (size_t)p.L * CH + (size_t)4 * CH * p.C);
-    if (p.C == 64) attn_cluster_kernel<64><<<4 * B, kAttnCThreads, csmem, st>>>(pt);
-    else attn_cluster_kernel<32><<<4 * B, kAttnCThreads, csmem, st>>>(pt);
-    DMD_LAUNCH_OK();
-    return 0;
-  }
-  if (p.C == 64) attn_kernel<64><<<B, kAttnThreads, smem, st>>>(pt);
-  else attn_kernel<32><<<B, kAttnThreads, smem, st>>>(pt);
+  // four CTAs per image (thread-block cluster), distributed shared memory for the head outputs
+  const int CH = p.C / 4;
+  const size_t csmem = sizeof(float) * ((size_t)p.L * (p.C + 1) * 2 + (size_t)p.L * (3 * CH + 4) + (size_t)p.L * CH + (size_t)4 * CH * p.C);
+  if (p.C == 64) attn_cluster_kernel<64><<<4 * B, kAttnCThreads, csmem, st>>>(pt);
+  else attn_cluster_kernel<32><<<4 * B, kAttnCThreads, csmem, st>>>(pt);
   DMD_LAUNCH_OK();
   return 0;
 }
@@ -543,10 +512,9 @@ static int linear_launch(const float* in, const float* W, const float* bias, flo
   if (init_kernels()) return 1;
   // enough blocks to cover the SMs: 8, 16 or 32 output features per block
   const int by = (B + 31) / 32;
-  const int forceJ = tune_int("DMD_LINEAR_J", 0);
-  if (forceJ == 4 || (forceJ == 0 && (long long)((F + 31) / 32) * by >= 2 * kPlanSms))
+  if ((long long)((F + 31) / 32) * by >= 2 * kPlanSms)
     linear_kernel<4><<<dim3((F + 31) / 32, by), 256, (size_t)(32 + 32) * kLinChunk * sizeof(float), st>>>(in, W, bias, out, B, K, F, silu, accumulate, hw_perm);
-  else if (forceJ == 2 || (forceJ == 0 && (long long)((F + 15) / 16) * by >= kPlanSms))
+  else if ((long long)((F + 15) / 16) * by >= kPlanSms)
     linear_kernel<2><<<dim3((F + 15) / 16, by), 256, (size_t)(16 + 32) * kLinChunk * sizeof(float), st>>>(in, W, bias, out, B, K, F, silu, accumulate, hw_perm);
   else
     linear_kernel<1><<<dim3((F + 7) / 8, by), 256, (size_t)(8 + 32) * kLinChunk * sizeof(float), st>>>(in, W, bias, out, B, K, F, silu, accumulate, hw_perm);
@@ -876,7 +844,6 @@ struct ConvW {          // one nn.Conv2d
   int w_idx, b_idx;     // indices into the state_dict pointer list
   int Cout, CoutPad, CinReal, Cin, taps, c0_real, c0_store;
   int precise = 0;      // split-fp16 in one launch: K = 3 * Cin
-  int trs = 0;          // forward weights in the tap-row-stacked layout (3x3, non-split)
   int three_pass = 0;   // split-fp16 as three launches (A_hi W_hi, A_lo W_hi, A_hi W_lo): 3 * Cin weights would crowd out the slab ring
   size_t pk_off;        // byte offset into the packed-weight buffer
   size_t pk_lo_off = 0; // three_pass: the low-part pack
@@ -1098,9 +1065,6 @@ struct Walker {  // assigns state_dict indices in module registration order and 
     const size_t w1 = (size_t)taps * c.Cin * c.CoutPad * 2;
     c.precise = split && 3 * w1 <= 120 * 1024;
     c.three_pass = split && !c.precise;
-    // tap-row-stacked weight layout: opt-in (DMD_CONV_TRS=1).  The conv kernel addresses each tap inside it, so the layout
-    // changes the weight packing only, not the tensor-core work
-    c.trs = (taps == 9 && !split && 3 * c.CoutPad <= 256 && tune_int("DMD_CONV_TRS", 0) != 0) ? 1 : 0;
     c.pk_off = take(w1 * (c.precise ? 3 : 1));
     if (c.three_pass) c.pk_lo_off = take(w1);
     if (dgrad) {
@@ -1288,7 +1252,7 @@ struct PlanBuilder {
     }
     const bool split = cw.precise || cw.three_pass;
     d.src0 = raw ? in.r0 : in.n0; d.src1 = in.C1 ? (raw ? in.r1 : in.n1) : nullptr;
-    d.precise = cw.precise; d.wpk_layout = cw.trs;
+    d.precise = cw.precise;
     if (split) { d.src0_lo = raw ? in.rl0 : in.nl0; d.src1_lo = in.C1 ? in.rl1 : nullptr; }
     d.C0 = in.C0; d.C1 = in.C1; d.B = pl->B; d.H = in.H; d.W = in.W; d.taps = cw.taps; d.stride = stride;
     d.wpk = pk(cw.pk_off); d.bias = P(cw.b_idx);
@@ -1520,7 +1484,7 @@ struct BwdBuilder {
   void wgrad(const ConvW& cw, const uint8_t* gy, const uint8_t* act, int Ca, int Cin, int ci_off, int H, int W) {
     BOp b; b.kind = B_WGRAD; b.goff = G(cw.w_idx);
     if (wgrad_fill(gy ? gy : (const void*)1, round_up(cw.Cout, 16), act ? act : (const void*)1, Ca, pl->B, H, W, cw.taps,
-                   pl->partial ? pl->partial : (float*)1, cw.Cout, Cin, cw.CinReal, ci_off, pl->scale ? pl->scale + 1 : (const float*)1, 1, 0, &b.wg)) { err = 1; return; }
+                   pl->partial ? pl->partial : (float*)1, cw.Cout, Cin, cw.CinReal, ci_off, pl->scale ? pl->scale + 1 : (const float*)1, 1, &b.wg)) { err = 1; return; }
     push(b);
   }
   void norm_bwd(const Tens& x, const float* gy, int mode, const FilmW* film, int c_off, int ctot, int gamma_idx, int beta_idx,
@@ -1835,7 +1799,7 @@ extern "C" size_t dmd_denoiser_packed_bytes(const dmd_denoiser* h) { return h->c
 
 static int pack_one(const ModelCore& m, const ConvW& c, cudaStream_t st) {
   const float* w = m.ptrs[c.w_idx];
-  if (dmd_pack_conv_weight(w, m.packed + c.pk_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, c.trs ? 3 : c.precise, st)) return 1;
+  if (dmd_pack_conv_weight(w, m.packed + c.pk_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, c.precise, st)) return 1;
   if (c.three_pass && dmd_pack_conv_weight(w, m.packed + c.pk_lo_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, 2, st)) return 1;
   for (int k = 0; k < c.nsrcT; ++k)  // backward-data packs (transposed, flipped), one per concat source
     if (dmd_pack_conv_weight_dgrad(w, m.packed + c.pkT_off[k], c.Cout, c.CinReal, c.srcOff[k], c.srcC[k], c.taps, st)) return 1;
@@ -2467,7 +2431,7 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
   const float* inv = sc.scale + 1;
   auto wgrad = [&](const ConvW& cw, const uint8_t* gy, const uint8_t* act, int Ca, int hw) -> int {
     WgradLaunch L;
-    if (wgrad_fill(gy, round_up(cw.Cout, 16), act, Ca, B, hw, hw, cw.taps, sc.partial, cw.Cout, cw.CinReal, cw.CinReal, 0, inv, 1, 0, &L)) return 1;
+    if (wgrad_fill(gy, round_up(cw.Cout, 16), act, Ca, B, hw, hw, cw.taps, sc.partial, cw.Cout, cw.CinReal, cw.CinReal, 0, inv, 1, &L)) return 1;
     return wgrad_launch(L, G(cw.w_idx), st);
   };
   // spatial size of every level's input

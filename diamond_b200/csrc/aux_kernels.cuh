@@ -274,7 +274,7 @@ __global__ void lstm_gates_kernel(const float* __restrict__ gates, const float* 
 }
 
 // ------------------------------------------------------------------------------------------------
-// SelfAttention2d (blocks.py:51-72), one CTA (512 threads) per image, L = 64 tokens, C in {32, 64}, head_dim 8.
+// SelfAttention2d (blocks.py:51-72), C in {32, 64}, head_dim 8.
 //   xn = GroupNorm(x) ; qkv = 1x1 ; att = softmax(q k^T / sqrt(d)) ; y = att v ; out = xn + out_proj(y)
 // NOTE the residual is added to the NORMED x (blocks.py:64 rebinding, :72).  Input stats come from the producer's
 // epilogue; output stats (for the next AdaGroupNorm) are accumulated here.
@@ -295,130 +295,12 @@ struct AttnParams {
   float* scratch = nullptr;  // L != 64: q | k | v of every token, [B][3][C/8][L][8] (attn_qkv_kernel -> attn_stream_kernel)
 };
 
-constexpr int kAttnThreads = 512;
+constexpr int kAttnThreads = 512;   // attn_bwd_kernel: one CTA per image
 constexpr int kAttnL = 64;
 
-template <int C>
-__global__ void __launch_bounds__(kAttnThreads) attn_kernel(const AttnParams p) {
-  constexpr int L = kAttnL, C3 = 3 * C, XP = C + 1, QP = C3 + 4, HEADS = C / 8;
-  extern __shared__ __align__(16) float sm_attn[];
-  float* xs = sm_attn;          // [L][XP]   normed x
-  float* qkv = xs + L * XP;     // [L][QP]   (QP*4 bytes is a multiple of 16: rows are float4-addressable)
-  float* ys = qkv + L * QP;     // [L][XP]
-  const int n = blockIdx.x, tid = threadIdx.x;
-  if (n == 0 && tid == 0) ktrace_stamp(p.ktrace);
-  const int G = C / p.gs;
-  const float* xg = p.x + (size_t)n * L * C;
-  for (int i = tid; i < L * C; i += kAttnThreads) {
-    const int l = i / C, c = i - l * C;
-    const int g = c / p.gs;
-    const double cnt = (double)L * p.gs;
-    const double mean = p.st_in[((size_t)n * G + g) * 2] / cnt;
-    double var = p.st_in[((size_t)n * G + g) * 2 + 1] / cnt - mean * mean;
-    var = var > 0.0 ? var : 0.0;
-    const float rstd = (float)(1.0 / sqrt(var + (double)p.eps));
-    xs[l * XP + c] = (xg[i] - (float)mean) * rstd * p.gamma[c] + p.beta[c];
-  }
-  __syncthreads();
-  // ---- qkv projection.  thread = (token l, output group og of NO outputs); warp = 32 tokens, one og (weights broadcast)
-  {
-    constexpr int NG = kAttnThreads / L;  // 8 output groups
-    constexpr int NO = C3 / NG;           // 24 (C=64) or 12 (C=32) outputs per thread
-    const int l = tid % L, og = tid / L;
-    float acc[NO];
-#pragma unroll
-    for (int i = 0; i < NO; ++i) acc[i] = __ldg(p.bqkv + og * NO + i);
-    for (int c4 = 0; c4 < C / 4; ++c4) {
-      const float x0 = xs[l * XP + 4 * c4], x1 = xs[l * XP + 4 * c4 + 1], x2 = xs[l * XP + 4 * c4 + 2], x3 = xs[l * XP + 4 * c4 + 3];
-#pragma unroll
-      for (int i = 0; i < NO; ++i) {
-        const float4 w = __ldg(reinterpret_cast<const float4*>(p.wqkv + (size_t)(og * NO + i) * C) + c4);
-        acc[i] = fmaf(w.x, x0, acc[i]); acc[i] = fmaf(w.y, x1, acc[i]);
-        acc[i] = fmaf(w.z, x2, acc[i]); acc[i] = fmaf(w.w, x3, acc[i]);
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < NO; ++i) qkv[l * QP + og * NO + i] = acc[i];
-  }
-  __syncthreads();
-  // ---- attention: item = (head h, query l); K/V rows are warp-broadcast float4 reads
-  for (int it = tid; it < HEADS * L; it += kAttnThreads) {
-    const int h = it / L, l = it - h * L;
-    float q[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) q[e] = qkv[l * QP + h * 8 + e] * 0.35355339059327373f;  // 1/sqrt(8)
-    float sc[L];
-    float mx = -INFINITY;
-#pragma unroll
-    for (int j = 0; j < L; ++j) {
-      const float4 k0 = *reinterpret_cast<const float4*>(qkv + j * QP + C + h * 8);
-      const float4 k1 = *reinterpret_cast<const float4*>(qkv + j * QP + C + h * 8 + 4);
-      float sj = q[0] * k0.x;
-      sj = fmaf(q[1], k0.y, sj); sj = fmaf(q[2], k0.z, sj); sj = fmaf(q[3], k0.w, sj);
-      sj = fmaf(q[4], k1.x, sj); sj = fmaf(q[5], k1.y, sj); sj = fmaf(q[6], k1.z, sj); sj = fmaf(q[7], k1.w, sj);
-      sc[j] = sj;
-      mx = fmaxf(mx, sj);
-    }
-    float den = 0.f;
-#pragma unroll
-    for (int j = 0; j < L; ++j) { sc[j] = expf(sc[j] - mx); den += sc[j]; }
-    const float inv = 1.0f / den;
-    float y[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-#pragma unroll
-    for (int j = 0; j < L; ++j) {
-      const float4 v0 = *reinterpret_cast<const float4*>(qkv + j * QP + 2 * C + h * 8);
-      const float4 v1 = *reinterpret_cast<const float4*>(qkv + j * QP + 2 * C + h * 8 + 4);
-      const float pj = sc[j] * inv;
-      y[0] = fmaf(pj, v0.x, y[0]); y[1] = fmaf(pj, v0.y, y[1]); y[2] = fmaf(pj, v0.z, y[2]); y[3] = fmaf(pj, v0.w, y[3]);
-      y[4] = fmaf(pj, v1.x, y[4]); y[5] = fmaf(pj, v1.y, y[5]); y[6] = fmaf(pj, v1.z, y[6]); y[7] = fmaf(pj, v1.w, y[7]);
-    }
-#pragma unroll
-    for (int e = 0; e < 8; ++e) ys[l * XP + h * 8 + e] = y[e];
-  }
-  __syncthreads();
-  // ---- out projection + residual on normed x; output statistics.  thread = (token l, NO2 outputs)
-  {
-    constexpr int NG = kAttnThreads / L;  // 8
-    constexpr int NO2 = C / NG;           // 8 or 4 consecutive outputs: always inside one GroupNorm group
-    const int l = tid % L, og = tid / L;
-    float acc[NO2];
-#pragma unroll
-    for (int i = 0; i < NO2; ++i) acc[i] = __ldg(p.bout + og * NO2 + i);
-    for (int c4 = 0; c4 < C / 4; ++c4) {
-      const float y0 = ys[l * XP + 4 * c4], y1 = ys[l * XP + 4 * c4 + 1], y2 = ys[l * XP + 4 * c4 + 2], y3 = ys[l * XP + 4 * c4 + 3];
-#pragma unroll
-      for (int i = 0; i < NO2; ++i) {
-        const float4 w = __ldg(reinterpret_cast<const float4*>(p.wout + (size_t)(og * NO2 + i) * C) + c4);
-        acc[i] = fmaf(w.x, y0, acc[i]); acc[i] = fmaf(w.y, y1, acc[i]);
-        acc[i] = fmaf(w.z, y2, acc[i]); acc[i] = fmaf(w.w, y3, acc[i]);
-      }
-    }
-    float* og_ptr = p.out + (size_t)n * L * C + (size_t)l * C + og * NO2;
-    float a = 0.f, b = 0.f;
-#pragma unroll
-    for (int i = 0; i < NO2; ++i) {
-      const float v = xs[l * XP + og * NO2 + i] + acc[i];
-      og_ptr[i] = v;
-      a += v; b += v * v;
-    }
-    if (p.ostats) {
-#pragma unroll
-      for (int off = 16; off > 0; off >>= 1) {
-        a += __shfl_xor_sync(0xffffffffu, a, off);
-        b += __shfl_xor_sync(0xffffffffu, b, off);
-      }
-      if ((tid & 31) == 0) {
-        const int g = (og * NO2) / p.gs;
-        atomicAdd(p.ostats + ((size_t)n * G + g) * 2, (double)a);
-        atomicAdd(p.ostats + ((size_t)n * G + g) * 2 + 1, (double)b);
-      }
-    }
-  }
-}
-
 // ------------------------------------------------------------------------------------------------
-// SelfAttention2d on a CLUSTER of four CTAs per image (same math as attn_kernel above, same parameter block).
-// The one-CTA-per-image kernel keeps only 32 SMs busy at the benchmark batch and runs ~5 k instructions per thread.  Here cluster rank r owns C/4 channels = C/32 heads:
+// SelfAttention2d at L = 64 (the 8x8 level of a 64x64 frame) on a CLUSTER of four CTAs per image.
+// One CTA per image would keep only 32 SMs busy at the benchmark batch.  Here cluster rank r owns C/4 channels = C/32 heads:
 //   every CTA   : GroupNorm(x) for all channels (its q/k/v rows contract over all of them)
 //   rank r      : q, k, v rows of its heads -> softmax(q k^T / sqrt(d)) v with the 64 keys split over 2 (C=64) or 4 (C=32)
 //                 threads per (head, query) and merged with shuffles -> its C/4 channels of y in ITS shared memory
@@ -597,7 +479,7 @@ __global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(kAttnCThreads) attn_
 }
 
 // ------------------------------------------------------------------------------------------------
-// SelfAttention2d over any token count L >= 1 (same math as attn_kernel, same parameter block plus p.scratch), in two launches
+// SelfAttention2d over any token count L >= 1 (same math as attn_cluster_kernel, same parameter block plus p.scratch), in two launches
 // of grid (ceil(L / 32), B):
 //   attn_qkv_kernel   : 32 tokens per CTA: GroupNorm(x) from the producer's statistics, the qkv 1x1 projection into p.scratch,
 //                       head-major [B][3][C/8][L][8] (q, k, v), so that the keys of one head are contiguous
@@ -610,7 +492,7 @@ constexpr int kAttnTile = 32;        // tokens (queries) per CTA
 constexpr int kAttnQkvThreads = 256;
 constexpr int kAttnSThreads = 512;
 
-// (float) mean and rstd of every group of image n (as attn_kernel computes them), for the first C / gs threads
+// (float) mean and rstd of every group of image n (as attn_cluster_kernel computes them), for the first C / gs threads
 __device__ __forceinline__ void attn_group_stats(const AttnParams& p, int n, float (*smr)[2]) {
   const int G = p.C / p.gs;
   if ((int)threadIdx.x < G) {
@@ -860,28 +742,6 @@ __global__ void pack_conv_weight_kernel(const float* __restrict__ w, __half* __r
     if (co < Cout && cr >= 0 && cr < CinReal) v = w[((size_t)co * CinReal + cr) * taps + t];
     const __half hi = __float2half_rn(v);
     wpk[i] = (precise != 2 && seg < 2) ? hi : __float2half_rn(v - __half2float(hi));
-  }
-}
-
-// Tap-row-stacked packing (conv_tc.cuh addresses tap (dy, dx) inside it): [dy 3][Cin/8][3 * CoutPad][8] fp16, column n = dx * CoutPad + co of kernel
-// row dy holds W[co][ci][dy][dx]; channel mapping (c0_real / c0_store / concat) as in pack_conv_weight_kernel.
-__global__ void pack_conv_weight_trs_kernel(const float* __restrict__ w, __half* __restrict__ wpk, int Cout, int CoutPad, int CinReal,
-                                            int Cin, int c0_real, int c0_store) {
-  const int N3 = 3 * CoutPad;
-  const int total = 3 * Cin * N3;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    const int e = i & 7;
-    const int n = (i >> 3) % N3;
-    const int j = (i >> 3) / N3 % (Cin >> 3);
-    const int dy = (i >> 3) / N3 / (Cin >> 3);
-    const int dx = n / CoutPad, co = n - dx * CoutPad;
-    const int ci = j * 8 + e;
-    int cr = -1;
-    if (ci < c0_store) cr = ci < c0_real ? ci : -1;
-    else cr = c0_real + (ci - c0_store);
-    float v = 0.f;
-    if (co < Cout && cr >= 0 && cr < CinReal) v = w[((size_t)co * CinReal + cr) * 9 + dy * 3 + dx];
-    wpk[i] = __float2half_rn(v);
   }
 }
 

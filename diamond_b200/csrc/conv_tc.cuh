@@ -74,7 +74,7 @@ struct ConvParams {
   int B, H, W;          // conv input size
   int taps;             // 9 (3x3, pad 1) or 1 (1x1)
   int stride;           // 1 or 2 (stride 2 == stride-1 result sampled at even (y,x); exact for k=3,p=1)
-  const __half* wpk;    // [taps][Cin/8][CoutPad][8], or [dy][Cin/8][3*CoutPad][8] when trs
+  const __half* wpk;    // [taps][Cin/8][CoutPad][8]
   const float* bias;    // [Cout] or null
   int Cout, CoutPad;
   const float* resid;   // NHWC [B][Ho][Wo][Cout] or null
@@ -86,8 +86,9 @@ struct ConvParams {
   unsigned long long plane_bytes;  // bytes of one chunk plane (same geometry for both sources)
   int P, Palloc;        // halo positions, odd allocation pitch
   int num_tiles, stages;
-  int trs;              // weights in the tap-row-stacked layout (dmd_pack_conv_weight precise = 3): tap (dy, dx) is the column
-                        // block dx * CoutPad of kernel row dy
+  int trs;              // always 0 (conv_fill).  The consumer prologue still selects its B-descriptor constants on it: without a
+                        // runtime select the compiler recomputes them inside the slab loop, 18 more instructions per slab that
+                        // made the 3x3 64->64 conv 4 % slower (H100 80GB HBM3, 700 W)
   FastDiv dPW, dPH;
   long long* ktrace;    // diagnostics: globaltimer stamp when the kernel's inputs are ready, or null
 };

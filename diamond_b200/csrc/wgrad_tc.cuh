@@ -38,7 +38,6 @@ struct WgradParams {
   int num_tiles, stages;
   int Pb;                       // activation positions per stage (128 + 2*halo), PbAlloc = Pb | 1
   float* partial;               // [gridDim.x][taps][64][N]
-  int dbg;                      // bit 0: swap the LBO/SBO roles of the MN-major descriptors (bring-up probe)
 };
 
 struct WgradSmem { uint32_t a_off, b_off, a_bytes, b_bytes, total; };
@@ -102,8 +101,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const WgradPara
     const int ky = warp >> 2;                 // kernel row of this warpgroup
     const int ntap = p.taps == 9 ? 3 : (ky == 0 ? 1 : 0);
     // MN-major no-swizzle: K groups (8 positions) are 128 B apart; MN groups (8 channels) one plane apart
-    uint32_t a_lbo = 128, a_sbo = kTileM * 16, b_lbo = 128, b_sbo = PbAlloc * 16;
-    if (p.dbg & 1) { uint32_t t = a_lbo; a_lbo = a_sbo; a_sbo = t; t = b_lbo; b_lbo = b_sbo; b_sbo = t; }
+    const uint32_t a_lbo = 128, a_sbo = kTileM * 16, b_lbo = 128, b_sbo = PbAlloc * 16;
     const uint64_t a_hi = gmma_desc_hi(a_sbo), b_hi = gmma_desc_hi(b_sbo);
     const uint32_t a_lo0 = ((smem_u32(sA) >> 4) & 0x3FFFu) | (((a_lbo >> 4) & 0x3FFFu) << 16);
     const uint32_t b_lo0 = ((smem_u32(sB) >> 4) & 0x3FFFu) | (((b_lbo >> 4) & 0x3FFFu) << 16);

@@ -39,7 +39,8 @@ def nhwc_to_nchw(x: Tensor, c: Optional[int] = None) -> Tensor:
 def pack_conv_weight(w: Tensor, cin_pad: int, c0_real: Optional[int] = None, c0_store: Optional[int] = None,
                      precise: bool = False, trs: bool = False) -> Tuple[Tensor, int]:
     """torch weight [Cout][Cin][k][k] -> fp16 operand [taps][cin_pad/8][CoutPad][8]; returns (packed, CoutPad).
-    trs=True: the tap-row-stacked layout of 3x3 kernels (pass trs=True to the conv call as well)."""
+    trs: see _reject_removed."""
+    _reject_removed(trs=trs)
     _cuda(w)
     cout, cin, kh, kw = w.shape
     taps = kh * kw
@@ -48,8 +49,17 @@ def pack_conv_weight(w: Tensor, cin_pad: int, c0_real: Optional[int] = None, c0_
     c0_store = c0_real if c0_store is None else c0_store
     out = torch.empty(taps * cin_pad * cout_pad * (3 if precise else 1), device=w.device, dtype=torch.float16)
     _lib.check(_lib.lib().dmd_pack_conv_weight(w.data_ptr(), out.data_ptr(), cout, cout_pad, cin, cin_pad, taps,
-                                              c0_real, c0_store, 3 if trs else int(precise), _lib.current_stream()))
+                                              c0_real, c0_store, int(precise), _lib.current_stream()))
     return out, cout_pad
+
+
+def _reject_removed(trs: bool = False, debug: int = 0) -> None:
+    """`trs` (the tap-row-stacked weight layout) and `debug` (kernel debug switches) name options the kernels no longer
+    have.  Callers such as bench.py still pass their defaults, which are accepted; anything else raises."""
+    if trs:
+        raise ValueError("trs=True: only the tap-major weight layout is supported")
+    if debug:
+        raise ValueError(f"debug={debug}: the kernels have no debug switches")
 
 
 def gn_stats(x: Tensor, gs: int) -> Tensor:
@@ -104,9 +114,10 @@ def prep_act(src0: Tensor, *, src1: Optional[Tensor] = None, upsample: bool = Fa
 def conv2d_operand(n0: Tensor, n1: Optional[Tensor], c0: int, c1: int, b: int, h: int, w: int, wpk: Tensor, cout: int,
                    cout_pad: int, taps: int = 9, *, bias: Optional[Tensor] = None, stride: int = 1,
                    residual: Optional[Tensor] = None, out_gs: int = 0, out: Optional[Tensor] = None,
-                   ostats: Optional[Tensor] = None, debug: int = 0, debug_buf: Optional[Tensor] = None,
-                   lo0: Optional[Tensor] = None, lo1: Optional[Tensor] = None, xproj=None, trs: bool = False):
-    """wgmma conv on already prepared PLC16 operand(s) (one kernel launch)."""
+                   ostats: Optional[Tensor] = None, lo0: Optional[Tensor] = None, lo1: Optional[Tensor] = None,
+                   xproj=None, trs: bool = False):
+    """wgmma conv on already prepared PLC16 operand(s) (one kernel launch).  trs: see _reject_removed."""
+    _reject_removed(trs=trs)
     _cuda(n0, n1, wpk, bias, residual)
     ho, wo = h // stride, w // stride
     if out is None:
@@ -117,10 +128,8 @@ def conv2d_operand(n0: Tensor, n1: Optional[Tensor], c0: int, c1: int, b: int, h
     d.src0, d.src1, d.C0, d.C1 = n0.data_ptr(), _lib.ptr(n1), c0, c1
     d.B, d.H, d.W, d.taps, d.stride = b, h, w, taps, stride
     d.wpk, d.bias, d.Cout, d.CoutPad = wpk.data_ptr(), _lib.ptr(bias), cout, cout_pad
-    d.residual, d.out, d.out_stats, d.out_gs, d.debug = _lib.ptr(residual), out.data_ptr(), _lib.ptr(ostats), out_gs, debug
-    d.debug_buf = _lib.ptr(debug_buf)
+    d.residual, d.out, d.out_stats, d.out_gs = _lib.ptr(residual), out.data_ptr(), _lib.ptr(ostats), out_gs
     d.precise, d.src0_lo, d.src1_lo = int(lo0 is not None), _lib.ptr(lo0), _lib.ptr(lo1)
-    d.wpk_layout = int(trs)
     if xproj is not None:  # fused split-fp16 1x1 projection: (hi0, hi1, lo0, lo1, C0, C1, wpk_x, bias_x)
         xh0, xh1, xl0, xl1, xc0, xc1, wpk_x, bias_x = xproj
         d.xsrc0, d.xsrc1, d.xsrc0_lo, d.xsrc1_lo = xh0.data_ptr(), _lib.ptr(xh1), xl0.data_ptr(), _lib.ptr(xl1)
@@ -134,10 +143,11 @@ def conv2d_fprop(src0: Tensor, wpk: Tensor, cout: int, cout_pad: int, cin_pad: i
                  prologue: int = 0, silu: bool = False, stats0: Optional[Tensor] = None, stats1: Optional[Tensor] = None,
                  gs0: int = 0, gs1: int = 0, film: Optional[Tensor] = None, film_off: int = 0,
                  gamma: Optional[Tensor] = None, beta: Optional[Tensor] = None, eps: float = 1e-5,
-                 residual: Optional[Tensor] = None, out_gs: int = 0, debug: int = 0, debug_buf: Optional[Tensor] = None,
+                 residual: Optional[Tensor] = None, out_gs: int = 0, debug: int = 0,
                  precise: bool = False, trs: bool = False) -> Tuple[Tensor, Optional[Tensor]]:
     """The reference's `conv(act(norm(cat(x, skip))))` on NHWC fp32 tensors: one prep launch + one wgmma conv launch.
-    precise=True: split-fp16 operands (weights must be packed with precise=True)."""
+    precise=True: split-fp16 operands (weights must be packed with precise=True).  debug, trs: see _reject_removed."""
+    _reject_removed(trs=trs, debug=debug)
     res = prep_act(src0, src1=src1, upsample=upsample, mode=prologue, silu=silu, stats0=stats0, stats1=stats1,
                    gs0=gs0, gs1=gs1, film=film, film_off=film_off, gamma=gamma, beta=beta, eps=eps, split=precise)
     n0, n1, _, _, h, w = res[:6]
@@ -146,7 +156,7 @@ def conv2d_fprop(src0: Tensor, wpk: Tensor, cout: int, cout_pad: int, cin_pad: i
     if c0 + c1 != cin_pad:
         raise ValueError(f"operand channels {c0}+{c1} do not match the packed weights ({cin_pad})")
     return conv2d_operand(n0, n1, c0, c1, src0.shape[0], h, w, wpk, cout, cout_pad, taps, bias=bias, stride=stride,
-                          residual=residual, out_gs=out_gs, debug=debug, debug_buf=debug_buf, lo0=lo0, lo1=lo1, trs=trs)
+                          residual=residual, out_gs=out_gs, lo0=lo0, lo1=lo1)
 
 
 def attn_fwd(x: Tensor, stats_in: Tensor, gamma: Tensor, beta: Tensor, wqkv: Tensor, bqkv: Tensor, wout: Tensor,
@@ -225,7 +235,9 @@ _partial = {}
 def conv2d_wgrad(grad_op: Tensor, cg: int, act_op: Tensor, ca: int, b: int, h: int, w: int, cout: int, cin: int, taps: int = 9, *,
                  dw: Optional[Tensor] = None, cin_tot: Optional[int] = None, ci_off: int = 0, inv_scale: Optional[Tensor] = None,
                  accumulate: bool = False, debug: int = 0) -> Tensor:
-    """wgmma weight gradient from two PLC16 operands (dL/dy with `cg` stored channels, conv input with `ca`)."""
+    """wgmma weight gradient from two PLC16 operands (dL/dy with `cg` stored channels, conv input with `ca`).  debug: see
+    _reject_removed."""
+    _reject_removed(debug=debug)
     _cuda(grad_op, act_op)
     lib = _lib.lib()
     cin_tot = cin if cin_tot is None else cin_tot
@@ -238,7 +250,7 @@ def conv2d_wgrad(grad_op: Tensor, cg: int, act_op: Tensor, ca: int, b: int, h: i
     d = _lib.WgradDesc()
     d.grad, d.act, d.Cg, d.Ca, d.B, d.H, d.W, d.taps = grad_op.data_ptr(), act_op.data_ptr(), cg, ca, b, h, w, taps
     d.dW, d.Cout, d.Cin, d.CinTot, d.ci_off = dw.data_ptr(), cout, cin, cin_tot, ci_off
-    d.inv_scale, d.accumulate, d.partial, d.partial_bytes, d.debug = _lib.ptr(inv_scale), int(accumulate), part.data_ptr(), part.numel(), debug
+    d.inv_scale, d.accumulate, d.partial, d.partial_bytes = _lib.ptr(inv_scale), int(accumulate), part.data_ptr(), part.numel()
     _lib.check(lib.dmd_conv2d_wgrad(C.byref(d), _lib.current_stream()))
     return dw
 

@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define DMD_VERSION 100
+#define DMD_VERSION 101
 /* Headroom of the backward loss scale: max|S * dL/d(output)| is put in [2^(E-1), 2^E), E = DMD_LOSS_SCALE_EXP, so an inner
  * gradient up to 65504 / 2^E (just under 2^(16-E)) times the largest output gradient is finite in the fp16 tensor-core operands.
  * E = 8 (headroom 256x) costs nothing measurable against E = 12 (16x) on either training fixture: fp16 keeps its relative
@@ -70,9 +70,7 @@ int dmd_pack_conv_weight(const float* w, void* wpk, int Cout, int CoutPad, int C
                          int c0_real, int c0_store, int precise, void* stream);
 /* precise = 1: split-fp16 packing [W_hi | W_hi | W_lo] (3*Cin channels per tap) for dmd_conv_desc.precise convs: the
  * product is evaluated as A_hi W_hi + A_lo W_hi + A_hi W_lo on the tensor cores, i.e. to ~2^-22 instead of 2^-11.  Used
- * for the layers whose input is the raw residual stream (1x1 skip projections, conv_in) and for conv_out.
- * precise = 3: the tap-row-stacked layout [dy][Cin/8][3*CoutPad][8] of 3x3 kernels (dmd_conv_desc.wpk_layout = 1): the
- * three taps of a kernel row side by side as column blocks dx*CoutPad (conv_tc.cuh addresses each tap inside its row). */
+ * for the layers whose input is the raw residual stream (1x1 skip projections, conv_in) and for conv_out. */
 
 /* Activation operand ("PLC16": padded-linear, chunk-major fp16; layout in diamond_b200/csrc/conv_tc.cuh).  One pass over
  * an NHWC fp32 tensor applies what the reference runs on a conv INPUT — GroupNorm (blocks.py:28) or AdaGroupNorm
@@ -122,10 +120,7 @@ typedef struct dmd_conv_desc {
   float* out;            /* NHWC [B][Ho][Wo][Cout] */
   double* out_stats;     /* [B][Cout/out_gs][2], accumulated (caller zeroes) or NULL */
   int out_gs;
-  int debug;             /* reserved: must be 0 (rejected otherwise) */
-  void* debug_buf;       /* reserved: must be NULL (rejected otherwise) */
   int precise;           /* 1: split-fp16 (needs src*_lo and weights packed with precise = 1) */
-  int wpk_layout;        /* 0: tap-major weights ; 1: tap-row-stacked (dmd_pack_conv_weight precise = 3; 3x3, non-split only) */
   const void* src0_lo;
   const void* src1_lo;
   /* Optional fused 1x1 projection accumulated into the same output: out += W_x . cat(x0, x1) + b_x  (the skip path
@@ -160,7 +155,6 @@ typedef struct dmd_wgrad_desc {
   int accumulate;        /* dW += instead of dW = */
   void* partial;         /* workspace of dmd_wgrad_partial_bytes() */
   size_t partial_bytes;
-  int debug;             /* bring-up only; 0 */
 } dmd_wgrad_desc;
 size_t dmd_wgrad_partial_bytes(void);
 int dmd_conv2d_wgrad(const dmd_wgrad_desc* d, void* stream);
@@ -183,8 +177,9 @@ int dmd_prep_plan(const dmd_prep_desc* d, int* blocks, int* pos_per_block, int* 
 int dmd_gn_stats(const float* x, double* stats, int B, int HW, int C, int gs, void* stream);
 
 /* SelfAttention2d.forward (blocks.py:62-72), L = H*W = 64 tokens, C in {32, 64}, head_dim 8, groups of gs channels (gs a
- * multiple of 8 dividing C): out = xn + out_proj(softmax(q k^T / sqrt(8)) v) with xn = GroupNorm(x) from the producer's
- * statistics stats_in [B][C/gs][2]; out_stats (or NULL) [B][C/gs][2] += (sum, sumsq) of out. */
+ * multiple of 8 dividing C, and at L = 64 a multiple of C/4, as every model's gs = 32 is): out = xn + out_proj(softmax(q k^T
+ * / sqrt(8)) v) with xn = GroupNorm(x) from the producer's statistics stats_in [B][C/gs][2]; out_stats (or NULL) [B][C/gs][2]
+ * += (sum, sumsq) of out. */
 int dmd_attn_fwd(const float* x, const double* stats_in, const float* gamma, const float* beta, const float* wqkv,
                  const float* bqkv, const float* wout, const float* bout, float* out, double* out_stats, int B, int L,
                  int C, int gs, float eps, void* stream);

@@ -27,7 +27,7 @@ from oracle import torch_oracle as O  # noqa: E402
 from diamond_b200.models.diffusion import (Denoiser, DenoiserConfig, DiffusionSampler, DiffusionSamplerConfig,  # noqa: E402
                                            InnerModelConfig)
 
-ATTN_KERNELS = ("attn_qkv_kernel", "attn_stream_kernel", "attn_cluster_kernel", "attn_kernel")
+ATTN_KERNELS = ("attn_qkv_kernel", "attn_stream_kernel", "attn_cluster_kernel")
 
 
 def flops_per_forward(inner: O.InnerCfg, b: int, h: int, w: int):

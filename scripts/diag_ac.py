@@ -57,7 +57,7 @@ def main():
                 d = p.grad.double() - r
                 num += float(d.pow(2).sum()); den += float(r.pow(2).sum())
                 rows.append((k, float(d.norm() / r.norm().clamp_min(1e-30)), float(r.norm())))
-            print(f"B={b} steps={steps} pdl_off={os.environ.get('DMD_NO_PDL')}: "
+            print(f"B={b} steps={steps}: "
                   f"loss {float(loss):.6f} ref {float(ref_loss):.6f}  whole-grad rel err {(num / den) ** 0.5:.3e}", flush=True)
             if b == batches[0]:
                 for k, e, n in rows:

@@ -16,7 +16,7 @@ def _declared():
 
 def test_library_built_and_loads():
     assert os.path.exists(_lib.LIB_PATH), "run __graft_entry__.build() first"
-    assert _lib.lib().dmd_version() == 100
+    assert _lib.lib().dmd_version() == 101
 
 
 def test_every_declared_symbol_is_exported_and_bound():
@@ -33,5 +33,5 @@ def test_every_declared_symbol_is_exported_and_bound():
 def test_struct_sizes_match_header_layout():
     # natural alignment, 64-bit pointers: guards against field drift between the header and the ctypes mirror
     assert ctypes.sizeof(_lib.DenoiserConfigC) == 4 * 4 + 3 * 8 * 4 + 4 + 2 * 4
-    assert ctypes.sizeof(_lib.ConvDesc) == 192 and ctypes.sizeof(_lib.PrepDesc) == 176
+    assert ctypes.sizeof(_lib.ConvDesc) == 176 and ctypes.sizeof(_lib.PrepDesc) == 176
     assert ctypes.sizeof(_lib.SamplerConfigC) == 40

@@ -27,7 +27,7 @@ def _h(x):
 
 
 def _run_conv(dev, b, h, w, c0, c1, cout, taps=9, upsample=False, stride=1, prologue=0, silu=False, residual=False,
-              want_stats=False, seed=0, debug=0, precise=False, trs=False):
+              want_stats=False, seed=0, precise=False):
     from diamond_b200 import ops
 
     g = torch.Generator().manual_seed(seed)
@@ -66,7 +66,7 @@ def _run_conv(dev, b, h, w, c0, c1, cout, taps=9, upsample=False, stride=1, prol
     s0 = ops.nchw_to_nhwc(x0.to(dev), c0s)
     s1 = ops.nchw_to_nhwc(x1.to(dev)) if c1 else None
     cin_pad = ops.round_up(c0s, 16) + (ops.round_up(c1, 16) if c1 else 0)
-    wpk, cout_pad = ops.pack_conv_weight(wt.to(dev), cin_pad, c0_real=c0, c0_store=ops.round_up(c0s, 16), precise=precise, trs=trs)
+    wpk, cout_pad = ops.pack_conv_weight(wt.to(dev), cin_pad, c0_real=c0, c0_store=ops.round_up(c0s, 16), precise=precise)
     kw = {}
     if prologue:
         gs0 = gs if c0 % gs == 0 else c0
@@ -78,7 +78,7 @@ def _run_conv(dev, b, h, w, c0, c1, cout, taps=9, upsample=False, stride=1, prol
         prologue=prologue, silu=silu, film=film.to(dev) if film is not None else None, film_off=5,
         gamma=gamma.to(dev) if gamma is not None else None, beta=beta.to(dev) if beta is not None else None,
         residual=ops.nchw_to_nhwc(res.to(dev)) if residual else None,
-        out_gs=(32 if cout % 32 == 0 else 0) if want_stats else 0, debug=debug, precise=precise, trs=trs, **kw)
+        out_gs=(32 if cout % 32 == 0 else 0) if want_stats else 0, precise=precise, **kw)
     got = ops.nhwc_to_nchw(out).cpu()
     torch.cuda.synchronize()
     return got, ref32, ref16, (st.cpu() if st is not None else None)
@@ -114,32 +114,6 @@ def test_conv_plain(case):
     assert _rel(got, ref32) < 2e-3, ("fp32 reference", _rel(got, ref32))
 
 
-# row-stacked weights hold 3 * CoutPad columns, at most 256 (CoutPad <= 80)
-@pytest.mark.parametrize("case", [c for c in CASES if c.get("taps", 9) == 9 and c["cout"] <= 80],
-                         ids=lambda c: "-".join(f"{k}{v}" for k, v in c.items()))
-def test_conv_row_stacked_taps(case):
-    """The tap-row-stacked weight layout of the 3x3 convs (the three taps of a kernel row side by side, N = 3 * Cout; the kernel
-    addresses each tap inside its row, conv_tc.cuh) -- same results as the tap-major layout."""
-    dev = _dev()
-    got, ref32, ref16, _ = _run_conv(dev, trs=True, **case)
-    assert got.shape == ref32.shape
-    assert _rel(got, ref16) < 2e-5, ("fp16-operand reference", _rel(got, ref16))
-    assert _rel(got, ref32) < 2e-3, ("fp32 reference", _rel(got, ref32))
-
-
-@pytest.mark.parametrize("shape", [dict(b=2, h=64, w=64, c0=64, c1=0, cout=64), dict(b=3, h=16, w=16, c0=64, c1=64, cout=64),
-                                   dict(b=4, h=8, w=8, c0=64, c1=0, cout=64), dict(b=32, h=64, w=64, c0=64, c1=0, cout=64)],
-                         ids=["64x64", "16x16cat", "8x8", "bench"])
-def test_conv_row_stacked_norm_prologue_residual_stats(shape):
-    dev = _dev()
-    got, ref32, _, st = _run_conv(dev, prologue=1, silu=True, residual=True, want_stats=True, seed=3, trs=True, **shape)
-    assert _rel(got, ref32) < 2e-3, _rel(got, ref32)
-    b, c, h, w = got.shape
-    v = got.double().reshape(b, c // 32, 32 * h * w)
-    want = torch.stack([v.sum(-1), (v * v).sum(-1)], -1)
-    assert torch.allclose(st, want, rtol=1e-5, atol=1e-3), float((st - want).abs().max())
-
-
 @pytest.mark.parametrize("prologue,silu", [(1, True), (2, True), (1, False)])
 @pytest.mark.parametrize("shape", [dict(b=2, h=64, w=64, c0=64, c1=0, cout=64), dict(b=3, h=16, w=16, c0=64, c1=64, cout=64),
                                    dict(b=4, h=8, w=8, c0=64, c1=0, cout=64), dict(b=2, h=32, w=32, c0=128, c1=0, cout=64),
@@ -170,8 +144,7 @@ def test_conv_precise_split_fp16(case):
     assert _rel(got, ref32) < 5e-6, _rel(got, ref32)
 
 
-@pytest.mark.parametrize("trs", [False, True], ids=["tap-major", "row-stacked"])
-def test_conv_with_fused_skip_projection(trs):
+def test_conv_with_fused_skip_projection():
     """ResBlock tail (blocks.py:142-145): conv2(silu(norm2(t))) + proj(cat(x, skip)) in ONE launch — the 1x1 projection is
     extra K (split-fp16, centre tap) accumulated into the same accumulator tile."""
     dev = _dev()
@@ -188,10 +161,10 @@ def test_conv_with_fused_skip_projection(trs):
     n0 = ops.prep_act(tn)[0]
     res = ops.prep_act(xn, src1=sn, also_raw=False, split=True)  # raw mode: main operand = raw hi, lo parts via split
     xh0, xh1, xl0, xl1 = res[0], res[1], res[6], res[7]
-    wpk2, cp = ops.pack_conv_weight(w2.to(dev), 64, trs=trs)
+    wpk2, cp = ops.pack_conv_weight(w2.to(dev), 64)
     wpkx, _ = ops.pack_conv_weight(wp.to(dev), 128, precise=True)
     out, _ = ops.conv2d_operand(n0, None, 64, 0, b, h, w, wpk2, 64, cp, bias=b2.to(dev),
-                                xproj=(xh0, xh1, xl0, xl1, 64, 64, wpkx, bp.to(dev)), trs=trs)
+                                xproj=(xh0, xh1, xl0, xl1, 64, 64, wpkx, bp.to(dev)))
     got = ops.nhwc_to_nchw(out).cpu()
     assert _rel(got, ref) < 2e-5, _rel(got, ref)
 

@@ -45,7 +45,7 @@ def _dev():
 
 def _case(id_, b, h, w, c0, cout, **kw):
     d = dict(id=id_, b=b, h=h, w=w, c0=c0, c1=0, cout=cout, taps=9, stride=1, upsample=False, prologue=False, residual=False,
-             gs=0, trs=False, precise=False, xproj=False, regime=())
+             gs=0, precise=False, xproj=False, regime=())
     d.update(kw)
     return d
 
@@ -57,7 +57,6 @@ def _case(id_, b, h, w, c0, cout, **kw):
 # change without a straddling tile in between).  "uneven" is not claimed where it rests on the all-padding tail tile alone.
 CASES = [
     _case("d0-64x64-tapmajor", 32, 64, 64, 64, 64, gs=32, regime=("wrap", "multi")),
-    _case("d0-64x64-rowstacked", 32, 64, 64, 64, 64, gs=32, trs=True, regime=("wrap", "multi")),
     _case("resblock-64x64-adagn-silu-residual", 32, 64, 64, 64, 64, gs=32, prologue=True, residual=True, regime=("wrap", "multi")),
     _case("concat-64x64", 16, 64, 64, 64, 64, c1=64, gs=32, regime=("wrap", "multi")),
     _case("concat-16x16", 64, 16, 16, 64, 64, c1=64, gs=32, regime=("wrap", "mixed")),
@@ -119,7 +118,6 @@ def _plan(c):
         d.out_stats, d.out_gs = p, c["gs"]
     if c["precise"]:
         d.precise, d.src0_lo, d.src1_lo = 1, p, (p if c["c1"] else None)
-    d.wpk_layout = int(c["trs"])
     if c["xproj"]:
         d.xsrc0, d.xsrc1, d.xsrc0_lo, d.xsrc1_lo, d.xC0, d.xC1, d.wpk_x = p, p, p, p, 64, 64, p
     info = _lib.ConvPlanInfo()
@@ -241,7 +239,7 @@ class Run:
         res = ops.prep_act(self.x0, src1=self.x1, upsample=c["upsample"], split=c["precise"], **kw)
         self.n0, self.n1 = res[0], res[1]
         self.lo0, self.lo1 = (res[6], res[7]) if c["precise"] else (None, None)
-        self.wpk, self.cout_pad = ops.pack_conv_weight(self.wt, cin, precise=c["precise"], trs=c["trs"])
+        self.wpk, self.cout_pad = ops.pack_conv_weight(self.wt, cin, precise=c["precise"])
         self.xproj = None
         if c["xproj"]:   # ResBlock tail: + proj(cat(x, skip)), split-fp16 operands, centre tap
             xs, sk = torch.randn(b, hs, ws, 64, device=dev, generator=g) * 2, torch.randn(b, hs, ws, 64, device=dev, generator=g) + 0.5
@@ -297,7 +295,7 @@ class Run:
             ost.zero_()
         ops.conv2d_operand(self.n0, self.n1, c["c0"], c["c1"], b, self.h, self.w, self.wpk, cout, self.cout_pad, c["taps"],
                            bias=self.bias, stride=c["stride"], residual=self.resid, out_gs=c["gs"], out=out, ostats=ost,
-                           lo0=self.lo0, lo1=self.lo1, xproj=self.xproj, trs=c["trs"])
+                           lo0=self.lo0, lo1=self.lo1, xproj=self.xproj)
         torch.cuda.synchronize()
         _check_guards(obuf, out, NAN32)
         assert not bool(out.isnan().any()), "output elements left unwritten"

@@ -1,6 +1,7 @@
 """CPU: shape validation, error behaviour and launch planning of the conv / prep entry points, through the host-only
 C-ABI twins dmd_conv_plan / dmd_prep_plan (same code path as dmd_conv2d_fprop / dmd_prep_act up to the launch).  Pointers
-are dummies: the plan functions only test them for NULL."""
+are dummies: the plan functions only test them for NULL.  dmd_attn_fwd's shape checks come before any CUDA call, so its
+rejections are tested through the entry point itself."""
 import ctypes as C
 
 import pytest
@@ -83,10 +84,20 @@ def test_conv_tiles_per_level(hw, tiles):
     (dict(C0=64, C1=64, src1=P, W=600, H=8, B=1), "shared memory too small"),
     (dict(src0=0), "null src0/out/wpk"),
     (dict(wpk_x=P), "bad fused projection operands"),
-    (dict(debug=1), "debug / debug_buf must be 0"),
 ])
 def test_conv_rejections_fail_loudly(kw, needle):
     rc, _, err = _conv(**kw)
+    assert rc != 0 and needle in err, err
+
+
+@pytest.mark.parametrize("c,gs,needle", [
+    (64, 8, "needs gs a multiple of C/4"),       # attn_cluster_kernel credits each CTA's C/4 channels to one group
+    (48, 16, "unsupported shape"),
+], ids=["c64-gs8", "c48"])
+def test_attn_rejections_fail_loudly(c, gs, needle):
+    """dmd_attn_fwd checks the shape before any CUDA call, so null pointers do."""
+    rc = _lib.lib().dmd_attn_fwd(*[None] * 10, 2, 64, c, gs, 1e-5, None)
+    err = _lib.lib().dmd_last_error().decode()
     assert rc != 0 and needle in err, err
 
 
