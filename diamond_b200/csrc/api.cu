@@ -923,7 +923,8 @@ struct Plan {
   const int64_t* t_act = nullptr;                         // the forward's action tensor (embedding gradient)
   float *tA = nullptr, *tB = nullptr, *tC = nullptr;      // fp32 NHWC temporaries (largest activation)
   uint8_t *gyA = nullptr, *gyB = nullptr;                 // PLC16 gradient operands
-  float *gF = nullptr;                                    // scaled dL/d(model output), NHWC with 8 channels
+  float *gF = nullptr;                                    // scaled dL/d(model output), NHWC with gF_ch channels
+  int gF_ch = 0;                                          // round_up(img_channels, 8): the padded channels are zero
   float *dfilm = nullptr, *nsum = nullptr, *partial = nullptr, *scale = nullptr;
   float *dcond = nullptr, *dh = nullptr, *cpre = nullptr, *dpre = nullptr, *de = nullptr;
   unsigned int* amax = nullptr;
@@ -1588,6 +1589,8 @@ struct BwdBuilder {
         colsum(r.o.grad, (long long)B * H * W, cw.Cout, cw.Cout, cw.b_idx);
         replay(r.in1);
         wgrad(cw, pl->gyA, r.in1.n0, cw.c0_store, cw.c0_real, 0, H, W);
+        if (err) return fail("backward plan: conv_in weight gradient over %d input channels (%d after padding to 16) cannot be built: %s",
+                             cw.c0_real, cw.c0_store, g_err.c_str());
       } else {
         return fail("backward plan: record %d of kind %d belongs to a model's own head", i, r.kind);
       }
@@ -1626,13 +1629,13 @@ int build_denoiser_bwd(const dmd_denoiser* h, BwdBuilder& bw) {
   Plan* pl = bw.pl;
   const int B = pl->B;
   bw.begin();
-  {   // the last record: gF is the scaled gradient of the model output, NHWC x 8 channels
+  {   // the last record: gF is the scaled gradient of the model output, NHWC x gF_ch channels
     const Rec& r = pl->tape.back();
     if (r.kind != R_OUT) return fail("denoiser backward plan: the tape does not end with the output head");
     const ConvW& cw = *r.cw;
     const int H = r.x.H, W = r.x.W;
-    bw.gprep(pl->gF, 8, H, W, 0, pl->gyA);
-    bw.colsum(pl->gF, (long long)B * H * W, 8, cw.Cout, cw.b_idx);
+    bw.gprep(pl->gF, pl->gF_ch, H, W, 0, pl->gyA);
+    bw.colsum(pl->gF, (long long)B * H * W, pl->gF_ch, cw.Cout, cw.b_idx);
     bw.replay(r.in1);
     bw.wgrad(cw, pl->gyA, r.in1.n0, round_up(r.x.C, 16), r.x.C, 0, H, W);
     bw.dgrad(cw, 0, pl->gyA, H, W, pl->tA, false);
@@ -1676,7 +1679,7 @@ int make_train_plan(const ModelCore& core, int cmax, int gF_ch, Plan* pl, int B,
   pl->tA = (float*)bb.take(act_bytes); pl->tB = (float*)bb.take(act_bytes); pl->tC = (float*)bb.take(act_bytes);
   const size_t op_bytes = plc16_bytes(B, H, W, cmax);
   pl->gyA = (uint8_t*)bb.take(op_bytes); pl->gyB = (uint8_t*)bb.take(op_bytes);
-  pl->gF = (float*)bb.take((size_t)B * H * W * gF_ch * 4);
+  pl->gF = (float*)bb.take((size_t)B * H * W * gF_ch * 4); pl->gF_ch = gF_ch;
   if (init_kernels()) return 1;
   pl->partial = (float*)bb.take(wgrad_partial_bytes(g_num_sms));
   const int CC = core.cond_channels;
@@ -1704,7 +1707,8 @@ template <class Cfg> int widest_channels(const Cfg& c) {  // at least 16
   return cmax;
 }
 int make_denoiser_train_plan(const dmd_denoiser* h, Plan* pl, int B, int H, int W, uint8_t* base, size_t* total) {
-  return make_train_plan(h->core, widest_channels(h->cfg), 8, pl, B, H, W, 1, base, total,
+  // gF: one channel per output channel, padded to 8 (the gradient-operand prep reads multiples of 8)
+  return make_train_plan(h->core, widest_channels(h->cfg), round_up(h->cfg.img_channels, 8), pl, B, H, W, 1, base, total,
                          [h](PlanBuilder& pb) { return pb.build(h); }, [h](BwdBuilder& bw) { return build_denoiser_bwd(h, bw); });
 }
 
@@ -1782,6 +1786,15 @@ extern "C" dmd_denoiser* dmd_denoiser_create(const dmd_denoiser_config* cfg) {
   if (cfg->cond_channels % 32 || cfg->cond_channels > 256 || cfg->cond_channels % cfg->num_steps_conditioning) { fail("denoiser_create: cond_channels must be a multiple of 32 (<= 256) and of num_steps_conditioning"); return nullptr; }
   for (int i = 0; i < cfg->num_levels; ++i)
     if (cfg->channels[i] % 32 || cfg->channels[i] > 64) { fail("denoiser_create: channels must be 32 or 64 per level (got %d)", cfg->channels[i]); return nullptr; }
+  {   // conv_in's operand: 16, 32 or 64 channels after padding (the operand prep and the wgrad kernel; at 128 the forward
+      // computes a wrong model output)
+    const int cin = (cfg->num_steps_conditioning + 1) * cfg->img_channels, cp = round_up(cin, 16);
+    if (cfg->img_channels < 1 || (cp != 16 && cp != 32 && cp != 64)) {
+      fail("denoiser_create: conv_in over (num_steps_conditioning + 1) * img_channels = %d input channels (%d after padding to 16) "
+           "is not supported: it takes 16, 32 or 64", cin, cp);
+      return nullptr;
+    }
+  }
   if (init_kernels()) return nullptr;
   dmd_denoiser* h = new dmd_denoiser();
   h->cfg = *cfg;
@@ -2011,7 +2024,7 @@ extern "C" int dmd_denoiser_backward(dmd_denoiser* h, int B, int H, int W, const
   if (clear_backward(h->core, pl, grads, st)) return 1;
   // loss scale from the incoming gradient, then the scaled NHWC gradient of the model output
   if (loss_scale_launch(grad_out, (long long)B * C * HW, pl.amax, pl.scale, st)) return 1;
-  nchw_to_nhwc_scaled_kernel<<<dim3((HW + 255) / 256, B), 256, 0, st>>>(grad_out, pl.gF, pl.scale, C, 8, HW);
+  nchw_to_nhwc_scaled_kernel<<<dim3((HW + 255) / 256, B), 256, 0, st>>>(grad_out, pl.gF, pl.scale, C, pl.gF_ch, HW);
   DMD_LAUNCH_OK();
   return run_backward(h->core, pl, grads, st);
 }

@@ -360,7 +360,9 @@ int dmd_inner_model_forward(dmd_denoiser* h, int B, int H, int W, const float* n
  * EVERY parameter into one flat fp32 buffer (16-byte aligned slices, layout from dmd_denoiser_grad_layout, state_dict
  * order; buffers such as noise_emb.weight get zeros).  Convolutions run on wgmma (dgrad = fprop with transposed weights,
  * wgrad = dmd_conv2d_wgrad), gradients carry a power-of-two loss scale chosen from max|grad_out| on the device.  The flat
- * buffer is what a data-parallel step all-reduces in ONE collective (utils.py:105-106 wraps each model in DDP instead). */
+ * buffer is what a data-parallel step all-reduces in ONE collective (utils.py:105-106 wraps each model in DDP instead).
+ * The output gradient is held NHWC with round_up(img_channels, 8) channels.  conv_in takes (num_steps_conditioning + 1) *
+ * img_channels input channels that round up to 16, 32 or 64: dmd_denoiser_create refuses other configs, naming conv_in. */
 size_t dmd_denoiser_train_workspace_bytes(const dmd_denoiser* h, int B, int H, int W);
 /* offsets / numels: n = dmd_denoiser_num_tensors entries (floats); returns the total length of the flat buffer. */
 long long dmd_denoiser_grad_layout(const dmd_denoiser* h, long long* offsets, long long* numels, int n);

@@ -2,6 +2,8 @@
 the residual-stream layers (conv_in, 1x1 projections) exact as the split-fp16 kernels make them.
 
 - QConv: conv2d whose forward / dgrad / wgrad operands are rounded per layer (oracle/grad_error_budget.py's backward budget).
+- grad_errors(): the whole-gradient and per-tensor errors of that rounding against exact autograd, for any loss over a state
+  dict (the denoiser, reward / termination and actor-critic training tests bound the native gradients by it).
 - fp16_forward(): a context that patches F.conv2d (and optionally F.group_norm) for a forward pass of the oracle, which calls
   both through the module attribute.  Its GroupNorm can move each (image, group) (sum, sumsq) by +-1 fp32 ulp under a seed:
   the spread that a valid regrouping of the conv epilogue's fp32 partial sums produces.
@@ -68,6 +70,64 @@ class QConv(torch.autograd.Function):
         gw = torch.nn.grad.conv2d_weight(_h(x) if mode[2] else x, w.shape, gwy, stride=stride, padding=padding)
         gb = gy.sum(dim=(0, 2, 3)) if has_b else None
         return gx, gw, gb, None, None, None, None
+
+
+MODE_MAIN, MODE_STREAM = (1, 1, 1), (0, 1, 1)   # the kernels' rounding: fp16 everywhere, but split-fp16 stream layers forward
+
+
+def grad_errors(loss_fn, sd, stream, out_key=None, exp=None, mode_main=MODE_MAIN, mode_stream=MODE_STREAM):
+    """The backward error budget of the kernels' operand rounding at one model's own inputs.
+
+    loss_fn(sd) -> scalar loss, computing every conv through F.conv2d with weights taken from sd; sd: the state dict, its
+    leaves with requires_grad set.  stream(name): True for the layers the kernels run split-fp16 in the forward (conv_in /
+    conv0, the 1x1 projections and skips).  out_key: the model's single output conv, whose dL/dy fixes one loss scale per
+    backward call with max|S dL/dy| in [2^(exp-1), 2^exp) when exp is given (the denoiser, exp = DMD_LOSS_SCALE_EXP); without
+    it every gradient operand gets a per-tensor scale.  Gradients are exact autograd at sd's dtype, once as is and once with
+    every conv replaced by QConv.  Returns (loss, emulated loss, whole-gradient relative L2 error, {name: relative L2 error},
+    {name: exact gradient})."""
+
+    def grads(emulate):
+        params = {k: v.detach().clone().requires_grad_(v.requires_grad) for k, v in sd.items()}
+        names = {id(v): k for k, v in params.items()}
+
+        def conv2d(x, w, b=None, stride=1, padding=0, dilation=1, groups=1):
+            assert dilation == 1 and groups == 1
+            k = names.get(id(w))
+            mode = mode_stream if k is not None and stream(k) else mode_main
+            return QConv.apply(x, w, b, stride, padding, mode, k is not None and k == out_key)
+
+        F.conv2d = conv2d if emulate else _real_conv2d
+        _SCALE["exp"], _SCALE["S"] = exp, None
+        try:
+            loss = loss_fn(params)
+            loss.backward()
+        finally:
+            F.conv2d = _real_conv2d
+            _SCALE["exp"], _SCALE["S"] = None, None
+        return float(loss.detach()), {k: v.grad for k, v in params.items() if v.grad is not None}
+
+    l0, g0 = grads(False)
+    l1, g1 = grads(True)
+    assert set(g0) == set(g1)
+    num = math.sqrt(sum(float((g1[k] - g0[k]).double().pow(2).sum()) for k in g0))
+    den = math.sqrt(sum(float(g0[k].double().pow(2).sum()) for k in g0))
+    per = {k: float((g1[k] - g0[k]).double().norm() / g0[k].double().norm().clamp_min(1e-30)) for k in g0}
+    return l0, l1, num / den, per, g0
+
+
+def denoiser_stream(sd):
+    """grad_errors' stream predicate for InnerModel: conv_in and every 1x1 conv (projections, attention)."""
+    return lambda k: k == "conv_in.weight" or (sd[k].dim() == 4 and sd[k].shape[-1] == 1)
+
+
+def rew_end_stream(sd):
+    """The same for RewEndModel: its encoder's conv_in and every 1x1 conv."""
+    return lambda k: k == "encoder.conv_in.weight" or (sd[k].dim() == 4 and sd[k].shape[-1] == 1)
+
+
+def actor_critic_stream(sd):
+    """The same for ActorCritic, whose encoder runs every conv split-fp16 in the forward (conv0, the 3x3s, the skips)."""
+    return lambda k: sd[k].dim() == 4
 
 
 def _ulp_step(s, gen):

@@ -15,18 +15,16 @@ of a smaller E: gradients far below max|dL/d(output)| fall into the fp16 subnorm
 `--gain k` multiplies conv_out.weight by k, which makes inner gradients ~0.29 k times the output gradient (default net): the
 headroom a trained network may need; an overflowing operand shows up as a non-finite error.
 """
-import math
 import os
 import sys
 
 import numpy as np
 import torch
-import torch.nn.functional as F
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import torch_oracle as O  # noqa: E402
-from oracle.fp16_emulation import QConv, _SCALE, _real_conv2d  # noqa: E402
+from oracle.fp16_emulation import denoiser_stream, grad_errors  # noqa: E402
 from oracle.make_golden import CASES, TRAIN_CASES  # noqa: E402
 
 
@@ -38,35 +36,20 @@ def run(case_name, mode_main, mode_stream, exp=None, gain=1.0):
     c = CASES[tc["case"]]
     g = np.load(os.path.join(ROOT, "tests", "golden", case_name + ".npz"))
     inner = c["inner"]
+    sd = O.seeded_state_dict(O.inner_model_shapes(inner), c["wseed"])
+    sd["conv_out.weight"] *= gain
+    for k, v in sd.items():
+        if k != "noise_emb.weight":
+            v.requires_grad_(True)
+    draws = [tuple(torch.from_numpy(g[k][i]) for k in ("raw_sigma", "raw_offset", "raw_noise")) for i in range(tc["seq"])]
 
-    def grads(patched):
-        sd = O.seeded_state_dict(O.inner_model_shapes(inner), c["wseed"])
-        sd["conv_out.weight"] *= gain
-        for k, v in sd.items():
-            if k != "noise_emb.weight":
-                v.requires_grad_(True)
-        draws = [tuple(torch.from_numpy(g[k][i]) for k in ("raw_sigma", "raw_offset", "raw_noise")) for i in range(tc["seq"])]
+    def loss_fn(p):
+        return O.denoiser_loss(torch.from_numpy(g["obs"]), torch.from_numpy(g["act"]), torch.from_numpy(g["mask_padding"]),
+                               draws, p, O.DenoiserCfg(inner=inner), O.SigmaDistCfg())
 
-        def conv2d(x, w, b=None, stride=1, padding=0):
-            stream = w.shape[-1] == 1 or w.shape[1] == (inner.num_steps_conditioning + 1) * inner.img_channels
-            return QConv.apply(x, w, b, stride, padding, mode_stream if stream else mode_main, w.shape[0] == inner.img_channels)
-
-        F.conv2d = conv2d if patched else _real_conv2d
-        _SCALE["exp"], _SCALE["S"] = exp, None
-        try:
-            loss = O.denoiser_loss(torch.from_numpy(g["obs"]), torch.from_numpy(g["act"]), torch.from_numpy(g["mask_padding"]),
-                                   draws, sd, O.DenoiserCfg(inner=inner), O.SigmaDistCfg())
-            loss.backward()
-        finally:
-            F.conv2d = _real_conv2d
-        return loss.item(), {k: v.grad for k, v in sd.items() if v.grad is not None}
-
-    l0, g0 = grads(False)
-    l1, g1 = grads(True)
-    num = math.sqrt(sum(float((g1[k] - g0[k]).double().pow(2).sum()) for k in g0))
-    den = math.sqrt(sum(float(g0[k].double().pow(2).sum()) for k in g0))
-    per = sorted(((float((g1[k] - g0[k]).norm() / g0[k].norm().clamp_min(1e-30)), k) for k in g0), reverse=True)
-    return abs(l1 - l0) / abs(l0), num / den, per[:3]
+    l0, l1, whole, per, _ = grad_errors(loss_fn, sd, denoiser_stream(sd), "conv_out.weight", exp, mode_main, mode_stream)
+    worst = sorted(((e, k) for k, e in per.items()), reverse=True)
+    return abs(l1 - l0) / abs(l0), whole, worst[:3]
 
 
 def per_call_rows(name, exps, gain=1.0):
