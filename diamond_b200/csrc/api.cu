@@ -224,6 +224,7 @@ static int init_kernels() {
     DMD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(attn_cluster_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(attn_cluster_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
+    DMD_CUDA(cudaFuncSetAttribute(attn_cluster_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 168 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(linear_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
@@ -380,7 +381,7 @@ struct WgradLaunch { WgradParams wp; WgradReduceParams rp; size_t smem; int grid
 static size_t wgrad_partial_bytes(int num_sms) { return (size_t)num_sms * kWgTaps * 64 * 64 * sizeof(float); }
 
 static int wgrad_fill(const void* grad, int Cg, const void* act, int Ca, int B, int H, int W, int taps, float* partial,
-                      int Cout, int Cin, int CinTot, int ci_off, const float* inv_scale, int accumulate, WgradLaunch* L) {
+                      int Cout, int Cin, int CinTot, int ci_off, const float* inv_scale, int accumulate, WgradLaunch* L, int co_off = 0) {
   DMD_CHECK(grad && act && partial, "wgrad: null operand / partial buffer");
   DMD_CHECK(taps == 9 || taps == 1, "wgrad: taps must be 1 or 9");
   DMD_CHECK(Cg % 8 == 0 && Cg > 0 && Cg <= 64, "wgrad: gradient operand channels must be a multiple of 8, <= 64 (got %d)", Cg);
@@ -408,7 +409,7 @@ static int wgrad_fill(const void* grad, int Cg, const void* act, int Ca, int B, 
   L->grid = wp.num_tiles < g_num_sms ? wp.num_tiles : g_num_sms;
   WgradReduceParams& rp = L->rp;
   rp.partial = partial; rp.nparts = L->grid; rp.N = Ca;
-  rp.Cout = Cout; rp.Cin = Cin; rp.CinTot = CinTot; rp.ci_off = ci_off; rp.taps = taps;
+  rp.Cout = Cout; rp.Cin = Cin; rp.CinTot = CinTot; rp.ci_off = ci_off; rp.co_off = co_off; rp.taps = taps;
   rp.inv_scale = inv_scale; rp.accumulate = accumulate;
   return 0;
 }
@@ -474,8 +475,9 @@ static size_t attn_scratch_bytes(int B, int L, int C) { return L == kAttnL ? 0 :
 // L = 64 (the 8x8 level of a 64x64 frame): one launch of attn_cluster_kernel.  Any other L: attn_qkv_kernel, then
 // attn_stream_kernel, through p.scratch (attn_scratch_bytes)
 static int attn_launch(const AttnParams& p, int B, cudaStream_t st) {
-  DMD_CHECK((p.C == 64 || p.C == 32) && p.L >= 1 && p.C % p.gs == 0 && p.gs % 8 == 0,
-            "attn: unsupported shape L=%d C=%d gs=%d (C in {32, 64}, groups of a multiple of 8 channels)", p.L, p.C, p.gs);
+  // the kernels keep (mean, rstd) of at most 8 groups
+  DMD_CHECK((p.C == 128 || p.C == 64 || p.C == 32) && p.L >= 1 && p.C % p.gs == 0 && p.gs % 8 == 0 && p.C / p.gs <= 8,
+            "attn: unsupported shape L=%d C=%d gs=%d (C in {32, 64, 128}, at most 8 groups of a multiple of 8 channels)", p.L, p.C, p.gs);
   // attn_cluster_kernel adds the output statistics of each CTA's C/4 channels to one GroupNorm group
   DMD_CHECK(p.L != kAttnL || p.gs % (p.C / 4) == 0, "attn: L=%d needs gs a multiple of C/4 (C=%d gs=%d)", kAttnL, p.C, p.gs);
   if (init_kernels()) return 1;
@@ -485,11 +487,13 @@ static int attn_launch(const AttnParams& p, int B, cudaStream_t st) {
     const dim3 grid((p.L + kAttnTile - 1) / kAttnTile, B);
     AttnParams pa = p;
     pa.ktrace = kt_slot("attn qkv", (int)(grid.x * grid.y), p.L);
-    if (p.C == 64) attn_qkv_kernel<64><<<grid, kAttnQkvThreads, 0, st>>>(pa);
+    if (p.C == 128) attn_qkv_kernel<128><<<grid, kAttnQkvThreads, 0, st>>>(pa);
+    else if (p.C == 64) attn_qkv_kernel<64><<<grid, kAttnQkvThreads, 0, st>>>(pa);
     else attn_qkv_kernel<32><<<grid, kAttnQkvThreads, 0, st>>>(pa);
     DMD_LAUNCH_OK();
     pa.ktrace = kt_slot("attn softmax", (int)(grid.x * grid.y), p.L);
-    if (p.C == 64) attn_stream_kernel<64><<<grid, kAttnSThreads, 0, st>>>(pa);
+    if (p.C == 128) attn_stream_kernel<128><<<grid, kAttnSThreads, 0, st>>>(pa);
+    else if (p.C == 64) attn_stream_kernel<64><<<grid, kAttnSThreads, 0, st>>>(pa);
     else attn_stream_kernel<32><<<grid, kAttnSThreads, 0, st>>>(pa);
     DMD_LAUNCH_OK();
     return 0;
@@ -499,7 +503,8 @@ static int attn_launch(const AttnParams& p, int B, cudaStream_t st) {
   // four CTAs per image (thread-block cluster), distributed shared memory for the head outputs
   const int CH = p.C / 4;
   const size_t csmem = sizeof(float) * ((size_t)p.L * (p.C + 1) * 2 + (size_t)p.L * (3 * CH + 4) + (size_t)p.L * CH + (size_t)4 * CH * p.C);
-  if (p.C == 64) attn_cluster_kernel<64><<<4 * B, kAttnCThreads, csmem, st>>>(pt);
+  if (p.C == 128) attn_cluster_kernel<128><<<4 * B, kAttnCThreads, csmem, st>>>(pt);   // 162 KB
+  else if (p.C == 64) attn_cluster_kernel<64><<<4 * B, kAttnCThreads, csmem, st>>>(pt);
   else attn_cluster_kernel<32><<<4 * B, kAttnCThreads, csmem, st>>>(pt);
   DMD_LAUNCH_OK();
   return 0;
@@ -840,6 +845,11 @@ namespace {
 
 constexpr float kGnEps = 1e-5f;  // blocks.py:13
 
+// Packed weights the conv kernel keeps resident next to its slab ring: the 128 -> 64 and 64 -> 128 3x3 convs (144 KB) fit
+// at the widths the 64-channel nets run, a 128 -> 128 3x3 conv (288 KB) does not
+constexpr size_t kResidentWeightMax = 144 * 1024;
+constexpr int kMaxConvChunks = 4;   // 256 input channels (a 128-channel level's up-path concat) in chunks of 64
+struct ConvChunk { int src, c_off, C; size_t pk_off; };   // input channels [c_off, c_off + C) of concat source src, and their pack
 struct ConvW {          // one nn.Conv2d
   int w_idx, b_idx;     // indices into the state_dict pointer list
   int Cout, CoutPad, CinReal, Cin, taps, c0_real, c0_store;
@@ -847,8 +857,14 @@ struct ConvW {          // one nn.Conv2d
   int three_pass = 0;   // split-fp16 as three launches (A_hi W_hi, A_lo W_hi, A_hi W_lo): 3 * Cin weights would crowd out the slab ring
   size_t pk_off;        // byte offset into the packed-weight buffer
   size_t pk_lo_off = 0; // three_pass: the low-part pack
-  // backward-data packs (transposed, tap-flipped; one per source of a channel concat), training only
+  // K split: more than kMaxCin input channels, or weights over kResidentWeightMax, run as one launch per chunk of input
+  // channels (each with its own pack at chunk[j].pk_off; pk_off is then unused), accumulating into the output in place
+  int nchunks = 0; ConvChunk chunk[kMaxConvChunks] = {};
+  // backward-data packs (transposed, tap-flipped; one per source of a channel concat), training only.  A pack over more than
+  // kResidentWeightMax bytes is split the same way, over the gradient channels: widthT channels per chunk, one pack each at
+  // pkTc_off[k][j] (pkT_off[k] is then unused)
   int nsrcT = 0; int srcC[2] = {0, 0}; int srcOff[2] = {0, 0}; size_t pkT_off[2] = {0, 0};
+  int widthT = 0; size_t pkTc_off[2][kMaxConvChunks] = {};
 };
 struct FilmW { int w_idx, b_idx, C, off; };  // AdaGroupNorm.linear ; off = row offset into the batched FiLM GEMM
 struct ResBlockW {
@@ -874,7 +890,7 @@ struct Operand {
 
 // backward op list (training).  Parameter-gradient destinations are OFFSETS into the caller's flat gradient buffer.
 enum BKind { B_PREP = 0, B_CONV, B_WGRAD, B_COLSUM, B_NORM1, B_NORM2, B_AFFINE, B_POOL, B_ATTN, B_MEMSET, B_SGEMM, B_FILMW,
-             B_LINEAR, B_DSILU, B_EMB };
+             B_LINEAR, B_DSILU, B_EMB, B_ATTN_RECOMP, B_ATTN_CORE };
 struct BOp {
   int kind = 0;
   PrepParams prep; int prep_nsrc = 1;
@@ -885,6 +901,8 @@ struct BOp {
   int chunks = 0;                             // sgemm: split-K chunk count (<= 1: no split)
   const float* src = nullptr; float* dst = nullptr; long long rows = 0; int C = 0, Creal = 0, H = 0, W = 0, acc = 0;
   AttnBwdParams ab; long long goffs[6] = {-1, -1, -1, -1, -1, -1};
+  // split attention backward (C = 128): ap recomputes q | k | v into ap.scratch; the buffers of attn_core_bwd_kernel
+  AttnParams ap; float *at_xn = nullptr, *at_gy = nullptr, *at_y = nullptr, *at_gqkv = nullptr, *at_gxn = nullptr;
   void* ms_ptr = nullptr; size_t ms_bytes = 0;
   // sgemm: C = alpha * op(A) op(B); c_goff >= 0 -> C lives in the gradient buffer
   const float *ga = nullptr, *gb = nullptr; float* gc = nullptr; long long sam = 0, sak = 0, sbk = 0, sbn = 0, ldc = 0, c_goff = -1;
@@ -1054,7 +1072,7 @@ struct dmd_rew_end {
 namespace {
 
 struct Walker {  // assigns state_dict indices in module registration order and packed-buffer offsets
-  ModelCore* m; size_t pk = 0;
+  ModelCore* m; size_t pk = 0; int err = 0;
   int next(long long n) { m->numel.push_back(n); return (int)m->numel.size() - 1; }
   size_t take(size_t bytes) { const size_t off = pk; pk = (pk + bytes + 255) & ~(size_t)255; return off; }
   // split: split-fp16 forward (error ~2^-22), in one launch with K = 3 * Cin when those weights take at most 120 KB of shared
@@ -1064,14 +1082,41 @@ struct Walker {  // assigns state_dict indices in module registration order and 
     c.Cout = cout; c.CoutPad = round_up(cout, 16); c.CinReal = cin_real; c.taps = taps;
     c.c0_real = c0_real; c.c0_store = c0_store; c.Cin = round_up(c0_store + c1, 16);
     const size_t w1 = (size_t)taps * c.Cin * c.CoutPad * 2;
-    c.precise = split && 3 * w1 <= 120 * 1024;
-    c.three_pass = split && !c.precise;
-    c.pk_off = take(w1 * (c.precise ? 3 : 1));
-    if (c.three_pass) c.pk_lo_off = take(w1);
+    if (c.Cin > kMaxCin || w1 > kResidentWeightMax) {
+      // chunks of at most kMaxCin channels whose weights stay resident; split-fp16 chunks run in one launch each (K = 3 x chunk)
+      const int f = split ? 3 : 1;
+      const size_t limit = split ? 120 * 1024 : kResidentWeightMax;
+      int width = kMaxCin;
+      while (width > 16 && (size_t)taps * width * c.CoutPad * 2 * f > limit) width /= 2;
+      c.precise = split;
+      const int srcw[2] = {c0_store, c1};
+      for (int k = 0; k < 2; ++k)
+        for (int s = 0; s < srcw[k]; s += width) {
+          if (c.nchunks == kMaxConvChunks) { err = fail("plan: a %d -> %d conv needs more than %d K-split chunks", cin_real, cout, kMaxConvChunks); return c; }
+          ConvChunk& ch = c.chunk[c.nchunks++];
+          ch.src = k; ch.c_off = s; ch.C = srcw[k] - s < width ? srcw[k] - s : width;
+          ch.pk_off = take((size_t)taps * ch.C * c.CoutPad * 2 * f);
+        }
+    } else {
+      c.precise = split && 3 * w1 <= 120 * 1024;
+      c.three_pass = split && !c.precise;
+      c.pk_off = take(w1 * (c.precise ? 3 : 1));
+      if (c.three_pass) c.pk_lo_off = take(w1);
+    }
     if (dgrad) {
       c.nsrcT = c1 ? 2 : 1;
       c.srcC[0] = c0_real; c.srcC[1] = c1; c.srcOff[0] = 0; c.srcOff[1] = c0_real;
-      for (int k = 0; k < c.nsrcT; ++k) c.pkT_off[k] = take((size_t)taps * round_up(cout, 16) * round_up(c.srcC[k], 16) * 2);
+      int cmaxT = 16;
+      for (int k = 0; k < c.nsrcT; ++k) cmaxT = round_up(c.srcC[k], 16) > cmaxT ? round_up(c.srcC[k], 16) : cmaxT;
+      if ((size_t)taps * c.CoutPad * cmaxT * 2 > kResidentWeightMax) {
+        c.widthT = c.CoutPad;
+        while (c.widthT > 16 && (size_t)taps * c.widthT * cmaxT * 2 > kResidentWeightMax) c.widthT /= 2;
+        if (c.CoutPad / c.widthT > kMaxConvChunks) { err = fail("plan: the dgrad of a %d -> %d conv needs more than %d chunks", cin_real, cout, kMaxConvChunks); return c; }
+        for (int k = 0; k < c.nsrcT; ++k)
+          for (int j = 0; j * c.widthT < c.CoutPad; ++j) c.pkTc_off[k][j] = take((size_t)taps * c.widthT * round_up(c.srcC[k], 16) * 2);
+      } else {
+        for (int k = 0; k < c.nsrcT; ++k) c.pkT_off[k] = take((size_t)taps * round_up(cout, 16) * round_up(c.srcC[k], 16) * 2);
+      }
     }
     return c;
   }
@@ -1133,7 +1178,7 @@ int build_structure(dmd_denoiser* h) {
   h->i_normout_w = w.next(c.channels[0]); h->i_normout_b = w.next(c.channels[0]);
   h->conv_out = w.conv(c.img_channels, c.channels[0], 9, c.channels[0], c.channels[0], 0);  // split-fp16 here costs 3x on an N=16 conv for 3.2e-4
   h->core.finish(w.pk);
-  return 0;
+  return w.err;
 }
 
 // ---- descriptors shared by the plan builders and the actor-critic's immediate-mode launches
@@ -1262,6 +1307,25 @@ struct PlanBuilder {
     d.out_stats = out_stats ? (out.stats ? out.stats : (double*)1) : nullptr; d.out_gs = out.gs;
     if (split && (!d.src0_lo || (in.C1 && !d.src1_lo))) { fail("plan: precise conv without low operand parts"); err = 1; return; }
     if (in.C0 + in.C1 != cw.Cin) { fail("plan: operand channels %d+%d do not match the packed weights (%d)", in.C0, in.C1, cw.Cin); err = 1; return; }
+    if (cw.nchunks) {   // K split, as the three-pass split-fp16 conv: bias and residual with the first launch, statistics with the last
+      if (xproj) { fail("plan: a K-split conv cannot carry a fused projection"); err = 1; return; }
+      const size_t plane = (size_t)plc_geometry(pl->B, in.H, in.W).Qalloc * 16;   // one PLC16 plane holds 8 channels
+      for (int j = 0; j < cw.nchunks; ++j) {
+        const ConvChunk& ch = cw.chunk[j];
+        const uint8_t* hi = (const uint8_t*)(ch.src ? d.src1 : d.src0);
+        const uint8_t* lo = (const uint8_t*)(ch.src ? d.src1_lo : d.src0_lo);
+        dmd_conv_desc dc = d;
+        dc.src0 = hi + (size_t)(ch.c_off / 8) * plane; dc.src0_lo = lo ? lo + (size_t)(ch.c_off / 8) * plane : nullptr;
+        dc.src1 = dc.src1_lo = nullptr; dc.C0 = ch.C; dc.C1 = 0;
+        dc.wpk = pk(ch.pk_off);
+        if (j > 0) { dc.bias = nullptr; dc.residual = dc.out; }
+        if (j + 1 < cw.nchunks) dc.out_stats = nullptr;
+        Op op; op.kind = OP_CONV;
+        if (conv_fill(&dc, &op.conv, &op.smem, &op.cols)) { err = 1; return; }
+        pl->ops.push_back(op);
+      }
+      return;
+    }
     for (int pass = 0; pass < (cw.three_pass ? 3 : 1); ++pass) {
       const dmd_conv_desc dp = cw.three_pass ? conv_pass(d, pass, pk(cw.pk_lo_off)) : d;
       Op op; op.kind = OP_CONV;
@@ -1278,8 +1342,10 @@ struct PlanBuilder {
     conv(rb.c1, in1, false, 1, nullptr, t, true);
     Operand in2 = prep(t, nullptr, 0, 1, &rb.n2, 0, 0, true, false);
     Tens o = tensor(rb.cout, H, W, true);
-    // x + r: r is the block input itself, or proj(input) fused into conv2's accumulator (no r tensor, no extra launch)
-    if (rb.has_proj) conv(rb.c2, in2, false, 1, nullptr, o, true, &rb.proj, &in1);
+    // x + r: r is the block input itself, or proj(input) fused into conv2's accumulator (no r tensor, no extra launch).  When
+    // either is K-split, proj(input) runs first into o and conv2 accumulates onto it
+    if (rb.has_proj && !rb.c2.nchunks && !rb.proj.nchunks) conv(rb.c2, in2, false, 1, nullptr, o, true, &rb.proj, &in1);
+    else if (rb.has_proj) { conv(rb.proj, in1, true, 1, nullptr, o, false); conv(rb.c2, in2, false, 1, &o, o, true); }
     else conv(rb.c2, in2, false, 1, &x, o, true);
     Rec rec; rec.kind = R_RES; rec.rb = &rb; rec.x = x; rec.has_skip = skip != nullptr; if (skip) rec.skip = *skip;
     rec.t = t; rec.o = o; rec.in1 = in1; rec.in2 = in2;
@@ -1476,22 +1542,41 @@ struct BwdBuilder {
     BOp b; b.kind = B_COLSUM; b.src = g; b.rows = rows; b.C = C; b.Creal = Creal; b.goff = G(idx); b.goff2 = idx2 >= 0 ? G(idx2) : -1;
     push(b);
   }
+  // one launch, or with split transposed packs (ConvW::widthT) one per chunk of gradient channels, accumulating in place
   void dgrad(const ConvW& cw, int k, const uint8_t* gy, int H, int W, float* out, bool accumulate) {
-    const dmd_conv_desc d = dgrad_desc(cw, k, core->packed + cw.pkT_off[k], gy, pl->B, H, W, out, accumulate);
-    BOp b; b.kind = B_CONV;
-    if (conv_fill(&d, &b.conv, &b.smem, &b.cols)) { err = 1; return; }
-    push(b);
+    const int nch = cw.widthT ? cw.CoutPad / cw.widthT : 1;
+    const size_t plane = (size_t)plc_geometry(pl->B, H, W).Qalloc * 16;   // one PLC16 plane holds 8 channels
+    for (int j = 0; j < nch; ++j) {
+      const void* wpk = core->packed + (cw.widthT ? cw.pkTc_off[k][j] : cw.pkT_off[k]);
+      dmd_conv_desc d = dgrad_desc(cw, k, wpk, gy, pl->B, H, W, out, accumulate || j > 0);
+      if (cw.widthT) { d.src0 = gy + (size_t)(j * cw.widthT / 8) * plane; d.C0 = cw.widthT; }
+      BOp b; b.kind = B_CONV;
+      if (conv_fill(&d, &b.conv, &b.smem, &b.cols)) { err = 1; return; }
+      push(b);
+    }
   }
+  // the weight gradient kernel takes at most 64 gradient and 64 activation channels: one launch per 64 x 64 (Cout, Cin) block
   void wgrad(const ConvW& cw, const uint8_t* gy, const uint8_t* act, int Ca, int Cin, int ci_off, int H, int W) {
-    BOp b; b.kind = B_WGRAD; b.goff = G(cw.w_idx);
-    if (wgrad_fill(gy ? gy : (const void*)1, round_up(cw.Cout, 16), act ? act : (const void*)1, Ca, pl->B, H, W, cw.taps,
-                   pl->partial ? pl->partial : (float*)1, cw.Cout, Cin, cw.CinReal, ci_off, pl->scale ? pl->scale + 1 : (const float*)1, 1, &b.wg)) { err = 1; return; }
-    push(b);
+    const int Cg = round_up(cw.Cout, 16);
+    const size_t plane = (size_t)plc_geometry(pl->B, H, W).Qalloc * 16;
+    for (int co = 0; co < Cg; co += 64)
+      for (int ca = 0; ca < Ca; ca += 64) {
+        BOp b; b.kind = B_WGRAD; b.goff = G(cw.w_idx);
+        const int cg_n = Cg - co < 64 ? Cg - co : 64, ca_n = Ca - ca < 64 ? Ca - ca : 64;
+        const int cout_n = cw.Cout - co < 64 ? cw.Cout - co : 64, cin_n = Cin - ca < 64 ? Cin - ca : 64;
+        if (cin_n <= 0) continue;
+        const uint8_t* g = (gy ? gy : (const uint8_t*)1) + (size_t)(co / 8) * plane;
+        const uint8_t* a = (act ? act : (const uint8_t*)1) + (size_t)(ca / 8) * plane;
+        if (wgrad_fill(g, cg_n, a, ca_n, pl->B, H, W, cw.taps, pl->partial ? pl->partial : (float*)1, cout_n, cin_n, cw.CinReal, ci_off + ca,
+                       pl->scale ? pl->scale + 1 : (const float*)1, 1, &b.wg, co)) { err = 1; return; }
+        push(b);
+      }
   }
   void norm_bwd(const Tens& x, const float* gy, int mode, const FilmW* film, int c_off, int ctot, int gamma_idx, int beta_idx,
-                float* gx, const float* addend, bool accumulate) {
+                float* gx, const float* addend, bool accumulate, bool silu = true) {
     const int R = core->film_rows;
     NormBwdParams nb = gn_bwd_params(x.data, gy, x.stats, pl->B, x.H * x.W, x.C, x.gs, P(gamma_idx), P(beta_idx), pl->nsum, gx, addend, accumulate);
+    nb.act = silu ? 1 : 0;
     if (mode == 1) {   // AdaGroupNorm: FiLM rows in place of gamma / beta, their gradients in place of the per-channel sums
       nb.mode = 1; nb.gamma = nb.beta = nullptr; nb.c_off = c_off;
       nb.film = pl->film; nb.film_stride = R; nb.film_off = film->off; nb.film_ctot = ctot;
@@ -1509,13 +1594,44 @@ struct BwdBuilder {
     BOp b2 = b1; b2.kind = B_NORM2; push(b2);
   }
 
+  // SelfAttention2d backward at C = 128, L = 64 (bwd_kernels.cuh): x = o, g_out = gout, g_x assigned to o.grad.  Buffers in tB
+  // (q | k | v, g_qkv) and tC (xn, g_y, y, g_xn); the weight-gradient products split K over tA
+  void attn_split(const ResBlockW& rb, const Tens& o, const float* gout) {
+    const int C = rb.cout, rows = pl->B * kAttnL;
+    const long long n = (long long)rows * C;
+    if (6 * n > pl->tmp_floats) { err = fail("backward plan: attention temporaries (%lld floats) exceed tB", 6 * n); return; }
+    BOp b; b.kind = B_ATTN_RECOMP;
+    b.ap = AttnParams{o.data, o.stats, P(rb.an_w), P(rb.an_b), P(rb.qkv_w), P(rb.qkv_b), P(rb.op_w), P(rb.op_b), nullptr, nullptr, kAttnL, C, o.gs, kGnEps};
+    b.ap.scratch = pl->tB; b.ap.out = const_cast<float*>(gout);   // attn_core_bwd_kernel reads g_out from ap.out
+    b.at_gqkv = pl->tB + 3 * n;
+    b.at_xn = pl->tC; b.at_gy = pl->tC + n; b.at_y = pl->tC + 2 * n; b.at_gxn = pl->tC + 3 * n;
+    push(b);
+    sgemm(gout, C, 1, P(rb.op_w), C, 1, b.at_gy, -1, C, rows, C, C, 0, 0);                       // g_y = g_out Wo
+    BOp c = b; c.kind = B_ATTN_CORE; push(c);
+    sgemm(gout, 1, C, b.at_y, C, 1, nullptr, G(rb.op_w), C, C, C, rows, 1, 1); split_k();        // dWo += g_out^T y
+    colsum(gout, rows, C, C, rb.op_b);
+    sgemm(b.at_gqkv, 1, 3 * C, b.at_xn, C, 1, nullptr, G(rb.qkv_w), C, 3 * C, C, rows, 1, 1); split_k();   // dWqkv += g_qkv^T xn
+    colsum(b.at_gqkv, rows, 3 * C, 3 * C, rb.qkv_b);
+    sgemm(b.at_gqkv, 3 * C, 1, P(rb.qkv_w), C, 1, b.at_gxn, -1, C, rows, C, 3 * C, 0, 1);      // g_xn += g_qkv Wqkv
+    norm_bwd(o, b.at_gxn, 2, nullptr, 0, C, rb.an_w, rb.an_b, o.grad, nullptr, false, false);
+  }
+  void split_k() {   // the last sgemm contracts over every token of the batch: split K across the SMs, partials in tA
+    BOp& s = pl->bops.back();
+    const long long fit = pl->tmp_floats / ((long long)s.M * s.N);
+    int splits = s.K / 256; if (splits > 32) splits = 32; if (splits > fit) splits = (int)fit;
+    if (splits > 1) s.chunks = splits;
+  }
+
   // ResBlock.forward (blocks.py:141-147) backward
   void resblock(const Rec& r) {
     const ResBlockW& rb = *r.rb;
     const int H = r.o.H, W = r.o.W, B = pl->B;
     const long long pix = (long long)B * H * W;
     Tens o = r.o;
-    if (rb.has_attn) {  // attention consumes o alone: its backward ASSIGNS o's gradient
+    if (rb.has_attn && rb.cout > 64) {
+      attn_split(rb, o, r.a.grad);
+      ginit[o.gid] = 1;
+    } else if (rb.has_attn) {  // attention consumes o alone: its backward ASSIGNS o's gradient
       BOp b; b.kind = B_ATTN;
       b.ab = AttnBwdParams{o.data, o.stats, P(rb.an_w), P(rb.an_b), P(rb.qkv_w), P(rb.qkv_b), P(rb.op_w), r.a.grad, o.grad,
                            nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, pl->scale ? pl->scale + 1 : nullptr, H * W, rb.cout, o.gs, kGnEps};
@@ -1675,6 +1791,8 @@ int make_train_plan(const ModelCore& core, int cmax, int gF_ch, Plan* pl, int B,
   if (base) { PlanBuilder pb{&core, pl, &bb, &sb}; if (fwd(pb)) return 1; } else bb.off = b0.off;
   // backward temporaries
   pl->tmp_floats = (long long)B * H * W * cmax;
+  // the split attention backward at C = 128 (BwdBuilder::attn_split) keeps six [B][64][C] buffers in tB and four in tC
+  if (cmax > 64 && pl->tmp_floats < 6ll * B * kAttnL * cmax) pl->tmp_floats = 6ll * B * kAttnL * cmax;
   const size_t act_bytes = (size_t)pl->tmp_floats * 4;
   pl->tA = (float*)bb.take(act_bytes); pl->tB = (float*)bb.take(act_bytes); pl->tC = (float*)bb.take(act_bytes);
   const size_t op_bytes = plc16_bytes(B, H, W, cmax);
@@ -1701,6 +1819,9 @@ int make_train_plan(const ModelCore& core, int cmax, int gF_ch, Plan* pl, int B,
   return 0;
 }
 
+// U-Net / encoder level widths the executors build: GroupNorm groups of 32, and at most kMaxCin channels per operand source
+// (wider convs run K-split)
+bool level_width_ok(int c) { return c == 32 || c == 64 || c == 128; }
 template <class Cfg> int widest_channels(const Cfg& c) {  // at least 16
   int cmax = 16;
   for (int i = 0; i < c.num_levels; ++i) cmax = c.channels[i] > cmax ? c.channels[i] : cmax;
@@ -1785,7 +1906,7 @@ extern "C" dmd_denoiser* dmd_denoiser_create(const dmd_denoiser_config* cfg) {
   if (!cfg || cfg->num_levels < 1 || cfg->num_levels > DMD_MAX_LEVELS) { fail("denoiser_create: bad config"); return nullptr; }
   if (cfg->cond_channels % 32 || cfg->cond_channels > 256 || cfg->cond_channels % cfg->num_steps_conditioning) { fail("denoiser_create: cond_channels must be a multiple of 32 (<= 256) and of num_steps_conditioning"); return nullptr; }
   for (int i = 0; i < cfg->num_levels; ++i)
-    if (cfg->channels[i] % 32 || cfg->channels[i] > 64) { fail("denoiser_create: channels must be 32 or 64 per level (got %d)", cfg->channels[i]); return nullptr; }
+    if (!level_width_ok(cfg->channels[i])) { fail("denoiser_create: channels must be 32, 64 or 128 per level, at most 128 (got %d at level %d)", cfg->channels[i], i); return nullptr; }
   {   // conv_in's operand: 16, 32 or 64 channels after padding (the operand prep and the wgrad kernel; at 128 the forward
       // computes a wrong model output)
     const int cin = (cfg->num_steps_conditioning + 1) * cfg->img_channels, cp = round_up(cin, 16);
@@ -1798,7 +1919,7 @@ extern "C" dmd_denoiser* dmd_denoiser_create(const dmd_denoiser_config* cfg) {
   if (init_kernels()) return nullptr;
   dmd_denoiser* h = new dmd_denoiser();
   h->cfg = *cfg;
-  build_structure(h);
+  if (build_structure(h)) { delete h; return nullptr; }
   return h;
 }
 extern "C" void dmd_denoiser_destroy(dmd_denoiser* h) {
@@ -1812,10 +1933,21 @@ extern "C" size_t dmd_denoiser_packed_bytes(const dmd_denoiser* h) { return h->c
 
 static int pack_one(const ModelCore& m, const ConvW& c, cudaStream_t st) {
   const float* w = m.ptrs[c.w_idx];
-  if (dmd_pack_conv_weight(w, m.packed + c.pk_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, c.precise, st)) return 1;
+  for (int j = 0; j < c.nchunks; ++j) {   // stored channel i of a chunk is real channel ci_off + i (c0_store = 0, c0_real = ci_off)
+    const ConvChunk& ch = c.chunk[j];
+    const int ci_off = (ch.src ? c.c0_real : 0) + ch.c_off;
+    if (dmd_pack_conv_weight(w, m.packed + ch.pk_off, c.Cout, c.CoutPad, c.CinReal, ch.C, c.taps, ci_off, 0, c.precise, st)) return 1;
+  }
+  if (!c.nchunks && dmd_pack_conv_weight(w, m.packed + c.pk_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, c.precise, st)) return 1;
   if (c.three_pass && dmd_pack_conv_weight(w, m.packed + c.pk_lo_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, 2, st)) return 1;
-  for (int k = 0; k < c.nsrcT; ++k)  // backward-data packs (transposed, flipped), one per concat source
-    if (dmd_pack_conv_weight_dgrad(w, m.packed + c.pkT_off[k], c.Cout, c.CinReal, c.srcOff[k], c.srcC[k], c.taps, st)) return 1;
+  for (int k = 0; k < c.nsrcT; ++k) {  // backward-data packs (transposed, flipped), one per concat source (and gradient chunk)
+    if (!c.widthT) { if (dmd_pack_conv_weight_dgrad(w, m.packed + c.pkT_off[k], c.Cout, c.CinReal, c.srcOff[k], c.srcC[k], c.taps, st)) return 1; continue; }
+    for (int j = 0; j * c.widthT < c.CoutPad; ++j) {   // output channels [j * widthT, ...) of the weight: its rows are outermost
+      const int co0 = j * c.widthT, n = c.Cout - co0 < c.widthT ? c.Cout - co0 : c.widthT;
+      if (dmd_pack_conv_weight_dgrad(w + (size_t)co0 * c.CinReal * c.taps, m.packed + c.pkTc_off[k][j], n, c.CinReal, c.srcOff[k], c.srcC[k],
+                                     c.taps, st)) return 1;
+    }
+  }
   return 0;
 }
 static int pack_rb(const ModelCore& m, const ResBlockW& r, cudaStream_t st) {
@@ -1954,6 +2086,20 @@ int run_backward(const ModelCore& core, Plan& pl, float* grads, cudaStream_t st)
         if (attn_bwd_launch(ab, B, st)) return 1;
         break;
       }
+      case B_ATTN_RECOMP: {
+        const dim3 grid(kAttnL / kAttnTile, B);
+        attn_qkv_kernel<128><<<grid, kAttnQkvThreads, 0, st>>>(b.ap);
+        DMD_LAUNCH_OK();
+        const long long total = (long long)B * kAttnL * b.ap.C;
+        attn_xn_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(b.ap.x, b.ap.st_in, b.ap.gamma, b.ap.beta, b.at_xn, kAttnL, b.ap.C,
+                                                                       b.ap.gs, b.ap.eps, total);
+        DMD_LAUNCH_OK();
+        break;
+      }
+      case B_ATTN_CORE:
+        attn_core_bwd_kernel<<<dim3(b.ap.C / 8, B), kAttnCoreThreads, 0, st>>>(b.ap.scratch, b.at_gy, b.ap.out, b.at_y, b.at_gqkv, b.at_gxn, b.ap.C);
+        DMD_LAUNCH_OK();
+        break;
       case B_MEMSET: DMD_CUDA(cudaMemsetAsync(b.ms_ptr, 0, b.ms_bytes, st)); break;
       case B_SGEMM:   // the long-K product (dcond = dfilm Wf, K = all FiLM rows) is split; its partials live in tA
         if (sgemm_launch(b.ga, b.sam, b.sak, b.gb, b.sbk, b.sbn, b.c_goff >= 0 ? grads + b.c_goff : b.gc, b.ldc, b.M, b.N, b.K,
@@ -2685,7 +2831,7 @@ extern "C" dmd_rew_end* dmd_rew_end_create(const dmd_rew_end_config* cfg) {
   if (!cfg || cfg->num_levels < 1 || cfg->num_levels >= DMD_MAX_LEVELS) { fail("rew_end_create: bad config"); return nullptr; }
   if (cfg->cond_channels % 32 || cfg->cond_channels > 256) { fail("rew_end_create: cond_channels must be a multiple of 32, <= 256"); return nullptr; }
   for (int i = 0; i < cfg->num_levels; ++i)
-    if (cfg->channels[i] % 32 || cfg->channels[i] > 64) { fail("rew_end_create: channels must be 32 or 64 per level (got %d)", cfg->channels[i]); return nullptr; }
+    if (!level_width_ok(cfg->channels[i])) { fail("rew_end_create: channels must be 32, 64 or 128 per level, at most 128 (got %d at level %d)", cfg->channels[i], i); return nullptr; }
   if (cfg->lstm_dim % 4) { fail("rew_end_create: lstm_dim must be a multiple of 4"); return nullptr; }
   if (init_kernels()) return nullptr;
   dmd_rew_end* h = new dmd_rew_end();
@@ -2711,6 +2857,7 @@ extern "C" dmd_rew_end* dmd_rew_end_create(const dmd_rew_end_config* cfg) {
   h->i_wih = w.next(4 * D * K); h->i_whh = w.next(4 * D * D); h->i_bih = w.next(4 * D); h->i_bhh = w.next(4 * D);
   h->i_h0w = w.next(D * D); h->i_h0b = w.next(D); h->i_h2w = w.next(5 * D);
   h->core.finish(w.pk);
+  if (w.err) { delete h; return nullptr; }
   return h;
 }
 extern "C" void dmd_rew_end_destroy(dmd_rew_end* h) { delete h; }

@@ -314,7 +314,7 @@ __global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(kAttnCThreads) attn_
   namespace cg = cooperative_groups;
   constexpr int L = kAttnL, XP = C + 1, CH = C / 4, HL = CH / 8;      // CH channels / HL heads per CTA
   constexpr int Q3 = 3 * CH, QP = Q3 + 4;                            // local q | k | v row, float4-addressable
-  constexpr int KS = kAttnCThreads / (HL * L);                       // threads per (head, query): 2 (C=64) or 4 (C=32)
+  constexpr int KS = kAttnCThreads / (HL * L);                       // threads per (head, query): 1 (C=128), 2 (C=64) or 4 (C=32)
   constexpr int KPT = L / KS;                                        // keys per thread
   extern __shared__ __align__(16) float sm_attn[];
   float* xs = sm_attn;              // [L][XP]  normed x
@@ -359,7 +359,7 @@ __global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(kAttnCThreads) attn_
   // ---- local q | k | v rows: thread = (token l, output group og of NO outputs)
   {
     constexpr int NG = kAttnCThreads / L;   // 4
-    constexpr int NO = Q3 / NG;             // 12 (C=64) or 6 (C=32)
+    constexpr int NO = Q3 / NG;             // 24 (C=128), 12 (C=64) or 6 (C=32)
     const int l = tid % L, og = tid / L;
     float acc[NO];
     int row[NO];
@@ -440,7 +440,7 @@ __global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(kAttnCThreads) attn_
   // ---- out projection of THIS rank's channels + residual on normed x; statistics.  thread = (token l, NO2 outputs)
   {
     constexpr int NG = kAttnCThreads / L;   // 4
-    constexpr int NO2 = CH / NG;            // 4 (C=64) or 2 (C=32) consecutive outputs
+    constexpr int NO2 = CH / NG;            // 8 (C=128), 4 (C=64) or 2 (C=32) consecutive outputs
     const int l = tid % L, og = tid / L;
     const int oc0 = r * CH + og * NO2;
     float acc[NO2];
@@ -509,7 +509,7 @@ template <int C>
 __global__ void __launch_bounds__(kAttnQkvThreads) attn_qkv_kernel(const AttnParams p) {
   constexpr int TQ = kAttnTile, C3 = 3 * C, XP = C + 1, HEADS = C / 8;
   constexpr int NG = kAttnQkvThreads / TQ;   // 8 output groups
-  constexpr int NO = C3 / NG;                // 24 (C=64) or 12 (C=32) outputs per thread
+  constexpr int NO = C3 / NG;                // 48 (C=128), 24 (C=64) or 12 (C=32) outputs per thread
   __shared__ float xs[TQ * XP];
   __shared__ float smr[8][2];
   const int n = blockIdx.y, l0 = blockIdx.x * TQ, tid = threadIdx.x, L = p.L;
@@ -549,8 +549,8 @@ __global__ void __launch_bounds__(kAttnQkvThreads) attn_qkv_kernel(const AttnPar
 template <int C>
 __global__ void __launch_bounds__(kAttnSThreads) attn_stream_kernel(const AttnParams p) {
   constexpr int TQ = kAttnTile, XP = C + 1, HEADS = C / 8;
-  constexpr int KS = kAttnSThreads / (HEADS * TQ);   // threads per (head, query): 2 (C=64) or 4 (C=32)
-  constexpr int KPT = 32, TK = KS * KPT;             // keys per thread and per tile (64 or 128): 32 KB of K / V either way
+  constexpr int KS = kAttnSThreads / (HEADS * TQ);   // threads per (head, query): 1 (C=128), 2 (C=64) or 4 (C=32)
+  constexpr int KPT = C == 128 ? 16 : 32, TK = KS * KPT;   // keys per thread / tile: 32 KB of K / V, 16 KB at C=128 (48 KB static)
   __shared__ __align__(16) float kv[2 * HEADS * TK * 8];   // [k | v][head][TK][8]
   __shared__ float ys[TQ * XP];
   __shared__ float smr[8][2];
@@ -632,7 +632,7 @@ __global__ void __launch_bounds__(kAttnSThreads) attn_stream_kernel(const AttnPa
   __syncthreads();
   // ---- out projection + residual on normed x; statistics.  thread = (token l, NO2 outputs); a warp = 32 tokens of one og
   constexpr int NG = kAttnSThreads / TQ;   // 16
-  constexpr int NO2 = C / NG;              // 4 or 2 consecutive outputs: inside one GroupNorm group (gs % 8 == 0)
+  constexpr int NO2 = C / NG;              // 8, 4 or 2 consecutive outputs: inside one GroupNorm group (gs % 8 == 0)
   const int l = tid % TQ, og = tid / TQ;
   float acc[NO2];
 #pragma unroll

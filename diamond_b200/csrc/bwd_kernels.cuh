@@ -728,4 +728,94 @@ __global__ void pack_conv_weight_T_kernel(const float* __restrict__ w, __half* _
   }
 }
 
+// ------------------------------------------------------------------------------------------------ attention backward, C = 128
+// At C = 128 the one-CTA backward above would need 343 KB of shared memory, so it is split (api.cu BwdBuilder::attn_split):
+// attn_qkv_kernel<128> recomputes q | k | v into scratch ([B][3][16][64][8], head-major), attn_xn_kernel the normed input,
+// sgemm gives g_y = g_out Wo, then attn_core_bwd_kernel runs one CTA per (head, image) and the projection gradients and
+// g_xn += g_qkv Wqkv are sgemm / colsum launches, the GroupNorm backward the two-pass norm backward without SiLU.
+
+// xn = GroupNorm(x) (gamma, beta) from the producer's statistics, NHWC [B][L][C] -> [B][L][C]
+__global__ void attn_xn_kernel(const float* __restrict__ x, const double* __restrict__ st_in, const float* __restrict__ gamma,
+                               const float* __restrict__ beta, float* __restrict__ xn, int L, int C, int gs, float eps, long long total) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int c = (int)(i % C);
+  const long long n = i / ((long long)L * C);
+  const int G = C / gs, g = c / gs;
+  const double cnt = (double)L * gs;
+  const double mean = st_in[(n * G + g) * 2] / cnt;
+  double var = st_in[(n * G + g) * 2 + 1] / cnt - mean * mean;
+  var = var > 0.0 ? var : 0.0;
+  xn[i] = (x[i] - (float)mean) * (float)(1.0 / sqrt(var + (double)eps)) * gamma[c] + beta[c];
+}
+
+// One CTA of kAttnL threads per (head h, image n), L = 64 tokens, head_dim 8.  In: qkv (attn_qkv_kernel layout), gy = g_y,
+// gout = g_out (both NHWC [B][L][C]).  Out: y (attention output before out_proj, NHWC), gqkv ([B][L][3C], q | k | v rows as
+// in Wqkv), gxn = g_out (head h's channels; the g_qkv Wqkv product is added to it afterwards).
+//   P = softmax(q k^T / sqrt 8), y = P v, g_v = P^T g_y, g_s = P o (g_y v^T - rowsum(g_y o y)), g_q = g_s k / sqrt 8,
+//   g_k = g_s^T q / sqrt 8
+constexpr int kAttnCoreThreads = kAttnL;
+__global__ void __launch_bounds__(kAttnCoreThreads) attn_core_bwd_kernel(const float* __restrict__ qkv, const float* __restrict__ gy,
+                                                                        const float* __restrict__ gout, float* __restrict__ y,
+                                                                        float* __restrict__ gqkv, float* __restrict__ gxn, int C) {
+  constexpr int L = kAttnL, LP = L + 1;
+  __shared__ float q[L][8], k[L][8], v[L][8], g[L][8], P[L][LP], S[L][LP];
+  const int h = blockIdx.x, n = blockIdx.y, i = threadIdx.x, HEADS = C / 8;
+  const float* base = qkv + (size_t)n * 3 * C * L;
+  const size_t row = ((size_t)n * L + i) * C + h * 8;
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    q[i][e] = base[((size_t)h * L + i) * 8 + e];
+    k[i][e] = base[((size_t)(HEADS + h) * L + i) * 8 + e];
+    v[i][e] = base[((size_t)(2 * HEADS + h) * L + i) * 8 + e];
+    g[i][e] = gy[row + e];
+    gxn[row + e] = gout[row + e];
+  }
+  __syncthreads();
+  const float sc = 0.35355339059327373f;   // 1/sqrt(8)
+  // ---- row i: softmax, y_i, g_s row
+  float mx = -INFINITY;
+  for (int j = 0; j < L; ++j) {
+    float s = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) s = fmaf(q[i][e] * sc, k[j][e], s);
+    P[i][j] = s;
+    mx = fmaxf(mx, s);
+  }
+  float den = 0.f;
+  for (int j = 0; j < L; ++j) { const float pj = expf(P[i][j] - mx); P[i][j] = pj; den += pj; }
+  const float inv = 1.f / den;
+  float yi[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  for (int j = 0; j < L; ++j) {
+    const float pj = P[i][j] * inv;
+    P[i][j] = pj;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) yi[e] = fmaf(pj, v[j][e], yi[e]);
+  }
+  float D = 0.f;
+#pragma unroll
+  for (int e = 0; e < 8; ++e) { y[row + e] = yi[e]; D = fmaf(g[i][e], yi[e], D); }
+  float gq[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  for (int j = 0; j < L; ++j) {
+    float dp = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) dp = fmaf(g[i][e], v[j][e], dp);
+    const float ds = P[i][j] * (dp - D) * sc;
+    S[i][j] = ds;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) gq[e] = fmaf(ds, k[j][e], gq[e]);
+  }
+  __syncthreads();
+  // ---- column j = i: g_k, g_v
+  float gk[8] = {0, 0, 0, 0, 0, 0, 0, 0}, gv[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  for (int r = 0; r < L; ++r) {
+    const float ds = S[r][i], pr = P[r][i];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) { gk[e] = fmaf(ds, q[r][e], gk[e]); gv[e] = fmaf(pr, g[r][e], gv[e]); }
+  }
+  float* o = gqkv + ((size_t)n * L + i) * 3 * C + h * 8;
+#pragma unroll
+  for (int e = 0; e < 8; ++e) { o[e] = gq[e]; o[C + e] = gk[e]; o[2 * C + e] = gv[e]; }
+}
+
 }  // namespace dmd

@@ -164,6 +164,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const WgradPara
 struct WgradReduceParams {
   const float* partial; int nparts; int N;
   float* dW; int Cout, Cin, CinTot, ci_off, taps;
+  int co_off;                   // first output channel (row of dW) of this launch's 64-row block
   const float* inv_scale;       // device scalar or null (1.0)
   int accumulate;
 };
@@ -201,7 +202,7 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const WgradReducePara
   if (kg == 0 && live) {
     s = (part[0][o] + part[1][o]) + (part[2][o] + part[3][o]);
     if (p.inv_scale) s *= *p.inv_scale;
-    float* d = p.dW + ((size_t)co * p.CinTot + p.ci_off + ci) * p.taps + t;
+    float* d = p.dW + ((size_t)(p.co_off + co) * p.CinTot + p.ci_off + ci) * p.taps + t;
     *d = p.accumulate ? *d + s : s;
   }
 }

@@ -176,8 +176,8 @@ int dmd_prep_plan(const dmd_prep_desc* d, int* blocks, int* pos_per_block, int* 
 /* GroupNorm partial sums of an NHWC tensor: stats[n][g] += (sum, sumsq) (blocks.py:28,43). */
 int dmd_gn_stats(const float* x, double* stats, int B, int HW, int C, int gs, void* stream);
 
-/* SelfAttention2d.forward (blocks.py:62-72), L = H*W = 64 tokens, C in {32, 64}, head_dim 8, groups of gs channels (gs a
- * multiple of 8 dividing C, and at L = 64 a multiple of C/4, as every model's gs = 32 is): out = xn + out_proj(softmax(q k^T
+/* SelfAttention2d.forward (blocks.py:62-72), L = H*W = 64 tokens, C in {32, 64, 128}, head_dim 8, at most 8 groups of gs
+ * channels (gs a multiple of 8 dividing C, and at L = 64 a multiple of C/4, as every model's gs = 32 is): out = xn + out_proj(softmax(q k^T
  * / sqrt(8)) v) with xn = GroupNorm(x) from the producer's statistics stats_in [B][C/gs][2]; out_stats (or NULL) [B][C/gs][2]
  * += (sum, sumsq) of out. */
 int dmd_attn_fwd(const float* x, const double* stats_in, const float* gamma, const float* beta, const float* wqkv,
@@ -296,7 +296,7 @@ typedef struct dmd_denoiser_config {
   int cond_channels;
   int num_levels;
   int depths[DMD_MAX_LEVELS];
-  int channels[DMD_MAX_LEVELS];
+  int channels[DMD_MAX_LEVELS]; /* 32, 64 or 128 per level, in any mix */
   int attn_depths[DMD_MAX_LEVELS];
   int num_actions;
   float sigma_data;             /* DenoiserConfig */
@@ -415,7 +415,7 @@ typedef struct dmd_actor_critic_config {
   int img_channels;
   int img_size;
   int num_levels;
-  int channels[DMD_MAX_LEVELS];
+  int channels[DMD_MAX_LEVELS]; /* 32 or 64 per level */
   int down[DMD_MAX_LEVELS];
   int num_actions;
 } dmd_actor_critic_config;
@@ -468,7 +468,7 @@ typedef struct dmd_rew_end_config {
   int cond_channels;
   int num_levels;
   int depths[DMD_MAX_LEVELS];
-  int channels[DMD_MAX_LEVELS];
+  int channels[DMD_MAX_LEVELS]; /* 32, 64 or 128 per level, in any mix */
   int attn_depths[DMD_MAX_LEVELS];
   int num_actions;
 } dmd_rew_end_config;
