@@ -849,7 +849,8 @@ constexpr float kGnEps = 1e-5f;  // blocks.py:13
 // at the widths the 64-channel nets run, a 128 -> 128 3x3 conv (288 KB) does not
 constexpr size_t kResidentWeightMax = 144 * 1024;
 constexpr int kMaxConvChunks = 4;   // 256 input channels (a 128-channel level's up-path concat) in chunks of 64
-struct ConvChunk { int src, c_off, C; size_t pk_off; };   // input channels [c_off, c_off + C) of concat source src, and their pack
+// input channels [c_off, c_off + C) of concat source src, their pack, and (three-pass chunks) their low-part pack
+struct ConvChunk { int src, c_off, C; size_t pk_off, pk_lo_off; };
 struct ConvW {          // one nn.Conv2d
   int w_idx, b_idx;     // indices into the state_dict pointer list
   int Cout, CoutPad, CinReal, Cin, taps, c0_real, c0_store;
@@ -858,7 +859,8 @@ struct ConvW {          // one nn.Conv2d
   size_t pk_off;        // byte offset into the packed-weight buffer
   size_t pk_lo_off = 0; // three_pass: the low-part pack
   // K split: more than kMaxCin input channels, or weights over kResidentWeightMax, run as one launch per chunk of input
-  // channels (each with its own pack at chunk[j].pk_off; pk_off is then unused), accumulating into the output in place
+  // channels (each with its own pack at chunk[j].pk_off; pk_off is then unused), accumulating into the output in place.
+  // With three_pass, each chunk runs as three passes (its low-part pack at chunk[j].pk_lo_off; pk_lo_off is then unused)
   int nchunks = 0; ConvChunk chunk[kMaxConvChunks] = {};
   // backward-data packs (transposed, tap-flipped; one per source of a channel concat), training only.  A pack over more than
   // kResidentWeightMax bytes is split the same way, over the gradient channels: widthT channels per chunk, one pack each at
@@ -1088,14 +1090,23 @@ struct Walker {  // assigns state_dict indices in module registration order and 
       const size_t limit = split ? 120 * 1024 : kResidentWeightMax;
       int width = kMaxCin;
       while (width > 16 && (size_t)taps * width * c.CoutPad * 2 * f > limit) width /= 2;
-      c.precise = split;
       const int srcw[2] = {c0_store, c1};
+      auto nchunks_at = [&](int wd) { return (srcw[0] + wd - 1) / wd + (srcw[1] + wd - 1) / wd; };
+      if (split && nchunks_at(width) > kMaxConvChunks) {
+        // split-fp16 chunks that would each run in one launch are too narrow here (a 3x3 128 -> 128 conv: 8 chunks of 16).
+        // Instead every chunk runs as three passes, with kResidentWeightMax bytes of weights (64 channels at CoutPad 128)
+        c.three_pass = 1;
+        width = kMaxCin;
+        while (width > 16 && (size_t)taps * width * c.CoutPad * 2 > kResidentWeightMax) width /= 2;
+      }
+      c.precise = split && !c.three_pass;
       for (int k = 0; k < 2; ++k)
         for (int s = 0; s < srcw[k]; s += width) {
           if (c.nchunks == kMaxConvChunks) { err = fail("plan: a %d -> %d conv needs more than %d K-split chunks", cin_real, cout, kMaxConvChunks); return c; }
           ConvChunk& ch = c.chunk[c.nchunks++];
           ch.src = k; ch.c_off = s; ch.C = srcw[k] - s < width ? srcw[k] - s : width;
-          ch.pk_off = take((size_t)taps * ch.C * c.CoutPad * 2 * f);
+          ch.pk_off = take((size_t)taps * ch.C * c.CoutPad * 2 * (c.precise ? 3 : 1));
+          if (c.three_pass) ch.pk_lo_off = take((size_t)taps * ch.C * c.CoutPad * 2);
         }
     } else {
       c.precise = split && 3 * w1 <= 120 * 1024;
@@ -1211,6 +1222,66 @@ dmd_conv_desc conv_pass(dmd_conv_desc d, int pass, const void* wpk_lo) {
   if (pass < 2) d.out_stats = nullptr;
   return d;
 }
+// every launch of conv cw, given its one-launch description d: d itself, its three split-fp16 passes, or one launch (or three
+// passes) per K-split chunk.  Bias and residual go with the first launch, statistics with the last; the later launches
+// accumulate into the output in place.  plane: bytes of one PLC16 plane (8 channels) of the operand; pk: pack offset -> pointer
+template <class Pk, class Emit>
+int for_each_conv_launch(const ConvW& cw, const dmd_conv_desc& d, size_t plane, Pk pk, Emit emit) {
+  const int passes = cw.three_pass ? 3 : 1;
+  if (!cw.nchunks) {
+    for (int pass = 0; pass < passes; ++pass)
+      if (emit(cw.three_pass ? conv_pass(d, pass, pk(cw.pk_lo_off)) : d)) return 1;
+    return 0;
+  }
+  for (int j = 0; j < cw.nchunks; ++j) {
+    const ConvChunk& ch = cw.chunk[j];
+    const uint8_t* hi = (const uint8_t*)(ch.src ? d.src1 : d.src0);
+    const uint8_t* lo = (const uint8_t*)(ch.src ? d.src1_lo : d.src0_lo);
+    dmd_conv_desc dc = d;
+    dc.src0 = hi + (size_t)(ch.c_off / 8) * plane; dc.src0_lo = lo ? lo + (size_t)(ch.c_off / 8) * plane : nullptr;
+    dc.src1 = dc.src1_lo = nullptr; dc.C0 = ch.C; dc.C1 = 0;
+    dc.wpk = pk(ch.pk_off);
+    if (j > 0) { dc.bias = nullptr; dc.residual = dc.out; }
+    if (j + 1 < cw.nchunks) dc.out_stats = nullptr;
+    for (int pass = 0; pass < passes; ++pass)
+      if (emit(cw.three_pass ? conv_pass(dc, pass, pk(ch.pk_lo_off)) : dc)) return 1;
+  }
+  return 0;
+}
+// backward-data of source k of conv cw: one launch, or with split transposed packs (ConvW::widthT) one per chunk of gradient
+// channels, accumulating in place.  gy: the PLC16 gradient operand at B x H x W
+template <class Emit>
+int for_each_dgrad_launch(const ConvW& cw, int k, const uint8_t* packed, const uint8_t* gy, int B, int H, int W, float* out,
+                          bool accumulate, Emit emit) {
+  const int nch = cw.widthT ? cw.CoutPad / cw.widthT : 1;
+  const size_t plane = (size_t)plc_geometry(B, H, W).Qalloc * 16;   // one PLC16 plane holds 8 channels
+  for (int j = 0; j < nch; ++j) {
+    const void* wpk = packed + (cw.widthT ? cw.pkTc_off[k][j] : cw.pkT_off[k]);
+    dmd_conv_desc d = dgrad_desc(cw, k, wpk, gy, B, H, W, out, accumulate || j > 0);
+    if (cw.widthT) { d.src0 = gy + (size_t)(j * cw.widthT / 8) * plane; d.C0 = cw.widthT; }
+    if (emit(d)) return 1;
+  }
+  return 0;
+}
+// the weight gradient kernel takes at most 64 gradient and 64 activation channels: one launch per 64 x 64 (Cout, Cin) block.
+// gy / act: PLC16 operands at B x H x W with round_up(Cout, 16) / Ca channels; act channel i is input channel ci_off + i
+template <class Emit>
+int for_each_wgrad_launch(const ConvW& cw, const uint8_t* gy, const uint8_t* act, int Ca, int Cin, int ci_off, int B, int H, int W,
+                          float* partial, const float* inv_scale, Emit emit) {
+  const int Cg = round_up(cw.Cout, 16);
+  const size_t plane = (size_t)plc_geometry(B, H, W).Qalloc * 16;
+  for (int co = 0; co < Cg; co += 64)
+    for (int ca = 0; ca < Ca; ca += 64) {
+      const int cg_n = Cg - co < 64 ? Cg - co : 64, ca_n = Ca - ca < 64 ? Ca - ca : 64;
+      const int cout_n = cw.Cout - co < 64 ? cw.Cout - co : 64, cin_n = Cin - ca < 64 ? Cin - ca : 64;
+      if (cin_n <= 0) continue;
+      WgradLaunch L;
+      if (wgrad_fill(gy + (size_t)(co / 8) * plane, cg_n, act + (size_t)(ca / 8) * plane, ca_n, B, H, W, cw.taps, partial, cout_n, cin_n,
+                     cw.CinReal, ci_off + ca, inv_scale, 1, &L, co)) return 1;
+      if (emit(L)) return 1;
+    }
+  return 0;
+}
 // silu(GroupNorm(gamma, beta)) backward of x [B][HW][C] (mode 2): per-channel sums in nsum ([2][B][kMaxCin], zeroed before
 // pass 1), gx (+)= the input gradient (+ addend)
 NormBwdParams gn_bwd_params(const float* x, const float* gy, const double* stats, int B, int HW, int C, int gs, const float* gamma,
@@ -1307,31 +1378,14 @@ struct PlanBuilder {
     d.out_stats = out_stats ? (out.stats ? out.stats : (double*)1) : nullptr; d.out_gs = out.gs;
     if (split && (!d.src0_lo || (in.C1 && !d.src1_lo))) { fail("plan: precise conv without low operand parts"); err = 1; return; }
     if (in.C0 + in.C1 != cw.Cin) { fail("plan: operand channels %d+%d do not match the packed weights (%d)", in.C0, in.C1, cw.Cin); err = 1; return; }
-    if (cw.nchunks) {   // K split, as the three-pass split-fp16 conv: bias and residual with the first launch, statistics with the last
-      if (xproj) { fail("plan: a K-split conv cannot carry a fused projection"); err = 1; return; }
-      const size_t plane = (size_t)plc_geometry(pl->B, in.H, in.W).Qalloc * 16;   // one PLC16 plane holds 8 channels
-      for (int j = 0; j < cw.nchunks; ++j) {
-        const ConvChunk& ch = cw.chunk[j];
-        const uint8_t* hi = (const uint8_t*)(ch.src ? d.src1 : d.src0);
-        const uint8_t* lo = (const uint8_t*)(ch.src ? d.src1_lo : d.src0_lo);
-        dmd_conv_desc dc = d;
-        dc.src0 = hi + (size_t)(ch.c_off / 8) * plane; dc.src0_lo = lo ? lo + (size_t)(ch.c_off / 8) * plane : nullptr;
-        dc.src1 = dc.src1_lo = nullptr; dc.C0 = ch.C; dc.C1 = 0;
-        dc.wpk = pk(ch.pk_off);
-        if (j > 0) { dc.bias = nullptr; dc.residual = dc.out; }
-        if (j + 1 < cw.nchunks) dc.out_stats = nullptr;
-        Op op; op.kind = OP_CONV;
-        if (conv_fill(&dc, &op.conv, &op.smem, &op.cols)) { err = 1; return; }
-        pl->ops.push_back(op);
-      }
-      return;
-    }
-    for (int pass = 0; pass < (cw.three_pass ? 3 : 1); ++pass) {
-      const dmd_conv_desc dp = cw.three_pass ? conv_pass(d, pass, pk(cw.pk_lo_off)) : d;
+    if (cw.nchunks && xproj) { fail("plan: a K-split conv cannot carry a fused projection"); err = 1; return; }
+    const size_t plane = (size_t)plc_geometry(pl->B, in.H, in.W).Qalloc * 16;   // one PLC16 plane holds 8 channels
+    if (for_each_conv_launch(cw, d, plane, [&](size_t off) { return pk(off); }, [&](const dmd_conv_desc& dc) {
       Op op; op.kind = OP_CONV;
-      if (conv_fill(&dp, &op.conv, &op.smem, &op.cols)) { err = 1; return; }
+      if (conv_fill(&dc, &op.conv, &op.smem, &op.cols)) return 1;
       pl->ops.push_back(op);
-    }
+      return 0;
+    })) err = 1;
   }
 
   // ResBlock.forward (blocks.py:141-147)
@@ -1544,33 +1598,20 @@ struct BwdBuilder {
   }
   // one launch, or with split transposed packs (ConvW::widthT) one per chunk of gradient channels, accumulating in place
   void dgrad(const ConvW& cw, int k, const uint8_t* gy, int H, int W, float* out, bool accumulate) {
-    const int nch = cw.widthT ? cw.CoutPad / cw.widthT : 1;
-    const size_t plane = (size_t)plc_geometry(pl->B, H, W).Qalloc * 16;   // one PLC16 plane holds 8 channels
-    for (int j = 0; j < nch; ++j) {
-      const void* wpk = core->packed + (cw.widthT ? cw.pkTc_off[k][j] : cw.pkT_off[k]);
-      dmd_conv_desc d = dgrad_desc(cw, k, wpk, gy, pl->B, H, W, out, accumulate || j > 0);
-      if (cw.widthT) { d.src0 = gy + (size_t)(j * cw.widthT / 8) * plane; d.C0 = cw.widthT; }
+    if (for_each_dgrad_launch(cw, k, core->packed, gy, pl->B, H, W, out, accumulate, [&](const dmd_conv_desc& d) {
       BOp b; b.kind = B_CONV;
-      if (conv_fill(&d, &b.conv, &b.smem, &b.cols)) { err = 1; return; }
+      if (conv_fill(&d, &b.conv, &b.smem, &b.cols)) return 1;
       push(b);
-    }
+      return 0;
+    })) err = 1;
   }
-  // the weight gradient kernel takes at most 64 gradient and 64 activation channels: one launch per 64 x 64 (Cout, Cin) block
   void wgrad(const ConvW& cw, const uint8_t* gy, const uint8_t* act, int Ca, int Cin, int ci_off, int H, int W) {
-    const int Cg = round_up(cw.Cout, 16);
-    const size_t plane = (size_t)plc_geometry(pl->B, H, W).Qalloc * 16;
-    for (int co = 0; co < Cg; co += 64)
-      for (int ca = 0; ca < Ca; ca += 64) {
-        BOp b; b.kind = B_WGRAD; b.goff = G(cw.w_idx);
-        const int cg_n = Cg - co < 64 ? Cg - co : 64, ca_n = Ca - ca < 64 ? Ca - ca : 64;
-        const int cout_n = cw.Cout - co < 64 ? cw.Cout - co : 64, cin_n = Cin - ca < 64 ? Cin - ca : 64;
-        if (cin_n <= 0) continue;
-        const uint8_t* g = (gy ? gy : (const uint8_t*)1) + (size_t)(co / 8) * plane;
-        const uint8_t* a = (act ? act : (const uint8_t*)1) + (size_t)(ca / 8) * plane;
-        if (wgrad_fill(g, cg_n, a, ca_n, pl->B, H, W, cw.taps, pl->partial ? pl->partial : (float*)1, cout_n, cin_n, cw.CinReal, ci_off + ca,
-                       pl->scale ? pl->scale + 1 : (const float*)1, 1, &b.wg, co)) { err = 1; return; }
-        push(b);
-      }
+    if (for_each_wgrad_launch(cw, gy ? gy : (const uint8_t*)1, act ? act : (const uint8_t*)1, Ca, Cin, ci_off, pl->B, H, W,
+                              pl->partial ? pl->partial : (float*)1, pl->scale ? pl->scale + 1 : (const float*)1, [&](const WgradLaunch& L) {
+      BOp b; b.kind = B_WGRAD; b.goff = G(cw.w_idx); b.wg = L;
+      push(b);
+      return 0;
+    })) err = 1;
   }
   void norm_bwd(const Tens& x, const float* gy, int mode, const FilmW* film, int c_off, int ctot, int gamma_idx, int beta_idx,
                 float* gx, const float* addend, bool accumulate, bool silu = true) {
@@ -1937,9 +1978,10 @@ static int pack_one(const ModelCore& m, const ConvW& c, cudaStream_t st) {
     const ConvChunk& ch = c.chunk[j];
     const int ci_off = (ch.src ? c.c0_real : 0) + ch.c_off;
     if (dmd_pack_conv_weight(w, m.packed + ch.pk_off, c.Cout, c.CoutPad, c.CinReal, ch.C, c.taps, ci_off, 0, c.precise, st)) return 1;
+    if (c.three_pass && dmd_pack_conv_weight(w, m.packed + ch.pk_lo_off, c.Cout, c.CoutPad, c.CinReal, ch.C, c.taps, ci_off, 0, 2, st)) return 1;
   }
   if (!c.nchunks && dmd_pack_conv_weight(w, m.packed + c.pk_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, c.precise, st)) return 1;
-  if (c.three_pass && dmd_pack_conv_weight(w, m.packed + c.pk_lo_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, 2, st)) return 1;
+  if (!c.nchunks && c.three_pass && dmd_pack_conv_weight(w, m.packed + c.pk_lo_off, c.Cout, c.CoutPad, c.CinReal, c.Cin, c.taps, c.c0_real, c.c0_store, 2, st)) return 1;
   for (int k = 0; k < c.nsrcT; ++k) {  // backward-data packs (transposed, flipped), one per concat source (and gradient chunk)
     if (!c.widthT) { if (dmd_pack_conv_weight_dgrad(w, m.packed + c.pkT_off[k], c.Cout, c.CinReal, c.srcOff[k], c.srcC[k], c.taps, st)) return 1; continue; }
     for (int j = 0; j * c.widthT < c.CoutPad; ++j) {   // output channels [j * widthT, ...) of the weight: its rows are outermost
@@ -2348,6 +2390,10 @@ struct AcBuffers {
   float* x0; void* opnd; void* opnd_lo; std::vector<float*> r, y, pooled; std::vector<double*> st_in, st_y; float *gates, *hx, *cx; double* stats; size_t stats_bytes; size_t total;
 };
 
+// channels of the operand and gradient buffers that every level shares: the widest level, and never fewer than the 64 the
+// layouts of 32- and 64-channel nets have always had
+int ac_operand_channels(const dmd_actor_critic_config& c) { const int w = widest_channels(c); return w > 64 ? w : 64; }
+
 // lays out the workspace; base may be null (size query)
 int ac_layout(const dmd_actor_critic* h, int B, uint8_t* base, AcBuffers* o) {
   const dmd_actor_critic_config& c = h->cfg;
@@ -2363,8 +2409,9 @@ int ac_layout(const dmd_actor_critic* h, int B, uint8_t* base, AcBuffers* o) {
   o->stats = (double*)base; o->stats_bytes = (sb.off + 255) & ~(size_t)255;
   Bump bb{base ? base + o->stats_bytes : nullptr};
   o->x0 = (float*)bb.take((size_t)B * S * S * h->conv0.c0_store * 4);
-  o->opnd = bb.take(plc16_bytes(B, S, S, 64));  // one operand buffer: every conv's prep immediately precedes it on the stream
-  o->opnd_lo = bb.take(plc16_bytes(B, S, S, 64));  // its fp16 low part (split-fp16 forward)
+  const int cw = ac_operand_channels(c);
+  o->opnd = bb.take(plc16_bytes(B, S, S, cw));  // one operand buffer: every conv's prep immediately precedes it on the stream
+  o->opnd_lo = bb.take(plc16_bytes(B, S, S, cw));  // its fp16 low part (split-fp16 forward)
   float* cur = (float*)bb.take((size_t)B * S * S * c.channels[0] * 4);  // conv0 output
   o->r.assign(nl, nullptr); o->y.assign(nl, nullptr); o->pooled.assign(nl + 1, nullptr);
   o->pooled[0] = cur;
@@ -2385,7 +2432,7 @@ int ac_layout(const dmd_actor_critic* h, int B, uint8_t* base, AcBuffers* o) {
 extern "C" dmd_actor_critic* dmd_actor_critic_create(const dmd_actor_critic_config* cfg) {
   if (!cfg || cfg->num_levels < 1 || cfg->num_levels > DMD_MAX_LEVELS) { fail("actor_critic_create: bad config"); return nullptr; }
   for (int i = 0; i < cfg->num_levels; ++i)
-    if (cfg->channels[i] % 32 || cfg->channels[i] > 64) { fail("actor_critic_create: channels must be 32 or 64 (got %d)", cfg->channels[i]); return nullptr; }
+    if (!level_width_ok(cfg->channels[i])) { fail("actor_critic_create: channels must be 32, 64 or 128 per level, at most 128 (got %d at level %d)", cfg->channels[i], i); return nullptr; }
   if (cfg->lstm_dim % 4) { fail("actor_critic_create: lstm_dim must be a multiple of 4"); return nullptr; }
   if (init_kernels()) return nullptr;
   dmd_actor_critic* h = new dmd_actor_critic();
@@ -2410,6 +2457,7 @@ extern "C" dmd_actor_critic* dmd_actor_critic_create(const dmd_actor_critic_conf
   h->i_wih = w.next(4 * D * K); h->i_whh = w.next(4 * D * D); h->i_bih = w.next(4 * D); h->i_bhh = w.next(4 * D);
   h->i_cw = w.next(D); h->i_cb = w.next(1); h->i_aw = w.next((long long)cfg->num_actions * D); h->i_ab = w.next(cfg->num_actions);
   h->core.finish(w.pk);
+  if (w.err) { delete h; return nullptr; }
   return h;
 }
 extern "C" void dmd_actor_critic_destroy(dmd_actor_critic* h) { delete h; }
@@ -2454,11 +2502,9 @@ extern "C" int dmd_actor_critic_forward(dmd_actor_critic* h, int B, const float*
     d.B = B; d.H = hw; d.W = hw; d.taps = cw.taps; d.stride = 1;
     d.wpk = m.packed + cw.pk_off; d.bias = m.ptrs[cw.b_idx]; d.Cout = cw.Cout; d.CoutPad = cw.CoutPad;
     d.residual = resid; d.out = out; d.out_stats = st_out; d.out_gs = gn_group_size(cw.Cout);
-    for (int pass = 0; pass < (cw.three_pass ? 3 : 1); ++pass) {
-      dmd_conv_desc dp = cw.three_pass ? conv_pass(d, pass, m.packed + cw.pk_lo_off) : d;
-      if (dmd_conv2d_fprop(&dp, st)) return 1;
-    }
-    return 0;
+    const size_t plane = (size_t)plc_geometry(B, hw, hw).Qalloc * 16;   // one PLC16 plane holds 8 channels
+    return for_each_conv_launch(cw, d, plane, [&](size_t off) { return m.packed + off; },
+                                [&](const dmd_conv_desc& dc) { return dmd_conv2d_fprop(&dc, st); });
   };
   // conv0 feeds the first GroupNorm -> statistics in its epilogue
   if (run_conv(h->conv0, b.x0, h->conv0.c0_store, S, 0, 0, 0, nullptr, nullptr, b.pooled[0], b.st_in[0])) return 1;
@@ -2499,10 +2545,10 @@ struct AcScratch {
 int ac_scratch_layout(const dmd_actor_critic* h, int B, uint8_t* base, AcScratch* o) {
   const dmd_actor_critic_config& c = h->cfg;
   Bump bb{base};
-  const int S = c.img_size;
-  const size_t act = (size_t)B * S * S * 64 * 4;
+  const int S = c.img_size, cw = ac_operand_channels(c);
+  const size_t act = (size_t)B * S * S * cw * 4;
   o->g_a = (float*)bb.take(act); o->g_b = (float*)bb.take(act); o->tA = (float*)bb.take(act);
-  o->gy_op = (uint8_t*)bb.take(plc16_bytes(B, S, S, 64)); o->x_op = (uint8_t*)bb.take(plc16_bytes(B, S, S, 64));
+  o->gy_op = (uint8_t*)bb.take(plc16_bytes(B, S, S, cw)); o->x_op = (uint8_t*)bb.take(plc16_bytes(B, S, S, cw));
   const int D = c.lstm_dim, K = h->feat_c * h->feat_hw;
   o->dgates = (float*)bb.take((size_t)B * 4 * D * 4); o->g_h = (float*)bb.take((size_t)B * D * 4);
   o->g_xflat = (float*)bb.take((size_t)B * K * 4); o->x_flat = (float*)bb.take((size_t)B * K * 4);
@@ -2589,9 +2635,11 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
   }
   const float* inv = sc.scale + 1;
   auto wgrad = [&](const ConvW& cw, const uint8_t* gy, const uint8_t* act, int Ca, int hw) -> int {
-    WgradLaunch L;
-    if (wgrad_fill(gy, round_up(cw.Cout, 16), act, Ca, B, hw, hw, cw.taps, sc.partial, cw.Cout, cw.CinReal, cw.CinReal, 0, inv, 1, &L)) return 1;
-    return wgrad_launch(L, G(cw.w_idx), st);
+    return for_each_wgrad_launch(cw, gy, act, Ca, cw.CinReal, 0, B, hw, hw, sc.partial, inv,
+                                 [&](const WgradLaunch& L) { return wgrad_launch(L, G(cw.w_idx), st); });
+  };
+  auto dgrad = [&](const ConvW& cw, const uint8_t* gy, int hw, float* out, bool accumulate) -> int {
+    return for_each_dgrad_launch(cw, 0, m.packed, gy, B, hw, hw, out, accumulate, [&](const dmd_conv_desc& d) { return dmd_conv2d_fprop(&d, st); });
   };
   // spatial size of every level's input
   std::vector<int> size_in(h->levels.size() + 1);
@@ -2614,8 +2662,7 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
     pd = prep_desc(b.pooled[i], lv.cin, B, S, S, 0, 2, b.st_in[i], m.P(lv.gn_w), m.P(lv.gn_b), sc.x_op);
     if (dmd_prep_act(&pd, st)) return 1;
     if (wgrad(lv.conv, sc.gy_op, sc.x_op, round_up(lv.cin, 16), S)) return 1;
-    dmd_conv_desc cd = dgrad_desc(lv.conv, 0, m.packed + lv.conv.pkT_off[0], sc.gy_op, B, S, S, sc.tA, false);
-    if (dmd_conv2d_fprop(&cd, st)) return 1;
+    if (dgrad(lv.conv, sc.gy_op, S, sc.tA, false)) return 1;
     const NormBwdParams nb = gn_bwd_params(b.pooled[i], sc.tA, b.st_in[i], B, S * S, lv.cin, gn_group_size(lv.cin), m.P(lv.gn_w),
                                            m.P(lv.gn_b), sc.nsum, gx, lv.has_skip ? nullptr : gy, false);
     DMD_CUDA(cudaMemsetAsync(sc.nsum, 0, (size_t)2 * B * kMaxCin * 4, st));
@@ -2624,8 +2671,7 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
       pd = prep_desc(b.pooled[i], lv.cin, B, S, S, 0, 0, nullptr, nullptr, nullptr, sc.x_op);
       if (dmd_prep_act(&pd, st)) return 1;
       if (wgrad(lv.skip, sc.gy_op, sc.x_op, round_up(lv.cin, 16), S)) return 1;
-      cd = dgrad_desc(lv.skip, 0, m.packed + lv.skip.pkT_off[0], sc.gy_op, B, S, S, gx, true);
-      if (dmd_conv2d_fprop(&cd, st)) return 1;
+      if (dgrad(lv.skip, sc.gy_op, S, gx, true)) return 1;
     }
     g_cur = gx;
   }

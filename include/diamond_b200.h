@@ -415,7 +415,7 @@ typedef struct dmd_actor_critic_config {
   int img_channels;
   int img_size;
   int num_levels;
-  int channels[DMD_MAX_LEVELS]; /* 32 or 64 per level */
+  int channels[DMD_MAX_LEVELS]; /* 32, 64 or 128 per level, in any mix */
   int down[DMD_MAX_LEVELS];
   int num_actions;
 } dmd_actor_critic_config;
