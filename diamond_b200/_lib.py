@@ -142,6 +142,7 @@ SIGNATURES = {
     "dmd_denoiser_grad_layout": (C.c_longlong, [_vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), _i]),
     "dmd_inner_model_forward_train": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dmd_denoiser_backward": (_i, [_vp, _i, _i, _i, _vp, _vp, C.c_longlong, _vp, _vp]),
+    "dmd_denoiser_backward_accumulate": (_i, [_vp, _i, _i, _i, _vp, _vp, C.c_longlong, _vp, _vp]),
     "dmd_inner_model_forward_u8": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, C.POINTER(U8Frames), _vp, _vp, _vp, _sz, _vp]),
     "dmd_inner_model_forward_train_u8": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, C.POINTER(U8Frames), _vp, _vp, _vp, _sz, _vp]),
     "dmd_sampler_sample": (_i, [_vp, C.POINTER(SamplerConfigC), _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _i, _vp]),
@@ -167,6 +168,7 @@ SIGNATURES = {
     "dmd_rew_end_grad_layout": (C.c_longlong, [_vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), _i]),
     "dmd_rew_end_forward_train": (_i, [_vp, _i, _i] + [_vp] * 9 + [_vp, _sz, _vp]),
     "dmd_rew_end_backward": (_i, [_vp, _i, _i] + [_vp] * 5 + [C.c_longlong, _vp, _vp, _vp, _vp]),
+    "dmd_rew_end_backward_accumulate": (_i, [_vp, _i, _i] + [_vp] * 5 + [C.c_longlong, _vp, _vp, _vp, _vp]),
     "dmd_rew_end_predict_u8": (_i, [_vp, _i, _i, C.POINTER(U8Frames), C.POINTER(U8Frames)] + [_vp] * 7 + [_vp, _sz, _vp]),
     "dmd_rew_end_forward_train_u8": (_i, [_vp, _i, _i, C.POINTER(U8Frames), C.POINTER(U8Frames)] + [_vp] * 7 + [_vp, _sz, _vp]),
     "dmd_lambda_returns": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, C.c_double, C.c_double, _vp]),

@@ -1759,6 +1759,7 @@ struct BwdBuilder {
   // C (+)= alpha * op(A) op(B); c_goff >= 0: C is that slice of the gradient buffer
   void sgemm(const float* A, long long sam, long long sak, const float* Bm, long long sbk, long long sbn, float* C, long long c_goff,
              long long ldc, int M, int N, int K, int use_inv, int acc) {
+    if (c_goff >= 0 && !acc) { err = fail("backward plan: a product into the gradient buffer must add to it"); return; }
     BOp b; b.kind = B_SGEMM; b.ga = A; b.sam = sam; b.sak = sak; b.gb = Bm; b.sbk = sbk; b.sbn = sbn; b.gc = C; b.c_goff = c_goff; b.ldc = ldc;
     b.M = M; b.N = N; b.K = K; b.use_inv = use_inv; b.acc = acc; push(b);
   }
@@ -2098,14 +2099,18 @@ int ensure_train_plan(ModelCore& core, const char* who, int B, int H, int W, int
   return 0;
 }
 
-// start of every backward: the flat gradient buffer and the accumulators of the plan (dfilm, affine-norm sums, amax) cleared
-int clear_backward(const ModelCore& core, Plan& pl, float* grads, cudaStream_t st) {
-  DMD_CUDA(cudaMemsetAsync(grads, 0, (size_t)core.grad_total * 4, st));
+// start of every backward: the accumulators of the plan (dfilm, affine-norm sums, amax) cleared, and the caller's flat gradient
+// buffer too unless the call adds to it (the *_backward_accumulate entry points)
+int clear_backward(const ModelCore& core, Plan& pl, float* grads, int accumulate, cudaStream_t st) {
+  if (!accumulate) DMD_CUDA(cudaMemsetAsync(grads, 0, (size_t)core.grad_total * 4, st));
   DMD_CUDA(cudaMemsetAsync(pl.zero_begin, 0, pl.zero_bytes, st));
   return 0;
 }
 
-// the backward op list; the caller has cleared (clear_backward), set the loss scale and seeded the gradient the list starts from
+// the backward op list; the caller has cleared (clear_backward), set the loss scale and seeded the gradient the list starts from.
+// Every op that writes into `grads` ADDS to it (wgrad reduce with accumulate = 1, colsum / attention / embedding atomics, affine
+// and FiLM +=, sgemm into a c_goff slice with acc = 1, checked when the list is built), so an accumulating call is this same list
+// on a buffer that was not cleared
 int run_backward(const ModelCore& core, Plan& pl, float* grads, cudaStream_t st) {
   const int B = pl.B;
   const float* inv = pl.scale + 1;
@@ -2199,22 +2204,30 @@ extern "C" int dmd_inner_model_forward_train_u8(dmd_denoiser* h, int B, int H, i
   return run_wrap(h, *pl, noisy_rescaled, out, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 1.f, 0.f, st);
 }
 
-extern "C" int dmd_denoiser_backward(dmd_denoiser* h, int B, int H, int W, const float* grad_out, float* grads, long long grads_numel,
-                                     void* workspace, void* stream) {
-  DMD_CHECK(h && grad_out && grads && workspace, "denoiser_backward: null argument");
+static int denoiser_backward_impl(const char* who, dmd_denoiser* h, int B, int H, int W, const float* grad_out, float* grads,
+                                  long long grads_numel, int accumulate, void* workspace, void* stream) {
+  DMD_CHECK(h && grad_out && grads && workspace, "%s: null argument", who);
   Plan* plp = find_train_plan(h->core, B, H, W, 1, workspace);
-  DMD_CHECK(plp && plp->train, "denoiser_backward: no matching dmd_inner_model_forward_train on this workspace (B=%d H=%d W=%d)", B, H, W);
+  DMD_CHECK(plp && plp->train, "%s: no matching dmd_inner_model_forward_train on this workspace (B=%d H=%d W=%d)", who, B, H, W);
   Plan& pl = *plp;
-  DMD_CHECK(grads_numel >= h->core.grad_total, "denoiser_backward: gradient buffer too small (%lld < %lld floats)", grads_numel, h->core.grad_total);
-  DMD_CHECK(((uintptr_t)grads & 15) == 0, "denoiser_backward: gradient buffer must be 16-byte aligned");
+  DMD_CHECK(grads_numel >= h->core.grad_total, "%s: gradient buffer too small (%lld < %lld floats)", who, grads_numel, h->core.grad_total);
+  DMD_CHECK(((uintptr_t)grads & 15) == 0, "%s: gradient buffer must be 16-byte aligned", who);
   cudaStream_t st = (cudaStream_t)stream;
   const int HW = H * W, C = h->cfg.img_channels;
-  if (clear_backward(h->core, pl, grads, st)) return 1;
+  if (clear_backward(h->core, pl, grads, accumulate, st)) return 1;
   // loss scale from the incoming gradient, then the scaled NHWC gradient of the model output
   if (loss_scale_launch(grad_out, (long long)B * C * HW, pl.amax, pl.scale, st)) return 1;
   nchw_to_nhwc_scaled_kernel<<<dim3((HW + 255) / 256, B), 256, 0, st>>>(grad_out, pl.gF, pl.scale, C, pl.gF_ch, HW);
   DMD_LAUNCH_OK();
   return run_backward(h->core, pl, grads, st);
+}
+extern "C" int dmd_denoiser_backward(dmd_denoiser* h, int B, int H, int W, const float* grad_out, float* grads, long long grads_numel,
+                                     void* workspace, void* stream) {
+  return denoiser_backward_impl("denoiser_backward", h, B, H, W, grad_out, grads, grads_numel, 0, workspace, stream);
+}
+extern "C" int dmd_denoiser_backward_accumulate(dmd_denoiser* h, int B, int H, int W, const float* grad_out, float* grads,
+                                                long long grads_numel, void* workspace, void* stream) {
+  return denoiser_backward_impl("denoiser_backward_accumulate", h, B, H, W, grad_out, grads, grads_numel, 1, workspace, stream);
 }
 
 // ---------------------------------------------------------------------------------------------- sampler
@@ -3057,16 +3070,17 @@ extern "C" int dmd_rew_end_forward_train_u8(dmd_rew_end* h, int b, int t, const 
                                workspace_bytes, stream);
 }
 
-extern "C" int dmd_rew_end_backward(dmd_rew_end* h, int b, int t, const float* g_logits_rew, const float* g_logits_end,
-                                    const float* g_hx_out, const float* g_cx_out, float* grads, long long grads_numel,
-                                    float* g_hx_in, float* g_cx_in, void* workspace, void* stream) {
-  DMD_CHECK(h && g_logits_rew && g_logits_end && grads && workspace, "rew_end backward: null argument");
+namespace {
+int rew_end_backward_impl(const char* who, dmd_rew_end* h, int b, int t, const float* g_logits_rew, const float* g_logits_end,
+                          const float* g_hx_out, const float* g_cx_out, float* grads, long long grads_numel, int accumulate,
+                          float* g_hx_in, float* g_cx_in, void* workspace, void* stream) {
+  DMD_CHECK(h && g_logits_rew && g_logits_end && grads && workspace, "%s: null argument", who);
   const dmd_rew_end_config& c = h->cfg;
   Plan* plp = (b > 0 && t > 0) ? find_train_plan(h->core, b * t, c.img_size, c.img_size, t, workspace) : nullptr;
-  DMD_CHECK(plp && plp->train, "rew_end backward: no matching dmd_rew_end_forward_train on this workspace (b=%d t=%d)", b, t);
+  DMD_CHECK(plp && plp->train, "%s: no matching dmd_rew_end_forward_train on this workspace (b=%d t=%d)", who, b, t);
   const ModelCore& m = h->core;
-  DMD_CHECK(grads_numel >= m.grad_total, "rew_end backward: gradient buffer too small (%lld < %lld floats)", grads_numel, m.grad_total);
-  DMD_CHECK(((uintptr_t)grads & 15) == 0, "rew_end backward: gradient buffer must be 16-byte aligned");
+  DMD_CHECK(grads_numel >= m.grad_total, "%s: gradient buffer too small (%lld < %lld floats)", who, grads_numel, m.grad_total);
+  DMD_CHECK(((uintptr_t)grads & 15) == 0, "%s: gradient buffer must be 16-byte aligned", who);
   Plan& pl = *plp;
   cudaStream_t st = (cudaStream_t)stream;
   const int rows = b * t, D = c.lstm_dim, K = h->feat_c * h->feat_hw;
@@ -3075,7 +3089,8 @@ extern "C" int dmd_rew_end_backward(dmd_rew_end* h, int b, int t, const float* g
                    int M, int N, int Kd, int acc) -> int {
     return sgemm_launch(Am, sam, sak, Bm, sbk, sbn, C, ldc, M, N, Kd, nullptr, acc, 0, nullptr, st);
   };
-  if (clear_backward(m, pl, grads, st)) return 1;
+  // every write into `grads` below adds to it (sgemm with acc = 1, colsum), as run_backward's do
+  if (clear_backward(m, pl, grads, accumulate, st)) return 1;
   // ---- head (rew_end_model.py:54): logits = W2 silu(W0 y + b0); these gradients are fp32 and unscaled
   const float* y = pl.hseq + (size_t)b * D;
   merge_logits_kernel<<<(rows + 127) / 128, 128, 0, st>>>(g_logits_rew, g_logits_end, pl.g_tm, b, t);
@@ -3116,6 +3131,20 @@ extern "C" int dmd_rew_end_backward(dmd_rew_end* h, int b, int t, const float* g
   nchw_to_nhwc_scaled_kernel<<<dim3((h->feat_hw + 255) / 256, rows), 256, 0, st>>>(g_x, pl.feat.grad, pl.scale, h->feat_c, h->feat_c, h->feat_hw);
   DMD_LAUNCH_OK();
   return run_backward(m, pl, grads, st);
+}
+}  // namespace
+
+extern "C" int dmd_rew_end_backward(dmd_rew_end* h, int b, int t, const float* g_logits_rew, const float* g_logits_end,
+                                    const float* g_hx_out, const float* g_cx_out, float* grads, long long grads_numel,
+                                    float* g_hx_in, float* g_cx_in, void* workspace, void* stream) {
+  return rew_end_backward_impl("rew_end backward", h, b, t, g_logits_rew, g_logits_end, g_hx_out, g_cx_out, grads, grads_numel, 0,
+                               g_hx_in, g_cx_in, workspace, stream);
+}
+extern "C" int dmd_rew_end_backward_accumulate(dmd_rew_end* h, int b, int t, const float* g_logits_rew, const float* g_logits_end,
+                                               const float* g_hx_out, const float* g_cx_out, float* grads, long long grads_numel,
+                                               float* g_hx_in, float* g_cx_in, void* workspace, void* stream) {
+  return rew_end_backward_impl("rew_end backward_accumulate", h, b, t, g_logits_rew, g_logits_end, g_hx_out, g_cx_out, grads,
+                               grads_numel, 1, g_hx_in, g_cx_in, workspace, stream);
 }
 
 // ---------------------------------------------------------------------------------------------- optimizer (optim_kernels.cuh)

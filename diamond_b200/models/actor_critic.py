@@ -91,23 +91,6 @@ class ActorCritic(NativeStateMixin, nn.Module):
         cc.num_actions = int(c.num_actions)
         return cc
 
-    def _adopt_accumulated_grads(self) -> None:
-        """End of a backward pass (autograd engine callback): the flat buffer the BPTT nodes accumulated into becomes `.grad`
-        (added to an existing `.grad`, like AccumulateGrad) and is remembered as `last_flat_grad` for a one-collective all-reduce."""
-        flat = self.__dict__.pop("_grad_acc", None)
-        if flat is None:
-            return
-        offs, nums, _ = self._grad_views_layout()
-        for p, o, n in zip(self.parameters(), offs, nums):
-            if not p.requires_grad:
-                continue
-            g = flat[o:o + n].view_as(p)
-            if p.grad is None:
-                p.grad = g
-            else:
-                p.grad.add_(g)
-        self.last_flat_grad = flat
-
     def _native_forward(self, obs: Tensor, hx: Tensor, cx: Tensor, ws: Tensor):
         lib = _lib.lib()
         h = self._native()

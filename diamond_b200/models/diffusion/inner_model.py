@@ -114,7 +114,8 @@ class InnerModel(NativeStateMixin, nn.Module):
 
 class _InnerModelFn(torch.autograd.Function):
     """InnerModel.forward under autograd: forward = dmd_inner_model_forward_train (activations stay in the training
-    workspace), backward = dmd_denoiser_backward (all parameter gradients in one flat buffer, returned as views)."""
+    workspace), backward = dmd_denoiser_backward[_accumulate] (all parameter gradients in one flat buffer; see
+    NativeStateMixin._native_param_grads for how it reaches `.grad`)."""
 
     @staticmethod
     def forward(ctx, module, noisy, c_noise, obs, act, *params):
@@ -147,11 +148,11 @@ class _InnerModelFn(torch.autograd.Function):
         module = ctx.module
         h = module.native()
         b, hh, ww = ctx.shape
-        offs, nums, total = module._grad_views_layout()
-        flat = torch.empty(total, dtype=torch.float32, device=grad_out.device)
         g = grad_out.float().contiguous()
-        _lib.check(lib.dmd_denoiser_backward(h, b, hh, ww, g.data_ptr(), flat.data_ptr(), total, ctx.ws.data_ptr(), _lib.current_stream()))
-        grads = [flat[o:o + n].view_as(p) for o, n, p in zip(offs, nums, module.parameters())]
+
+        def run(flat, accumulate):
+            fn = lib.dmd_denoiser_backward_accumulate if accumulate else lib.dmd_denoiser_backward
+            _lib.check(fn(h, b, hh, ww, g.data_ptr(), flat.data_ptr(), flat.numel(), ctx.ws.data_ptr(), _lib.current_stream()))
+        grads = module._native_param_grads(ctx, run)
         module._release_ws(ctx.ws, module._WS_POOL_CAP)
-        module.last_flat_grad = flat   # one contiguous buffer: what a data-parallel step all-reduces in a single collective
         return (None, None, None, None, None, *grads)

@@ -196,8 +196,8 @@ def confusion_matrix(logits: Tensor, target: Tensor, num_classes: int) -> Tensor
 
 class _RewEndFn(torch.autograd.Function):
     """RewEndModel.predict_rew_end under autograd: forward = dmd_rew_end_forward_train (activations stay in the training
-    workspace), backward = dmd_rew_end_backward (all parameter gradients in one flat buffer, returned as views; the
-    gradients wrt a carried (hx, cx) when the caller's state requires them)."""
+    workspace), backward = dmd_rew_end_backward[_accumulate] (all parameter gradients in one flat buffer, see
+    NativeStateMixin._native_param_grads; the gradients wrt a carried (hx, cx) when the caller's state requires them)."""
 
     @staticmethod
     def forward(ctx, module, obs, act, next_obs, hx, cx, src, *params):
@@ -235,16 +235,16 @@ class _RewEndFn(torch.autograd.Function):
         module = ctx.module
         h = module._native()
         b, t = ctx.shape
-        offs, nums, total = module._grad_views_layout()
-        flat = torch.empty(total, dtype=torch.float32, device=g_rew.device)
         g_rew, g_end = g_rew.float().contiguous(), g_end.float().contiguous()
         g_hx = None if g_hx is None else g_hx.float().contiguous()
         g_cx = None if g_cx is None else g_cx.float().contiguous()
         g_hx_in = g_rew.new_empty(b, module.cfg.lstm_dim) if ctx.needs_input_grad[4] else None
         g_cx_in = g_rew.new_empty(b, module.cfg.lstm_dim) if ctx.needs_input_grad[5] else None
-        _lib.check(lib.dmd_rew_end_backward(h, b, t, g_rew.data_ptr(), g_end.data_ptr(), _lib.ptr(g_hx), _lib.ptr(g_cx), flat.data_ptr(),
-                                            total, _lib.ptr(g_hx_in), _lib.ptr(g_cx_in), ctx.ws.data_ptr(), _lib.current_stream()))
-        grads = [flat[o:o + n].view_as(p) for o, n, p in zip(offs, nums, module.parameters())]
+
+        def run(flat, accumulate):
+            fn = lib.dmd_rew_end_backward_accumulate if accumulate else lib.dmd_rew_end_backward
+            _lib.check(fn(h, b, t, g_rew.data_ptr(), g_end.data_ptr(), _lib.ptr(g_hx), _lib.ptr(g_cx), flat.data_ptr(), flat.numel(),
+                          _lib.ptr(g_hx_in), _lib.ptr(g_cx_in), ctx.ws.data_ptr(), _lib.current_stream()))
+        grads = module._native_param_grads(ctx, run)
         module._release_ws(ctx.ws, module._WS_POOL_CAP)
-        module.last_flat_grad = flat   # one contiguous buffer: what a data-parallel step all-reduces in a single collective
         return (None, None, None, None, g_hx_in, g_cx_in, None, *grads)

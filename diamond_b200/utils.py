@@ -125,6 +125,77 @@ class NativeStateMixin:
             self.__dict__["_state_tensor_cache"] = ts
         return ts
 
+    # ------------------------------------------------------------------ gradients of native backward nodes
+    # A native backward writes every parameter gradient into one flat fp32 buffer (layout: grad_layout()).  When a backward pass
+    # stores gradients into `.grad`, its nodes ADD into one buffer natively and `.grad` becomes views of it when the pass ends,
+    # so that a data-parallel step all-reduces the whole model in one collective (allreduce_native_gradients).  `_grad_acc` is
+    # the buffer of the running pass, `last_flat_grad` the one of the last pass.
+
+    def _adopt_accumulated_grads(self) -> None:
+        """End of a backward pass (autograd engine callback): the flat buffer the nodes accumulated into becomes `.grad` (added to
+        an existing `.grad`, like AccumulateGrad) and is remembered as `last_flat_grad` for a one-collective all-reduce."""
+        flat = self.__dict__.pop("_grad_acc", None)
+        if flat is None:
+            return
+        offs, nums, _ = self._grad_views_layout()
+        for p, o, n in zip(self.parameters(), offs, nums):
+            if not p.requires_grad:
+                continue
+            g = flat[o:o + n].view_as(p)
+            if p.grad is None:
+                p.grad = g
+            else:
+                p.grad.add_(g)
+        self.last_flat_grad = flat
+
+    def _engine_stores_grads(self, node) -> bool:
+        """True when the running backward pass stores the gradient of every trainable parameter into `.grad`
+        (`loss.backward()`), False when it hands gradients back to its caller (`torch.autograd.grad(loss, params)`) or skips
+        some parameters (`backward(inputs=...)`).  `node` is the native call's autograd node (its `ctx`); its last edges lead to
+        the parameters' AccumulateGrad nodes.  Asked once per pass (graph task); a new pass also drops the buffer of a pass that
+        died before its end."""
+        task = torch._C._current_graph_task_id()
+        cached = self.__dict__.get("_grad_task")
+        if cached is not None and cached[0] == task:
+            return cached[1]
+        self.__dict__.pop("_grad_acc", None)
+        n = len(self._grad_views_layout()[0])
+        accs = [f for f, _ in node.next_functions[-n:] if f is not None]
+        try:
+            stores = all(torch._C._will_engine_execute_node(f) for f in accs)
+        except RuntimeError:
+            # torch refuses the query for a leaf that torch.autograd.grad captures: that pass returns the gradients instead
+            stores = False
+        self.__dict__["_grad_task"] = (task, stores)
+        return stores
+
+    def _native_param_grads(self, node, run):
+        """The parameter gradients a native backward node returns to autograd.  `run(flat, accumulate)` makes the native call
+        that writes (accumulate False) or adds (True) every parameter gradient into the flat buffer `flat`.
+
+        Under `loss.backward()` the first node of the pass writes a new buffer and every later node of the pass (the autoregressive
+        steps of Denoiser.forward) adds to it; a callback at the end of the pass makes it `.grad`, so no per-tensor
+        AccumulateGrad runs inside a pass.  Otherwise (torch.autograd.grad, backward(inputs=...)) each node returns views of its
+        own buffer, as autograd expects."""
+        offs, nums, total = self._grad_views_layout()
+        dev = self.device
+        if not self._engine_stores_grads(node):
+            flat = torch.empty(total, dtype=torch.float32, device=dev)
+            run(flat, False)
+            self.last_flat_grad = flat
+            return [flat[o:o + n].view_as(p) for o, n, p in zip(offs, nums, self.parameters())]
+        flat = self.__dict__.get("_grad_acc")
+        if flat is not None:
+            run(flat, True)
+        else:
+            # first node of the pass.  The previous pass's buffer is released first: when the `.grad`s were set to None it is
+            # free, and the allocator can hand its memory back
+            self.__dict__.pop("last_flat_grad", None)
+            flat = self.__dict__["_grad_acc"] = torch.empty(total, dtype=torch.float32, device=dev)
+            run(flat, False)
+            torch.autograd.Variable._execution_engine.queue_callback(self._adopt_accumulated_grads)
+        return [None] * len(offs)
+
     def refresh_weights(self) -> None:
         self.__dict__["_state_tensor_cache"] = None
         self.__dict__["_wkey"] = None
@@ -137,7 +208,7 @@ class NativeStateMixin:
     # to ONE module object.  copy.deepcopy (EMA copies) and pickle (multiprocessing) go through __getstate__: the copy starts
     # without native state and builds its own on first use, so two objects never own -- and free -- the same handle.
     _NATIVE_RESET = ("_h", "_h_key", "_wkey", "_packed", "_ws")
-    _NATIVE_DROP = ("_state_tensor_cache", "_ws_pool", "_bwd_scratch", "_grad_acc", "_gv_layout", "last_flat_grad")
+    _NATIVE_DROP = ("_state_tensor_cache", "_ws_pool", "_bwd_scratch", "_grad_acc", "_grad_task", "_gv_layout", "last_flat_grad")
 
     def __getstate__(self):
         state = self.__dict__.copy()

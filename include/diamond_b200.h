@@ -24,7 +24,8 @@
  *   Kept -- must not be touched by the caller while the library relies on it:
  *     - a training workspace from dmd_inner_model_forward_train[_u8] / dmd_rew_end_forward_train[_u8] to its backward, and an
  *       actor-critic workspace from dmd_actor_critic_forward to its backward (it holds the activations);
- *     - the flat gradient buffer of dmd_actor_critic_backward_accumulate (it is added to);
+ *     - the flat gradient buffer of dmd_denoiser_backward_accumulate / dmd_rew_end_backward_accumulate /
+ *       dmd_actor_critic_backward_accumulate (it is added to);
  *     - the packed-weight buffers (conv packs, FiLM table and the FiLM gradient offsets, written by *_set_weights), the
  *       optimizer state (param, exp_avg, exp_avg_sq), and the frame / action rings a sampler reads (ring_head >= 0);
  *     - every input, including trajectory slot 0 and the churn noise `eps`.
@@ -371,6 +372,13 @@ int dmd_inner_model_forward_train(dmd_denoiser* h, int B, int H, int W, const fl
                                   void* workspace, size_t workspace_bytes, void* stream);
 int dmd_denoiser_backward(dmd_denoiser* h, int B, int H, int W, const float* grad_out, float* grads, long long grads_numel,
                           void* workspace, void* stream);
+/* Same, but ADDS every parameter gradient to what `grads` already holds (slots without a gradient, such as noise_emb.weight,
+ * are left as they are): the nodes of one backward pass (Denoiser.forward's autoregressive steps, denoiser.py:93-122)
+ * accumulate into ONE flat buffer, which a data-parallel step then all-reduces in one collective.  Launches what
+ * dmd_denoiser_backward launches, without its clear of `grads`; the sum differs from the plain call's result plus the prior
+ * contents only in fp32 addition order. */
+int dmd_denoiser_backward_accumulate(dmd_denoiser* h, int B, int H, int W, const float* grad_out, float* grads,
+                                     long long grads_numel, void* workspace, void* stream);
 
 /* dmd_inner_model_forward / dmd_inner_model_forward_train with the frame stack read from uint8 frames: obs holds the
  * num_steps_conditioning frames of each sample, f = 0 oldest, and its table the rescaled values obs / sigma_data (what
@@ -500,6 +508,11 @@ int dmd_rew_end_forward_train(dmd_rew_end* h, int b, int t, const float* obs, co
 int dmd_rew_end_backward(dmd_rew_end* h, int b, int t, const float* g_logits_rew, const float* g_logits_end,
                          const float* g_hx_out, const float* g_cx_out, float* grads, long long grads_numel,
                          float* g_hx_in, float* g_cx_in, void* workspace, void* stream);
+/* Same, but ADDS every parameter gradient to what `grads` already holds, as dmd_denoiser_backward_accumulate does (several
+ * predict_rew_end calls in one backward pass); g_hx_in / g_cx_in are written as by dmd_rew_end_backward. */
+int dmd_rew_end_backward_accumulate(dmd_rew_end* h, int b, int t, const float* g_logits_rew, const float* g_logits_end,
+                                    const float* g_hx_out, const float* g_cx_out, float* grads, long long grads_numel,
+                                    float* g_hx_in, float* g_cx_in, void* workspace, void* stream);
 /* dmd_rew_end_predict / dmd_rew_end_forward_train with obs / next_obs read from uint8 frames (frame (n, k) = step k of
  * segment n); both sources share one decode table (values as the fp32 entry points read them).  dmd_rew_end_backward is the
  * same after either forward.  Every argument is checked before any launch. */
