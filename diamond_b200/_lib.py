@@ -139,6 +139,7 @@ SIGNATURES = {
     "dmd_denoiser_forward": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dmd_inner_model_forward": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dmd_denoiser_train_workspace_bytes": (_sz, [_vp, _i, _i, _i]),
+    "dmd_denoiser_train_dcond_plan": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
     "dmd_denoiser_grad_layout": (C.c_longlong, [_vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), _i]),
     "dmd_inner_model_forward_train": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dmd_denoiser_backward": (_i, [_vp, _i, _i, _i, _vp, _vp, C.c_longlong, _vp, _vp]),

@@ -111,6 +111,10 @@ static inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 // SM count of the H100 SXM the launch shapes of the memory-bound kernels are planned for (grids of >= 2 blocks per SM).  A plan
 // does not depend on the device it is built on, so host-only planning (dmd_prep_plan) gives the same answer as a launch.
 constexpr int kPlanSms = 132;
+// widest conditioning vector (cond_channels) the denoiser and reward / termination model accept: film_wgrad_kernel covers it in
+// 256-column slices, and the split-K partials of dcond = dfilm Wf get their own buffer when the backward temporaries hold too few
+// (make_train_plan)
+constexpr int kMaxCondChannels = 2048;
 static inline int gn_group_size(int C) {  // blocks.py:12,27: num_groups = max(1, C // 32)
   int G = C / 32 > 1 ? C / 32 : 1;
   return C / G;
@@ -645,6 +649,12 @@ static void splitk_plan(int K, int chunks, int* kchunk, int* splits) {
   *kchunk = ((K + chunks - 1) / chunks + 15) / 16 * 16;
   *splits = (K + *kchunk - 1) / *kchunk;
 }
+// split count of dcond = dfilm Wf over `rows` FiLM rows: K chunks of at least 256 rows, at most 32 (28 for the default net)
+static int film_splits(int rows) { return rows / 256 < 32 ? rows / 256 : 32; }
+// dcond's split count may be capped by the partials the backward temporary tA holds, down to this many; below it the partials
+// get their own buffer.  Every net that trains at cond_channels <= 256 holds at least 8 (its bottom level is an 8 x 8 attention
+// level of >= 32 channels: tA >= B x 64 x 32 >= 8 x B x cond_channels floats), so those plans are capped as before.
+constexpr int kMinFilmSplits = 8;
 static long long splitk_partial_floats(int M, int N, int K, int chunks) {
   if (chunks <= 1) return 0;
   int kchunk, splits;
@@ -685,7 +695,8 @@ static int attn_bwd_launch(const AttnBwdParams& ab, int B, cudaStream_t st) {
 
 static int film_wgrad_launch(const float* dfilm, const float* cond, float* grads, const long long* woff, const long long* boff,
                              int B, int rows, int CC, const float* inv, cudaStream_t st) {
-  film_wgrad_kernel<<<(rows + 7) / 8, 256, 0, st>>>(dfilm, cond, grads, woff, boff, B, rows, CC, inv);
+  if (CC <= 256) film_wgrad_kernel<false><<<(rows + 7) / 8, 256, 0, st>>>(dfilm, cond, grads, woff, boff, B, rows, CC, inv);
+  else film_wgrad_kernel<true><<<dim3((rows + 7) / 8, (CC + 255) / 256), 256, 0, st>>>(dfilm, cond, grads, woff, boff, B, rows, CC, inv);
   DMD_LAUNCH_OK();
   return 0;
 }
@@ -782,7 +793,8 @@ extern "C" int dmd_sgemm(const float* A, long long sam, long long sak, const flo
 }
 extern "C" int dmd_film_wgrad(const float* dfilm, const float* cond, float* grads, const long long* woff, const long long* boff, int B, int rows,
                               int CC, const float* inv_scale, void* stream) {
-  DMD_CHECK(dfilm && cond && grads && woff && boff && B > 0 && rows > 0 && CC > 0 && CC <= 256, "film_wgrad: bad arguments (CC <= 256)");
+  DMD_CHECK(dfilm && cond && grads && woff && boff && B > 0 && rows > 0 && CC > 0 && CC <= kMaxCondChannels,
+            "film_wgrad: bad arguments (CC <= %d)", kMaxCondChannels);
   return film_wgrad_launch(dfilm, cond, grads, woff, boff, B, rows, CC, inv_scale, (cudaStream_t)stream);
 }
 extern "C" int dmd_embedding_bwd(const float* de, const int64_t* act, float* dE, int B, int CC, int T, int num_actions, const float* inv_scale,
@@ -901,6 +913,7 @@ struct BOp {
   long long goff = -1, goff2 = -1;            // flat-gradient offsets (floats)
   NormBwdParams nb;
   int chunks = 0;                             // sgemm: split-K chunk count (<= 1: no split)
+  float* part = nullptr;                      // sgemm: split-K partial buffer (nullptr: tA)
   const float* src = nullptr; float* dst = nullptr; long long rows = 0; int C = 0, Creal = 0, H = 0, W = 0, acc = 0;
   AttnBwdParams ab; long long goffs[6] = {-1, -1, -1, -1, -1, -1};
   // split attention backward (C = 128): ap recomputes q | k | v into ap.scratch; the buffers of attn_core_bwd_kernel
@@ -947,6 +960,9 @@ struct Plan {
   int gF_ch = 0;                                          // round_up(img_channels, 8): the padded channels are zero
   float *dfilm = nullptr, *nsum = nullptr, *partial = nullptr, *scale = nullptr;
   float *dcond = nullptr, *dh = nullptr, *cpre = nullptr, *dpre = nullptr, *de = nullptr;
+  float* film_part = nullptr;                             // split-K partials of dcond = dfilm Wf: tA, or its own buffer
+  int film_splits = 0;                                    // dcond's split count (<= 1: no split)
+  long long film_part_own = 0;                            // floats of film_part's own buffer (0: the partials live in tA)
   unsigned int* amax = nullptr;
   const long long *film_woff = nullptr, *film_boff = nullptr;   // the model's FiLM gradient offsets (in its packed buffer)
   uint8_t* zero_begin = nullptr; size_t zero_bytes = 0;   // region cleared at the start of every backward (dfilm, sums, amax)
@@ -1769,11 +1785,9 @@ struct BwdBuilder {
     { BOp b; b.kind = B_FILMW; push(b); }
     const float* Wf = core->packed ? (const float*)(core->packed + core->film_w_off) : nullptr;
     sgemm(pl->dfilm, R, 1, Wf, CC, 1, pl->dcond, -1, CC, B, CC, R, 0, 0);                       // dcond = dfilm Wf
-    {   // K = R (7168 rows for the default net) over a handful of 64 x 64 output tiles: split K across the SMs
-      const long long fit = pl->tmp_floats / ((long long)B * CC);   // partials live in tA
-      int splits = R / 256; if (splits > 32) splits = 32; if (splits > fit) splits = (int)fit;
-      if (splits > 1) pl->bops.back().chunks = splits;
-    }
+    // K = R (7168 rows for the default net) over a handful of 64 x 64 output tiles: split K across the SMs, partials in
+    // pl->film_part (make_train_plan chose the split count and the buffer)
+    if (pl->film_splits > 1) { pl->bops.back().chunks = pl->film_splits; pl->bops.back().part = pl->film_part; }
   }
   // nn.Embedding gradient of table `idx` from de [B][CC] (T embeddings of CC / T channels per row, actions pl->t_act [B][T])
   void embedding(const float* de, int idx, int T, int num_actions) {
@@ -1845,6 +1859,20 @@ int make_train_plan(const ModelCore& core, int cmax, int gF_ch, Plan* pl, int B,
   const int CC = core.cond_channels;
   pl->dcond = (float*)bb.take((size_t)B * CC * 4); pl->dh = (float*)bb.take((size_t)B * CC * 4); pl->cpre = (float*)bb.take((size_t)B * CC * 4);
   pl->dpre = (float*)bb.take((size_t)B * CC * 4); pl->de = (float*)bb.take((size_t)B * CC * 4);
+  {   // dcond = dfilm Wf: its partials live in tA, which caps the split count at what it holds, down to kMinFilmSplits; a
+      // wider cond whose partials tA cannot hold that many of keeps the full split count in a buffer of its own
+    const int want = film_splits(core.film_rows);
+    const long long fit = pl->tmp_floats / ((long long)B * CC);
+    pl->film_part_own = 0;
+    if (want <= fit || fit >= kMinFilmSplits) {
+      pl->film_splits = want <= fit ? want : (int)fit;
+      pl->film_part = pl->tA;
+    } else {
+      pl->film_splits = want;
+      pl->film_part_own = splitk_partial_floats(B, CC, core.film_rows, want);
+      pl->film_part = (float*)bb.take((size_t)pl->film_part_own * 4);
+    }
+  }
   pl->scale = (float*)bb.take(256);
   // zeroed at the start of every backward: dfilm, affine-norm sums, amax
   uint8_t* z0 = (uint8_t*)bb.take(0);
@@ -1946,7 +1974,12 @@ int ensure_plan(dmd_denoiser* h, int B, int H, int W, void* ws, size_t ws_bytes)
 
 extern "C" dmd_denoiser* dmd_denoiser_create(const dmd_denoiser_config* cfg) {
   if (!cfg || cfg->num_levels < 1 || cfg->num_levels > DMD_MAX_LEVELS) { fail("denoiser_create: bad config"); return nullptr; }
-  if (cfg->cond_channels % 32 || cfg->cond_channels > 256 || cfg->cond_channels % cfg->num_steps_conditioning) { fail("denoiser_create: cond_channels must be a multiple of 32 (<= 256) and of num_steps_conditioning"); return nullptr; }
+  if (cfg->num_steps_conditioning <= 0 || cfg->cond_channels <= 0 || cfg->cond_channels % 32 || cfg->cond_channels > kMaxCondChannels ||
+      cfg->cond_channels % cfg->num_steps_conditioning) {
+    fail("denoiser_create: cond_channels must be a multiple of 32 and of num_steps_conditioning (%d), at most %d; got %d",
+         cfg->num_steps_conditioning, kMaxCondChannels, cfg->cond_channels);
+    return nullptr;
+  }
   for (int i = 0; i < cfg->num_levels; ++i)
     if (!level_width_ok(cfg->channels[i])) { fail("denoiser_create: channels must be 32, 64 or 128 per level, at most 128 (got %d at level %d)", cfg->channels[i], i); return nullptr; }
   {   // conv_in's operand: 16, 32 or 64 channels after padding (the operand prep and the wgrad kernel; at 128 the forward
@@ -2148,9 +2181,10 @@ int run_backward(const ModelCore& core, Plan& pl, float* grads, cudaStream_t st)
         DMD_LAUNCH_OK();
         break;
       case B_MEMSET: DMD_CUDA(cudaMemsetAsync(b.ms_ptr, 0, b.ms_bytes, st)); break;
-      case B_SGEMM:   // the long-K product (dcond = dfilm Wf, K = all FiLM rows) is split; its partials live in tA
+      case B_SGEMM:   // the long-K products are split: dcond = dfilm Wf (K = all FiLM rows, partials in film_part) and the
+                      // attention weight gradients (K = every token of the batch, partials in tA)
         if (sgemm_launch(b.ga, b.sam, b.sak, b.gb, b.sbk, b.sbn, b.c_goff >= 0 ? grads + b.c_goff : b.gc, b.ldc, b.M, b.N, b.K,
-                         b.use_inv ? inv : nullptr, b.acc, b.chunks, pl.tA, st)) return 1;
+                         b.use_inv ? inv : nullptr, b.acc, b.chunks, b.part ? b.part : pl.tA, st)) return 1;
         break;
       case B_FILMW:
         if (film_wgrad_launch(pl.dfilm, pl.cond, grads, pl.film_woff, pl.film_boff, B, core.film_rows, core.cond_channels, inv, st)) return 1;
@@ -2172,6 +2206,14 @@ extern "C" size_t dmd_denoiser_train_workspace_bytes(const dmd_denoiser* h, int 
   Plan tmp; size_t need = 0;
   if (make_denoiser_train_plan(h, &tmp, B, H, W, nullptr, &need)) return 0;
   return need;
+}
+extern "C" int dmd_denoiser_train_dcond_plan(const dmd_denoiser* h, int B, int H, int W, int* splits, long long* own_partial_floats,
+                                             long long* temporary_floats) {
+  DMD_CHECK(splits && own_partial_floats && temporary_floats, "denoiser_train_dcond_plan: null output");
+  Plan tmp; size_t need = 0;
+  if (make_denoiser_train_plan(h, &tmp, B, H, W, nullptr, &need)) return 1;
+  *splits = tmp.film_splits; *own_partial_floats = tmp.film_part_own; *temporary_floats = tmp.tmp_floats;
+  return 0;
 }
 extern "C" long long dmd_denoiser_grad_layout(const dmd_denoiser* h, long long* offsets, long long* numels, int n) {
   return grad_layout(h ? &h->core : nullptr, offsets, numels, n);
@@ -2888,7 +2930,10 @@ int rew_end_head(const dmd_rew_end* h, int b, int t, const float* y, float* hid,
 
 extern "C" dmd_rew_end* dmd_rew_end_create(const dmd_rew_end_config* cfg) {
   if (!cfg || cfg->num_levels < 1 || cfg->num_levels >= DMD_MAX_LEVELS) { fail("rew_end_create: bad config"); return nullptr; }
-  if (cfg->cond_channels % 32 || cfg->cond_channels > 256) { fail("rew_end_create: cond_channels must be a multiple of 32, <= 256"); return nullptr; }
+  if (cfg->cond_channels <= 0 || cfg->cond_channels % 32 || cfg->cond_channels > kMaxCondChannels) {
+    fail("rew_end_create: cond_channels must be a multiple of 32, at most %d; got %d", kMaxCondChannels, cfg->cond_channels);
+    return nullptr;
+  }
   for (int i = 0; i < cfg->num_levels; ++i)
     if (!level_width_ok(cfg->channels[i])) { fail("rew_end_create: channels must be 32, 64 or 128 per level, at most 128 (got %d at level %d)", cfg->channels[i], i); return nullptr; }
   if (cfg->lstm_dim % 4) { fail("rew_end_create: lstm_dim must be a multiple of 4"); return nullptr; }

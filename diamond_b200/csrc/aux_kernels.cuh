@@ -160,7 +160,8 @@ __global__ void cond_embed_kernel(const float* __restrict__ cs, const float* __r
 
 // out[n][f] (+)= act( sum_k in[n][k] * W[f][k] + b[f] ),  K multiple of 4; K is processed in chunks of <= 256.
 // grid (ceil(F/(8J)), ceil(B/32)), 256 threads: warp w owns rows f = Jw..Jw+J-1 of the 8J-row tile, lane = sample n.
-// J = 1 gives small GEMMs (the conditioning MLP: F = 256) four times the blocks; the k order of each sum is the same.
+// J = 1 gives small GEMMs (the conditioning MLP: F = cond_channels, 32..2048) four times the blocks; the k order of each sum is
+// the same.  Any K and F are covered (K in chunks of kLinChunk, F in tiles of 8J rows); linear_launch picks J from the grid size.
 // hw_perm > 0: `in` is an NHWC tensor [B][hw_perm][K/hw_perm] read in NCHW-flatten order (k = c*hw + pix), i.e. the
 // x.flatten(start_dim=1) of actor_critic.py:71 without materialising the permutation.
 constexpr int kLinChunk = 256;

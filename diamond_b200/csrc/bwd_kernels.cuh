@@ -343,13 +343,16 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ partial, int spli
 // FiLM weight gradients through a row-pointer table: the 44 AdaGroupNorm.linear layers (blocks.py:39) were batched into one
 // [film_rows][CC] matrix for the forward; their gradients go back to 44 separate parameters.
 //   dW_row[f][k] += alpha * sum_n dfilm[n][f] * cond[n][k] ;  db_row[f] += alpha * sum_n dfilm[n][f]
-// grid (film_rows / 8), 256 threads = CC columns (CC <= 256); woff[f] / boff[f] are offsets into the flat gradient buffer.
+// grid (film_rows / 8, ceil(CC / 256)), 256 threads = the 256 cond columns of slice blockIdx.y (kSlices = false: CC <= 256, one
+// slice); the first 8 threads of slice 0 also sum the biases.  Each sum runs over n ascending whatever CC is.  woff[f] / boff[f]
+// are offsets into the flat gradient buffer.
+template <bool kSlices>
 __global__ void __launch_bounds__(256) film_wgrad_kernel(const float* __restrict__ dfilm, const float* __restrict__ cond,
                                                          float* __restrict__ grads, const long long* __restrict__ woff,
                                                          const long long* __restrict__ boff, int B, int rows, int CC,
                                                          const float* __restrict__ inv_scale) {
   __shared__ float sd[8][64];
-  const int f0 = blockIdx.x * 8, k = threadIdx.x;
+  const int f0 = blockIdx.x * 8, k = (kSlices ? blockIdx.y * 256 : 0) + threadIdx.x;   // k < 8: a bias row (slice 0)
   float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   float bsum = 0.f;
   for (int nb = 0; nb < B; nb += 64) {

@@ -259,7 +259,8 @@ int dmd_sgemm(const float* A, long long sam, long long sak, const float* B, long
               int M, int N, int K, const float* alpha, int accumulate, int chunks, float* partial, void* stream);
 
 /* FiLM linear weights (blocks.py:39) batched as rows of one matrix: grads[woff[f] + k] += inv_scale * sum_n dfilm[n][f] cond[n][k],
- * grads[boff[f]] += inv_scale * sum_n dfilm[n][f].  dfilm [B][rows], cond [B][CC], CC <= 256. */
+ * grads[boff[f]] += inv_scale * sum_n dfilm[n][f].  dfilm [B][rows], cond [B][CC], 0 < CC <= 2048.  Every write adds; each sum
+ * runs over n ascending.  One launch of ceil(rows / 8) x ceil(CC / 256) CTAs (one 256-column slice of cond per grid row). */
 int dmd_film_wgrad(const float* dfilm, const float* cond, float* grads, const long long* woff, const long long* boff, int B, int rows,
                    int CC, const float* inv_scale, void* stream);
 /* act_emb (inner_model.py:27-30): dE[act[n][t]][j] += inv_scale * de[n][t * CC/T + j]; act [B][T] int64 */
@@ -294,7 +295,7 @@ int dmd_loss_scale(const float* g, long long n, unsigned int* amax, float* scale
 typedef struct dmd_denoiser_config {
   int img_channels;             /* InnerModelConfig.img_channels */
   int num_steps_conditioning;   /* frame stack */
-  int cond_channels;
+  int cond_channels;            /* multiple of 32, at most 2048 */
   int num_levels;
   int depths[DMD_MAX_LEVELS];
   int channels[DMD_MAX_LEVELS]; /* 32, 64 or 128 per level, in any mix */
@@ -365,6 +366,11 @@ int dmd_inner_model_forward(dmd_denoiser* h, int B, int H, int W, const float* n
  * The output gradient is held NHWC with round_up(img_channels, 8) channels.  conv_in takes (num_steps_conditioning + 1) *
  * img_channels input channels that round up to 16, 32 or 64: dmd_denoiser_create refuses other configs, naming conv_in. */
 size_t dmd_denoiser_train_workspace_bytes(const dmd_denoiser* h, int B, int H, int W);
+/* The training plan's dcond = dfilm W_film product at B x H x W (no device work): its split-K count, the floats of the partial
+ * buffer it has to itself (0: the partials share the backward temporary, which caps the count at what it holds down to 8),
+ * and the floats of that temporary.  Returns nonzero (dmd_last_error) where the workspace query would fail. */
+int dmd_denoiser_train_dcond_plan(const dmd_denoiser* h, int B, int H, int W, int* splits, long long* own_partial_floats,
+                                  long long* temporary_floats);
 /* offsets / numels: n = dmd_denoiser_num_tensors entries (floats); returns the total length of the flat buffer. */
 long long dmd_denoiser_grad_layout(const dmd_denoiser* h, long long* offsets, long long* numels, int n);
 int dmd_inner_model_forward_train(dmd_denoiser* h, int B, int H, int W, const float* noisy_rescaled, const float* c_noise,
@@ -473,7 +479,7 @@ typedef struct dmd_rew_end_config {
   int lstm_dim;
   int img_channels;
   int img_size;
-  int cond_channels;
+  int cond_channels;            /* multiple of 32, at most 2048 */
   int num_levels;
   int depths[DMD_MAX_LEVELS];
   int channels[DMD_MAX_LEVELS]; /* 32, 64 or 128 per level, in any mix */
