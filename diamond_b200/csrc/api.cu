@@ -127,6 +127,10 @@ static size_t plc16_bytes(int B, int H, int W, int C) {
 }
 extern "C" size_t dmd_plc16_bytes(int B, int H, int W, int C) { return plc16_bytes(B, H, W, C); }
 
+// The statistics epilogue keeps kStatSlots images per 128-position tile, so the (padded) input image must hold at least 64
+// positions: 7x7 and up.  The executors follow a conv on a smaller image with gn_stats instead (PlanBuilder::conv).
+static bool conv_epilogue_stats_fit(int H, int W) { const Plc g = plc_geometry(1, H, W); return g.PH * g.PW >= 64; }
+
 static int conv_fill(const dmd_conv_desc* d, ConvParams* p, size_t* smem, int* acc_cols) {
   DMD_CHECK(d->src0 && d->out && d->wpk, "conv: null src0/out/wpk");
   DMD_CHECK(d->taps == 9 || d->taps == 1, "conv: taps must be 1 or 9 (got %d)", d->taps);
@@ -177,7 +181,7 @@ static int conv_fill(const dmd_conv_desc* d, ConvParams* p, size_t* smem, int* a
   p->P = kTileM + 2 * halo; p->Palloc = p->P | 1;
   if (d->out_stats) {
     const int L4 = d->Cout / 4;
-    DMD_CHECK(g.PH * g.PW >= 64, "conv: image too small for the statistics epilogue (a tile may touch at most %d images)", kStatSlots);
+    DMD_CHECK(conv_epilogue_stats_fit(d->H, d->W), "conv: image too small for the statistics epilogue (a tile may touch at most %d images)", kStatSlots);
     DMD_CHECK(d->Cout % 4 == 0 && (L4 == 4 || L4 == 8 || L4 == 16 || L4 == 32), "conv: out_stats needs Cout in {16,32,64,128} (got %d)", d->Cout);
     DMD_CHECK(d->out_gs == 16 || d->out_gs == 32 || d->out_gs == 64 || d->out_gs == 128, "conv: out_gs must be 16/32/64/128");
     DMD_CHECK(d->Cout % d->out_gs == 0 && d->Cout / d->out_gs <= kMaxOutGroups, "conv: bad output groups");
@@ -229,8 +233,10 @@ static int init_kernels() {
     DMD_CUDA(cudaFuncSetAttribute(attn_cluster_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(attn_cluster_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(attn_cluster_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 168 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    DMD_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    DMD_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<64, kAttnL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    DMD_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<32, kAttnL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    DMD_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<64, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    DMD_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<32, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(linear_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(linear_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     DMD_CUDA(cudaFuncSetAttribute(linear_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
@@ -302,11 +308,14 @@ static int prep_fill(const dmd_prep_desc* d, PrepParams* p, int* nsrc) {
   p->film = d->film; p->film_stride = d->film_stride; p->film_off = d->film_off; p->film_ctot = d->C0 + d->C1;
   p->gamma = d->gamma; p->beta = d->beta; p->eps = d->eps;
   const Plc g = plc_geometry(d->B, p->H, p->W);
-  DMD_CHECK(g.PH * g.PW >= 32, "prep: image too small");
-  // a block touches at most 2 images; low-resolution levels get smaller blocks so that the grid still covers the SMs
+  // 4x4 (25 padded positions) is the smallest image the executors build
+  DMD_CHECK(g.PH * g.PW >= 25, "prep: image too small (%dx%d; 4x4 is the smallest)", p->H, p->W);
+  // a block touches at most 2 images (at most PH * PW positions); low-resolution levels get smaller blocks so that the grid
+  // still covers the SMs.  Multiples of 32 positions, 16 on images of fewer than 32 (4x4, 4x5)
   int ppb = g.PH * g.PW >= 256 ? 256 : (g.PH * g.PW / 32) * 32;
   while (ppb > 64 && (g.Qalloc + ppb - 1) / ppb < 2 * kPlanSms) ppb >>= 1;
   ppb = (ppb / 32) * 32;
+  if (ppb == 0) ppb = 16;
   p->pos_per_block = ppb;
   // both kernels keep (mean, rstd) of at most 4 groups per image slot in shared memory, for every source
   DMD_CHECK(d->mode == 0 || (d->C0 / (d->gs0 > 0 ? d->gs0 : 8) <= 4 && d->C1 / (d->gs1 > 0 ? d->gs1 : 8) <= 4),
@@ -531,11 +540,12 @@ static int linear_launch(const float* in, const float* W, const float* bias, flo
   return 0;
 }
 
-// MaxPool2d(2) + GroupNorm partial sums of the pooled tensor; H, W: the pre-pool size.  The statistics are reduced over aligned
+// MaxPool2d(2) + GroupNorm partial sums of the pooled tensor; H, W: the pre-pool size, pooled to H/2 x W/2 with floor
+// division like nn.MaxPool2d (an odd last row / column is in no window).  The statistics are reduced over aligned
 // segments of min(gs, 32) lanes, i.e. consecutive channels of one pixel: a segment stays inside one group when gs is a power
 // of two <= 32 or a multiple of 32, and warps start on a group boundary when C % 32 == 0 or 256 % C == 0.
 static int maxpool2_stats_launch(const float* x, float* y, double* stats, int B, int H, int W, int C, int gs, cudaStream_t st) {
-  DMD_CHECK(H % 2 == 0 && W % 2 == 0, "maxpool2_stats: H=%d, W=%d must be even", H, W);
+  DMD_CHECK(H >= 2 && W >= 2, "maxpool2_stats: H=%d, W=%d must be at least 2", H, W);
   DMD_CHECK((long long)(H / 2) * (W / 2) * C < (1ll << 31), "maxpool2_stats: image too large for 32-bit indices");
   if (stats) DMD_CHECK(gs > 0 && C % gs == 0 && (gs % 32 == 0 || (gs <= 32 && (gs & (gs - 1)) == 0)) && (C % 32 == 0 || 256 % C == 0),
                        "maxpool2_stats: statistics need gs a power of two <= 32 or a multiple of 32, and C %% 32 == 0 or 256 %% C == 0 (C=%d gs=%d)", C, gs);
@@ -560,6 +570,7 @@ extern "C" int dmd_linear(const float* in, const float* W, const float* bias, fl
 }
 extern "C" int dmd_maxpool2_stats(const float* x, float* y, double* stats, int B, int H, int W, int C, int gs, void* stream) {
   DMD_CHECK(x && y && B > 0 && H > 0 && W > 0 && C > 0, "maxpool2_stats: bad arguments");
+  DMD_CHECK(H % 2 == 0 && W % 2 == 0, "maxpool2_stats: H=%d, W=%d must be even", H, W);
   return maxpool2_stats_launch(x, y, stats, B, H, W, C, gs, (cudaStream_t)stream);
 }
 extern "C" int dmd_lstm_gates(const float* gates, const float* c_in, float* h_out, float* c_out, int B, int Hd, void* stream) {
@@ -683,12 +694,18 @@ static int sgemm_launch(const float* A, long long sam, long long sak, const floa
 static size_t attn_bwd_smem(int L, int C) {
   return sizeof(float) * ((size_t)L * (C + 1) * 4 + (size_t)L * (3 * C + 4) * 2 + (size_t)(C / 8) * L * 3);
 }
+// L = 64 runs the instantiation with a compile-time token count, 1 <= L < 64 the one that reads it from ab.L
 static int attn_bwd_launch(const AttnBwdParams& ab, int B, cudaStream_t st) {
-  DMD_CHECK((ab.C == 64 || ab.C == 32) && ab.L == kAttnL && ab.gs > 0 && ab.C % ab.gs == 0 && ab.C / ab.gs <= 4,
-            "attention backward: unsupported shape L=%d C=%d gs=%d", ab.L, ab.C, ab.gs);
+  DMD_CHECK((ab.C == 64 || ab.C == 32) && ab.L >= 1 && ab.L <= kAttnL && ab.gs > 0 && ab.C % ab.gs == 0 && ab.C / ab.gs <= 4,
+            "attention backward: unsupported shape L=%d C=%d gs=%d (1 <= L <= %d)", ab.L, ab.C, ab.gs, kAttnL);
   const size_t smem = attn_bwd_smem(ab.L, ab.C);
-  if (ab.C == 64) attn_bwd_kernel<64><<<B, kAttnThreads, smem, st>>>(ab);
-  else attn_bwd_kernel<32><<<B, kAttnThreads, smem, st>>>(ab);
+  if (ab.L == kAttnL) {
+    if (ab.C == 64) attn_bwd_kernel<64, kAttnL><<<B, kAttnThreads, smem, st>>>(ab);
+    else attn_bwd_kernel<32, kAttnL><<<B, kAttnThreads, smem, st>>>(ab);
+  } else {
+    if (ab.C == 64) attn_bwd_kernel<64, 0><<<B, kAttnThreads, smem, st>>>(ab);
+    else attn_bwd_kernel<32, 0><<<B, kAttnThreads, smem, st>>>(ab);
+  }
   DMD_LAUNCH_OK();
   return 0;
 }
@@ -720,6 +737,7 @@ static int dsilu_mul_launch(const float* pre, const float* dh, float* out, long 
 }
 // H, W: the pre-pool size
 static int maxpool2_bwd_launch(const float* y, const float* gp, float* gy, int B, int H, int W, int C, cudaStream_t st) {
+  DMD_CHECK(H >= 2 && W >= 2, "maxpool2_bwd: H=%d, W=%d must be at least 2", H, W);
   const int total = (H / 2) * (W / 2) * C;
   maxpool2_bwd_kernel<<<dim3((total + 255) / 256, B), 256, 0, st>>>(y, gp, gy, H, W, C);
   DMD_LAUNCH_OK();
@@ -890,8 +908,9 @@ struct ResBlockW {
 
 struct Tens { float* data; double* stats; int C, H, W, gs; float* grad = nullptr; int gid = -1; };
 
-enum OpKind { OP_CONV = 0, OP_ATTN = 1, OP_PREP = 2, OP_RESIZE = 4 };
-struct Op { int kind; ConvParams conv; size_t smem; int cols; AttnParams attn; PrepParams prep; int prep_nsrc; ResizeParams rs; };
+enum OpKind { OP_CONV = 0, OP_ATTN = 1, OP_PREP = 2, OP_RESIZE = 4, OP_STATS = 5 };
+struct StatsOp { const float* x; double* stats; int HW, C, gs; };   // GroupNorm partial sums of x (dmd_gn_stats)
+struct Op { int kind; ConvParams conv; size_t smem; int cols; AttnParams attn; PrepParams prep; int prep_nsrc; ResizeParams rs; StatsOp gn; };
 constexpr int kScratchSlots = 10;  // round-robin pool of PLC16 operand buffers (each lives from its prep to the next conv)
 
 // PLC16 operands produced by one prep launch (op = index of that launch in Plan::ops, replayed by the backward pass)
@@ -1392,6 +1411,9 @@ struct PlanBuilder {
     d.Cout = cw.Cout; d.CoutPad = cw.CoutPad;
     d.residual = resid ? (resid->data ? resid->data : (const float*)1) : nullptr; d.out = out.data ? out.data : (float*)1;
     d.out_stats = out_stats ? (out.stats ? out.stats : (double*)1) : nullptr; d.out_gs = out.gs;
+    // below 7x7 the statistics come from gn_stats over the finished output (the same sums; one launch more)
+    const bool stats_after = d.out_stats && !conv_epilogue_stats_fit(in.H, in.W);
+    if (stats_after) d.out_stats = nullptr;
     if (split && (!d.src0_lo || (in.C1 && !d.src1_lo))) { fail("plan: precise conv without low operand parts"); err = 1; return; }
     if (in.C0 + in.C1 != cw.Cin) { fail("plan: operand channels %d+%d do not match the packed weights (%d)", in.C0, in.C1, cw.Cin); err = 1; return; }
     if (cw.nchunks && xproj) { fail("plan: a K-split conv cannot carry a fused projection"); err = 1; return; }
@@ -1402,6 +1424,11 @@ struct PlanBuilder {
       pl->ops.push_back(op);
       return 0;
     })) err = 1;
+    if (stats_after) {
+      Op op; op.kind = OP_STATS;
+      op.gn = StatsOp{out.data ? out.data : (const float*)1, out.stats ? out.stats : (double*)1, out.H * out.W, out.C, out.gs};
+      pl->ops.push_back(op);
+    }
   }
 
   // ResBlock.forward (blocks.py:141-147)
@@ -1420,9 +1447,9 @@ struct PlanBuilder {
     Rec rec; rec.kind = R_RES; rec.rb = &rb; rec.x = x; rec.has_skip = skip != nullptr; if (skip) rec.skip = *skip;
     rec.t = t; rec.o = o; rec.in1 = in1; rec.in2 = in2;
     if (!rb.has_attn) { record(rec); return o; }
-    if (pl->train && H * W != kAttnL) {
-      fail("training: the attention backward (attn_bwd_kernel) is built for 8x8 = 64 tokens only; this plan has an attention block "
-           "over %dx%d = %d tokens (inference runs at any token count)", H, W, H * W);
+    if (pl->train && H * W > kAttnL) {
+      fail("training: the attention backward (attn_bwd_kernel) is built for at most %d tokens (8x8); this plan has an attention block "
+           "over %dx%d = %d tokens (inference runs at any token count)", kAttnL, H, W, H * W);
       err = 1;
       return o;
     }
@@ -1651,14 +1678,14 @@ struct BwdBuilder {
     BOp b2 = b1; b2.kind = B_NORM2; push(b2);
   }
 
-  // SelfAttention2d backward at C = 128, L = 64 (bwd_kernels.cuh): x = o, g_out = gout, g_x assigned to o.grad.  Buffers in tB
-  // (q | k | v, g_qkv) and tC (xn, g_y, y, g_xn); the weight-gradient products split K over tA
+  // SelfAttention2d backward at C = 128, L = H * W <= 64 (bwd_kernels.cuh): x = o, g_out = gout, g_x assigned to o.grad.
+  // Buffers in tB (q | k | v, g_qkv) and tC (xn, g_y, y, g_xn); the weight-gradient products split K over tA
   void attn_split(const ResBlockW& rb, const Tens& o, const float* gout) {
-    const int C = rb.cout, rows = pl->B * kAttnL;
+    const int C = rb.cout, L = o.H * o.W, rows = pl->B * L;
     const long long n = (long long)rows * C;
     if (6 * n > pl->tmp_floats) { err = fail("backward plan: attention temporaries (%lld floats) exceed tB", 6 * n); return; }
     BOp b; b.kind = B_ATTN_RECOMP;
-    b.ap = AttnParams{o.data, o.stats, P(rb.an_w), P(rb.an_b), P(rb.qkv_w), P(rb.qkv_b), P(rb.op_w), P(rb.op_b), nullptr, nullptr, kAttnL, C, o.gs, kGnEps};
+    b.ap = AttnParams{o.data, o.stats, P(rb.an_w), P(rb.an_b), P(rb.qkv_w), P(rb.qkv_b), P(rb.op_w), P(rb.op_b), nullptr, nullptr, L, C, o.gs, kGnEps};
     b.ap.scratch = pl->tB; b.ap.out = const_cast<float*>(gout);   // attn_core_bwd_kernel reads g_out from ap.out
     b.at_gqkv = pl->tB + 3 * n;
     b.at_xn = pl->tC; b.at_gy = pl->tC + n; b.at_y = pl->tC + 2 * n; b.at_gxn = pl->tC + 3 * n;
@@ -1941,6 +1968,7 @@ int run_forward(dmd_denoiser* h, Plan& pl, const float* noisy, const float* sigm
       else if (prep_launch(op.prep, op.prep_nsrc, st)) return 1;
     }
     else if (op.kind == OP_RESIZE) { if (resize_launch(op.rs, st)) return 1; }
+    else if (op.kind == OP_STATS) { if (dmd_gn_stats(op.gn.x, op.gn.stats, pl.B, op.gn.HW, op.gn.C, op.gn.gs, st)) return 1; }
     else { if (attn_launch(op.attn, pl.B, st)) return 1; }
   }
   return 0;
@@ -2167,17 +2195,22 @@ int run_backward(const ModelCore& core, Plan& pl, float* grads, cudaStream_t st)
         break;
       }
       case B_ATTN_RECOMP: {
-        const dim3 grid(kAttnL / kAttnTile, B);
+        const dim3 grid((b.ap.L + kAttnTile - 1) / kAttnTile, B);
         attn_qkv_kernel<128><<<grid, kAttnQkvThreads, 0, st>>>(b.ap);
         DMD_LAUNCH_OK();
-        const long long total = (long long)B * kAttnL * b.ap.C;
-        attn_xn_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(b.ap.x, b.ap.st_in, b.ap.gamma, b.ap.beta, b.at_xn, kAttnL, b.ap.C,
+        const long long total = (long long)B * b.ap.L * b.ap.C;
+        attn_xn_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(b.ap.x, b.ap.st_in, b.ap.gamma, b.ap.beta, b.at_xn, b.ap.L, b.ap.C,
                                                                        b.ap.gs, b.ap.eps, total);
         DMD_LAUNCH_OK();
         break;
       }
       case B_ATTN_CORE:
-        attn_core_bwd_kernel<<<dim3(b.ap.C / 8, B), kAttnCoreThreads, 0, st>>>(b.ap.scratch, b.at_gy, b.ap.out, b.at_y, b.at_gqkv, b.at_gxn, b.ap.C);
+        if (b.ap.L == kAttnL)
+          attn_core_bwd_kernel<kAttnL><<<dim3(b.ap.C / 8, B), kAttnCoreThreads, 0, st>>>(b.ap.scratch, b.at_gy, b.ap.out, b.at_y, b.at_gqkv,
+                                                                                        b.at_gxn, b.ap.C, b.ap.L);
+        else
+          attn_core_bwd_kernel<0><<<dim3(b.ap.C / 8, B), kAttnCoreThreads, 0, st>>>(b.ap.scratch, b.at_gy, b.ap.out, b.at_y, b.at_gqkv,
+                                                                                   b.at_gxn, b.ap.C, b.ap.L);
         DMD_LAUNCH_OK();
         break;
       case B_MEMSET: DMD_CUDA(cudaMemsetAsync(b.ms_ptr, 0, b.ms_bytes, st)); break;
@@ -2557,9 +2590,12 @@ extern "C" int dmd_actor_critic_forward(dmd_actor_critic* h, int B, const float*
     d.B = B; d.H = hw; d.W = hw; d.taps = cw.taps; d.stride = 1;
     d.wpk = m.packed + cw.pk_off; d.bias = m.ptrs[cw.b_idx]; d.Cout = cw.Cout; d.CoutPad = cw.CoutPad;
     d.residual = resid; d.out = out; d.out_stats = st_out; d.out_gs = gn_group_size(cw.Cout);
+    const bool stats_after = st_out && !conv_epilogue_stats_fit(hw, hw);   // as PlanBuilder::conv
+    if (stats_after) d.out_stats = nullptr;
     const size_t plane = (size_t)plc_geometry(B, hw, hw).Qalloc * 16;   // one PLC16 plane holds 8 channels
-    return for_each_conv_launch(cw, d, plane, [&](size_t off) { return m.packed + off; },
-                                [&](const dmd_conv_desc& dc) { return dmd_conv2d_fprop(&dc, st); });
+    if (for_each_conv_launch(cw, d, plane, [&](size_t off) { return m.packed + off; },
+                             [&](const dmd_conv_desc& dc) { return dmd_conv2d_fprop(&dc, st); })) return 1;
+    return stats_after ? dmd_gn_stats(out, st_out, B, hw * hw, cw.Cout, d.out_gs, st) : 0;
   };
   // conv0 feeds the first GroupNorm -> statistics in its epilogue
   if (run_conv(h->conv0, b.x0, h->conv0.c0_store, S, 0, 0, 0, nullptr, nullptr, b.pooled[0], b.st_in[0])) return 1;
@@ -2888,6 +2924,7 @@ int rew_end_encode(const dmd_rew_end* h, Plan& pl, int b, int t, const float* ob
   for (const Op& op : pl.ops) {
     if (op.kind == OP_CONV) { if (conv_launch(op.conv, op.smem, op.cols, st)) return 1; }
     else if (op.kind == OP_PREP) { if (prep_launch(op.prep, op.prep_nsrc, st)) return 1; }
+    else if (op.kind == OP_STATS) { if (dmd_gn_stats(op.gn.x, op.gn.stats, pl.B, op.gn.HW, op.gn.C, op.gn.gs, st)) return 1; }
     else { if (attn_launch(op.attn, pl.B, st)) return 1; }
   }
   return 0;

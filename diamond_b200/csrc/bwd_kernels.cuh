@@ -392,8 +392,9 @@ __global__ void embedding_bwd_kernel(const float* __restrict__ de, const int64_t
 }
 
 // ------------------------------------------------------------------------------------------------ attention backward
-// SelfAttention2d (blocks.py:51-72) backward, one CTA per image (L = 64 tokens, C in {32, 64}, head_dim 8).  The forward
-// is recomputed in shared memory (normed x, qkv, per-row softmax statistics), then:
+// SelfAttention2d (blocks.py:51-72) backward, one CTA per image (L <= 64 tokens, C in {32, 64}, head_dim 8).  kL = 64: the
+// token count is a compile-time constant (the 8x8 level of a 64x64 frame); kL = 0: any L from 1 to 64, read from p.L, the same
+// arithmetic in the same order.  The forward is recomputed in shared memory (normed x, qkv, per-row softmax statistics), then:
 //   out = xn + Wo y + bo              ->  g_xn = g_out,  g_y = Wo^T g_out,  dWo += g_out (x) y,  dbo += sum g_out
 //   y = P v, P = softmax(q k^T / sqrt d)  ->  g_v = P^T g_y,  g_s = P o (g_y v^T - rowsum(P o g_y v^T)),  g_q = g_s k / sqrt d,
 //                                             g_k = g_s^T q / sqrt d
@@ -411,9 +412,11 @@ struct AttnBwdParams {
   float eps;
 };
 
-template <int C>
+template <int C, int kL>
 __global__ void __launch_bounds__(kAttnThreads) attn_bwd_kernel(const AttnBwdParams p) {
-  constexpr int L = kAttnL, C3 = 3 * C, XP = C + 1, QP = C3 + 4, HEADS = C / 8;
+  static_assert(kL == kAttnL || kL == 0, "attn_bwd_kernel: kL is 64 or 0 (runtime token count)");
+  constexpr int C3 = 3 * C, XP = C + 1, QP = C3 + 4, HEADS = C / 8;
+  const int L = kL ? kL : p.L;
   extern __shared__ __align__(16) float sm_ab[];
   float* xh = sm_ab;              // [L][XP]  xhat = (x - mean) * rstd
   float* qkv = xh + L * XP;       // [L][QP]
@@ -443,20 +446,23 @@ __global__ void __launch_bounds__(kAttnThreads) attn_bwd_kernel(const AttnBwdPar
     gxn[l * XP + c] = gg[i];
   }
   __syncthreads();
-  // ---- qkv = Wqkv xn + b   (xn = xhat * gamma + beta)
+  // ---- qkv = Wqkv xn + b   (xn = xhat * gamma + beta); item (token l, output group og): at L = 64 one per thread
   {
-    constexpr int NG = kAttnThreads / L, NO = C3 / NG;
-    const int l = tid % L, og = tid / L;
-    float acc[NO];
+    constexpr int NG = kAttnThreads / kAttnL, NO = C3 / NG;
+    auto project = [&](int l, int og) {
+      float acc[NO];
 #pragma unroll
-    for (int i = 0; i < NO; ++i) acc[i] = __ldg(p.bqkv + og * NO + i);
-    for (int c = 0; c < C; ++c) {
-      const float xn = fmaf(xh[l * XP + c], __ldg(p.gamma + c), __ldg(p.beta + c));
+      for (int i = 0; i < NO; ++i) acc[i] = __ldg(p.bqkv + og * NO + i);
+      for (int c = 0; c < C; ++c) {
+        const float xn = fmaf(xh[l * XP + c], __ldg(p.gamma + c), __ldg(p.beta + c));
 #pragma unroll
-      for (int i = 0; i < NO; ++i) acc[i] = fmaf(__ldg(p.wqkv + (size_t)(og * NO + i) * C + c), xn, acc[i]);
-    }
+        for (int i = 0; i < NO; ++i) acc[i] = fmaf(__ldg(p.wqkv + (size_t)(og * NO + i) * C + c), xn, acc[i]);
+      }
 #pragma unroll
-    for (int i = 0; i < NO; ++i) qkv[l * QP + og * NO + i] = acc[i];
+      for (int i = 0; i < NO; ++i) qkv[l * QP + og * NO + i] = acc[i];
+    };
+    if (kL) project(tid % L, tid / L);
+    else for (int it = tid; it < L * NG; it += kAttnThreads) project(it % L, it / L);
   }
   __syncthreads();
   // ---- pass A1: softmax row statistics and y, item = (head, query)
@@ -582,19 +588,20 @@ __global__ void __launch_bounds__(kAttnThreads) attn_bwd_kernel(const AttnBwdPar
   }
   __syncthreads();
   // ---- GroupNorm backward (affine)
+  float* const red = kL ? ys : qkv;   // two rows of per-channel sums: ys holds only one at L = 1, qkv is free as well
   if (tid < C) {
     float a = 0.f, b = 0.f;
     for (int l = 0; l < L; ++l) { const float g = gys[l * XP + tid]; a += g; b += g * xh[l * XP + tid]; }
     atomicAdd(p.dbeta + tid, a * alpha);
     atomicAdd(p.dgamma + tid, b * alpha);
     const float ga = __ldg(p.gamma + tid);
-    ys[tid] = ga * a;              // per-channel sums of g_xhat and g_xhat * xhat (ys is free now)
-    ys[XP + tid] = ga * b;
+    red[tid] = ga * a;             // per-channel sums of g_xhat and g_xhat * xhat (ys is free now)
+    red[XP + tid] = ga * b;
   }
   __syncthreads();
   if (tid < G) {
     float m1 = 0.f, m2 = 0.f;
-    for (int c = tid * p.gs; c < (tid + 1) * p.gs; ++c) { m1 += ys[c]; m2 += ys[XP + c]; }
+    for (int c = tid * p.gs; c < (tid + 1) * p.gs; ++c) { m1 += red[c]; m2 += red[XP + c]; }
     const float cnt = (float)L * p.gs;
     s_g1[tid] = m1 / cnt; s_g2[tid] = m2 / cnt;
   }
@@ -608,7 +615,9 @@ __global__ void __launch_bounds__(kAttnThreads) attn_bwd_kernel(const AttnBwdPar
 
 // ------------------------------------------------------------------------------------------------ actor-critic pieces
 // MaxPool2d(2) backward (actor_critic.py:109): the gradient of a pooled element goes to the window position that holds the
-// maximum (the first one in window order on an exact tie, like ATen).  y: pre-pool NHWC [B][H][W][C]; gp: NHWC [B][H/2][W/2][C].
+// maximum (the first one in window order on an exact tie, like ATen).  y: pre-pool NHWC [B][H][W][C]; gp: NHWC
+// [B][H/2][W/2][C], floor division: at an odd H (W) the last row (column) is in no window, and the threads of the last window
+// row (column) write its zero gradient.
 __global__ void maxpool2_bwd_kernel(const float* __restrict__ y, const float* __restrict__ gp, float* __restrict__ gy, int H, int W, int C) {
   const int n = blockIdx.y;
   const int Ho = H >> 1, Wo = W >> 1;
@@ -624,6 +633,10 @@ __global__ void maxpool2_bwd_kernel(const float* __restrict__ y, const float* __
   const float g = gp[(size_t)n * Ho * Wo * C + i];
 #pragma unroll
   for (int k = 0; k < 4; ++k) gy[o[k]] = k == am ? g : 0.f;
+  const bool last_col = (W & 1) && xo == Wo - 1, last_row = (H & 1) && yo == Ho - 1;
+  if (last_col) { gy[base + 2 * C] = 0.f; gy[base + (size_t)W * C + 2 * C] = 0.f; }
+  if (last_row) { gy[base + (size_t)2 * W * C] = 0.f; gy[base + (size_t)2 * W * C + C] = 0.f; }
+  if (last_col && last_row) gy[base + (size_t)2 * W * C + 2 * C] = 0.f;
 }
 
 // LSTMCell backward (actor_critic.py:46,72; torch gate order i, f, g, o).  gates: pre-activations [B][4H] of the forward;
@@ -752,63 +765,74 @@ __global__ void attn_xn_kernel(const float* __restrict__ x, const double* __rest
   xn[i] = (x[i] - (float)mean) * (float)(1.0 / sqrt(var + (double)eps)) * gamma[c] + beta[c];
 }
 
-// One CTA of kAttnL threads per (head h, image n), L = 64 tokens, head_dim 8.  In: qkv (attn_qkv_kernel layout), gy = g_y,
-// gout = g_out (both NHWC [B][L][C]).  Out: y (attention output before out_proj, NHWC), gqkv ([B][L][3C], q | k | v rows as
-// in Wqkv), gxn = g_out (head h's channels; the g_qkv Wqkv product is added to it afterwards).
+// One CTA of kAttnL threads per (head h, image n), L <= 64 tokens, head_dim 8; thread i owns token i (threads i >= L only
+// meet the barriers).  kL = 64: L is a compile-time constant; kL = 0: any L from 1 to 64, passed in Lrt.  In: qkv
+// (attn_qkv_kernel layout), gy = g_y, gout = g_out (both NHWC [B][L][C]).  Out: y (attention output before out_proj, NHWC),
+// gqkv ([B][L][3C], q | k | v rows as in Wqkv), gxn = g_out (head h's channels; the g_qkv Wqkv product is added to it
+// afterwards).
 //   P = softmax(q k^T / sqrt 8), y = P v, g_v = P^T g_y, g_s = P o (g_y v^T - rowsum(g_y o y)), g_q = g_s k / sqrt 8,
 //   g_k = g_s^T q / sqrt 8
 constexpr int kAttnCoreThreads = kAttnL;
+template <int kL>
 __global__ void __launch_bounds__(kAttnCoreThreads) attn_core_bwd_kernel(const float* __restrict__ qkv, const float* __restrict__ gy,
                                                                         const float* __restrict__ gout, float* __restrict__ y,
-                                                                        float* __restrict__ gqkv, float* __restrict__ gxn, int C) {
-  constexpr int L = kAttnL, LP = L + 1;
-  __shared__ float q[L][8], k[L][8], v[L][8], g[L][8], P[L][LP], S[L][LP];
+                                                                        float* __restrict__ gqkv, float* __restrict__ gxn, int C, int Lrt) {
+  static_assert(kL == kAttnL || kL == 0, "attn_core_bwd_kernel: kL is 64 or 0 (runtime token count)");
+  constexpr int LM = kAttnL, LP = LM + 1;
+  const int L = kL ? kL : Lrt;
+  __shared__ float q[LM][8], k[LM][8], v[LM][8], g[LM][8], P[LM][LP], S[LM][LP];
   const int h = blockIdx.x, n = blockIdx.y, i = threadIdx.x, HEADS = C / 8;
+  const bool own = kL || i < L;
   const float* base = qkv + (size_t)n * 3 * C * L;
   const size_t row = ((size_t)n * L + i) * C + h * 8;
+  if (own) {
 #pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    q[i][e] = base[((size_t)h * L + i) * 8 + e];
-    k[i][e] = base[((size_t)(HEADS + h) * L + i) * 8 + e];
-    v[i][e] = base[((size_t)(2 * HEADS + h) * L + i) * 8 + e];
-    g[i][e] = gy[row + e];
-    gxn[row + e] = gout[row + e];
+    for (int e = 0; e < 8; ++e) {
+      q[i][e] = base[((size_t)h * L + i) * 8 + e];
+      k[i][e] = base[((size_t)(HEADS + h) * L + i) * 8 + e];
+      v[i][e] = base[((size_t)(2 * HEADS + h) * L + i) * 8 + e];
+      g[i][e] = gy[row + e];
+      gxn[row + e] = gout[row + e];
+    }
   }
   __syncthreads();
   const float sc = 0.35355339059327373f;   // 1/sqrt(8)
-  // ---- row i: softmax, y_i, g_s row
-  float mx = -INFINITY;
-  for (int j = 0; j < L; ++j) {
-    float s = 0.f;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) s = fmaf(q[i][e] * sc, k[j][e], s);
-    P[i][j] = s;
-    mx = fmaxf(mx, s);
-  }
-  float den = 0.f;
-  for (int j = 0; j < L; ++j) { const float pj = expf(P[i][j] - mx); P[i][j] = pj; den += pj; }
-  const float inv = 1.f / den;
-  float yi[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  for (int j = 0; j < L; ++j) {
-    const float pj = P[i][j] * inv;
-    P[i][j] = pj;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) yi[e] = fmaf(pj, v[j][e], yi[e]);
-  }
-  float D = 0.f;
-#pragma unroll
-  for (int e = 0; e < 8; ++e) { y[row + e] = yi[e]; D = fmaf(g[i][e], yi[e], D); }
   float gq[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  for (int j = 0; j < L; ++j) {
-    float dp = 0.f;
+  if (own) {
+    // ---- row i: softmax, y_i, g_s row
+    float mx = -INFINITY;
+    for (int j = 0; j < L; ++j) {
+      float s = 0.f;
 #pragma unroll
-    for (int e = 0; e < 8; ++e) dp = fmaf(g[i][e], v[j][e], dp);
-    const float ds = P[i][j] * (dp - D) * sc;
-    S[i][j] = ds;
+      for (int e = 0; e < 8; ++e) s = fmaf(q[i][e] * sc, k[j][e], s);
+      P[i][j] = s;
+      mx = fmaxf(mx, s);
+    }
+    float den = 0.f;
+    for (int j = 0; j < L; ++j) { const float pj = expf(P[i][j] - mx); P[i][j] = pj; den += pj; }
+    const float inv = 1.f / den;
+    float yi[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    for (int j = 0; j < L; ++j) {
+      const float pj = P[i][j] * inv;
+      P[i][j] = pj;
 #pragma unroll
-    for (int e = 0; e < 8; ++e) gq[e] = fmaf(ds, k[j][e], gq[e]);
+      for (int e = 0; e < 8; ++e) yi[e] = fmaf(pj, v[j][e], yi[e]);
+    }
+    float D = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) { y[row + e] = yi[e]; D = fmaf(g[i][e], yi[e], D); }
+    for (int j = 0; j < L; ++j) {
+      float dp = 0.f;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) dp = fmaf(g[i][e], v[j][e], dp);
+      const float ds = P[i][j] * (dp - D) * sc;
+      S[i][j] = ds;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) gq[e] = fmaf(ds, k[j][e], gq[e]);
+    }
   }
   __syncthreads();
+  if (!own) return;
   // ---- column j = i: g_k, g_v
   float gk[8] = {0, 0, 0, 0, 0, 0, 0, 0}, gv[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   for (int r = 0; r < L; ++r) {

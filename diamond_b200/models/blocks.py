@@ -57,7 +57,7 @@ class AdaGroupNorm(_NativeOnly):  # blocks.py:34-45
 class SelfAttention2d(_NativeOnly):  # blocks.py:51-72
     """Multi-head self-attention over the H*W positions (head_dim 8) with a residual connection.  Executed by `attn_cluster_kernel`
     (a 4-CTA cluster per image exchanging K / V through distributed shared memory; 64 positions), by `attn_qkv_kernel` +
-    `attn_stream_kernel` at any other number of positions (inference), and `attn_bwd_kernel` (64 positions)."""
+    `attn_stream_kernel` at any other number of positions (inference), and `attn_bwd_kernel` (up to 64 positions)."""
 
     def __init__(self, in_channels: int, head_dim: int = ATTN_HEAD_DIM) -> None:
         super().__init__()

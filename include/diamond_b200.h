@@ -177,7 +177,8 @@ int dmd_prep_plan(const dmd_prep_desc* d, int* blocks, int* pos_per_block, int* 
 /* GroupNorm partial sums of an NHWC tensor: stats[n][g] += (sum, sumsq) (blocks.py:28,43). */
 int dmd_gn_stats(const float* x, double* stats, int B, int HW, int C, int gs, void* stream);
 
-/* SelfAttention2d.forward (blocks.py:62-72), L = H*W = 64 tokens, C in {32, 64, 128}, head_dim 8, at most 8 groups of gs
+/* SelfAttention2d.forward (blocks.py:62-72), L = H*W = 64 tokens (dmd_attn_fwd_scratch: any L; the backward, dmd_attn_bwd and
+ * the training plans: 1 <= L <= 64), C in {32, 64, 128}, head_dim 8, at most 8 groups of gs
  * channels (gs a multiple of 8 dividing C, and at L = 64 a multiple of C/4, as every model's gs = 32 is): out = xn + out_proj(softmax(q k^T
  * / sqrt(8)) v) with xn = GroupNorm(x) from the producer's statistics stats_in [B][C/gs][2]; out_stats (or NULL) [B][C/gs][2]
  * += (sum, sumsq) of out. */
@@ -247,7 +248,9 @@ int dmd_norm_bwd(const dmd_norm_bwd_desc* d, int pass, void* stream);
 int dmd_norm_affine_grad(const dmd_norm_bwd_desc* d, float* dgamma, float* dbeta, const float* inv_scale, void* stream);
 
 /* SelfAttention2d backward (blocks.py:62-72), the forward of dmd_attn_fwd: gx (NHWC [B][L][C]) is ASSIGNED; the six parameter
- * gradients are ADDED (times inv_scale).  L = 64, C in {32, 64}. */
+ * gradients are ADDED (times inv_scale).  Any L from 1 to 64 (L = 64: an 8x8 level; fewer: the deepest level of a frame
+ * below 64x64, e.g. 16 or 25 tokens at 32x32 or 40x40 with four levels), C in {32, 64}; L > 64 is refused (one CTA per image
+ * keeps every token in shared memory).  The training plans run C = 128 through their own split path over the same L. */
 int dmd_attn_bwd(const float* x, const double* stats_in, const float* gamma, const float* beta, const float* wqkv, const float* bqkv,
                  const float* wout, const float* gout, float* gx, float* dgamma, float* dbeta, float* dwqkv, float* dbqkv,
                  float* dwout, float* dbout, const float* inv_scale, int B, int L, int C, int gs, float eps, void* stream);
@@ -340,8 +343,10 @@ int dmd_denoiser_set_weights(dmd_denoiser* h, const float* const* ptrs_host, int
 /* H, W need not be multiples of 2^(levels-1): like UNet.forward (blocks.py:225-229,245) the executor zero-pads the conv_in
  * output at the bottom / right, runs the U-Net on the padded size and crops before norm_out / conv_out (inference entry
  * points; the training entry points reject such sizes).  Attention runs over any token count at inference, and the workspace
- * includes its scratch; the training entry points reject an attention block over other than 8x8 = 64 positions (the attention
- * backward is built for 64 tokens only) before any launch. */
+ * includes its scratch; the training entry points reject an attention block over more than 8x8 = 64 positions (the attention
+ * backward is built for at most 64 tokens) before any launch.  Levels as small as 4x4 are built (32x32 frames with four
+ * levels): a conv on a level below 7x7 gets its GroupNorm statistics from one gn_stats launch after it, since the conv's
+ * statistics epilogue keeps at most three images per tile; levels below 4x4 are refused by the operand prep. */
 size_t dmd_denoiser_workspace_bytes(const dmd_denoiser* h, int B, int H, int W);
 
 /* One Denoiser.denoise / compute_model_output call.  noisy (B,C,H,W), sigma (B) or (1), obs (B,T*C,H,W),
