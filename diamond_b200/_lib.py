@@ -135,6 +135,7 @@ SIGNATURES = {
     "dmd_denoiser_num_tensors": (_i, [_vp]),
     "dmd_denoiser_packed_bytes": (_sz, [_vp]),
     "dmd_denoiser_set_weights": (_i, [_vp, C.POINTER(_vp), _i, _vp, _vp]),
+    "dmd_denoiser_set_deterministic": (_i, [_vp, _i]),
     "dmd_denoiser_workspace_bytes": (_sz, [_vp, _i, _i, _i]),
     "dmd_denoiser_forward": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dmd_inner_model_forward": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
@@ -152,6 +153,7 @@ SIGNATURES = {
     "dmd_actor_critic_num_tensors": (_i, [_vp]),
     "dmd_actor_critic_packed_bytes": (_sz, [_vp]),
     "dmd_actor_critic_set_weights": (_i, [_vp, C.POINTER(_vp), _i, _vp, _vp]),
+    "dmd_actor_critic_set_deterministic": (_i, [_vp, _i]),
     "dmd_actor_critic_workspace_bytes": (_sz, [_vp, _i]),
     "dmd_actor_critic_forward": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dmd_actor_critic_backward_scratch_bytes": (_sz, [_vp, _i]),
@@ -163,6 +165,7 @@ SIGNATURES = {
     "dmd_rew_end_num_tensors": (_i, [_vp]),
     "dmd_rew_end_packed_bytes": (_sz, [_vp]),
     "dmd_rew_end_set_weights": (_i, [_vp, C.POINTER(_vp), _i, _vp, _vp]),
+    "dmd_rew_end_set_deterministic": (_i, [_vp, _i]),
     "dmd_rew_end_workspace_bytes": (_sz, [_vp, _i]),
     "dmd_rew_end_predict": (_i, [_vp, _i, _i] + [_vp] * 9 + [_vp, _sz, _vp]),
     "dmd_rew_end_train_workspace_bytes": (_sz, [_vp, _i, _i]),

@@ -471,15 +471,26 @@ extern "C" int dmd_pack_conv_weight(const float* w, void* wpk, int Cout, int Cou
   return 0;
 }
 
-extern "C" int dmd_gn_stats(const float* x, double* stats, int B, int HW, int C, int gs, void* stream) {
+// GroupNorm sums of an NHWC tensor, added to stats[B][C / gs][2].  det (torch.use_deterministic_algorithms): one cluster of
+// kGnDetSplit CTAs owns each (image, group) and sums it in a fixed order, in place of the fp64 atomics of up to 64 blocks per image
+static int gn_stats_launch(const float* x, double* stats, int B, int HW, int C, int gs, bool det, cudaStream_t st) {
   DMD_CHECK(x && stats && gs > 0 && C % gs == 0, "gn_stats: bad arguments");
+  if (det) {
+    DMD_CHECK(B <= 65535 && (long long)kGnDetSplit * (C / gs) < (1ll << 31), "gn_stats: B=%d or %d groups out of range", B, C / gs);
+    gn_stats_det_kernel<<<dim3(kGnDetSplit * (C / gs), B), kGnDetThreads, 0, st>>>(x, stats, HW, C, gs);
+    DMD_LAUNCH_OK();
+    return 0;
+  }
   long long per = (long long)HW * C;
   int chunks = (int)((per + 256 * 64 - 1) / (256 * 64));
   if (chunks < 1) chunks = 1;
   if (chunks > 64) chunks = 64;
-  gn_stats_kernel<<<dim3(chunks, B), 256, 0, (cudaStream_t)stream>>>(x, stats, HW, C, gs);
+  gn_stats_kernel<<<dim3(chunks, B), 256, 0, st>>>(x, stats, HW, C, gs);
   DMD_LAUNCH_OK();
   return 0;
+}
+extern "C" int dmd_gn_stats(const float* x, double* stats, int B, int HW, int C, int gs, void* stream) {
+  return gn_stats_launch(x, stats, B, HW, C, gs, false, (cudaStream_t)stream);
 }
 
 // scratch of the any-L attention path (q, k, v of every token); L = 64 runs in one launch without scratch
@@ -623,11 +634,22 @@ static int loss_scale_launch(const float* g, long long n, unsigned int* amax_bit
   return 0;
 }
 
-// column sums: up to 592 blocks of 256 / (Cb / 4) row lanes, at least 8 rows per lane
-static int colsum_launch(const float* x, float* out, float* out2, const float* inv, long long rows, int C, int Creal, cudaStream_t st) {
+// column sums: up to 592 blocks of 256 / (Cb / 4) row lanes, at least 8 rows per lane.  part (deterministic mode): each block
+// stores its sums to part[block][C] (part_bytes of room) and colsum_reduce_kernel adds them in block order, in place of the
+// atomics.  The block count depends on rows and C only, so the order does too.
+static int colsum_launch(const float* x, float* out, float* out2, const float* inv, long long rows, int C, int Creal, cudaStream_t st,
+                         float* part = nullptr, size_t part_bytes = 0) {
   const int L4 = (C < 256 ? C : 256) >> 2, lanes = 256 / L4;
   long long blocks = (rows + (long long)lanes * 8 - 1) / ((long long)lanes * 8);
   blocks = blocks > 592 ? 592 : (blocks < 1 ? 1 : blocks);
+  if (part) {
+    DMD_CHECK((size_t)blocks * C * sizeof(float) <= part_bytes, "colsum: partials (%lld x %d floats) exceed the partial buffer", blocks, C);
+    colsum_part_kernel<<<dim3((unsigned)blocks, (C + 255) / 256), 256, 0, st>>>(x, part, rows, C);
+    DMD_LAUNCH_OK();
+    colsum_reduce_kernel<<<(Creal + 255) / 256, 256, 0, st>>>(part, (int)blocks, C, Creal, out, out2, inv);
+    DMD_LAUNCH_OK();
+    return 0;
+  }
   colsum_kernel<<<dim3((unsigned)blocks, (C + 255) / 256), 256, 0, st>>>(x, out, out2, inv, rows, C, Creal);
   DMD_LAUNCH_OK();
   return 0;
@@ -640,8 +662,10 @@ static int norm_bwd_ppb(int B, int HW) {
   while (ppb > 32 && (long long)B * ((HW + ppb - 1) / ppb) < 2 * kPlanSms) ppb >>= 1;
   return ppb;
 }
-static int norm_bwd_launch(const NormBwdParams& nb, int pass, cudaStream_t st) {
-  const int ppb = norm_bwd_ppb(nb.B, nb.HW);
+// det (deterministic mode): pass 1 runs one block per image, so each per-(image, channel) sum has one writer, whose single
+// atomic add onto the cleared sum is exact and order-free
+static int norm_bwd_launch(const NormBwdParams& nb, int pass, cudaStream_t st, bool det = false) {
+  const int ppb = det && pass == 1 ? nb.HW : norm_bwd_ppb(nb.B, nb.HW);
   const dim3 grid((nb.HW + ppb - 1) / ppb, nb.B);
   if (pass == 1) norm_bwd_pass1_kernel<<<grid, kNormThreads, 0, st>>>(nb, ppb);
   else norm_bwd_pass2_kernel<<<grid, kNormThreads, 0, st>>>(nb, ppb);
@@ -718,8 +742,9 @@ static int film_wgrad_launch(const float* dfilm, const float* cond, float* grads
   return 0;
 }
 static int embedding_bwd_launch(const float* de, const int64_t* act, float* dE, int B, int CC, int T, int num_actions, const float* inv,
-                                cudaStream_t st) {
-  embedding_bwd_kernel<<<(B * CC + 255) / 256, 256, 0, st>>>(de, act, dE, B, CC, T, num_actions, inv);
+                                cudaStream_t st, bool det = false) {
+  if (det) embedding_bwd_det_kernel<<<(num_actions * (CC / T) + 255) / 256, 256, 0, st>>>(de, act, dE, B, CC, T, num_actions, inv);
+  else embedding_bwd_kernel<<<(B * CC + 255) / 256, 256, 0, st>>>(de, act, dE, B, CC, T, num_actions, inv);
   DMD_LAUNCH_OK();
   return 0;
 }
@@ -855,13 +880,13 @@ extern "C" int dmd_loss_scale(const float* g, long long n, unsigned int* amax, f
 
 // ---------------------------------------------------------------------------------------------- denoiser executor
 // zero-pad / crop copy of an NHWC tensor, then the GroupNorm partial sums of the result (the consumer's prologue reads them)
-static int resize_launch(const ResizeParams& p, cudaStream_t st) {
+static int resize_launch(const ResizeParams& p, cudaStream_t st, bool det = false) {
   const long long total = (long long)p.B * p.Hd * p.Wd * (p.C / 4);
   long long blocks = (total + 255) / 256;
   if (blocks > kPlanSms * 16) blocks = kPlanSms * 16;
   resize_nhwc_kernel<<<(int)blocks, 256, 0, st>>>(p);
   DMD_LAUNCH_OK();
-  if (p.stats) return dmd_gn_stats(p.dst, p.stats, p.B, p.Hd * p.Wd, p.C, p.gs, st);
+  if (p.stats) return gn_stats_launch(p.dst, p.stats, p.B, p.Hd * p.Wd, p.C, p.gs, det, st);
   return 0;
 }
 extern "C" int dmd_resize_nhwc(const float* src, float* dst, int B, int Hs, int Ws, int Hd, int Wd, int C, double* stats, int gs, void* stream) {
@@ -958,6 +983,7 @@ struct Rec {
 struct Plan {
   int B = 0, H = 0, W = 0;
   int T = 1;   // time-major plans (reward / termination): B = T x segments rows
+  bool det = false;   // deterministic mode (torch.use_deterministic_algorithms): fixed-order statistics and gradient sums
   long long tmp_floats = 0;   // training: floats in each of tA / tB / tC
   uint8_t* base = nullptr;
   size_t bytes = 0;
@@ -978,6 +1004,7 @@ struct Plan {
   float *gF = nullptr;                                    // scaled dL/d(model output), NHWC with gF_ch channels
   int gF_ch = 0;                                          // round_up(img_channels, 8): the padded channels are zero
   float *dfilm = nullptr, *nsum = nullptr, *partial = nullptr, *scale = nullptr;
+  size_t partial_bytes = 0;   // wgrad split-K partials; between weight gradients, the deterministic colsum partials
   float *dcond = nullptr, *dh = nullptr, *cpre = nullptr, *dpre = nullptr, *de = nullptr;
   float* film_part = nullptr;                             // split-K partials of dcond = dfilm Wf: tA, or its own buffer
   int film_splits = 0;                                    // dcond's split count (<= 1: no split)
@@ -1028,6 +1055,8 @@ struct ModelCore {
   // training plans, one per live training workspace (an autoregressive Denoiser.forward holds several forwards before
   // their backwards run); kept apart from the inference plan so that imagination and training can alternate
   std::vector<std::unique_ptr<Plan>> tplans;
+  // deterministic mode (dmd_*_set_deterministic, torch.use_deterministic_algorithms): part of every plan's cache key
+  bool det = false;
 
   const float* P(int idx) const { return ptrs.empty() ? nullptr : ptrs[idx]; }
   // once every tensor is registered: 16-byte aligned gradient slices, and the FiLM table behind the pk bytes of conv packs
@@ -1091,7 +1120,7 @@ struct dmd_denoiser {
   std::vector<SamplerGraph> graphs;     // one per distinct (buffers, ring head): a WorldModelEnv replays T of them round-robin
   unsigned long long graph_clock = 0;
   cudaStream_t cap_stream = nullptr;
-  int need_B = 0, need_H = 0, need_W = 0; size_t need_bytes = 0;
+  int need_B = 0, need_H = 0, need_W = 0; bool need_det = false; size_t need_bytes = 0;
 };
 
 // Reward / termination model (executor below dmd_lambda_returns): the encoder is built from the U-Net's ResBlocks
@@ -1411,8 +1440,9 @@ struct PlanBuilder {
     d.Cout = cw.Cout; d.CoutPad = cw.CoutPad;
     d.residual = resid ? (resid->data ? resid->data : (const float*)1) : nullptr; d.out = out.data ? out.data : (float*)1;
     d.out_stats = out_stats ? (out.stats ? out.stats : (double*)1) : nullptr; d.out_gs = out.gs;
-    // below 7x7 the statistics come from gn_stats over the finished output (the same sums; one launch more)
-    const bool stats_after = d.out_stats && !conv_epilogue_stats_fit(in.H, in.W);
+    // below 7x7, and in deterministic mode, the statistics come from gn_stats over the finished output (the same sums; one
+    // launch more)
+    const bool stats_after = d.out_stats && (pl->det || !conv_epilogue_stats_fit(in.H, in.W));
     if (stats_after) d.out_stats = nullptr;
     if (split && (!d.src0_lo || (in.C1 && !d.src1_lo))) { fail("plan: precise conv without low operand parts"); err = 1; return; }
     if (in.C0 + in.C1 != cw.Cin) { fail("plan: operand channels %d+%d do not match the packed weights (%d)", in.C0, in.C1, cw.Cin); err = 1; return; }
@@ -1424,11 +1454,12 @@ struct PlanBuilder {
       pl->ops.push_back(op);
       return 0;
     })) err = 1;
-    if (stats_after) {
-      Op op; op.kind = OP_STATS;
-      op.gn = StatsOp{out.data ? out.data : (const float*)1, out.stats ? out.stats : (double*)1, out.H * out.W, out.C, out.gs};
-      pl->ops.push_back(op);
-    }
+    if (stats_after) stats_of(out);
+  }
+  void stats_of(const Tens& t) {
+    Op op; op.kind = OP_STATS;
+    op.gn = StatsOp{t.data ? t.data : (const float*)1, t.stats ? t.stats : (double*)1, t.H * t.W, t.C, t.gs};
+    pl->ops.push_back(op);
   }
 
   // ResBlock.forward (blocks.py:141-147)
@@ -1457,7 +1488,9 @@ struct PlanBuilder {
     Op op; op.kind = OP_ATTN;
     op.attn = AttnParams{o.data, o.stats, P(rb.an_w), P(rb.an_b), P(rb.qkv_w), P(rb.qkv_b), P(rb.op_w), P(rb.op_b), a.data, a.stats, H * W, rb.cout, o.gs, kGnEps};
     if (H * W != kAttnL) op.attn.scratch = (float*)bump->take(attn_scratch_bytes(pl->B, H * W, rb.cout));
+    if (pl->det) op.attn.ostats = nullptr;
     pl->ops.push_back(op);
+    if (pl->det) stats_of(a);
     rec.a = a;
     record(rec);
     return a;
@@ -1599,12 +1632,12 @@ int make_plan(const dmd_denoiser* h, Plan* pl, int B, int H, int W, uint8_t* bas
   pl->B = B; pl->H = H; pl->W = W; pl->ops.clear();
   // pass 1: stats region size (tiny) — run the builder on null bases
   Bump b0{nullptr}, s0{nullptr};
-  { Plan tmp; tmp.B = B; tmp.H = H; tmp.W = W; PlanBuilder pb{&h->core, &tmp, &b0, &s0}; if (pb.build(h)) return 1; }
+  { Plan tmp; tmp.B = B; tmp.H = H; tmp.W = W; tmp.det = h->core.det; PlanBuilder pb{&h->core, &tmp, &b0, &s0}; if (pb.build(h)) return 1; }
   const size_t stats_bytes = (s0.off + 255) & ~(size_t)255;
   if (total) *total = stats_bytes + b0.off + 256;
   if (!base) return 0;
   Bump sb{base}, bb{base + stats_bytes};
-  pl->base = base; pl->stats = (double*)base; pl->stats_bytes = stats_bytes;
+  pl->base = base; pl->stats = (double*)base; pl->stats_bytes = stats_bytes; pl->det = h->core.det;
   PlanBuilder pb{&h->core, pl, &bb, &sb};
   if (pb.build(h)) return 1;
   pl->bytes = stats_bytes + bb.off;
@@ -1678,7 +1711,9 @@ struct BwdBuilder {
     BOp b2 = b1; b2.kind = B_NORM2; push(b2);
   }
 
-  // SelfAttention2d backward at C = 128, L = H * W <= 64 (bwd_kernels.cuh): x = o, g_out = gout, g_x assigned to o.grad.
+  // SelfAttention2d backward at C = 128, and at every C in deterministic mode (attn_bwd_kernel adds its parameter gradients
+  // with atomics; here they are fixed-order sgemm / colsum launches), L = H * W <= 64 (bwd_kernels.cuh): x = o, g_out = gout,
+  // g_x assigned to o.grad.
   // Buffers in tB (q | k | v, g_qkv) and tC (xn, g_y, y, g_xn); the weight-gradient products split K over tA
   void attn_split(const ResBlockW& rb, const Tens& o, const float* gout) {
     const int C = rb.cout, L = o.H * o.W, rows = pl->B * L;
@@ -1712,7 +1747,7 @@ struct BwdBuilder {
     const int H = r.o.H, W = r.o.W, B = pl->B;
     const long long pix = (long long)B * H * W;
     Tens o = r.o;
-    if (rb.has_attn && rb.cout > 64) {
+    if (rb.has_attn && (rb.cout > 64 || pl->det)) {
       attn_split(rb, o, r.a.grad);
       ginit[o.gid] = 1;
     } else if (rb.has_attn) {  // attention consumes o alone: its backward ASSIGNS o's gradient
@@ -1864,25 +1899,28 @@ using FwdPlanFn = std::function<int(PlanBuilder&)>;
 using BwdPlanFn = std::function<int(BwdBuilder&)>;
 int make_train_plan(const ModelCore& core, int cmax, int gF_ch, Plan* pl, int B, int H, int W, int T, uint8_t* base, size_t* total,
                     const FwdPlanFn& fwd, const BwdPlanFn& bwd) {
-  pl->train = true; pl->n_grad_tensors = 0; pl->tape.clear();
+  const bool det = core.det;
+  pl->train = true; pl->n_grad_tensors = 0; pl->tape.clear(); pl->det = det;
   pl->B = B; pl->H = H; pl->W = W; pl->T = T; pl->ops.clear(); pl->bops.clear();
   Bump b0{nullptr}, s0{nullptr};
-  { Plan tmp; tmp.train = true; tmp.B = B; tmp.H = H; tmp.W = W; tmp.T = T; PlanBuilder pb{&core, &tmp, &b0, &s0}; if (fwd(pb)) return 1; }
+  { Plan tmp; tmp.train = true; tmp.det = det; tmp.B = B; tmp.H = H; tmp.W = W; tmp.T = T; PlanBuilder pb{&core, &tmp, &b0, &s0}; if (fwd(pb)) return 1; }
   const size_t stats_bytes = (s0.off + 255) & ~(size_t)255;
   Bump sb{base}, bb{base ? base + stats_bytes : nullptr};
   if (base) { pl->base = base; pl->stats = (double*)base; pl->stats_bytes = stats_bytes; }
   if (base) { PlanBuilder pb{&core, pl, &bb, &sb}; if (fwd(pb)) return 1; } else bb.off = b0.off;
   // backward temporaries
   pl->tmp_floats = (long long)B * H * W * cmax;
-  // the split attention backward at C = 128 (BwdBuilder::attn_split) keeps six [B][64][C] buffers in tB and four in tC
-  if (cmax > 64 && pl->tmp_floats < 6ll * B * kAttnL * cmax) pl->tmp_floats = 6ll * B * kAttnL * cmax;
+  // the split attention backward at C = 128, and at every C in deterministic mode (BwdBuilder::attn_split), keeps six
+  // [B][64][C] buffers in tB and four in tC
+  if ((cmax > 64 || det) && pl->tmp_floats < 6ll * B * kAttnL * cmax) pl->tmp_floats = 6ll * B * kAttnL * cmax;
   const size_t act_bytes = (size_t)pl->tmp_floats * 4;
   pl->tA = (float*)bb.take(act_bytes); pl->tB = (float*)bb.take(act_bytes); pl->tC = (float*)bb.take(act_bytes);
   const size_t op_bytes = plc16_bytes(B, H, W, cmax);
   pl->gyA = (uint8_t*)bb.take(op_bytes); pl->gyB = (uint8_t*)bb.take(op_bytes);
   pl->gF = (float*)bb.take((size_t)B * H * W * gF_ch * 4); pl->gF_ch = gF_ch;
   if (init_kernels()) return 1;
-  pl->partial = (float*)bb.take(wgrad_partial_bytes(g_num_sms));
+  pl->partial_bytes = wgrad_partial_bytes(g_num_sms);
+  pl->partial = (float*)bb.take(pl->partial_bytes);
   const int CC = core.cond_channels;
   pl->dcond = (float*)bb.take((size_t)B * CC * 4); pl->dh = (float*)bb.take((size_t)B * CC * 4); pl->cpre = (float*)bb.take((size_t)B * CC * 4);
   pl->dpre = (float*)bb.take((size_t)B * CC * 4); pl->de = (float*)bb.take((size_t)B * CC * 4);
@@ -1967,8 +2005,8 @@ int run_forward(dmd_denoiser* h, Plan& pl, const float* noisy, const float* sigm
       if (op.prep.film != nullptr && op.prep.film != film) { PrepParams pp = op.prep; pp.film = film; if (prep_launch(pp, op.prep_nsrc, st)) return 1; }
       else if (prep_launch(op.prep, op.prep_nsrc, st)) return 1;
     }
-    else if (op.kind == OP_RESIZE) { if (resize_launch(op.rs, st)) return 1; }
-    else if (op.kind == OP_STATS) { if (dmd_gn_stats(op.gn.x, op.gn.stats, pl.B, op.gn.HW, op.gn.C, op.gn.gs, st)) return 1; }
+    else if (op.kind == OP_RESIZE) { if (resize_launch(op.rs, st, pl.det)) return 1; }
+    else if (op.kind == OP_STATS) { if (gn_stats_launch(op.gn.x, op.gn.stats, pl.B, op.gn.HW, op.gn.C, op.gn.gs, pl.det, st)) return 1; }
     else { if (attn_launch(op.attn, pl.B, st)) return 1; }
   }
   return 0;
@@ -1986,7 +2024,7 @@ int run_wrap(dmd_denoiser* h, Plan& pl, const float* x, float* model_out, float*
 int ensure_plan(dmd_denoiser* h, int B, int H, int W, void* ws, size_t ws_bytes) {
   DMD_CHECK(h->core.ready(), "denoiser: call dmd_denoiser_set_weights first");
   Plan& pl = h->plan;
-  if (pl.B == B && pl.H == H && pl.W == W && pl.base == (uint8_t*)ws) return 0;
+  if (pl.B == B && pl.H == H && pl.W == W && pl.base == (uint8_t*)ws && pl.det == h->core.det) return 0;
   // size and validate on a scratch plan: the cached plan is replaced only after every check has passed, and is
   // invalidated (never left half-written) if the real build fails
   size_t need = 0;
@@ -2080,6 +2118,18 @@ extern "C" int dmd_denoiser_set_weights(dmd_denoiser* h, const float* const* ptr
   return 0;
 }
 
+// deterministic mode: plans, sampler graphs and workspace queries made while it is on use the fixed-order arms
+extern "C" int dmd_denoiser_set_deterministic(dmd_denoiser* h, int on) {
+  DMD_CHECK(h, "denoiser_set_deterministic: null handle");
+  h->core.det = on != 0;
+  return 0;
+}
+extern "C" int dmd_rew_end_set_deterministic(dmd_rew_end* h, int on) {
+  DMD_CHECK(h, "rew_end_set_deterministic: null handle");
+  h->core.det = on != 0;
+  return 0;
+}
+
 extern "C" size_t dmd_denoiser_workspace_bytes(const dmd_denoiser* h, int B, int H, int W) {
   Plan tmp; size_t need = 0;
   if (make_plan(h, &tmp, B, H, W, nullptr, &need)) return 0;
@@ -2132,9 +2182,10 @@ extern "C" int dmd_inner_model_forward_u8(dmd_denoiser* h, int B, int H, int W, 
 // ---------------------------------------------------------------------------------------------- training entry points
 namespace {
 
-Plan* find_train_plan(ModelCore& core, int B, int H, int W, int T, const void* ws) {
+// any_mode: a backward finds the plan its forward ran on (one per workspace) in whichever mode that forward was planned
+Plan* find_train_plan(ModelCore& core, int B, int H, int W, int T, const void* ws, bool any_mode = false) {
   for (auto& p : core.tplans)
-    if (p->B == B && p->H == H && p->W == W && p->T == T && p->base == (const uint8_t*)ws) return p.get();
+    if (p->B == B && p->H == H && p->W == W && p->T == T && p->base == (const uint8_t*)ws && (any_mode || p->det == core.det)) return p.get();
   return nullptr;
 }
 
@@ -2181,9 +2232,10 @@ int run_backward(const ModelCore& core, Plan& pl, float* grads, cudaStream_t st)
       case B_CONV: if (conv_launch(b.conv, b.smem, b.cols, st)) return 1; break;
       case B_WGRAD: if (wgrad_launch(b.wg, grads + b.goff, st)) return 1; break;
       case B_COLSUM:
-        if (colsum_launch(b.src, grads + b.goff, b.goff2 >= 0 ? grads + b.goff2 : nullptr, inv, b.rows, b.C, b.Creal, st)) return 1;
+        if (colsum_launch(b.src, grads + b.goff, b.goff2 >= 0 ? grads + b.goff2 : nullptr, inv, b.rows, b.C, b.Creal, st,
+                          pl.det ? pl.partial : nullptr, pl.partial_bytes)) return 1;
         break;
-      case B_NORM1: if (norm_bwd_launch(b.nb, 1, st)) return 1; break;
+      case B_NORM1: if (norm_bwd_launch(b.nb, 1, st, pl.det)) return 1; break;
       case B_NORM2: if (norm_bwd_launch(b.nb, 2, st)) return 1; break;
       case B_AFFINE: if (affine_param_grad_launch(b.nb, grads + b.goff, grads + b.goff2, inv, st)) return 1; break;
       case B_POOL: if (sumpool2_launch(b.src, b.dst, B, b.H, b.W, b.C, b.acc, st)) return 1; break;
@@ -2196,7 +2248,9 @@ int run_backward(const ModelCore& core, Plan& pl, float* grads, cudaStream_t st)
       }
       case B_ATTN_RECOMP: {
         const dim3 grid((b.ap.L + kAttnTile - 1) / kAttnTile, B);
-        attn_qkv_kernel<128><<<grid, kAttnQkvThreads, 0, st>>>(b.ap);
+        if (b.ap.C == 128) attn_qkv_kernel<128><<<grid, kAttnQkvThreads, 0, st>>>(b.ap);
+        else if (b.ap.C == 64) attn_qkv_kernel<64><<<grid, kAttnQkvThreads, 0, st>>>(b.ap);
+        else attn_qkv_kernel<32><<<grid, kAttnQkvThreads, 0, st>>>(b.ap);
         DMD_LAUNCH_OK();
         const long long total = (long long)B * b.ap.L * b.ap.C;
         attn_xn_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(b.ap.x, b.ap.st_in, b.ap.gamma, b.ap.beta, b.at_xn, b.ap.L, b.ap.C,
@@ -2225,7 +2279,7 @@ int run_backward(const ModelCore& core, Plan& pl, float* grads, cudaStream_t st)
       case B_LINEAR: if (linear_launch(b.lin_in, b.lin_w, b.lin_b, b.lin_out, B, b.lin_K, b.lin_F, 0, st)) return 1; break;
       case B_DSILU: if (dsilu_mul_launch(b.src, b.ga, b.dst, b.rows, st)) return 1; break;
       case B_EMB:
-        if (embedding_bwd_launch(b.src, pl.t_act, grads + b.goff, B, b.C, b.emb_T, b.emb_actions, inv, st)) return 1;
+        if (embedding_bwd_launch(b.src, pl.t_act, grads + b.goff, B, b.C, b.emb_T, b.emb_actions, inv, st, pl.det)) return 1;
         break;
       default: return fail("backward: unknown op kind %d", b.kind);
     }
@@ -2282,7 +2336,7 @@ extern "C" int dmd_inner_model_forward_train_u8(dmd_denoiser* h, int B, int H, i
 static int denoiser_backward_impl(const char* who, dmd_denoiser* h, int B, int H, int W, const float* grad_out, float* grads,
                                   long long grads_numel, int accumulate, void* workspace, void* stream) {
   DMD_CHECK(h && grad_out && grads && workspace, "%s: null argument", who);
-  Plan* plp = find_train_plan(h->core, B, H, W, 1, workspace);
+  Plan* plp = find_train_plan(h->core, B, H, W, 1, workspace, true);
   DMD_CHECK(plp && plp->train, "%s: no matching dmd_inner_model_forward_train on this workspace (B=%d H=%d W=%d)", who, B, H, W);
   Plan& pl = *plp;
   DMD_CHECK(grads_numel >= h->core.grad_total, "%s: gradient buffer too small (%lld < %lld floats)", who, grads_numel, h->core.grad_total);
@@ -2397,9 +2451,9 @@ extern "C" int dmd_sampler_sample(dmd_denoiser* h, const dmd_sampler_config* sc,
   const int n = sc->num_sigmas, T = c.num_steps_conditioning;
   DMD_CHECK(ring_head >= -1 && ring_head < T, "sampler: ring_head must be -1 (contiguous stacks) or a slot index < %d", T);
   if (init_kernels()) return 1;
-  if (h->need_B != B || h->need_H != H || h->need_W != W) {
+  if (h->need_B != B || h->need_H != H || h->need_W != W || h->need_det != h->core.det) {
     h->need_bytes = dmd_denoiser_workspace_bytes(h, B, H, W);
-    h->need_B = B; h->need_H = H; h->need_W = W;
+    h->need_B = B; h->need_H = H; h->need_W = W; h->need_det = h->core.det;
   }
   DMD_CHECK(h->need_bytes > 0, "sampler: %s", g_err.c_str());
   DMD_CHECK(workspace_bytes >= h->need_bytes, "sampler: workspace too small (%zu < %zu)", workspace_bytes, h->need_bytes);
@@ -2562,6 +2616,11 @@ extern "C" int dmd_actor_critic_set_weights(dmd_actor_critic* h, const float* co
   return 0;
 }
 
+extern "C" int dmd_actor_critic_set_deterministic(dmd_actor_critic* h, int on) {
+  DMD_CHECK(h, "actor_critic_set_deterministic: null handle");
+  h->core.det = on != 0;
+  return 0;
+}
 extern "C" size_t dmd_actor_critic_workspace_bytes(const dmd_actor_critic* h, int B) {
   AcBuffers b; ac_layout(h, B, nullptr, &b); return b.total;
 }
@@ -2577,6 +2636,7 @@ extern "C" int dmd_actor_critic_forward(dmd_actor_critic* h, int B, const float*
   cudaStream_t st = (cudaStream_t)stream;
   AcBuffers b; ac_layout(h, B, (uint8_t*)workspace, &b);
   DMD_CHECK(workspace_bytes >= b.total, "ac forward: workspace too small (%zu < %zu)", workspace_bytes, b.total);
+  const bool det = m.det;
   DMD_CUDA(cudaMemsetAsync(b.stats, 0, b.stats_bytes, st));
   int S = c.img_size;
   if (dmd_nchw_to_nhwc(obs, b.x0, B, c.img_channels, h->conv0.c0_store, S * S, st)) return 1;
@@ -2590,12 +2650,12 @@ extern "C" int dmd_actor_critic_forward(dmd_actor_critic* h, int B, const float*
     d.B = B; d.H = hw; d.W = hw; d.taps = cw.taps; d.stride = 1;
     d.wpk = m.packed + cw.pk_off; d.bias = m.ptrs[cw.b_idx]; d.Cout = cw.Cout; d.CoutPad = cw.CoutPad;
     d.residual = resid; d.out = out; d.out_stats = st_out; d.out_gs = gn_group_size(cw.Cout);
-    const bool stats_after = st_out && !conv_epilogue_stats_fit(hw, hw);   // as PlanBuilder::conv
+    const bool stats_after = st_out && (det || !conv_epilogue_stats_fit(hw, hw));   // as PlanBuilder::conv
     if (stats_after) d.out_stats = nullptr;
     const size_t plane = (size_t)plc_geometry(B, hw, hw).Qalloc * 16;   // one PLC16 plane holds 8 channels
     if (for_each_conv_launch(cw, d, plane, [&](size_t off) { return m.packed + off; },
                              [&](const dmd_conv_desc& dc) { return dmd_conv2d_fprop(&dc, st); })) return 1;
-    return stats_after ? dmd_gn_stats(out, st_out, B, hw * hw, cw.Cout, d.out_gs, st) : 0;
+    return stats_after ? gn_stats_launch(out, st_out, B, hw * hw, cw.Cout, d.out_gs, det, st) : 0;
   };
   // conv0 feeds the first GroupNorm -> statistics in its epilogue
   if (run_conv(h->conv0, b.x0, h->conv0.c0_store, S, 0, 0, 0, nullptr, nullptr, b.pooled[0], b.st_in[0])) return 1;
@@ -2608,8 +2668,9 @@ extern "C" int dmd_actor_critic_forward(dmd_actor_critic* h, int B, const float*
     double* st_y = lv.down ? nullptr : b.st_in[i + 1];
     if (run_conv(lv.conv, x, lv.cin, S, 2, lv.gn_w, lv.gn_b, b.st_in[i], r, b.y[i], st_y)) return 1;
     if (lv.down) {
-      if (maxpool2_stats_launch(b.y[i], b.pooled[i + 1], i + 1 < h->levels.size() ? b.st_in[i + 1] : nullptr, B, S, S, lv.cout,
-                                gn_group_size(lv.cout), st)) return 1;
+      double* st_pool = i + 1 < h->levels.size() ? b.st_in[i + 1] : nullptr;
+      if (maxpool2_stats_launch(b.y[i], b.pooled[i + 1], det ? nullptr : st_pool, B, S, S, lv.cout, gn_group_size(lv.cout), st)) return 1;
+      if (det && st_pool && gn_stats_launch(b.pooled[i + 1], st_pool, B, (S / 2) * (S / 2), lv.cout, gn_group_size(lv.cout), true, st)) return 1;
       S /= 2;
     }
   }
@@ -2631,7 +2692,7 @@ extern "C" int dmd_actor_critic_forward(dmd_actor_critic* h, int B, const float*
 namespace {
 
 struct AcScratch {
-  float *g_a, *g_b, *tA; uint8_t *gy_op, *x_op; float *dgates, *g_h, *g_xflat, *x_flat, *nsum, *scale, *partial; unsigned int* amax; size_t total;
+  float *g_a, *g_b, *tA; uint8_t *gy_op, *x_op; float *dgates, *g_h, *g_xflat, *x_flat, *nsum, *scale, *partial; unsigned int* amax; size_t total, partial_bytes;
 };
 int ac_scratch_layout(const dmd_actor_critic* h, int B, uint8_t* base, AcScratch* o) {
   const dmd_actor_critic_config& c = h->cfg;
@@ -2646,7 +2707,8 @@ int ac_scratch_layout(const dmd_actor_critic* h, int B, uint8_t* base, AcScratch
   o->nsum = (float*)bb.take((size_t)2 * B * kMaxCin * 4);
   o->scale = (float*)bb.take(256); o->amax = (unsigned int*)bb.take(256);
   if (init_kernels()) return 1;
-  o->partial = (float*)bb.take(wgrad_partial_bytes(g_num_sms));
+  o->partial_bytes = wgrad_partial_bytes(g_num_sms);
+  o->partial = (float*)bb.take(o->partial_bytes);
   o->total = bb.off + 256;
   return 0;
 }
@@ -2698,7 +2760,7 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
     return sgemm_launch(Am, sam, sak, Bm, sbk, sbn, C, ldc, M, N, Kd, nullptr, acc, 0, nullptr, st);
   };
   auto colsum = [&](const float* x, long long rows, int C, int Creal, float* out, float* out2, const float* inv) -> int {
-    return colsum_launch(x, out, out2, inv, rows, C, Creal, st);
+    return colsum_launch(x, out, out2, inv, rows, C, Creal, st, m.det ? sc.partial : nullptr, sc.partial_bytes);
   };
   if (!accumulate) DMD_CUDA(cudaMemsetAsync(grads, 0, (size_t)m.grad_total * 4, st));
   DMD_CUDA(cudaMemsetAsync(sc.amax, 0, 256, st));
@@ -2757,7 +2819,7 @@ static int ac_backward_impl(dmd_actor_critic* h, int B, const float* hx_in, cons
     const NormBwdParams nb = gn_bwd_params(b.pooled[i], sc.tA, b.st_in[i], B, S * S, lv.cin, gn_group_size(lv.cin), m.P(lv.gn_w),
                                            m.P(lv.gn_b), sc.nsum, gx, lv.has_skip ? nullptr : gy, false);
     DMD_CUDA(cudaMemsetAsync(sc.nsum, 0, (size_t)2 * B * kMaxCin * 4, st));
-    if (norm_bwd_launch(nb, 1, st) || affine_param_grad_launch(nb, G(lv.gn_w), G(lv.gn_b), inv, st) || norm_bwd_launch(nb, 2, st)) return 1;
+    if (norm_bwd_launch(nb, 1, st, m.det) || affine_param_grad_launch(nb, G(lv.gn_w), G(lv.gn_b), inv, st) || norm_bwd_launch(nb, 2, st)) return 1;
     if (lv.has_skip) {  // 1x1 skip projection on the raw input
       pd = prep_desc(b.pooled[i], lv.cin, B, S, S, 0, 0, nullptr, nullptr, nullptr, sc.x_op);
       if (dmd_prep_act(&pd, st)) return 1;
@@ -2855,9 +2917,9 @@ __global__ void merge_logits_kernel(const float* __restrict__ g_rew, const float
 int rew_end_layout(const dmd_rew_end* h, int B, uint8_t* base, RewEndLayout* o, size_t* total) {
   const int S = h->cfg.img_size;
   Plan& pl = o->plan;
-  pl.train = false; pl.B = B; pl.H = S; pl.W = S; pl.ops.clear();
+  pl.train = false; pl.B = B; pl.H = S; pl.W = S; pl.det = h->core.det; pl.ops.clear();
   Bump b0{nullptr}, s0{nullptr};
-  { Plan tmp; tmp.B = B; tmp.H = S; tmp.W = S; PlanBuilder pb{&h->core, &tmp, &b0, &s0}; if (pb.build_rew_end(h, &o->feat)) return 1; }
+  { Plan tmp; tmp.B = B; tmp.H = S; tmp.W = S; tmp.det = h->core.det; PlanBuilder pb{&h->core, &tmp, &b0, &s0}; if (pb.build_rew_end(h, &o->feat)) return 1; }
   const size_t stats_bytes = (s0.off + 255) & ~(size_t)255;
   Bump sb{base}, bb{base ? base + stats_bytes : nullptr};
   if (base) {
@@ -2924,7 +2986,7 @@ int rew_end_encode(const dmd_rew_end* h, Plan& pl, int b, int t, const float* ob
   for (const Op& op : pl.ops) {
     if (op.kind == OP_CONV) { if (conv_launch(op.conv, op.smem, op.cols, st)) return 1; }
     else if (op.kind == OP_PREP) { if (prep_launch(op.prep, op.prep_nsrc, st)) return 1; }
-    else if (op.kind == OP_STATS) { if (dmd_gn_stats(op.gn.x, op.gn.stats, pl.B, op.gn.HW, op.gn.C, op.gn.gs, st)) return 1; }
+    else if (op.kind == OP_STATS) { if (gn_stats_launch(op.gn.x, op.gn.stats, pl.B, op.gn.HW, op.gn.C, op.gn.gs, pl.det, st)) return 1; }
     else { if (attn_launch(op.attn, pl.B, st)) return 1; }
   }
   return 0;
@@ -3038,7 +3100,7 @@ int rew_end_predict(dmd_rew_end* h, int b, int t, const float* obs, const float*
   const int rows = b * t, D = c.lstm_dim;
   RewEndLayout& o = h->lay;
   Plan& pl = o.plan;
-  if (pl.B != rows || pl.base != (uint8_t*)workspace) {
+  if (pl.B != rows || pl.base != (uint8_t*)workspace || pl.det != h->core.det) {
     // size and validate on a scratch layout; the cached one is invalidated (never left half-written) if the real build fails
     size_t need = 0;
     { RewEndLayout tmp; if (rew_end_layout(h, rows, nullptr, &tmp, &need)) return 1; }
@@ -3158,7 +3220,7 @@ int rew_end_backward_impl(const char* who, dmd_rew_end* h, int b, int t, const f
                           float* g_hx_in, float* g_cx_in, void* workspace, void* stream) {
   DMD_CHECK(h && g_logits_rew && g_logits_end && grads && workspace, "%s: null argument", who);
   const dmd_rew_end_config& c = h->cfg;
-  Plan* plp = (b > 0 && t > 0) ? find_train_plan(h->core, b * t, c.img_size, c.img_size, t, workspace) : nullptr;
+  Plan* plp = (b > 0 && t > 0) ? find_train_plan(h->core, b * t, c.img_size, c.img_size, t, workspace, true) : nullptr;
   DMD_CHECK(plp && plp->train, "%s: no matching dmd_rew_end_forward_train on this workspace (b=%d t=%d)", who, b, t);
   const ModelCore& m = h->core;
   DMD_CHECK(grads_numel >= m.grad_total, "%s: gradient buffer too small (%lld < %lld floats)", who, grads_numel, m.grad_total);
@@ -3182,7 +3244,7 @@ int rew_end_backward_impl(const char* who, dmd_rew_end* h, int b, int t, const f
   if (linear_launch(y, m.ptrs[h->i_h0w], m.ptrs[h->i_h0b], pl.hpre, rows, D, D, 0, st)) return 1;  // the forward's pre-activation
   if (dsilu_mul_launch(pl.hpre, pl.g_hid, pl.g_pre, (long long)rows * D, st)) return 1;
   if (sgemm(pl.g_pre, 1, D, y, D, 1, G(h->i_h0w), D, D, D, rows, 1)) return 1;                    // dW0 += g_pre^T y
-  if (colsum_launch(pl.g_pre, G(h->i_h0b), nullptr, nullptr, rows, D, D, st)) return 1;
+  if (colsum_launch(pl.g_pre, G(h->i_h0b), nullptr, nullptr, rows, D, D, st, pl.det ? pl.partial : nullptr, pl.partial_bytes)) return 1;
   if (sgemm(pl.g_pre, D, 1, m.ptrs[h->i_h0w], D, 1, pl.g_y, D, rows, D, D, 0)) return 1;          // g_y = g_pre W0
   // ---- LSTM (rew_end_model.py:53), back through time: g_h of step k = g_y[k] (+ g_hx_out at the last step) + dgates_{k+1} W_hh
   const float* Whh = m.ptrs[h->i_whh];
@@ -3206,7 +3268,7 @@ int rew_end_backward_impl(const char* who, dmd_rew_end* h, int b, int t, const f
   if (dmd_nhwc_to_nchw(pl.feat.data, x_flat, rows, h->feat_c, h->feat_c, h->feat_hw, st)) return 1;
   if (sgemm(pl.dgates, 1, 4 * D, x_flat, K, 1, G(h->i_wih), K, 4 * D, K, rows, 1)) return 1;     // dW_ih += dgates^T x
   if (sgemm(pl.dgates, 1, 4 * D, pl.hseq, D, 1, G(h->i_whh), D, 4 * D, D, rows, 1)) return 1;    // dW_hh += dgates^T [h_in; y[:-1]]
-  if (colsum_launch(pl.dgates, G(h->i_bih), G(h->i_bhh), nullptr, rows, 4 * D, 4 * D, st)) return 1;
+  if (colsum_launch(pl.dgates, G(h->i_bih), G(h->i_bhh), nullptr, rows, 4 * D, 4 * D, st, pl.det ? pl.partial : nullptr, pl.partial_bytes)) return 1;
   if (sgemm(pl.dgates, 4 * D, 1, m.ptrs[h->i_wih], K, 1, g_x, K, rows, K, 4 * D, 0)) return 1;   // g_x = dgates W_ih
   // ---- encoder: the feature gradient enters the fp16 tensor-core path with a loss scale, NHWC in the last tensor's gradient
   if (loss_scale_launch(g_x, (long long)rows * K, pl.amax, pl.scale, st)) return 1;

@@ -391,6 +391,61 @@ __global__ void embedding_bwd_kernel(const float* __restrict__ de, const int64_t
   atomicAdd(dE + (size_t)a * E + (k % E), de[i] * (inv_scale ? *inv_scale : 1.f));
 }
 
+// ------------------------------------------------------------------------------------------------ deterministic arms
+// What torch.use_deterministic_algorithms selects in place of the fp32 atomics above: every sum has one owner and a fixed order.
+
+// colsum_kernel's row chunks, each block's column sums stored (unscaled) to part[blockIdx.x][C] instead of added to `out`
+__global__ void __launch_bounds__(256) colsum_part_kernel(const float* __restrict__ x, float* __restrict__ part, long long rows, int C) {
+  __shared__ float cs_sm[1024];
+  const int cbase = blockIdx.y * 256;
+  const int Cb = min(256, C - cbase);
+  const int L4 = Cb >> 2;
+  const int lanes = 256 / L4;
+  const int c4 = threadIdx.x % L4, rl = threadIdx.x / L4;
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (rl < lanes) {
+    for (long long r = (long long)blockIdx.x * lanes + rl; r < rows; r += (long long)gridDim.x * lanes) {
+      const float4 v = __ldg(reinterpret_cast<const float4*>(x + r * C + cbase) + c4);
+      acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+    }
+    reinterpret_cast<float4*>(cs_sm + (size_t)rl * Cb)[c4] = acc;
+  }
+  __syncthreads();
+  if ((int)threadIdx.x < Cb) {
+    float s = 0.f;
+    for (int k = 0; k < lanes; ++k) s += cs_sm[(size_t)k * Cb + threadIdx.x];
+    part[(size_t)blockIdx.x * C + cbase + threadIdx.x] = s;
+  }
+}
+// out[c] (and out2[c]) += inv_scale * sum over the nparts block sums of part, in block order
+__global__ void colsum_reduce_kernel(const float* __restrict__ part, int nparts, int C, int Creal, float* __restrict__ out,
+                                     float* __restrict__ out2, const float* __restrict__ inv_scale) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= Creal) return;
+  float s = 0.f;
+  for (int b = 0; b < nparts; ++b) s += part[(size_t)b * C + c];
+  s *= inv_scale ? *inv_scale : 1.f;
+  out[c] += s;
+  if (out2) out2[c] += s;
+}
+
+// embedding_bwd_kernel gathered: one thread per table entry (a, j) walks the batch rows and their T actions in order
+__global__ void embedding_bwd_det_kernel(const float* __restrict__ de, const int64_t* __restrict__ act, float* __restrict__ dE,
+                                         int B, int CC, int T, int num_actions, const float* __restrict__ inv_scale) {
+  const int E = CC / T;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= num_actions * E) return;
+  const int a = i / E, j = i - a * E;
+  float s = 0.f;
+  for (int n = 0; n < B; ++n)
+    for (int t = 0; t < T; ++t) {
+      long long an = act[(size_t)n * T + t];
+      an = an < 0 ? 0 : (an >= num_actions ? num_actions - 1 : an);
+      if (an == a) s += de[(size_t)n * CC + t * E + j] * (inv_scale ? *inv_scale : 1.f);
+    }
+  dE[i] += s;
+}
+
 // ------------------------------------------------------------------------------------------------ attention backward
 // SelfAttention2d (blocks.py:51-72) backward, one CTA per image (L <= 64 tokens, C in {32, 64}, head_dim 8).  kL = 64: the
 // token count is a compile-time constant (the 8x8 level of a 64x64 frame); kL = 0: any L from 1 to 64, read from p.L, the same

@@ -76,6 +76,8 @@ class NativeStateMixin:
             arr = (C.c_void_p * n)(*[t.data_ptr() for t in tensors])
             _lib.check(getattr(lib, pre + "set_weights")(self._h, arr, n, self._packed.data_ptr(), _lib.current_stream()))
             self._wkey = wkey
+        # torch.use_deterministic_algorithms selects the native fixed-order reductions; the handle keys its plans on it
+        _lib.check(getattr(lib, pre + "set_deterministic")(self._h, int(torch.are_deterministic_algorithms_enabled())))
         return self._h
 
     def _native(self):

@@ -339,6 +339,13 @@ size_t dmd_denoiser_packed_bytes(const dmd_denoiser* h);
 /* ptrs_host: host array of device pointers, in InnerModel.state_dict() order (fp32, torch layouts).
  * Re-packs the tensor-core copies; call again after every optimizer step / load_state_dict. */
 int dmd_denoiser_set_weights(dmd_denoiser* h, const float* const* ptrs_host, int n_ptrs, void* packed, void* stream);
+/* Deterministic mode (on != 0; torch.are_deterministic_algorithms_enabled() on the Python side, which sets it before every
+ * call): every forward, sampler and backward call of the handle is bit-reproducible on the same GPU model and build, whatever
+ * the workspace address, the CTA schedule or other work on the GPU.  GroupNorm statistics, bias / affine / FiLM / embedding
+ * gradients and the attention parameter gradients then come from fixed-order reductions instead of atomics.  The mode is part
+ * of every cached plan's and sampler graph's key; off (the default) runs exactly the kernels it always did.  The same holds
+ * for dmd_rew_end_set_deterministic and dmd_actor_critic_set_deterministic. */
+int dmd_denoiser_set_deterministic(dmd_denoiser* h, int on);
 
 /* H, W need not be multiples of 2^(levels-1): like UNet.forward (blocks.py:225-229,245) the executor zero-pads the conv_in
  * output at the bottom / right, runs the U-Net on the padded size and crops before norm_out / conv_out (inference entry
@@ -446,6 +453,7 @@ void dmd_actor_critic_destroy(dmd_actor_critic* h);
 int dmd_actor_critic_num_tensors(const dmd_actor_critic* h);          /* == len(ActorCritic.state_dict()) */
 size_t dmd_actor_critic_packed_bytes(const dmd_actor_critic* h);
 int dmd_actor_critic_set_weights(dmd_actor_critic* h, const float* const* ptrs_host, int n_ptrs, void* packed, void* stream);
+int dmd_actor_critic_set_deterministic(dmd_actor_critic* h, int on);
 size_t dmd_actor_critic_workspace_bytes(const dmd_actor_critic* h, int B);
 /* obs (B,C,S,S) NCHW; hx_in/cx_in (B,lstm_dim); outputs: logits (B,A), val (B), hx_out/cx_out (B,lstm_dim). */
 int dmd_actor_critic_forward(dmd_actor_critic* h, int B, const float* obs, const float* hx_in, const float* cx_in,
@@ -497,6 +505,7 @@ void dmd_rew_end_destroy(dmd_rew_end* h);
 int dmd_rew_end_num_tensors(const dmd_rew_end* h);           /* == len(RewEndModel.state_dict()) */
 size_t dmd_rew_end_packed_bytes(const dmd_rew_end* h);
 int dmd_rew_end_set_weights(dmd_rew_end* h, const float* const* ptrs_host, int n_ptrs, void* packed, void* stream);
+int dmd_rew_end_set_deterministic(dmd_rew_end* h, int on);
 size_t dmd_rew_end_workspace_bytes(const dmd_rew_end* h, int rows);  /* rows = b * t */
 /* obs / next_obs (b, t, C, S, S), act (b, t) int64, hx_in / cx_in (b, lstm_dim) or NULL (zero state).
  * logits_rew (b, t, 3), logits_end (b, t, 2), hx_out / cx_out (b, lstm_dim). */
