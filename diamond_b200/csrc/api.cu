@@ -1074,10 +1074,12 @@ struct ModelCore {
     film_boff_off = pk; pk += (size_t)film_rows * 8; pk = (pk + 255) & ~(size_t)255;
     packed_bytes = pk;
   }
-  int upload_film_offsets(cudaStream_t st) const {
+  const uint8_t* film_offsets_at = nullptr;   // the packed buffer the offset tables were last uploaded into
+  int upload_film_offsets(cudaStream_t st) {
     if (film_rows == 0) return 0;
     DMD_CUDA(cudaMemcpyAsync(packed + film_woff_off, film_woff_h.data(), (size_t)film_rows * 8, cudaMemcpyHostToDevice, st));
     DMD_CUDA(cudaMemcpyAsync(packed + film_boff_off, film_boff_h.data(), (size_t)film_rows * 8, cudaMemcpyHostToDevice, st));
+    film_offsets_at = packed;
     return 0;
   }
   // adopts the caller's tensors (`module`.state_dict() order); *moved: a tensor or the packed buffer is not where it was
@@ -2103,19 +2105,43 @@ static int pack_rb(const ModelCore& m, const ResBlockW& r, cudaStream_t st) {
   return 0;
 }
 
-extern "C" int dmd_denoiser_set_weights(dmd_denoiser* h, const float* const* ptrs_host, int n_ptrs, void* packed, void* stream) {
-  DMD_CHECK(h, "set_weights: null argument");
-  cudaStream_t st = (cudaStream_t)stream;
-  bool moved = false;
-  if (h->core.set_weights("InnerModel", ptrs_host, n_ptrs, packed, &moved)) return 1;
-  if (moved) { h->plan.B = 0; h->core.tplans.clear(); for (auto& g : h->graphs) g.valid = false; }
+static int pack_denoiser(const dmd_denoiser* h, cudaStream_t st) {
   const ModelCore& m = h->core;
-  if (m.upload_film_offsets(st) || pack_one(m, h->conv_in, st) || pack_one(m, h->conv_out, st)) return 1;
+  if (pack_one(m, h->conv_in, st) || pack_one(m, h->conv_out, st)) return 1;
   for (auto& lv : h->d_blocks) for (auto& r : lv) if (pack_rb(m, r, st)) return 1;
   for (auto& lv : h->u_blocks) for (auto& r : lv) if (pack_rb(m, r, st)) return 1;
   for (auto& r : h->mid) if (pack_rb(m, r, st)) return 1;
   for (int i = 1; i < h->cfg.num_levels; ++i) if (pack_one(m, h->downs[i], st) || pack_one(m, h->ups[i], st)) return 1;
   return 0;
+}
+
+// A CUDA graph the caller captures (torch.compile's cudagraphs) replays without the host-side check that re-packs changed
+// weights: the inference entry points therefore enqueue the packs as the first captured work whenever `st` is capturing, and
+// every replay packs the fp32 parameters as they are then.  Inside a capture set_weights only adopts the tensors; the FiLM
+// offset tables (a pageable host->device copy) must already be on the device from an uncaptured call into the same buffer.
+static int stream_capturing(cudaStream_t st, bool* on) {
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  DMD_CUDA(cudaStreamIsCapturing(st, &cap));
+  *on = cap != cudaStreamCaptureStatusNone;
+  return 0;
+}
+static int set_weights_tail(ModelCore& m, cudaStream_t st, bool* pack_now) {
+  bool cap = false;
+  if (stream_capturing(st, &cap)) return 1;
+  DMD_CHECK(!cap || m.film_rows == 0 || m.film_offsets_at == m.packed,
+            "set_weights: the first call with a packed buffer cannot be captured (its FiLM offset tables are a host upload)");
+  *pack_now = !cap;
+  return cap ? 0 : m.upload_film_offsets(st);
+}
+
+extern "C" int dmd_denoiser_set_weights(dmd_denoiser* h, const float* const* ptrs_host, int n_ptrs, void* packed, void* stream) {
+  DMD_CHECK(h, "set_weights: null argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  bool moved = false, pack_now = false;
+  if (h->core.set_weights("InnerModel", ptrs_host, n_ptrs, packed, &moved)) return 1;
+  if (moved) { h->plan.B = 0; h->core.tplans.clear(); for (auto& g : h->graphs) g.valid = false; }
+  if (set_weights_tail(h->core, st, &pack_now)) return 1;
+  return pack_now ? pack_denoiser(h, st) : 0;
 }
 
 // deterministic mode: plans, sampler graphs and workspace queries made while it is on use the fixed-order arms
@@ -2464,9 +2490,10 @@ extern "C" int dmd_sampler_sample(dmd_denoiser* h, const dmd_sampler_config* sc,
     const long long chw = (long long)c.img_channels * H * W;
     io.sv = StackView{T, ring_head, (long long)B * chw, chw, (long long)B, 1};
   }
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  DMD_CUDA(cudaStreamIsCapturing(st, &cap));
-  if (!use_graph || cap != cudaStreamCaptureStatusNone) return sampler_body(h, sc, io, st);
+  bool cap = false;
+  if (stream_capturing(st, &cap)) return 1;
+  if (cap) return pack_denoiser(h, st) || sampler_body(h, sc, io, st);   // inside the caller's graph: no graph of our own
+  if (!use_graph) return sampler_body(h, sc, io, st);
 
   const float churn[4] = {sc->s_churn, sc->s_tmin, sc->s_tmax, sc->s_noise};
   SamplerGraph* g = nullptr;
@@ -3067,17 +3094,22 @@ extern "C" void dmd_rew_end_destroy(dmd_rew_end* h) { delete h; }
 extern "C" int dmd_rew_end_num_tensors(const dmd_rew_end* h) { return h->core.n_tensors; }
 extern "C" size_t dmd_rew_end_packed_bytes(const dmd_rew_end* h) { return h->core.packed_bytes; }
 
-extern "C" int dmd_rew_end_set_weights(dmd_rew_end* h, const float* const* ptrs_host, int n_ptrs, void* packed, void* stream) {
-  DMD_CHECK(h, "set_weights: null argument");
-  cudaStream_t st = (cudaStream_t)stream;
-  bool moved = false;
-  if (h->core.set_weights("RewEndModel", ptrs_host, n_ptrs, packed, &moved)) return 1;
-  if (moved) { h->lay.plan.B = 0; h->core.tplans.clear(); }   // plans bake parameter and packed-weight addresses in
+static int pack_rew_end(const dmd_rew_end* h, cudaStream_t st) {
   const ModelCore& m = h->core;
-  if (m.upload_film_offsets(st) || pack_one(m, h->conv_in, st)) return 1;
+  if (pack_one(m, h->conv_in, st)) return 1;
   for (auto& lv : h->blocks) for (auto& r : lv) if (pack_rb(m, r, st)) return 1;
   for (int i = 1; i < h->cfg.num_levels; ++i) if (pack_one(m, h->downs[i], st)) return 1;
   return 0;
+}
+
+extern "C" int dmd_rew_end_set_weights(dmd_rew_end* h, const float* const* ptrs_host, int n_ptrs, void* packed, void* stream) {
+  DMD_CHECK(h, "set_weights: null argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  bool moved = false, pack_now = false;
+  if (h->core.set_weights("RewEndModel", ptrs_host, n_ptrs, packed, &moved)) return 1;
+  if (moved) { h->lay.plan.B = 0; h->core.tplans.clear(); }   // plans bake parameter and packed-weight addresses in
+  if (set_weights_tail(h->core, st, &pack_now)) return 1;
+  return pack_now ? pack_rew_end(h, st) : 0;
 }
 
 extern "C" size_t dmd_rew_end_workspace_bytes(const dmd_rew_end* h, int rows) {
@@ -3107,6 +3139,8 @@ int rew_end_predict(dmd_rew_end* h, int b, int t, const float* obs, const float*
     DMD_CHECK(workspace_bytes >= need, "rew_end predict: workspace too small (%zu < %zu)", workspace_bytes, need);
     if (rew_end_layout(h, rows, (uint8_t*)workspace, &o, nullptr)) { pl.B = 0; pl.base = nullptr; pl.ops.clear(); return 1; }
   }
+  bool cap = false;
+  if (stream_capturing(st, &cap) || (cap && pack_rew_end(h, st))) return 1;
   if (rew_end_encode(h, pl, b, t, obs, next_obs, act, nullptr, st, u8)) return 1;
   const float* hprev = hx_in; const float* cprev = cx_in;
   if (!hx_in) { DMD_CUDA(cudaMemsetAsync(o.hc[0], 0, (size_t)b * D * 4, st)); hprev = o.hc[0]; }

@@ -18,7 +18,9 @@ from torch import Tensor
 from torch.distributions.categorical import Categorical
 
 from .. import frames as frames_u8
+from .. import torch_ops
 from ..models.diffusion import Denoiser, DiffusionSampler, DiffusionSamplerConfig
+from ..models.rew_end_model import RewEndModel
 
 ResetOutput = Tuple[torch.FloatTensor, Dict[str, Any]]
 StepOutput = Tuple[Tensor, Tensor, Tensor, Tensor, Dict[str, Any]]
@@ -131,7 +133,19 @@ class WorldModelEnv:
         self._write_stacks(slice(None), obs, act)
         self.hx_rew_end, self.cx_rew_end = hx.clone(), cx.clone()
         self.ep_len = torch.zeros(self.num_envs, dtype=torch.long, device=obs.device)
+        self._prepare_compiled_calls()
         return self._frames[self._slot(t - 1)].clone(), {}
+
+    def _prepare_compiled_calls(self) -> None:
+        """predict_next_obs / predict_rew_end may be compiled (trainer.py:182-184).  What they keep between calls is made here,
+        outside the compiled region: the sampler's buffers, both native handles, their workspaces and op keys.  The rings and
+        the carried LSTM state are marked static, so CUDA graphs read and write them in place."""
+        if self._use_ring_sampler and "sample" not in self.sampler.__dict__:
+            self.sampler.prepare_ring(self._frames)
+        if isinstance(self.rew_end_model, RewEndModel):
+            self.rew_end_model.predict_workspace(self.num_envs)
+            torch_ops.key_of(self.rew_end_model)
+        torch_ops.mark_static(self._frames, self._acts, self.hx_rew_end, self.cx_rew_end)
 
     @torch.no_grad()
     def reset_dead(self, dead: torch.BoolTensor) -> None:  # world_model_env.py:55-62
@@ -178,7 +192,7 @@ class WorldModelEnv:
         if self._use_ring_sampler and "sample" not in self.sampler.__dict__:
             # native path: the sampler reads the ring in place; the new frame lands in the slot that is about to be freed.
             # It is still logical slot 0 (read by every denoising step) -- the final Euler update writes it last, in stream order.
-            traj = self.sampler.sample_ring(self._frames, self._acts, self._head, self._frames[self._head])
+            traj = self.sampler.sample_ring(self._frames, self._acts, self._head)
             return self._frames[self._head], traj.unbind(0)
         return self.sampler.sample(self.obs_buffer, self.act_buffer)
 
@@ -186,8 +200,15 @@ class WorldModelEnv:
     def predict_rew_end(self, next_obs: Tensor) -> Tuple[Tensor, Tensor]:  # world_model_env.py:95-105
         t = self._frames.size(0)
         last = self._slot(t - 1)
-        logits_rew, logits_end, (self.hx_rew_end, self.cx_rew_end) = self.rew_end_model.predict_rew_end(
+        logits_rew, logits_end, (hx, cx) = self.rew_end_model.predict_rew_end(
             self._frames[last].unsqueeze(1), self._acts[last].unsqueeze(1), next_obs, (self.hx_rew_end, self.cx_rew_end))
+        if torch.compiler.is_compiling():
+            # a CUDA graph's outputs are overwritten by its next replay: the carried state stays in the static buffers made by
+            # reset, which reset_dead writes in place between replays
+            self.hx_rew_end.copy_(hx)
+            self.cx_rew_end.copy_(cx)
+        else:
+            self.hx_rew_end, self.cx_rew_end = hx, cx
         rew = Categorical(logits=logits_rew, validate_args=False).sample().squeeze(1) - 1.0  # {-1, 0, 1}
         end = Categorical(logits=logits_end, validate_args=False).sample().squeeze(1)
         return rew, end

@@ -6,7 +6,7 @@ from typing import List, Tuple
 import torch
 from torch import Tensor
 
-from ... import _lib
+from ... import _lib, torch_ops
 from .denoiser import Denoiser
 
 
@@ -46,6 +46,7 @@ class DiffusionSampler:
         self._sc = _lib.SamplerConfigC(self._n_sig, self._sig_arr, int(cfg.order), float(cfg.s_churn), float(cfg.s_tmin),
                                        float(min(cfg.s_tmax, 3.0e38)), 1.0)
         self._gamma = min(cfg.s_churn / (self._n_sig - 1), 2**0.5 - 1)
+        self._ws_bytes = {}   # (b, h, w, deterministic) -> the denoiser's inference workspace size
         self._buf = {}   # persistent device buffers per (B, C, H, W): the native call (a CUDA graph) uses them in place
 
     def _buffers(self, b: int, t: int, c: int, h: int, w: int, device):
@@ -73,14 +74,24 @@ class DiffusionSampler:
                 if self.cfg.s_tmin <= sigma <= self.cfg.s_tmax:
                     eps[i].copy_(torch.randn(*traj.shape[1:], device=traj.device) * self.cfg.s_noise)
 
-    def _run(self, obs: Tensor, act: Tensor, ring_head: int, buf, out_x, b: int, h: int, w: int) -> None:
+    def _workspace(self, b: int, h: int, w: int) -> Tensor:
+        """The denoiser's inference workspace for (b, h, w).  Its size is asked of the native layer once per shape and mode, so
+        that a compiled caller traces this as plain attribute reads (the shape is seen first by WorldModelEnv.reset)."""
+        im = self.denoiser.inner_model
+        key = (b, h, w, torch.are_deterministic_algorithms_enabled())
+        sizes = self._ws_bytes
+        if key not in sizes:
+            den = self.denoiser
+            sizes[key] = _lib.lib().dmd_denoiser_workspace_bytes(im.native(den.cfg.sigma_data, den.cfg.sigma_offset_noise), b, h, w)
+        return im.workspace(sizes[key])
+
+    def _sample_native(self, obs: Tensor, act: Tensor, ring_head: int, traj: Tensor, eps, out_x, ws: Tensor) -> None:
         lib = _lib.lib()
         den = self.denoiser
-        im = den.inner_model
-        hnd = im.native(den.cfg.sigma_data, den.cfg.sigma_offset_noise)
-        ws = im.workspace(lib.dmd_denoiser_workspace_bytes(hnd, b, h, w))
+        hnd = den.inner_model.native(den.cfg.sigma_data, den.cfg.sigma_offset_noise)
+        b, h, w = traj.shape[1], traj.shape[3], traj.shape[4]
         _lib.check(lib.dmd_sampler_sample(hnd, C.byref(self._sc), b, h, w, obs.data_ptr(), act.data_ptr(), ring_head,
-                                          buf["traj"].data_ptr(), _lib.ptr(buf["eps"]), _lib.ptr(out_x), ws.data_ptr(), ws.numel(),
+                                          traj.data_ptr(), _lib.ptr(eps), _lib.ptr(out_x), ws.data_ptr(), ws.numel(),
                                           int(self.use_cuda_graph), _lib.current_stream()))
 
     @torch.no_grad()
@@ -91,18 +102,30 @@ class DiffusionSampler:
         buf["obs"].copy_(prev_obs.reshape(b, t * c, h, w))   # stable addresses: the captured graph is replayed as is
         buf["act"].copy_(prev_act)
         self._draw_noise(buf)
-        self._run(buf["obs"], buf["act"], -1, buf, None, b, h, w)
+        self._sample_native(buf["obs"], buf["act"], -1, buf["traj"], buf["eps"], None, self._workspace(b, h, w))
         traj = buf["traj"].clone()                           # the caller owns what it gets; the buffers are reused next call
         return traj[-1], list(traj.unbind(0))
 
+    def prepare_ring(self, frames: Tensor) -> None:
+        """Creates what sample_ring(frames, ...) keeps between calls -- its buffers, the native handle with packed weights and
+        the workspace -- outside any compiled region, and marks the buffers static for the CUDA graphs of a compiled caller."""
+        t, b, c, h, w = frames.size()
+        self._check_stack(t, c)
+        buf = self._buffers(b, t, c, h, w, frames.device)
+        self._workspace(b, h, w)
+        torch_ops.key_of(self)
+        torch_ops.mark_static(buf["traj"], buf["eps"])
+
     @torch.no_grad()
-    def sample_ring(self, frames: Tensor, acts: Tensor, head: int, out_frame: Tensor) -> Tensor:
+    def sample_ring(self, frames: Tensor, acts: Tensor, head: int) -> Tensor:
         """The WorldModelEnv path: `frames` (T, B, C, H, W) / `acts` (T, B) are the environment's resident ring buffers with
-        logical slot k at physical slot (head + k) % T; the new frame is written straight into `out_frame` (a ring slot).
-        Nothing is staged or rolled.  Returns the trajectory buffer (num_sigmas, B, C, H, W), valid until the next call."""
+        logical slot k at physical slot (head + k) % T; the new frame is written straight into the ring slot `frames[head]`.
+        Nothing is staged or rolled.  Returns the trajectory buffer (num_sigmas, B, C, H, W), valid until the next call.
+        One `diamond_b200::sample_ring` op, so that torch.compile traces it whole."""
         t, b, c, h, w = frames.size()
         self._check_stack(t, c)
         buf = self._buffers(b, t, c, h, w, frames.device)
         self._draw_noise(buf)
-        self._run(frames, acts, head, buf, out_frame, b, h, w)
+        torch_ops.sample_ring(torch_ops.key_of(self), frames, acts, head, buf["traj"], buf["eps"], self._workspace(b, h, w),
+                              self.denoiser.inner_model._state_tensors())
         return buf["traj"]

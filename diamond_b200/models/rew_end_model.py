@@ -19,7 +19,7 @@ import torch.nn.functional as F
 from torch import Tensor
 from torch.autograd.function import once_differentiable
 
-from .. import _lib
+from .. import _lib, torch_ops
 from .. import frames as frames_u8
 from ..utils import NativeStateMixin, init_lstm
 from .blocks import Downsample, ResBlocks, _NativeOnly, conv3x3
@@ -79,6 +79,7 @@ class RewEndModel(NativeStateMixin, nn.Module):
 
     # a training workspace holds one forward's activations until its backward has run
     _WS_POOL_CAP = 2
+    _ws_bytes = None   # rows, deterministic -> inference workspace size
 
     def predict_rew_end(self, obs: Tensor, act: Tensor, next_obs: Tensor, hx_cx: Optional[Tuple[Tensor, Tensor]] = None,
                         kinds: Optional[Tuple[Tensor, Tensor]] = None) -> Tuple[Tensor, Tensor, Tuple[Tensor, Tensor]]:
@@ -108,34 +109,58 @@ class RewEndModel(NativeStateMixin, nn.Module):
     @torch.no_grad()
     def _predict(self, obs: Tensor, act: Tensor, next_obs: Tensor, hx_cx: Optional[Tuple[Tensor, Tensor]] = None,
                  kinds: Optional[Tuple[Tensor, Tensor]] = None) -> Tuple[Tensor, Tensor, Tuple[Tensor, Tensor]]:
-        lib = _lib.lib()
-        h = self._native()
-        b, t, c, hh, ww = obs.shape
-        dev = obs.device
+        b, t = obs.shape[:2]
         src = self._u8_sources(obs, next_obs, kinds)
         act_ = act.long().contiguous()
         hx = cx = None
         if hx_cx is not None:
             hx, cx = hx_cx[0].reshape(b, -1).float().contiguous(), hx_cx[1].reshape(b, -1).float().contiguous()
-        rew = torch.empty(b, t, 3, device=dev)
-        end = torch.empty(b, t, 2, device=dev)
-        hx_o = torch.empty(b, self.cfg.lstm_dim, device=dev)
-        cx_o = torch.empty(b, self.cfg.lstm_dim, device=dev)
-        need = lib.dmd_rew_end_workspace_bytes(h, b * t)
-        if need == 0:
-            raise RuntimeError("diamond_b200: " + lib.dmd_last_error().decode())
-        if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        ws = self.predict_workspace(b * t)
         if src is not None:
+            lib = _lib.lib()
+            h = self._native()
+            rew, end, hx_o, cx_o = self._new_outputs(b, t, obs.device)
             _lib.check(lib.dmd_rew_end_predict_u8(h, b, t, C.byref(src[0].c_struct()), C.byref(src[1].c_struct()), act_.data_ptr(),
                                                   _lib.ptr(hx), _lib.ptr(cx), rew.data_ptr(), end.data_ptr(), hx_o.data_ptr(),
-                                                  cx_o.data_ptr(), self._ws.data_ptr(), self._ws.numel(), _lib.current_stream()))
+                                                  cx_o.data_ptr(), ws.data_ptr(), ws.numel(), _lib.current_stream()))
             return rew, end, (hx_o.unsqueeze(0), cx_o.unsqueeze(0))
-        obs_, nxt_ = obs.float().contiguous(), next_obs.float().contiguous()
-        _lib.check(lib.dmd_rew_end_predict(h, b, t, obs_.data_ptr(), nxt_.data_ptr(), act_.data_ptr(), _lib.ptr(hx), _lib.ptr(cx),
-                                           rew.data_ptr(), end.data_ptr(), hx_o.data_ptr(), cx_o.data_ptr(), self._ws.data_ptr(),
-                                           self._ws.numel(), _lib.current_stream()))
+        # one diamond_b200::rew_end_predict op, so that torch.compile traces it whole
+        rew, end, hx_o, cx_o = torch_ops.rew_end_predict(torch_ops.key_of(self), obs.float().contiguous(), act_,
+                                                         next_obs.float().contiguous(), hx, cx, ws, self._state_tensors())
         return rew, end, (hx_o.unsqueeze(0), cx_o.unsqueeze(0))
+
+    def _new_outputs(self, b: int, t: int, dev):
+        d = self.cfg.lstm_dim
+        return (torch.empty(b, t, 3, device=dev), torch.empty(b, t, 2, device=dev), torch.empty(b, d, device=dev),
+                torch.empty(b, d, device=dev))
+
+    def _predict_native(self, obs: Tensor, act: Tensor, next_obs: Tensor, hx: Optional[Tensor], cx: Optional[Tensor], ws: Tensor):
+        """dmd_rew_end_predict on fp32 frames (the body of the diamond_b200::rew_end_predict op)."""
+        lib = _lib.lib()
+        h = self._native()
+        b, t = obs.shape[:2]
+        rew, end, hx_o, cx_o = self._new_outputs(b, t, obs.device)
+        _lib.check(lib.dmd_rew_end_predict(h, b, t, obs.data_ptr(), next_obs.data_ptr(), act.data_ptr(), _lib.ptr(hx), _lib.ptr(cx),
+                                           rew.data_ptr(), end.data_ptr(), hx_o.data_ptr(), cx_o.data_ptr(), ws.data_ptr(),
+                                           ws.numel(), _lib.current_stream()))
+        return rew, end, hx_o, cx_o
+
+    def predict_workspace(self, rows: int) -> Tensor:
+        """The inference workspace for `rows` = b * t frames.  Its size is asked of the native layer once per row count and
+        mode, so that a compiled caller traces this as plain attribute reads (WorldModelEnv.reset sees its shape first)."""
+        key = (rows, torch.are_deterministic_algorithms_enabled())
+        sizes = self._ws_bytes
+        if sizes is None:
+            sizes = self._ws_bytes = {}
+        if key not in sizes:
+            need = _lib.lib().dmd_rew_end_workspace_bytes(self._native(), rows)
+            if need == 0:
+                raise RuntimeError("diamond_b200: " + _lib.lib().dmd_last_error().decode())
+            sizes[key] = need
+        dev = self.device
+        if self._ws is None or self._ws.numel() < sizes[key] or self._ws.device != dev:
+            self._ws = torch.empty(sizes[key], dtype=torch.uint8, device=dev)
+        return self._ws
 
     def forward(self, batch):  # rew_end_model.py:57-90
         obs = batch.obs[:, :-1]

@@ -210,7 +210,8 @@ class NativeStateMixin:
     # to ONE module object.  copy.deepcopy (EMA copies) and pickle (multiprocessing) go through __getstate__: the copy starts
     # without native state and builds its own on first use, so two objects never own -- and free -- the same handle.
     _NATIVE_RESET = ("_h", "_h_key", "_wkey", "_packed", "_ws")
-    _NATIVE_DROP = ("_state_tensor_cache", "_ws_pool", "_bwd_scratch", "_grad_acc", "_grad_task", "_gv_layout", "last_flat_grad")
+    _NATIVE_DROP = ("_state_tensor_cache", "_ws_pool", "_bwd_scratch", "_grad_acc", "_grad_task", "_gv_layout", "last_flat_grad",
+                    "_ws_bytes", "_op_key")
 
     def __getstate__(self):
         state = self.__dict__.copy()
