@@ -107,6 +107,7 @@ SIGNATURES = {
     "dmd_wgrad_partial_bytes": (_sz, []),
     "dmd_conv2d_wgrad": (_i, [C.POINTER(WgradDesc), _vp]),
     "dmd_gn_stats": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
+    "dmd_gn_stats_det": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "dmd_attn_fwd": (_i, [_vp] * 10 + [_i, _i, _i, _i, _f, _vp]),
     "dmd_attn_scratch_bytes": (_sz, [_i, _i, _i]),
     "dmd_attn_fwd_scratch": (_i, [_vp] * 10 + [_i, _i, _i, _i, _f, _vp, _sz, _vp]),
@@ -117,13 +118,19 @@ SIGNATURES = {
     "dmd_lstm_gates": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp]),
     "dmd_resize_nhwc": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "dmd_norm_bwd": (_i, [C.POINTER(NormBwdDesc), _i, _vp]),
+    "dmd_norm_bwd_det": (_i, [C.POINTER(NormBwdDesc), _i, _vp]),
     "dmd_norm_affine_grad": (_i, [C.POINTER(NormBwdDesc), _vp, _vp, _vp, _vp]),
     "dmd_attn_bwd": (_i, [_vp] * 16 + [_i, _i, _i, _i, _f, _vp]),
+    "dmd_attn_split_bwd_workspace_bytes": (_sz, [_i, _i, _i]),
+    "dmd_attn_split_bwd": (_i, [_vp] * 10 + [C.POINTER(_ll), _vp, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
     "dmd_sgemm_partial_floats": (_ll, [_i, _i, _i, _i]),
     "dmd_sgemm": (_i, [_vp, _ll, _ll, _vp, _ll, _ll, _vp, _ll, _i, _i, _i, _vp, _i, _i, _vp, _vp]),
     "dmd_film_wgrad": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "dmd_embedding_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "dmd_embedding_bwd_det": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "dmd_colsum": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _vp]),
+    "dmd_colsum_partial_bytes": (_sz, [_ll, _i]),
+    "dmd_colsum_det": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _vp, _sz, _vp]),
     "dmd_sumpool2": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "dmd_dsilu_mul": (_i, [_vp, _vp, _vp, _ll, _vp]),
     "dmd_maxpool2_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),

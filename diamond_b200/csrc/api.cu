@@ -477,6 +477,7 @@ static int gn_stats_launch(const float* x, double* stats, int B, int HW, int C, 
   DMD_CHECK(x && stats && gs > 0 && C % gs == 0, "gn_stats: bad arguments");
   if (det) {
     DMD_CHECK(B <= 65535 && (long long)kGnDetSplit * (C / gs) < (1ll << 31), "gn_stats: B=%d or %d groups out of range", B, C / gs);
+    DMD_CHECK(C % 4 == 0 && gs % 4 == 0, "gn_stats: deterministic sums need C and gs multiples of 4 (C=%d gs=%d)", C, gs);
     gn_stats_det_kernel<<<dim3(kGnDetSplit * (C / gs), B), kGnDetThreads, 0, st>>>(x, stats, HW, C, gs);
     DMD_LAUNCH_OK();
     return 0;
@@ -491,6 +492,10 @@ static int gn_stats_launch(const float* x, double* stats, int B, int HW, int C, 
 }
 extern "C" int dmd_gn_stats(const float* x, double* stats, int B, int HW, int C, int gs, void* stream) {
   return gn_stats_launch(x, stats, B, HW, C, gs, false, (cudaStream_t)stream);
+}
+extern "C" int dmd_gn_stats_det(const float* x, double* stats, int B, int HW, int C, int gs, void* stream) {
+  DMD_CHECK(B > 0 && HW > 0 && C > 0, "gn_stats_det: bad arguments");
+  return gn_stats_launch(x, stats, B, HW, C, gs, true, (cudaStream_t)stream);
 }
 
 // scratch of the any-L attention path (q, k, v of every token); L = 64 runs in one launch without scratch
@@ -637,13 +642,17 @@ static int loss_scale_launch(const float* g, long long n, unsigned int* amax_bit
 // column sums: up to 592 blocks of 256 / (Cb / 4) row lanes, at least 8 rows per lane.  part (deterministic mode): each block
 // stores its sums to part[block][C] (part_bytes of room) and colsum_reduce_kernel adds them in block order, in place of the
 // atomics.  The block count depends on rows and C only, so the order does too.
+static long long colsum_blocks(long long rows, int C) {
+  const int L4 = (C < 256 ? C : 256) >> 2, lanes = 256 / L4;
+  const long long blocks = (rows + (long long)lanes * 8 - 1) / ((long long)lanes * 8);
+  return blocks > 592 ? 592 : (blocks < 1 ? 1 : blocks);
+}
+static size_t colsum_partial_bytes(long long rows, int C) { return (size_t)colsum_blocks(rows, C) * C * sizeof(float); }
 static int colsum_launch(const float* x, float* out, float* out2, const float* inv, long long rows, int C, int Creal, cudaStream_t st,
                          float* part = nullptr, size_t part_bytes = 0) {
-  const int L4 = (C < 256 ? C : 256) >> 2, lanes = 256 / L4;
-  long long blocks = (rows + (long long)lanes * 8 - 1) / ((long long)lanes * 8);
-  blocks = blocks > 592 ? 592 : (blocks < 1 ? 1 : blocks);
+  const long long blocks = colsum_blocks(rows, C);
   if (part) {
-    DMD_CHECK((size_t)blocks * C * sizeof(float) <= part_bytes, "colsum: partials (%lld x %d floats) exceed the partial buffer", blocks, C);
+    DMD_CHECK(colsum_partial_bytes(rows, C) <= part_bytes, "colsum: partials (%lld x %d floats) exceed the partial buffer", blocks, C);
     colsum_part_kernel<<<dim3((unsigned)blocks, (C + 255) / 256), 256, 0, st>>>(x, part, rows, C);
     DMD_LAUNCH_OK();
     colsum_reduce_kernel<<<(Creal + 255) / 256, 256, 0, st>>>(part, (int)blocks, C, Creal, out, out2, inv);
@@ -812,6 +821,12 @@ extern "C" int dmd_norm_bwd(const dmd_norm_bwd_desc* d, int pass, void* stream) 
   DMD_CHECK(pass == 1 || (pass == 2 && d->gx), "norm_bwd: pass must be 1 or 2 (pass 2 writes gx)");
   return norm_bwd_launch(nb, pass, (cudaStream_t)stream);
 }
+extern "C" int dmd_norm_bwd_det(const dmd_norm_bwd_desc* d, int pass, void* stream) {
+  NormBwdParams nb;
+  if (norm_bwd_params(d, &nb)) return 1;
+  DMD_CHECK(pass == 1 || (pass == 2 && d->gx), "norm_bwd_det: pass must be 1 or 2 (pass 2 writes gx)");
+  return norm_bwd_launch(nb, pass, (cudaStream_t)stream, true);
+}
 extern "C" int dmd_norm_affine_grad(const dmd_norm_bwd_desc* d, float* dgamma, float* dbeta, const float* inv_scale, void* stream) {
   NormBwdParams nb;
   if (norm_bwd_params(d, &nb)) return 1;
@@ -845,9 +860,20 @@ extern "C" int dmd_embedding_bwd(const float* de, const int64_t* act, float* dE,
   DMD_CHECK(de && act && dE && B > 0 && T > 0 && CC % T == 0 && num_actions > 0, "embedding_bwd: bad arguments");
   return embedding_bwd_launch(de, act, dE, B, CC, T, num_actions, inv_scale, (cudaStream_t)stream);
 }
+extern "C" int dmd_embedding_bwd_det(const float* de, const int64_t* act, float* dE, int B, int CC, int T, int num_actions,
+                                     const float* inv_scale, void* stream) {
+  DMD_CHECK(de && act && dE && B > 0 && T > 0 && CC % T == 0 && num_actions > 0, "embedding_bwd_det: bad arguments");
+  return embedding_bwd_launch(de, act, dE, B, CC, T, num_actions, inv_scale, (cudaStream_t)stream, true);
+}
 extern "C" int dmd_colsum(const float* x, float* out, float* out2, const float* inv_scale, long long rows, int C, int Creal, void* stream) {
   DMD_CHECK(x && out && rows > 0 && C > 0 && C % 4 == 0 && Creal <= C, "colsum: bad arguments (C a multiple of 4, Creal <= C)");
   return colsum_launch(x, out, out2, inv_scale, rows, C, Creal, (cudaStream_t)stream);
+}
+extern "C" size_t dmd_colsum_partial_bytes(long long rows, int C) { return rows > 0 && C > 0 ? colsum_partial_bytes(rows, C) : 0; }
+extern "C" int dmd_colsum_det(const float* x, float* out, float* out2, const float* inv_scale, long long rows, int C, int Creal,
+                              void* partial, size_t partial_bytes, void* stream) {
+  DMD_CHECK(x && out && partial && rows > 0 && C > 0 && C % 4 == 0 && Creal <= C, "colsum_det: bad arguments (C a multiple of 4, Creal <= C)");
+  return colsum_launch(x, out, out2, inv_scale, rows, C, Creal, (cudaStream_t)stream, (float*)partial, partial_bytes);
 }
 extern "C" int dmd_sumpool2(const float* in, float* out, int B, int H, int W, int C, int accumulate, void* stream) {
   DMD_CHECK(in && out && B > 0 && H > 0 && W > 0 && C % 4 == 0, "sumpool2: bad arguments (C a multiple of 4)");
@@ -2245,75 +2271,135 @@ int clear_backward(const ModelCore& core, Plan& pl, float* grads, int accumulate
   return 0;
 }
 
+// one op of a backward op list; inv: the reciprocal of the loss scale (device scalar) the parameter gradients are multiplied by
+int run_bop(const ModelCore& core, const Plan& pl, const BOp& b, float* grads, const float* inv, cudaStream_t st) {
+  const int B = pl.B;
+  switch (b.kind) {
+    case B_PREP: if (prep_launch(b.prep, b.prep_nsrc, st)) return 1; break;
+    case B_CONV: if (conv_launch(b.conv, b.smem, b.cols, st)) return 1; break;
+    case B_WGRAD: if (wgrad_launch(b.wg, grads + b.goff, st)) return 1; break;
+    case B_COLSUM:
+      if (colsum_launch(b.src, grads + b.goff, b.goff2 >= 0 ? grads + b.goff2 : nullptr, inv, b.rows, b.C, b.Creal, st,
+                        pl.det ? pl.partial : nullptr, pl.partial_bytes)) return 1;
+      break;
+    case B_NORM1: if (norm_bwd_launch(b.nb, 1, st, pl.det)) return 1; break;
+    case B_NORM2: if (norm_bwd_launch(b.nb, 2, st)) return 1; break;
+    case B_AFFINE: if (affine_param_grad_launch(b.nb, grads + b.goff, grads + b.goff2, inv, st)) return 1; break;
+    case B_POOL: if (sumpool2_launch(b.src, b.dst, B, b.H, b.W, b.C, b.acc, st)) return 1; break;
+    case B_ATTN: {
+      AttnBwdParams ab = b.ab;
+      ab.dgamma = grads + b.goffs[0]; ab.dbeta = grads + b.goffs[1]; ab.dwqkv = grads + b.goffs[2]; ab.dbqkv = grads + b.goffs[3];
+      ab.dwout = grads + b.goffs[4]; ab.dbout = grads + b.goffs[5];
+      if (attn_bwd_launch(ab, B, st)) return 1;
+      break;
+    }
+    case B_ATTN_RECOMP: {
+      const dim3 grid((b.ap.L + kAttnTile - 1) / kAttnTile, B);
+      if (b.ap.C == 128) attn_qkv_kernel<128><<<grid, kAttnQkvThreads, 0, st>>>(b.ap);
+      else if (b.ap.C == 64) attn_qkv_kernel<64><<<grid, kAttnQkvThreads, 0, st>>>(b.ap);
+      else attn_qkv_kernel<32><<<grid, kAttnQkvThreads, 0, st>>>(b.ap);
+      DMD_LAUNCH_OK();
+      const long long total = (long long)B * b.ap.L * b.ap.C;
+      attn_xn_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(b.ap.x, b.ap.st_in, b.ap.gamma, b.ap.beta, b.at_xn, b.ap.L, b.ap.C,
+                                                                     b.ap.gs, b.ap.eps, total);
+      DMD_LAUNCH_OK();
+      break;
+    }
+    case B_ATTN_CORE:
+      if (b.ap.L == kAttnL)
+        attn_core_bwd_kernel<kAttnL><<<dim3(b.ap.C / 8, B), kAttnCoreThreads, 0, st>>>(b.ap.scratch, b.at_gy, b.ap.out, b.at_y, b.at_gqkv,
+                                                                                      b.at_gxn, b.ap.C, b.ap.L);
+      else
+        attn_core_bwd_kernel<0><<<dim3(b.ap.C / 8, B), kAttnCoreThreads, 0, st>>>(b.ap.scratch, b.at_gy, b.ap.out, b.at_y, b.at_gqkv,
+                                                                                 b.at_gxn, b.ap.C, b.ap.L);
+      DMD_LAUNCH_OK();
+      break;
+    case B_MEMSET: DMD_CUDA(cudaMemsetAsync(b.ms_ptr, 0, b.ms_bytes, st)); break;
+    case B_SGEMM:   // the long-K products are split: dcond = dfilm Wf (K = all FiLM rows, partials in film_part) and the
+                    // attention weight gradients (K = every token of the batch, partials in tA)
+      if (sgemm_launch(b.ga, b.sam, b.sak, b.gb, b.sbk, b.sbn, b.c_goff >= 0 ? grads + b.c_goff : b.gc, b.ldc, b.M, b.N, b.K,
+                       b.use_inv ? inv : nullptr, b.acc, b.chunks, b.part ? b.part : pl.tA, st)) return 1;
+      break;
+    case B_FILMW:
+      if (film_wgrad_launch(pl.dfilm, pl.cond, grads, pl.film_woff, pl.film_boff, B, core.film_rows, core.cond_channels, inv, st)) return 1;
+      break;
+    case B_LINEAR: if (linear_launch(b.lin_in, b.lin_w, b.lin_b, b.lin_out, B, b.lin_K, b.lin_F, 0, st)) return 1; break;
+    case B_DSILU: if (dsilu_mul_launch(b.src, b.ga, b.dst, b.rows, st)) return 1; break;
+    case B_EMB:
+      if (embedding_bwd_launch(b.src, pl.t_act, grads + b.goff, B, b.C, b.emb_T, b.emb_actions, inv, st, pl.det)) return 1;
+      break;
+    default: return fail("backward: unknown op kind %d", b.kind);
+  }
+  return 0;
+}
 // the backward op list; the caller has cleared (clear_backward), set the loss scale and seeded the gradient the list starts from.
 // Every op that writes into `grads` ADDS to it (wgrad reduce with accumulate = 1, colsum / attention / embedding atomics, affine
 // and FiLM +=, sgemm into a c_goff slice with acc = 1, checked when the list is built), so an accumulating call is this same list
 // on a buffer that was not cleared
 int run_backward(const ModelCore& core, Plan& pl, float* grads, cudaStream_t st) {
-  const int B = pl.B;
-  const float* inv = pl.scale + 1;
-  for (const BOp& b : pl.bops) {
-    switch (b.kind) {
-      case B_PREP: if (prep_launch(b.prep, b.prep_nsrc, st)) return 1; break;
-      case B_CONV: if (conv_launch(b.conv, b.smem, b.cols, st)) return 1; break;
-      case B_WGRAD: if (wgrad_launch(b.wg, grads + b.goff, st)) return 1; break;
-      case B_COLSUM:
-        if (colsum_launch(b.src, grads + b.goff, b.goff2 >= 0 ? grads + b.goff2 : nullptr, inv, b.rows, b.C, b.Creal, st,
-                          pl.det ? pl.partial : nullptr, pl.partial_bytes)) return 1;
-        break;
-      case B_NORM1: if (norm_bwd_launch(b.nb, 1, st, pl.det)) return 1; break;
-      case B_NORM2: if (norm_bwd_launch(b.nb, 2, st)) return 1; break;
-      case B_AFFINE: if (affine_param_grad_launch(b.nb, grads + b.goff, grads + b.goff2, inv, st)) return 1; break;
-      case B_POOL: if (sumpool2_launch(b.src, b.dst, B, b.H, b.W, b.C, b.acc, st)) return 1; break;
-      case B_ATTN: {
-        AttnBwdParams ab = b.ab;
-        ab.dgamma = grads + b.goffs[0]; ab.dbeta = grads + b.goffs[1]; ab.dwqkv = grads + b.goffs[2]; ab.dbqkv = grads + b.goffs[3];
-        ab.dwout = grads + b.goffs[4]; ab.dbout = grads + b.goffs[5];
-        if (attn_bwd_launch(ab, B, st)) return 1;
-        break;
-      }
-      case B_ATTN_RECOMP: {
-        const dim3 grid((b.ap.L + kAttnTile - 1) / kAttnTile, B);
-        if (b.ap.C == 128) attn_qkv_kernel<128><<<grid, kAttnQkvThreads, 0, st>>>(b.ap);
-        else if (b.ap.C == 64) attn_qkv_kernel<64><<<grid, kAttnQkvThreads, 0, st>>>(b.ap);
-        else attn_qkv_kernel<32><<<grid, kAttnQkvThreads, 0, st>>>(b.ap);
-        DMD_LAUNCH_OK();
-        const long long total = (long long)B * b.ap.L * b.ap.C;
-        attn_xn_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(b.ap.x, b.ap.st_in, b.ap.gamma, b.ap.beta, b.at_xn, b.ap.L, b.ap.C,
-                                                                       b.ap.gs, b.ap.eps, total);
-        DMD_LAUNCH_OK();
-        break;
-      }
-      case B_ATTN_CORE:
-        if (b.ap.L == kAttnL)
-          attn_core_bwd_kernel<kAttnL><<<dim3(b.ap.C / 8, B), kAttnCoreThreads, 0, st>>>(b.ap.scratch, b.at_gy, b.ap.out, b.at_y, b.at_gqkv,
-                                                                                        b.at_gxn, b.ap.C, b.ap.L);
-        else
-          attn_core_bwd_kernel<0><<<dim3(b.ap.C / 8, B), kAttnCoreThreads, 0, st>>>(b.ap.scratch, b.at_gy, b.ap.out, b.at_y, b.at_gqkv,
-                                                                                   b.at_gxn, b.ap.C, b.ap.L);
-        DMD_LAUNCH_OK();
-        break;
-      case B_MEMSET: DMD_CUDA(cudaMemsetAsync(b.ms_ptr, 0, b.ms_bytes, st)); break;
-      case B_SGEMM:   // the long-K products are split: dcond = dfilm Wf (K = all FiLM rows, partials in film_part) and the
-                      // attention weight gradients (K = every token of the batch, partials in tA)
-        if (sgemm_launch(b.ga, b.sam, b.sak, b.gb, b.sbk, b.sbn, b.c_goff >= 0 ? grads + b.c_goff : b.gc, b.ldc, b.M, b.N, b.K,
-                         b.use_inv ? inv : nullptr, b.acc, b.chunks, b.part ? b.part : pl.tA, st)) return 1;
-        break;
-      case B_FILMW:
-        if (film_wgrad_launch(pl.dfilm, pl.cond, grads, pl.film_woff, pl.film_boff, B, core.film_rows, core.cond_channels, inv, st)) return 1;
-        break;
-      case B_LINEAR: if (linear_launch(b.lin_in, b.lin_w, b.lin_b, b.lin_out, B, b.lin_K, b.lin_F, 0, st)) return 1; break;
-      case B_DSILU: if (dsilu_mul_launch(b.src, b.ga, b.dst, b.rows, st)) return 1; break;
-      case B_EMB:
-        if (embedding_bwd_launch(b.src, pl.t_act, grads + b.goff, B, b.C, b.emb_T, b.emb_actions, inv, st, pl.det)) return 1;
-        break;
-      default: return fail("backward: unknown op kind %d", b.kind);
-    }
-  }
+  for (const BOp& b : pl.bops)
+    if (run_bop(core, pl, b, grads, pl.scale + 1, st)) return 1;
   return 0;
 }
 
 }  // namespace
+
+// ---- per-op entry point of the split attention backward: BwdBuilder::attn_split's op list on a one-block model, run by
+// run_bop.  Workspace: the backward temporaries tA / tB / tC at the size attn_split needs (6 x B x L x C floats each; a
+// training plan's are at least that large, and split_k's split count is min(K / 256, 32) either way for C <= 128), the
+// deterministic column sums' partials and the norm backward's per-channel sums.
+static size_t attn_split_workspace(int B, int L, int C, uint8_t* base, Plan* pl) {
+  Bump bb{base};
+  const long long tmp = 6ll * B * L * C;
+  float* t[3];
+  for (float*& p : t) p = (float*)bb.take((size_t)tmp * 4);
+  const size_t part = std::max(colsum_partial_bytes((long long)B * L, C), colsum_partial_bytes((long long)B * L, 3 * C));
+  float* partial = (float*)bb.take(part);
+  float* nsum = (float*)bb.take((size_t)2 * B * kMaxCin * 4);
+  if (pl) {
+    pl->B = B; pl->tmp_floats = tmp; pl->tA = t[0]; pl->tB = t[1]; pl->tC = t[2];
+    pl->partial = partial; pl->partial_bytes = part; pl->nsum = nsum;
+  }
+  return bb.off;
+}
+extern "C" size_t dmd_attn_split_bwd_workspace_bytes(int B, int L, int C) {
+  return B > 0 && L > 0 && C > 0 ? attn_split_workspace(B, L, C, nullptr, nullptr) : 0;
+}
+extern "C" int dmd_attn_split_bwd(const float* x, const double* stats_in, const float* gamma, const float* beta, const float* wqkv,
+                                  const float* bqkv, const float* wout, const float* gout, float* gx, float* grads,
+                                  const long long* goffs, const float* inv_scale, int B, int L, int C, int gs, int det,
+                                  void* workspace, size_t workspace_bytes, void* stream) {
+  DMD_CHECK(x && stats_in && gamma && beta && wqkv && bqkv && wout && gout && gx && grads && goffs && workspace,
+            "attn_split_bwd: null argument");
+  DMD_CHECK((C == 32 || C == 64 || C == 128) && L >= 1 && L <= kAttnL && B >= 1 && B <= 65535,
+            "attn_split_bwd: unsupported shape B=%d L=%d C=%d (C in {32, 64, 128}, 1 <= L <= %d)", B, L, C, kAttnL);
+  DMD_CHECK(gs > 0 && gs % 8 == 0 && C % gs == 0 && C / gs <= 8, "attn_split_bwd: bad group size %d for C=%d", gs, C);
+  for (int i = 0; i < 6; ++i) DMD_CHECK(goffs[i] >= 0, "attn_split_bwd: gradient offset %d is negative", i);
+  DMD_CHECK(((uintptr_t)workspace & 255) == 0, "attn_split_bwd: workspace must be 256-byte aligned");
+  DMD_CHECK(workspace_bytes >= attn_split_workspace(B, L, C, nullptr, nullptr), "attn_split_bwd: workspace too small (%zu < %zu)",
+            workspace_bytes, attn_split_workspace(B, L, C, nullptr, nullptr));
+  if (init_kernels()) return 1;
+  // gamma, beta, Wqkv, bqkv, Wout, bout: state_dict tensors 0..5 of the one-block model (bout's value is not read)
+  ModelCore core;
+  core.ptrs = {gamma, beta, wqkv, bqkv, wout, nullptr};
+  core.goff.assign(goffs, goffs + 6);
+  core.n_tensors = 6;
+  ResBlockW rb{};
+  rb.cin = rb.cout = C; rb.has_attn = 1;
+  rb.an_w = 0; rb.an_b = 1; rb.qkv_w = 2; rb.qkv_b = 3; rb.op_w = 4; rb.op_b = 5;
+  Tens o{const_cast<float*>(x), const_cast<double*>(stats_in), C, 1, L, gs};
+  o.grad = gx;
+  Plan pl;
+  pl.det = det != 0;
+  attn_split_workspace(B, L, C, (uint8_t*)workspace, &pl);
+  BwdBuilder bw{&core, &pl};
+  bw.begin();
+  bw.attn_split(rb, o, gout);
+  if (bw.err) return 1;
+  for (const BOp& b : pl.bops)
+    if (run_bop(core, pl, b, grads, inv_scale, (cudaStream_t)stream)) return 1;
+  return 0;
+}
 
 extern "C" size_t dmd_denoiser_train_workspace_bytes(const dmd_denoiser* h, int B, int H, int W) {
   Plan tmp; size_t need = 0;

@@ -775,7 +775,7 @@ __global__ void gn_stats_kernel(const float* __restrict__ x, double* __restrict_
 
 // Deterministic GroupNorm sums (torch.use_deterministic_algorithms).  Each (group, image) is owned by one cluster of
 // kGnDetSplit CTAs; CTA r of the cluster takes the r-th of kGnDetSplit fixed, contiguous pixel ranges.  Thread t sums elements
-// t, t + blockDim, ... of its range in fp32 (four consecutive channels per load when C and gs are multiples of 4), the CTA adds
+// t, t + blockDim, ... of its range in fp32 (four consecutive channels per load: C and gs are multiples of 4), the CTA adds
 // its threads' sums in a fixed fp64 tree, and rank 0 adds the CTAs' sums in rank order through distributed shared memory.  So
 // the result depends on the tensor alone, not on scheduling or the SM count, and no partials buffer is needed.
 // stats[n][g] += (sum, sumsq) with a plain add (rank 0 is the slot's only writer).  grid: (kGnDetSplit * C / gs, B).
@@ -787,26 +787,17 @@ gn_stats_det_kernel(const float* __restrict__ x, double* __restrict__ stats, int
   cg::cluster_group cluster = cg::this_cluster();
   const int r = (int)cluster.block_rank();
   const int g = blockIdx.x / kGnDetSplit, n = blockIdx.y, G = C / gs;
-  const bool v4 = (C & 3) == 0 && (gs & 3) == 0;
-  const int q = v4 ? gs >> 2 : gs;
+  const int q = gs >> 2;
   const int per = (HW + kGnDetSplit - 1) / kGnDetSplit, p0 = min(HW, r * per), p1 = min(HW, p0 + per);
   const float* xb = x + ((size_t)n * HW + p0) * C + (size_t)g * gs;
   const long long total = (long long)(p1 - p0) * q;
   float s = 0.f, ss = 0.f;
-  if (v4) {
 #pragma unroll 4
-    for (long long i = threadIdx.x; i < total; i += kGnDetThreads) {
-      const long long pix = i / q;
-      const float4 v = __ldg(reinterpret_cast<const float4*>(xb + pix * C) + (i - pix * q));
-      s += (v.x + v.y) + (v.z + v.w);
-      ss += fmaf(v.x, v.x, v.y * v.y) + fmaf(v.z, v.z, v.w * v.w);
-    }
-  } else {
-    for (long long i = threadIdx.x; i < total; i += kGnDetThreads) {
-      const long long pix = i / q;
-      const float v = __ldg(xb + pix * C + (i - pix * q));
-      s += v; ss += v * v;
-    }
+  for (long long i = threadIdx.x; i < total; i += kGnDetThreads) {
+    const long long pix = i / q;
+    const float4 v = __ldg(reinterpret_cast<const float4*>(xb + pix * C) + (i - pix * q));
+    s += (v.x + v.y) + (v.z + v.w);
+    ss += fmaf(v.x, v.x, v.y * v.y) + fmaf(v.z, v.z, v.w * v.w);
   }
   __shared__ double rs[kGnDetThreads], rss[kGnDetThreads];
   rs[threadIdx.x] = s; rss[threadIdx.x] = ss;

@@ -62,12 +62,14 @@ def _reject_removed(trs: bool = False, debug: int = 0) -> None:
         raise ValueError(f"debug={debug}: the kernels have no debug switches")
 
 
-def gn_stats(x: Tensor, gs: int) -> Tensor:
-    """(sum, sumsq) per (image, group) of an NHWC tensor, fp64 [B][C/gs][2]."""
-    _cuda(x)
+def gn_stats(x: Tensor, gs: int, *, out: Optional[Tensor] = None, det: bool = False) -> Tensor:
+    """(sum, sumsq) per (image, group) of an NHWC tensor, fp64 [B][C/gs][2], added to `out` (default: zeros); det: the
+    fixed-order sums of deterministic mode."""
+    _cuda(x, out)
     b, h, w, c = x.shape
-    st = torch.zeros(b, c // gs, 2, device=x.device, dtype=torch.float64)
-    _lib.check(_lib.lib().dmd_gn_stats(x.data_ptr(), st.data_ptr(), b, h * w, c, gs, _lib.current_stream()))
+    st = torch.zeros(b, c // gs, 2, device=x.device, dtype=torch.float64) if out is None else out
+    fn = _lib.lib().dmd_gn_stats_det if det else _lib.lib().dmd_gn_stats
+    _lib.check(fn(x.data_ptr(), st.data_ptr(), b, h * w, c, gs, _lib.current_stream()))
     return st
 
 
@@ -267,10 +269,11 @@ def norm_bwd(x: Tensor, gy: Tensor, stats: Tensor, gs: int, gx: Tensor, sum_a: T
              act: bool = True, film: Optional[Tensor] = None, film_off: int = 0, film_ctot: int = 0, c_off: int = 0,
              gamma: Optional[Tensor] = None, beta: Optional[Tensor] = None, eps: float = 1e-5, addend: Optional[Tensor] = None,
              accumulate: bool = False, dgamma: Optional[Tensor] = None, dbeta: Optional[Tensor] = None,
-             inv_scale: Optional[Tensor] = None) -> None:
+             inv_scale: Optional[Tensor] = None, det: bool = False) -> None:
     """(Ada)GroupNorm [+ SiLU] backward of NHWC x [B][H][W][C] as the executors run it: pass 1 adds the per-channel sums to
     sum_a / sum_b (rows of sum_stride floats; they may be views into a larger buffer such as the FiLM gradient), then the
-    affine parameter gradients when dgamma / dbeta are given, then pass 2 writes (or adds to) gx."""
+    affine parameter gradients when dgamma / dbeta are given, then pass 2 writes (or adds to) gx.  det: pass 1 as
+    deterministic mode runs it."""
     _cuda(x, gy, stats, gx, film, gamma, beta, addend)
     lib = _lib.lib()
     b, c = x.shape[0], x.shape[-1]
@@ -282,7 +285,7 @@ def norm_bwd(x: Tensor, gy: Tensor, stats: Tensor, gs: int, gx: Tensor, sum_a: T
     d.sumA, d.sumB, d.sum_stride = sum_a.data_ptr(), sum_b.data_ptr(), sum_stride
     d.gx, d.addend, d.accumulate = gx.data_ptr(), _lib.ptr(addend), int(accumulate)
     st = _lib.current_stream()
-    _lib.check(lib.dmd_norm_bwd(C.byref(d), 1, st))
+    _lib.check((lib.dmd_norm_bwd_det if det else lib.dmd_norm_bwd)(C.byref(d), 1, st))
     if dgamma is not None:
         _lib.check(lib.dmd_norm_affine_grad(C.byref(d), dgamma.data_ptr(), dbeta.data_ptr(), _inv(inv_scale), st))
     _lib.check(lib.dmd_norm_bwd(C.byref(d), 2, st))
@@ -298,6 +301,23 @@ def attn_bwd(x: Tensor, stats_in: Tensor, gamma: Tensor, beta: Tensor, wqkv: Ten
     _lib.check(_lib.lib().dmd_attn_bwd(x.data_ptr(), stats_in.data_ptr(), gamma.data_ptr(), beta.data_ptr(), wqkv.data_ptr(),
                                        bqkv.data_ptr(), wout.data_ptr(), gout.data_ptr(), gx.data_ptr(), *[t.data_ptr() for t in pgrads],
                                        _inv(inv_scale), b, h * w, c, gs, eps, _lib.current_stream()))
+    return gx
+
+
+def attn_split_bwd(x: Tensor, stats_in: Tensor, gamma: Tensor, beta: Tensor, wqkv: Tensor, bqkv: Tensor, wout: Tensor, gout: Tensor,
+                   gs: int, grads: Tensor, goffs, inv_scale: Optional[Tensor] = None, det: bool = False) -> Tensor:
+    """The training plans' split SelfAttention2d backward of NHWC x [B][H][W][C] (H*W <= 64, C in {32, 64, 128}): returns g_x;
+    ADDS the parameter gradients (gamma, beta, Wqkv, bqkv, Wout, bout) to the flat buffer `grads` at the six float offsets
+    `goffs`."""
+    _cuda(x, stats_in, gamma, beta, wqkv, bqkv, wout, gout, grads, inv_scale)
+    lib = _lib.lib()
+    b, h, w, c = x.shape
+    gx = torch.empty_like(x)
+    ws = torch.empty(lib.dmd_attn_split_bwd_workspace_bytes(b, h * w, c), dtype=torch.uint8, device=x.device)
+    offs = (C.c_longlong * 6)(*[int(o) for o in goffs])
+    _lib.check(lib.dmd_attn_split_bwd(x.data_ptr(), stats_in.data_ptr(), gamma.data_ptr(), beta.data_ptr(), wqkv.data_ptr(),
+                                      bqkv.data_ptr(), wout.data_ptr(), gout.data_ptr(), gx.data_ptr(), grads.data_ptr(), offs,
+                                      _inv(inv_scale), b, h * w, c, gs, int(det), ws.data_ptr(), ws.numel(), _lib.current_stream()))
     return gx
 
 
@@ -322,21 +342,31 @@ def film_wgrad(dfilm: Tensor, cond: Tensor, grads: Tensor, woff: Tensor, boff: T
     return grads
 
 
-def embedding_bwd(de: Tensor, act: Tensor, de_table: Tensor, inv_scale: Optional[Tensor] = None) -> Tensor:
-    """de [B][T*E], act [B][T] int64 -> de_table [num_actions][E] += scattered rows."""
+def embedding_bwd(de: Tensor, act: Tensor, de_table: Tensor, inv_scale: Optional[Tensor] = None, det: bool = False) -> Tensor:
+    """de [B][T*E], act [B][T] int64 -> de_table [num_actions][E] += scattered rows; det: gathered in a fixed order."""
     _cuda(de, act, de_table)
     b, t = act.shape
-    _lib.check(_lib.lib().dmd_embedding_bwd(de.data_ptr(), act.data_ptr(), de_table.data_ptr(), b, de.shape[1], t, de_table.shape[0],
-                                            _inv(inv_scale), _lib.current_stream()))
+    fn = _lib.lib().dmd_embedding_bwd_det if det else _lib.lib().dmd_embedding_bwd
+    _lib.check(fn(de.data_ptr(), act.data_ptr(), de_table.data_ptr(), b, de.shape[1], t, de_table.shape[0],
+               _inv(inv_scale), _lib.current_stream()))
     return de_table
 
 
-def colsum(x: Tensor, out: Tensor, out2: Optional[Tensor] = None, inv_scale: Optional[Tensor] = None, creal: Optional[int] = None) -> Tensor:
-    """out[c] (and out2[c]) += sum over the rows of x [rows][C] for c < creal (default C)."""
-    _cuda(x, out, out2)
+def colsum(x: Tensor, out: Tensor, out2: Optional[Tensor] = None, inv_scale: Optional[Tensor] = None, creal: Optional[int] = None,
+           det: bool = False, partial: Optional[Tensor] = None) -> Tensor:
+    """out[c] (and out2[c]) += sum over the rows of x [rows][C] for c < creal (default C).  det: the block sums go through
+    `partial` (default: a buffer of dmd_colsum_partial_bytes) and are added in block order."""
+    _cuda(x, out, out2, partial)
+    lib = _lib.lib()
     rows, c = x.shape
-    _lib.check(_lib.lib().dmd_colsum(x.data_ptr(), out.data_ptr(), _lib.ptr(out2), _inv(inv_scale), rows, c,
-                                     c if creal is None else creal, _lib.current_stream()))
+    creal = c if creal is None else creal
+    if not det:
+        _lib.check(lib.dmd_colsum(x.data_ptr(), out.data_ptr(), _lib.ptr(out2), _inv(inv_scale), rows, c, creal, _lib.current_stream()))
+        return out
+    if partial is None:
+        partial = torch.empty(lib.dmd_colsum_partial_bytes(rows, c), dtype=torch.uint8, device=x.device)
+    _lib.check(lib.dmd_colsum_det(x.data_ptr(), out.data_ptr(), _lib.ptr(out2), _inv(inv_scale), rows, c, creal, partial.data_ptr(),
+                                  partial.numel() * partial.element_size(), _lib.current_stream()))
     return out
 
 

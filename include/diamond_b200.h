@@ -176,6 +176,9 @@ int dmd_prep_plan(const dmd_prep_desc* d, int* blocks, int* pos_per_block, int* 
 
 /* GroupNorm partial sums of an NHWC tensor: stats[n][g] += (sum, sumsq) (blocks.py:28,43). */
 int dmd_gn_stats(const float* x, double* stats, int B, int HW, int C, int gs, void* stream);
+/* The same sums as torch.use_deterministic_algorithms runs them: one cluster of 8 CTAs per (image, group) adds fixed pixel
+ * ranges in a fixed order, so the result does not depend on scheduling.  C and gs multiples of 4. */
+int dmd_gn_stats_det(const float* x, double* stats, int B, int HW, int C, int gs, void* stream);
 
 /* SelfAttention2d.forward (blocks.py:62-72), L = H*W = 64 tokens (dmd_attn_fwd_scratch: any L; the backward, dmd_attn_bwd and
  * the training plans: 1 <= L <= 64), C in {32, 64, 128}, head_dim 8, at most 8 groups of gs
@@ -244,6 +247,9 @@ typedef struct dmd_norm_bwd_desc {
   int accumulate;
 } dmd_norm_bwd_desc;
 int dmd_norm_bwd(const dmd_norm_bwd_desc* d, int pass, void* stream);
+/* dmd_norm_bwd in deterministic mode: pass 1 runs one block per image (each per-channel sum has one writer); pass 2 is
+ * dmd_norm_bwd's */
+int dmd_norm_bwd_det(const dmd_norm_bwd_desc* d, int pass, void* stream);
 /* affine GroupNorm parameters after pass 1: dgamma[c] += inv_scale * sum_n sumB[n][c], dbeta[c] += inv_scale * sum_n sumA[n][c] */
 int dmd_norm_affine_grad(const dmd_norm_bwd_desc* d, float* dgamma, float* dbeta, const float* inv_scale, void* stream);
 
@@ -254,6 +260,17 @@ int dmd_norm_affine_grad(const dmd_norm_bwd_desc* d, float* dgamma, float* dbeta
 int dmd_attn_bwd(const float* x, const double* stats_in, const float* gamma, const float* beta, const float* wqkv, const float* bqkv,
                  const float* wout, const float* gout, float* gx, float* dgamma, float* dbeta, float* dwqkv, float* dbqkv,
                  float* dwout, float* dbout, const float* inv_scale, int B, int L, int C, int gs, float eps, void* stream);
+/* The training plans' split attention backward (C = 128, and every C in deterministic mode), the same op list on one block:
+ * the forward's q | k | v and normed input recomputed, the attention core backward, then the projection gradients as sgemm /
+ * column-sum launches and the GroupNorm backward.  gx (NHWC [B][L][C]) is ASSIGNED; the parameter gradients are ADDED (times
+ * inv_scale) to grads + goffs[i], i = gamma, beta, Wqkv, bqkv, Wout, bout (goffs: 6 host offsets, in floats).  1 <= L <= 64,
+ * C in {32, 64, 128}, eps 1e-5; det: fixed-order column sums and norm backward sums.  workspace: 256-byte aligned,
+ * dmd_attn_split_bwd_workspace_bytes(B, L, C) bytes. */
+size_t dmd_attn_split_bwd_workspace_bytes(int B, int L, int C);
+int dmd_attn_split_bwd(const float* x, const double* stats_in, const float* gamma, const float* beta, const float* wqkv,
+                       const float* bqkv, const float* wout, const float* gout, float* gx, float* grads, const long long* goffs,
+                       const float* inv_scale, int B, int L, int C, int gs, int det, void* workspace, size_t workspace_bytes,
+                       void* stream);
 
 /* C[m][n] (+)= alpha * sum_k A[m*sam + k*sak] * B[k*sbk + n*sbn] (alpha: device scalar or NULL = 1).  chunks > 1 splits K into
  * 16-aligned ranges reduced in a fixed order through `partial` (dmd_sgemm_partial_floats floats; needs ldc == N). */
@@ -269,8 +286,16 @@ int dmd_film_wgrad(const float* dfilm, const float* cond, float* grads, const lo
 /* act_emb (inner_model.py:27-30): dE[act[n][t]][j] += inv_scale * de[n][t * CC/T + j]; act [B][T] int64 */
 int dmd_embedding_bwd(const float* de, const int64_t* act, float* dE, int B, int CC, int T, int num_actions, const float* inv_scale,
                       void* stream);
+/* deterministic mode: one thread per table entry walks the batch in order */
+int dmd_embedding_bwd_det(const float* de, const int64_t* act, float* dE, int B, int CC, int T, int num_actions, const float* inv_scale,
+                          void* stream);
 /* bias gradients: out[c] (and out2[c], if not NULL) += inv_scale * sum_rows x[row][c] for c < Creal; x [rows][C], C multiple of 4 */
 int dmd_colsum(const float* x, float* out, float* out2, const float* inv_scale, long long rows, int C, int Creal, void* stream);
+/* deterministic mode: each block stores its column sums to `partial` (at least dmd_colsum_partial_bytes(rows, C) bytes, or the
+ * call fails) and a second launch adds them in block order */
+size_t dmd_colsum_partial_bytes(long long rows, int C);
+int dmd_colsum_det(const float* x, float* out, float* out2, const float* inv_scale, long long rows, int C, int Creal, void* partial,
+                   size_t partial_bytes, void* stream);
 /* nearest-2x upsample adjoint: out [B][H][W][C] (+)= sum of the 2x2 blocks of in [B][2H][2W][C] */
 int dmd_sumpool2(const float* in, float* out, int B, int H, int W, int C, int accumulate, void* stream);
 /* out = dh * silu'(pre) */
