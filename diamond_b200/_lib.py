@@ -70,6 +70,17 @@ class ConvPlanInfo(C.Structure):  # dmd_conv_plan_info
                 ("smem_bytes", C.c_ulonglong), ("weight_bytes", C.c_ulonglong)]
 
 
+class ConvLayerShape(C.Structure):  # dmd_conv_layer_shape
+    _fields_ = [("Cin", _i), ("CoutPad", _i), ("nchunks", _i), ("precise", _i), ("three_pass", _i), ("widthT", _i), ("nsrcT", _i),
+                ("fprop_launches", _i), ("dgrad_launches", _i * 2), ("wgrad_launches", _i * 2), ("packed_bytes", C.c_ulonglong)]
+
+
+class ConvLayerLaunch(C.Structure):  # dmd_conv_layer_launch
+    _fields_ = [("src", _i * 4), ("plane", C.c_longlong * 4), ("C0", _i), ("C1", _i), ("precise", _i), ("wpk", C.c_longlong),
+                ("bias", _i), ("residual", _i), ("residual_is_out", _i), ("stats", _i), ("Cout", _i), ("CoutPad", _i),
+                ("co_off", _i), ("ci_off", _i), ("Cin", _i), ("Cg", _i)]
+
+
 class NormBwdDesc(C.Structure):  # dmd_norm_bwd_desc
     _fields_ = [("x", _vp), ("gy", _vp), ("stats", _vp), ("B", _i), ("HW", _i), ("C", _i), ("gs", _i), ("mode", _i), ("act", _i),
                 ("film", _vp), ("film_stride", _i), ("film_off", _i), ("film_ctot", _i), ("c_off", _i),
@@ -106,6 +117,16 @@ SIGNATURES = {
     "dmd_pack_conv_weight_dgrad": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "dmd_wgrad_partial_bytes": (_sz, []),
     "dmd_conv2d_wgrad": (_i, [C.POINTER(WgradDesc), _vp]),
+    "dmd_conv_layer_create": (_vp, [_i, _i, _i, _i, _i, _i, _i, _i]),
+    "dmd_conv_layer_destroy": (None, [_vp]),
+    "dmd_conv_layer_info": (_i, [_vp, C.POINTER(ConvLayerShape)]),
+    "dmd_conv_layer_pack": (_i, [_vp, _vp, _vp, _vp]),
+    "dmd_conv_layer_fprop": (_i, [_vp, _vp, C.POINTER(ConvDesc), _vp]),
+    "dmd_conv_layer_dgrad": (_i, [_vp, _vp, _i, _vp, _i, _i, _i, _vp, _i, _vp]),
+    "dmd_conv_layer_wgrad": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp, _vp, _vp]),
+    "dmd_conv_layer_fprop_plan": (_i, [_vp, C.POINTER(ConvDesc), C.POINTER(ConvLayerLaunch), _i, C.POINTER(_i)]),
+    "dmd_conv_layer_dgrad_plan": (_i, [_vp, _i, _i, _i, _i, _i, C.POINTER(ConvLayerLaunch), _i, C.POINTER(_i)]),
+    "dmd_conv_layer_wgrad_plan": (_i, [_vp, _i, _i, _i, _i, _i, _i, C.POINTER(ConvLayerLaunch), _i, C.POINTER(_i)]),
     "dmd_gn_stats": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "dmd_gn_stats_det": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "dmd_attn_fwd": (_i, [_vp] * 10 + [_i, _i, _i, _i, _f, _vp]),

@@ -389,8 +389,9 @@ extern "C" int dmd_conv2d_fprop(const dmd_conv_desc* d, void* stream) {
 // ---------------------------------------------------------------------------------------------- wgrad launcher
 // Fills the wgmma weight-gradient launch for one (gradient operand, activation operand) pair.  grad: PLC16, Cg stored
 // channels (<= 64); act: PLC16, Ca stored channels (16 / 32 / 64), both over B images of H x W (conv INPUT size; a
-// stride-2 conv passes its zero-inserted gradient).
-struct WgradLaunch { WgradParams wp; WgradReduceParams rp; size_t smem; int grid; };
+// stride-2 conv passes its zero-inserted gradient).  Like conv_fill, it touches no device: the device's part of the launch (its
+// SM count and zero buffer) is added by wgrad_launch.
+struct WgradLaunch { WgradParams wp; WgradReduceParams rp; size_t smem; };
 static size_t wgrad_partial_bytes(int num_sms) { return (size_t)num_sms * kWgTaps * 64 * 64 * sizeof(float); }
 
 static int wgrad_fill(const void* grad, int Cg, const void* act, int Ca, int B, int H, int W, int taps, float* partial,
@@ -400,14 +401,12 @@ static int wgrad_fill(const void* grad, int Cg, const void* act, int Ca, int B, 
   DMD_CHECK(Cg % 8 == 0 && Cg > 0 && Cg <= 64, "wgrad: gradient operand channels must be a multiple of 8, <= 64 (got %d)", Cg);
   DMD_CHECK(Ca == 16 || Ca == 32 || Ca == 64, "wgrad: activation operand channels must be 16, 32 or 64 (got %d)", Ca);
   DMD_CHECK(Cout > 0 && Cout <= Cg && Cin > 0 && Cin <= Ca && ci_off >= 0 && ci_off + Cin <= CinTot, "wgrad: bad channel counts");
-  if (init_kernels()) return 1;
   memset(L, 0, sizeof(*L));
   const Plc g = plc_geometry(B, H, W);
   const size_t plane = (size_t)g.Qalloc * 16;
   WgradParams& wp = L->wp;
   const int ng = Cg / 8;
   for (int j = 0; j < 8; ++j) wp.a_plane[j] = j < ng ? (const uint8_t*)grad + (size_t)j * plane : nullptr;
-  wp.zeros = g_zeros;
   wp.nB = Ca / 8;
   for (int j = 0; j < wp.nB; ++j) wp.b_plane[j] = (const uint8_t*)act + (size_t)j * plane;
   wp.taps = taps; wp.PW = g.PW; wp.halo = taps == 9 ? g.PW + 1 : 0;
@@ -419,20 +418,23 @@ static int wgrad_fill(const void* grad, int Cg, const void* act, int Ca, int B, 
   wp.stages = stages;
   wp.partial = partial;
   L->smem = wgrad_smem(wp.nB, wp.halo, stages).total;
-  L->grid = wp.num_tiles < g_num_sms ? wp.num_tiles : g_num_sms;
   WgradReduceParams& rp = L->rp;
-  rp.partial = partial; rp.nparts = L->grid; rp.N = Ca;
+  rp.partial = partial; rp.N = Ca;
   rp.Cout = Cout; rp.Cin = Cin; rp.CinTot = CinTot; rp.ci_off = ci_off; rp.co_off = co_off; rp.taps = taps;
   rp.inv_scale = inv_scale; rp.accumulate = accumulate;
   return 0;
 }
 static int wgrad_launch(const WgradLaunch& L, float* dW, cudaStream_t st) {
-  const int N = L.wp.nB * 8;
-  if (N == 16) { if (launch_pdl(wgrad_tc_kernel<16>, dim3(L.grid), dim3(kWgThreads), L.smem, st, L.wp)) return 1; }
-  else if (N == 32) { if (launch_pdl(wgrad_tc_kernel<32>, dim3(L.grid), dim3(kWgThreads), L.smem, st, L.wp)) return 1; }
-  else if (launch_pdl(wgrad_tc_kernel<64>, dim3(L.grid), dim3(kWgThreads), L.smem, st, L.wp)) return 1;
+  if (init_kernels()) return 1;
+  WgradParams wp = L.wp;
+  wp.zeros = g_zeros;
+  const int grid = wp.num_tiles < g_num_sms ? wp.num_tiles : g_num_sms;   // persistent: one CTA per SM, one partial each
+  const int N = wp.nB * 8;
+  if (N == 16) { if (launch_pdl(wgrad_tc_kernel<16>, dim3(grid), dim3(kWgThreads), L.smem, st, wp)) return 1; }
+  else if (N == 32) { if (launch_pdl(wgrad_tc_kernel<32>, dim3(grid), dim3(kWgThreads), L.smem, st, wp)) return 1; }
+  else if (launch_pdl(wgrad_tc_kernel<64>, dim3(grid), dim3(kWgThreads), L.smem, st, wp)) return 1;
   WgradReduceParams rp = L.rp;
-  rp.dW = dW;
+  rp.nparts = grid; rp.dW = dW;
   const int total = rp.taps * 64 * rp.N;
   wgrad_reduce_kernel<<<(total + 63) / 64, 256, 0, st>>>(rp);
   DMD_LAUNCH_OK();
@@ -2399,6 +2401,206 @@ extern "C" int dmd_attn_split_bwd(const float* x, const double* stats_in, const 
   for (const BOp& b : pl.bops)
     if (run_bop(core, pl, b, grads, inv_scale, (cudaStream_t)stream)) return 1;
   return 0;
+}
+
+// ---- per-layer entry points of one nn.Conv2d: the ConvW of Walker::conv on a one-conv model, packed by pack_one and launched
+// through the executors' own expansions (for_each_conv_launch, for_each_dgrad_launch, for_each_wgrad_launch).  The *_plan
+// twins run the same expansions on stand-in pointers and record what they emit, without a device.
+struct dmd_conv_layer { ModelCore core; ConvW cw; };
+
+extern "C" dmd_conv_layer* dmd_conv_layer_create(int cout, int cin_real, int taps, int c0_real, int c0_store, int c1, int split, int dgrad) {
+  // the walker itself refuses a conv that needs more than kMaxConvChunks K-split or backward-data chunks
+  if (!(cout > 0 && cout <= 128 && (taps == 1 || taps == 9) && c0_real > 0 && c0_real <= c0_store && c0_store % 16 == 0 && c1 >= 0 &&
+        c1 % 16 == 0 && cin_real == c0_real + c1)) {
+    fail("conv_layer: unsupported conv %d -> %d (taps %d, first source %d real in %d stored, second source %d)", cin_real, cout, taps,
+         c0_real, c0_store, c1);
+    return nullptr;
+  }
+  std::unique_ptr<dmd_conv_layer> h(new dmd_conv_layer());
+  Walker w{&h->core};
+  h->cw = w.conv(cout, cin_real, taps, c0_real, c0_store, c1, split != 0, dgrad != 0);
+  if (w.err) return nullptr;   // dmd_last_error() says why
+  h->core.finish(w.pk);
+  return h.release();
+}
+extern "C" void dmd_conv_layer_destroy(dmd_conv_layer* h) { delete h; }
+
+namespace {
+
+// the one-launch description of the layer's forward, as PlanBuilder::conv and the actor-critic's run_conv fill it: the caller's
+// operands, bias, residual, output and statistics, the layer's weights and split-fp16 mode.  plane: bytes of one PLC16 plane
+int layer_fprop_desc(const dmd_conv_layer* h, const uint8_t* packed, const dmd_conv_desc* d, dmd_conv_desc* o, size_t* plane) {
+  DMD_CHECK(h && packed && d && d->src0 && d->out, "conv_layer: null layer, packed buffer, descriptor, src0 or out");
+  const ConvW& cw = h->cw;
+  DMD_CHECK(d->C0 == cw.c0_store && d->C1 == cw.Cin - cw.c0_store, "conv_layer: operand channels %d+%d, the layer takes %d+%d", d->C0,
+            d->C1, cw.c0_store, cw.Cin - cw.c0_store);
+  const bool split = cw.precise || cw.three_pass;
+  if (split) DMD_CHECK(d->src0_lo && (!d->C1 || d->src1_lo), "conv_layer: a split-fp16 layer needs the low operand parts");
+  DMD_CHECK(!d->wpk_x, "conv_layer: a layer carries no fused projection");
+  DMD_CHECK(d->B > 0 && d->H > 0 && d->W > 0, "conv_layer: bad size %dx%dx%d", d->B, d->H, d->W);
+  *o = *d;
+  if (!split) o->src0_lo = o->src1_lo = nullptr;
+  o->wpk = packed + cw.pk_off; o->precise = cw.precise; o->taps = cw.taps; o->Cout = cw.Cout; o->CoutPad = cw.CoutPad;
+  *plane = (size_t)plc_geometry(d->B, d->H, d->W).Qalloc * 16;   // one PLC16 plane holds 8 channels
+  return 0;
+}
+
+int layer_wgrad_check(const dmd_conv_layer* h, int Ca, int Cin, int ci_off) {
+  DMD_CHECK(h, "conv_layer: null layer");
+  DMD_CHECK(Cin > 0 && Cin <= Ca && ci_off >= 0 && ci_off + Cin <= h->cw.CinReal, "conv_layer_wgrad: input channels [%d, %d + %d) of %d (Ca %d)",
+            ci_off, ci_off, Cin, h->cw.CinReal, Ca);
+  return 0;
+}
+
+// stand-in pointers of the host-only twins, far apart so that each pointer an expansion emits names the operand it points into
+// (0 src0 / gradient, 1 src1 / activation, 2 src0_lo, 3 src1_lo, 4 residual, 5 out, 6 bias, 7 statistics, 8 packed buffer)
+constexpr uintptr_t kTwinSpan = 1ull << 40;
+inline uint8_t* twin(int i) { return (uint8_t*)(kTwinSpan * (uintptr_t)(i + 1)); }
+void twin_locate(const void* p, size_t plane, int* which, long long* at) {
+  if (!p) { *which = -1; *at = 0; return; }
+  const uintptr_t u = (uintptr_t)p, off = u % kTwinSpan;
+  *which = (int)(u / kTwinSpan) - 1;
+  *at = off % plane ? -1 : (long long)(off / plane);
+}
+struct TwinRecorder {
+  dmd_conv_layer_launch* out; int cap; int n = 0;
+  dmd_conv_layer_launch* next() {
+    if (n >= cap) { fail("conv_layer plan: more than %d launches", cap); return nullptr; }
+    dmd_conv_layer_launch* L = out + n++;
+    memset(L, 0, sizeof(*L));
+    return L;
+  }
+  int conv(const dmd_conv_desc& x, size_t plane) {
+    ConvParams p; size_t smem; int cols;
+    if (conv_fill(&x, &p, &smem, &cols)) return 1;   // the launch's own checks, as dmd_conv_plan runs them
+    dmd_conv_layer_launch* L = next();
+    if (!L) return 1;
+    const void* srcs[4] = {x.src0, x.src1, x.src0_lo, x.src1_lo};
+    for (int i = 0; i < 4; ++i) twin_locate(srcs[i], plane, &L->src[i], &L->plane[i]);
+    L->C0 = x.C0; L->C1 = x.C1; L->precise = x.precise;
+    L->wpk = (long long)((const uint8_t*)x.wpk - twin(8));
+    L->bias = x.bias != nullptr; L->residual = x.residual && x.residual != x.out; L->residual_is_out = x.residual && x.residual == x.out;
+    L->stats = x.out_stats != nullptr;
+    L->Cout = x.Cout; L->CoutPad = x.CoutPad;
+    return 0;
+  }
+  int wgrad(const WgradLaunch& W, size_t plane) {
+    dmd_conv_layer_launch* L = next();
+    if (!L) return 1;
+    twin_locate(W.wp.a_plane[0], plane, &L->src[0], &L->plane[0]);
+    twin_locate(W.wp.b_plane[0], plane, &L->src[1], &L->plane[1]);
+    L->src[2] = L->src[3] = -1;
+    for (int j = 0; j < 8; ++j) L->Cg += W.wp.a_plane[j] ? 8 : 0;
+    L->C0 = W.rp.N;
+    L->co_off = W.rp.co_off; L->ci_off = W.rp.ci_off; L->Cout = W.rp.Cout; L->Cin = W.rp.Cin;
+    return 0;
+  }
+};
+
+int layer_fprop_twin(const dmd_conv_layer* h, const dmd_conv_desc* d, dmd_conv_layer_launch* out, int cap, int* n) {
+  DMD_CHECK(d && out && n, "conv_layer plan: null argument");
+  dmd_conv_desc s = *d;   // the caller's pointers say only which operands are present
+  const void** ps[8] = {&s.src0, &s.src1, &s.src0_lo, &s.src1_lo, (const void**)&s.residual, (const void**)&s.out, (const void**)&s.bias,
+                        (const void**)&s.out_stats};
+  for (int i = 0; i < 8; ++i) if (*ps[i]) *ps[i] = twin(i);
+  dmd_conv_desc dc; size_t plane;
+  if (layer_fprop_desc(h, twin(8), &s, &dc, &plane)) return 1;
+  TwinRecorder r{out, cap};
+  if (for_each_conv_launch(h->cw, dc, plane, [&](size_t off) { return twin(8) + off; },
+                           [&](const dmd_conv_desc& x) { return r.conv(x, plane); })) return 1;
+  *n = r.n;
+  return 0;
+}
+int layer_dgrad_twin(const dmd_conv_layer* h, int k, int B, int H, int W, int accumulate, dmd_conv_layer_launch* out, int cap, int* n) {
+  DMD_CHECK(h && out && n, "conv_layer plan: null argument");
+  DMD_CHECK(k >= 0 && k < h->cw.nsrcT, "conv_layer_dgrad: source %d has no backward-data pack (the layer has %d)", k, h->cw.nsrcT);
+  DMD_CHECK(B > 0 && H > 0 && W > 0, "conv_layer_dgrad: bad size %dx%dx%d", B, H, W);
+  const size_t plane = (size_t)plc_geometry(B, H, W).Qalloc * 16;
+  TwinRecorder r{out, cap};
+  if (for_each_dgrad_launch(h->cw, k, twin(8), twin(0), B, H, W, (float*)twin(5), accumulate != 0,
+                            [&](const dmd_conv_desc& x) { return r.conv(x, plane); })) return 1;
+  *n = r.n;
+  return 0;
+}
+int layer_wgrad_twin(const dmd_conv_layer* h, int Ca, int Cin, int ci_off, int B, int H, int W, dmd_conv_layer_launch* out, int cap, int* n) {
+  DMD_CHECK(out && n, "conv_layer plan: null argument");
+  if (layer_wgrad_check(h, Ca, Cin, ci_off)) return 1;
+  DMD_CHECK(B > 0 && H > 0 && W > 0, "conv_layer_wgrad: bad size %dx%dx%d", B, H, W);
+  const size_t plane = (size_t)plc_geometry(B, H, W).Qalloc * 16;
+  TwinRecorder r{out, cap};
+  if (for_each_wgrad_launch(h->cw, twin(0), twin(1), Ca, Cin, ci_off, B, H, W, (float*)twin(7), nullptr,
+                            [&](const WgradLaunch& L) { return r.wgrad(L, plane); })) return 1;
+  *n = r.n;
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int dmd_conv_layer_info(const dmd_conv_layer* h, dmd_conv_layer_shape* out) {
+  DMD_CHECK(h && out, "conv_layer_info: null argument");
+  const ConvW& cw = h->cw;
+  memset(out, 0, sizeof(*out));
+  out->Cin = cw.Cin; out->CoutPad = cw.CoutPad; out->nchunks = cw.nchunks; out->precise = cw.precise; out->three_pass = cw.three_pass;
+  out->widthT = cw.widthT; out->nsrcT = cw.nsrcT; out->packed_bytes = h->core.packed_bytes;
+  // launch counts at an 8 x 8 image, with both sources (and their low parts) present
+  dmd_conv_layer_launch L[3 * kMaxConvChunks];
+  const int cap = 3 * kMaxConvChunks, c1 = cw.Cin - cw.c0_store;
+  dmd_conv_desc d; memset(&d, 0, sizeof(d));
+  d.src0 = d.src0_lo = d.out = (float*)1; d.src1 = d.src1_lo = c1 ? (const void*)1 : nullptr;
+  d.C0 = cw.c0_store; d.C1 = c1; d.B = 1; d.H = d.W = 8; d.stride = 1;
+  if (layer_fprop_twin(h, &d, L, cap, &out->fprop_launches)) return 1;
+  for (int k = 0; k < cw.nsrcT; ++k)
+    if (layer_dgrad_twin(h, k, 1, 8, 8, 0, L, cap, &out->dgrad_launches[k])) return 1;
+  const int ca[2] = {cw.c0_store, c1}, cin[2] = {cw.c0_real, c1};
+  for (int k = 0; k < (c1 ? 2 : 1); ++k)
+    if (layer_wgrad_twin(h, ca[k], cin[k], k ? cw.c0_real : 0, 1, 8, 8, L, cap, &out->wgrad_launches[k])) return 1;
+  return 0;
+}
+extern "C" int dmd_conv_layer_fprop_plan(const dmd_conv_layer* h, const dmd_conv_desc* d, dmd_conv_layer_launch* out, int cap, int* n) {
+  return layer_fprop_twin(h, d, out, cap, n);
+}
+extern "C" int dmd_conv_layer_dgrad_plan(const dmd_conv_layer* h, int k, int B, int H, int W, int accumulate, dmd_conv_layer_launch* out,
+                                         int cap, int* n) {
+  return layer_dgrad_twin(h, k, B, H, W, accumulate, out, cap, n);
+}
+extern "C" int dmd_conv_layer_wgrad_plan(const dmd_conv_layer* h, int Ca, int Cin, int ci_off, int B, int H, int W,
+                                         dmd_conv_layer_launch* out, int cap, int* n) {
+  return layer_wgrad_twin(h, Ca, Cin, ci_off, B, H, W, out, cap, n);
+}
+
+extern "C" int dmd_conv_layer_pack(const dmd_conv_layer* h, const float* w, void* packed, void* stream) {
+  DMD_CHECK(h && w && packed, "conv_layer_pack: null argument");
+  DMD_CHECK(((uintptr_t)packed & 255) == 0, "conv_layer_pack: the packed buffer must be 256-byte aligned");
+  ModelCore m;   // the layer's weight (tensor 0) and packed buffer
+  m.ptrs = {w, nullptr};
+  m.packed = (uint8_t*)packed;
+  return pack_one(m, h->cw, (cudaStream_t)stream);
+}
+extern "C" int dmd_conv_layer_fprop(const dmd_conv_layer* h, const void* packed, const dmd_conv_desc* d, void* stream) {
+  dmd_conv_desc dc; size_t plane;
+  if (layer_fprop_desc(h, (const uint8_t*)packed, d, &dc, &plane)) return 1;
+  cudaStream_t st = (cudaStream_t)stream;
+  return for_each_conv_launch(h->cw, dc, plane, [&](size_t off) { return (const uint8_t*)packed + off; },
+                              [&](const dmd_conv_desc& x) { return dmd_conv2d_fprop(&x, st); });
+}
+extern "C" int dmd_conv_layer_dgrad(const dmd_conv_layer* h, const void* packed, int k, const void* gy, int B, int H, int W, float* out,
+                                    int accumulate, void* stream) {
+  DMD_CHECK(h && packed && gy && out, "conv_layer_dgrad: null argument");
+  DMD_CHECK(k >= 0 && k < h->cw.nsrcT, "conv_layer_dgrad: source %d has no backward-data pack (the layer has %d)", k, h->cw.nsrcT);
+  cudaStream_t st = (cudaStream_t)stream;
+  return for_each_dgrad_launch(h->cw, k, (const uint8_t*)packed, (const uint8_t*)gy, B, H, W, out, accumulate != 0,
+                               [&](const dmd_conv_desc& x) { return dmd_conv2d_fprop(&x, st); });
+}
+extern "C" int dmd_conv_layer_wgrad(const dmd_conv_layer* h, const void* gy, const void* act, int Ca, int Cin, int ci_off, int B, int H,
+                                    int W, void* partial, size_t partial_bytes, const float* inv_scale, float* dW, void* stream) {
+  DMD_CHECK(gy && act && partial && dW, "conv_layer_wgrad: null argument");
+  if (layer_wgrad_check(h, Ca, Cin, ci_off)) return 1;
+  if (init_kernels()) return 1;
+  DMD_CHECK(partial_bytes >= wgrad_partial_bytes(g_num_sms), "conv_layer_wgrad: partial buffer too small (%zu < %zu)", partial_bytes,
+            wgrad_partial_bytes(g_num_sms));
+  cudaStream_t st = (cudaStream_t)stream;
+  return for_each_wgrad_launch(h->cw, (const uint8_t*)gy, (const uint8_t*)act, Ca, Cin, ci_off, B, H, W, (float*)partial, inv_scale,
+                               [&](const WgradLaunch& L) { return wgrad_launch(L, dW, st); });
 }
 
 extern "C" size_t dmd_denoiser_train_workspace_bytes(const dmd_denoiser* h, int B, int H, int W) {

@@ -257,6 +257,104 @@ def conv2d_wgrad(grad_op: Tensor, cg: int, act_op: Tensor, ca: int, b: int, h: i
     return dw
 
 
+class ConvLayer:
+    """One nn.Conv2d as the executors build it (dmd_conv_layer_create): its K-split chunks, split-fp16 passes, backward-data
+    chunks and weight-gradient blocks are the executors' own.  The *_plan methods record those launches without a device."""
+
+    _PLAN_CAP = 16
+
+    def __init__(self, cout: int, cin_real: int, taps: int, c0_real: int, c0_store: int, c1: int = 0, split: bool = False,
+                 dgrad: bool = True):
+        lib = _lib.lib()
+        self.h = lib.dmd_conv_layer_create(cout, cin_real, taps, c0_real, c0_store, c1, int(split), int(dgrad))
+        if not self.h:
+            raise RuntimeError("diamond_b200: " + lib.dmd_last_error().decode("utf-8", "replace"))
+        self._destroy = lib.dmd_conv_layer_destroy
+        self.cout, self.cin_real, self.taps, self.c0_real, self.c0_store, self.c1 = cout, cin_real, taps, c0_real, c0_store, c1
+        s = _lib.ConvLayerShape()
+        _lib.check(lib.dmd_conv_layer_info(self.h, C.byref(s)))
+        self.info = {f: (list(getattr(s, f)) if f.endswith("_launches") and f != "fprop_launches" else getattr(s, f))
+                     for f, _ in s._fields_}
+
+    def __del__(self):
+        if getattr(self, "h", None):
+            self._destroy(self.h)
+            self.h = None
+
+    def pack(self, w: Tensor) -> Tensor:
+        """The layer's packs of the torch weight w [cout][cin_real][k][k] in a new buffer."""
+        _cuda(w)
+        packed = torch.empty(self.info["packed_bytes"], dtype=torch.uint8, device=w.device)
+        _lib.check(_lib.lib().dmd_conv_layer_pack(self.h, w.data_ptr(), packed.data_ptr(), _lib.current_stream()))
+        return packed
+
+    def _desc(self, n0, n1, lo0, lo1, b, h, w, stride, bias, residual, out, ostats, out_gs):
+        d = _lib.ConvDesc()
+        d.src0, d.src1, d.C0, d.C1 = n0, n1, self.c0_store, self.c1
+        d.src0_lo, d.src1_lo = lo0, lo1
+        d.B, d.H, d.W, d.stride = b, h, w, stride
+        d.bias, d.residual, d.out, d.out_stats, d.out_gs = bias, residual, out, ostats, out_gs
+        return d
+
+    def fprop(self, packed: Tensor, n0: Tensor, n1: Optional[Tensor], b: int, h: int, w: int, out: Tensor, *,
+              lo0: Optional[Tensor] = None, lo1: Optional[Tensor] = None, stride: int = 1, bias: Optional[Tensor] = None,
+              residual: Optional[Tensor] = None, ostats: Optional[Tensor] = None, out_gs: int = 0) -> Tensor:
+        """out (NHWC [b][h/stride][w/stride][cout]) = conv of the PLC16 operands (+ bias, + residual); ostats += its GroupNorm
+        (sum, sumsq) in groups of out_gs channels."""
+        _cuda(packed, n0, n1, lo0, lo1, bias, residual, out, ostats)
+        d = self._desc(n0.data_ptr(), _lib.ptr(n1), _lib.ptr(lo0), _lib.ptr(lo1), b, h, w, stride, _lib.ptr(bias), _lib.ptr(residual),
+                       out.data_ptr(), _lib.ptr(ostats), out_gs)
+        _lib.check(_lib.lib().dmd_conv_layer_fprop(self.h, packed.data_ptr(), C.byref(d), _lib.current_stream()))
+        return out
+
+    def dgrad(self, packed: Tensor, k: int, gy_op: Tensor, b: int, h: int, w: int, out: Tensor, accumulate: bool = False) -> Tensor:
+        """out (NHWC [b][h][w][channels of source k]) (+)= the input gradient of source k from the PLC16 gradient operand at the
+        conv input size."""
+        _cuda(packed, gy_op, out)
+        _lib.check(_lib.lib().dmd_conv_layer_dgrad(self.h, packed.data_ptr(), k, gy_op.data_ptr(), b, h, w, out.data_ptr(),
+                                                   int(accumulate), _lib.current_stream()))
+        return out
+
+    def wgrad(self, gy_op: Tensor, act_op: Tensor, ca: int, cin: int, ci_off: int, b: int, h: int, w: int, dw: Tensor,
+              inv_scale: Optional[Tensor] = None, partial: Optional[Tensor] = None) -> Tensor:
+        """dw [cout][cin_real][taps] += inv_scale * the weight gradient of input channels [ci_off, ci_off + cin) (act_op: ca
+        stored channels)."""
+        _cuda(gy_op, act_op, dw, inv_scale, partial)
+        lib = _lib.lib()
+        if partial is None:
+            partial = torch.empty(lib.dmd_wgrad_partial_bytes(), dtype=torch.uint8, device=dw.device)
+        _lib.check(lib.dmd_conv_layer_wgrad(self.h, gy_op.data_ptr(), act_op.data_ptr(), ca, cin, ci_off, b, h, w, partial.data_ptr(),
+                                            partial.numel() * partial.element_size(), _lib.ptr(inv_scale), dw.data_ptr(),
+                                            _lib.current_stream()))
+        return dw
+
+    @staticmethod
+    def _launches(buf, n):
+        return [{f: (list(getattr(buf[i], f)) if f in ("src", "plane") else getattr(buf[i], f)) for f, _ in _lib.ConvLayerLaunch._fields_}
+                for i in range(n.value)]
+
+    def fprop_plan(self, b: int, h: int, w: int, *, stride: int = 1, bias: bool = True, residual: bool = False, stats: bool = False,
+                   out_gs: int = 0, lo: Optional[bool] = None) -> list:
+        """The forward's launches (dicts of dmd_conv_layer_launch), recorded without a device; lo: pass low operand parts
+        (default: when the layer is split-fp16)."""
+        lo = bool(self.info["precise"] or self.info["three_pass"]) if lo is None else lo
+        d = self._desc(1, 1 if self.c1 else None, 1 if lo else None, 1 if (lo and self.c1) else None, b, h, w, stride,
+                       1 if bias else None, 1 if residual else None, 1, 1 if stats else None, out_gs)
+        buf, n = (_lib.ConvLayerLaunch * self._PLAN_CAP)(), C.c_int(0)
+        _lib.check(_lib.lib().dmd_conv_layer_fprop_plan(self.h, C.byref(d), buf, self._PLAN_CAP, C.byref(n)))
+        return self._launches(buf, n)
+
+    def dgrad_plan(self, k: int, b: int, h: int, w: int, accumulate: bool = False) -> list:
+        buf, n = (_lib.ConvLayerLaunch * self._PLAN_CAP)(), C.c_int(0)
+        _lib.check(_lib.lib().dmd_conv_layer_dgrad_plan(self.h, k, b, h, w, int(accumulate), buf, self._PLAN_CAP, C.byref(n)))
+        return self._launches(buf, n)
+
+    def wgrad_plan(self, ca: int, cin: int, ci_off: int, b: int, h: int, w: int) -> list:
+        buf, n = (_lib.ConvLayerLaunch * self._PLAN_CAP)(), C.c_int(0)
+        _lib.check(_lib.lib().dmd_conv_layer_wgrad_plan(self.h, ca, cin, ci_off, b, h, w, buf, self._PLAN_CAP, C.byref(n)))
+        return self._launches(buf, n)
+
+
 # ------------------------------------------------------------------------------------------------ backward kernels
 # One wrapper per C entry point of the CUDA-core backward kernels.  Outputs that the kernels accumulate into are passed in
 # by the caller; the launch geometry is the library's (the same launchers the training executors use).

@@ -174,6 +174,66 @@ typedef struct dmd_conv_plan_info {
 int dmd_conv_plan(const dmd_conv_desc* d, dmd_conv_plan_info* out);
 int dmd_prep_plan(const dmd_prep_desc* d, int* blocks, int* pos_per_block, int* sources);
 
+/* One nn.Conv2d as the denoiser, reward / termination and actor-critic executors build it: the arguments are those of their
+ * layer walker (cout output channels; cin_real input channels, the first source's c0_real of them stored as c0_store
+ * channels, then c1 of a second concat source; split: split-fp16 forward; dgrad: backward-data packs).  A conv over more than
+ * 128 input channels, or whose packed weights exceed 144 KB, runs as K-split chunks (split-fp16 chunks in one launch each, or
+ * as three passes A_hi W_hi, A_lo W_hi, A_hi W_lo); its backward-data packs over 144 KB run in chunks of widthT gradient
+ * channels; its weight gradient runs in 64 x 64 (Cout, Cin) blocks.  create returns NULL (dmd_last_error() says why) for a
+ * shape the walker refuses, such as one needing more than 4 K-split chunks. */
+typedef struct dmd_conv_layer dmd_conv_layer;
+dmd_conv_layer* dmd_conv_layer_create(int cout, int cin_real, int taps, int c0_real, int c0_store, int c1, int split, int dgrad);
+void dmd_conv_layer_destroy(dmd_conv_layer* h);
+typedef struct dmd_conv_layer_shape {
+  int Cin, CoutPad;      /* stored input channels (both sources), padded output channels */
+  int nchunks;           /* K-split chunks (0: none) */
+  int precise;           /* split-fp16 in one launch per chunk (K = 3 x chunk) */
+  int three_pass;        /* split-fp16 as three launches per chunk */
+  int widthT;            /* gradient channels per backward-data chunk (0: one launch per source) */
+  int nsrcT;             /* sources with backward-data packs (0: dgrad = 0) */
+  int fprop_launches;    /* launches of one forward */
+  int dgrad_launches[2]; /* launches of the backward-data of each source */
+  int wgrad_launches[2]; /* weight-gradient blocks of each source */
+  unsigned long long packed_bytes;   /* bytes of the packed buffer */
+} dmd_conv_layer_shape;
+int dmd_conv_layer_info(const dmd_conv_layer* h, dmd_conv_layer_shape* out);
+/* Writes every pack of the layer (forward chunks, low parts, transposed backward-data chunks) from the torch weight w
+ * [cout][cin_real][k][k] into `packed` (packed_bytes, 256-byte aligned). */
+int dmd_conv_layer_pack(const dmd_conv_layer* h, const float* w, void* packed, void* stream);
+/* The layer's forward from its one-launch description d: PLC16 operands src0 (C0 = c0_store channels) and src1 (C1 = c1), with
+ * their low parts src0_lo / src1_lo for a split layer; bias, residual, out, out_stats / out_gs as for dmd_conv2d_fprop.  wpk,
+ * precise, taps, Cout and CoutPad are the layer's own.  Bias and residual go with the first launch, statistics with the last;
+ * later launches add to out. */
+int dmd_conv_layer_fprop(const dmd_conv_layer* h, const void* packed, const dmd_conv_desc* d, void* stream);
+/* Backward-data of source k (0 or 1): out [B][H][W][channels of source k] (+)= the gradient wrt that source's input, from the
+ * PLC16 gradient operand gy (round16(cout) channels at the conv INPUT size B x H x W; a stride-2 conv passes it
+ * zero-inserted, dmd_prep_desc.upsample = 2) */
+int dmd_conv_layer_dgrad(const dmd_conv_layer* h, const void* packed, int k, const void* gy, int B, int H, int W, float* out,
+                         int accumulate, void* stream);
+/* Weight gradient of the input channels [ci_off, ci_off + Cin) from the PLC16 operand act (Ca stored channels, channel i =
+ * input channel ci_off + i) and gy as for dgrad: dW [cout][cin_real][taps] += inv_scale * the gradient (always accumulates).
+ * partial: dmd_wgrad_partial_bytes() bytes at least. */
+int dmd_conv_layer_wgrad(const dmd_conv_layer* h, const void* gy, const void* act, int Ca, int Cin, int ci_off, int B, int H, int W,
+                         void* partial, size_t partial_bytes, const float* inv_scale, float* dW, void* stream);
+/* Host-only twins of the three: the same expansions on stand-in pointers, touching no device.  The non-NULL pointers of d only
+ * say which operands are present.  Each launch is recorded (at most cap; *n of them) as: */
+typedef struct dmd_conv_layer_launch {
+  int src[4];            /* what the launch's src0, src1, src0_lo, src1_lo point into: 0 src0 (dgrad, wgrad: gy), 1 src1 (wgrad: act),
+                            2 src0_lo, 3 src1_lo; -1 NULL.  Weight-gradient blocks: src[0] gradient, src[1] activation operand */
+  long long plane[4];    /* ... at which PLC16 plane (8 channels) of it */
+  int C0, C1;            /* operand channels of the launch (weight-gradient blocks: C0 = activation channels) */
+  int precise;
+  long long wpk;         /* byte offset of the launch's weight pack in the packed buffer */
+  int bias, residual, residual_is_out, stats;   /* carries the bias / the caller's residual / out as residual / statistics */
+  int Cout, CoutPad;     /* output channels (weight-gradient blocks: of the block) */
+  int co_off, ci_off, Cin, Cg;   /* weight-gradient blocks: dW[co_off + co][ci_off + ci], Cg gradient operand channels */
+} dmd_conv_layer_launch;
+int dmd_conv_layer_fprop_plan(const dmd_conv_layer* h, const dmd_conv_desc* d, dmd_conv_layer_launch* out, int cap, int* n);
+int dmd_conv_layer_dgrad_plan(const dmd_conv_layer* h, int k, int B, int H, int W, int accumulate, dmd_conv_layer_launch* out, int cap,
+                              int* n);
+int dmd_conv_layer_wgrad_plan(const dmd_conv_layer* h, int Ca, int Cin, int ci_off, int B, int H, int W, dmd_conv_layer_launch* out,
+                              int cap, int* n);
+
 /* GroupNorm partial sums of an NHWC tensor: stats[n][g] += (sum, sumsq) (blocks.py:28,43). */
 int dmd_gn_stats(const float* x, double* stats, int B, int HW, int C, int gs, void* stream);
 /* The same sums as torch.use_deterministic_algorithms runs them: one cluster of 8 CTAs per (image, group) adds fixed pixel
