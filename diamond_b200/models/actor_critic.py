@@ -179,6 +179,7 @@ class _PredictActValueFn(torch.autograd.Function):
         ws = module._acquire_ws(lib.dmd_actor_critic_workspace_bytes(h, obs.size(0)))
         logits, val, hx_o, cx_o = module._native_forward(obs, hx.detach(), cx.detach(), ws)
         ctx.module, ctx.ws, ctx.b = module, ws, obs.size(0)
+        ctx.under_ddp = module._under_ddp()
         ctx.save_for_backward(hx.detach(), cx.detach(), hx_o)
         ctx.set_materialize_grads(False)
         return logits, val, hx_o, cx_o
@@ -206,7 +207,8 @@ class _PredictActValueFn(torch.autograd.Function):
         if module.accumulate_native_grads:
             # One flat gradient buffer per backward pass: every node of the BPTT graph ADDS into it natively, and a callback that the
             # autograd engine runs once the pass is complete hands it to the parameters.  (Returning ~40 gradient views per node
-            # instead makes autograd's AccumulateGrad launch ~40 tiny additions for each of the ~60 nodes of a rollout.)
+            # instead makes autograd's AccumulateGrad launch ~40 tiny additions for each of the ~60 nodes of a rollout.)  Under DDP
+            # one node hands autograd views of the buffer instead (NativeStateMixin._pass_param_grads).
             flat = module.__dict__.get("_grad_acc")
             if flat is None:
                 flat = module.__dict__["_grad_acc"] = torch.empty(total, dtype=torch.float32, device=dev)
@@ -215,7 +217,7 @@ class _PredictActValueFn(torch.autograd.Function):
             else:
                 _lib.check(lib.dmd_actor_critic_backward_accumulate(*args, flat.data_ptr(), total, *tail))
             module._release_ws(ctx.ws, module._WS_POOL_CAP)
-            return (None, None, g_hx_in, g_cx_in, *([None] * len(offs)))
+            return (None, None, g_hx_in, g_cx_in, *module._pass_param_grads(ctx, flat))
         flat = torch.empty(total, dtype=torch.float32, device=dev)
         _lib.check(lib.dmd_actor_critic_backward(*args, flat.data_ptr(), total, *tail))
         module._release_ws(ctx.ws, module._WS_POOL_CAP)

@@ -140,6 +140,7 @@ class _InnerModelFn(torch.autograd.Function):
                                                          obs_.data_ptr(), act_.data_ptr(), out.data_ptr(), ws.data_ptr(), ws.numel(),
                                                          _lib.current_stream()))
         ctx.module, ctx.shape, ctx.ws, ctx.keep = module, (b, hh, ww), ws, (noisy_, obs_, cn, act_)
+        ctx.under_ddp = module._under_ddp()
         return out
 
     @staticmethod

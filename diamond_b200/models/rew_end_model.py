@@ -251,6 +251,7 @@ class _RewEndFn(torch.autograd.Function):
                                                      rew.data_ptr(), end.data_ptr(), hx_o.data_ptr(), cx_o.data_ptr(), ws.data_ptr(),
                                                      ws.numel(), _lib.current_stream()))
         ctx.module, ctx.shape, ctx.ws = module, (b, t), ws
+        ctx.under_ddp = module._under_ddp()
         return rew, end, hx_o, cx_o
 
     @staticmethod

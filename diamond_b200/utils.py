@@ -1,10 +1,12 @@
 """The two helpers of the reference's src/utils.py that the mirrored models need (init_lstm utils.py:184-196)."""
 import ctypes as C
+import weakref
 from typing import Any, Dict, Tuple
 
 import torch
 import torch.nn as nn
 from torch import Tensor
+from torch.nn.parallel import DistributedDataParallel
 
 from . import _lib
 
@@ -132,22 +134,54 @@ class NativeStateMixin:
     # stores gradients into `.grad`, its nodes ADD into one buffer natively and `.grad` becomes views of it when the pass ends,
     # so that a data-parallel step all-reduces the whole model in one collective (allreduce_native_gradients).  `_grad_acc` is
     # the buffer of the running pass, `last_flat_grad` the one of the last pass.
+    #
+    # Under DistributedDataParallel that callback would come too late: DDP averages what the parameters' AccumulateGrad nodes
+    # receive, and its own end-of-pass callback, which runs after ours, overwrites `.grad` with that average.  A node made
+    # inside a DDP forward therefore hands autograd views of the pass's buffer instead (once per pass; every other node of
+    # the pass still adds natively and returns None).  Each AccumulateGrad node depends on every native node of the pass, so it
+    # runs after the last native add and passes the complete sum to DDP's hook once.
+
+    def _under_ddp(self) -> bool:
+        """True while a DistributedDataParallel wrapper whose module is this one or contains it runs its forward.  torch sets
+        `_active_ddp_module` for the duration of that forward only, so a native autograd Function asks here in its forward
+        and keeps the answer on its ctx for the backward.  The containment walk is cached per wrapper."""
+        ddp = DistributedDataParallel._active_ddp_module
+        if ddp is None:
+            return False
+        seen = self.__dict__.get("_ddp_wrappers")
+        if seen is None:
+            seen = self.__dict__["_ddp_wrappers"] = weakref.WeakKeyDictionary()
+        inside = seen.get(ddp)
+        if inside is None:
+            inside = seen[ddp] = any(m is self for m in ddp.module.modules())
+        return inside
+
+    def _pass_param_grads(self, node, flat):
+        """What a node that wrote or added its parameter gradients into the pass's buffer `flat` returns to autograd: views of
+        `flat` for the first node of the pass made inside a DDP forward (`node.under_ddp`), None for every other one."""
+        offs, nums, _ = self._grad_views_layout()
+        if getattr(node, "under_ddp", False) and self.__dict__.get("_grad_views") is not flat:
+            self.__dict__["_grad_views"] = flat
+            return [flat[o:o + n].view_as(p) for o, n, p in zip(offs, nums, self.parameters())]
+        return [None] * len(offs)
 
     def _adopt_accumulated_grads(self) -> None:
         """End of a backward pass (autograd engine callback): the flat buffer the nodes accumulated into becomes `.grad` (added to
-        an existing `.grad`, like AccumulateGrad) and is remembered as `last_flat_grad` for a one-collective all-reduce."""
+        an existing `.grad`, like AccumulateGrad) and is remembered as `last_flat_grad` for a one-collective all-reduce.  When a
+        node already handed autograd views of it (DDP), AccumulateGrad has stored them and only `last_flat_grad` is set."""
         flat = self.__dict__.pop("_grad_acc", None)
         if flat is None:
             return
-        offs, nums, _ = self._grad_views_layout()
-        for p, o, n in zip(self.parameters(), offs, nums):
-            if not p.requires_grad:
-                continue
-            g = flat[o:o + n].view_as(p)
-            if p.grad is None:
-                p.grad = g
-            else:
-                p.grad.add_(g)
+        if self.__dict__.pop("_grad_views", None) is not flat:
+            offs, nums, _ = self._grad_views_layout()
+            for p, o, n in zip(self.parameters(), offs, nums):
+                if not p.requires_grad:
+                    continue
+                g = flat[o:o + n].view_as(p)
+                if p.grad is None:
+                    p.grad = g
+                else:
+                    p.grad.add_(g)
         self.last_flat_grad = flat
 
     def _engine_stores_grads(self, node) -> bool:
@@ -161,6 +195,7 @@ class NativeStateMixin:
         if cached is not None and cached[0] == task:
             return cached[1]
         self.__dict__.pop("_grad_acc", None)
+        self.__dict__.pop("_grad_views", None)
         n = len(self._grad_views_layout()[0])
         accs = [f for f, _ in node.next_functions[-n:] if f is not None]
         try:
@@ -177,8 +212,8 @@ class NativeStateMixin:
 
         Under `loss.backward()` the first node of the pass writes a new buffer and every later node of the pass (the autoregressive
         steps of Denoiser.forward) adds to it; a callback at the end of the pass makes it `.grad`, so no per-tensor
-        AccumulateGrad runs inside a pass.  Otherwise (torch.autograd.grad, backward(inputs=...)) each node returns views of its
-        own buffer, as autograd expects."""
+        AccumulateGrad runs inside a pass (under DDP one node returns views of it instead, see `_pass_param_grads`).  Otherwise
+        (torch.autograd.grad, backward(inputs=...)) each node returns views of its own buffer, as autograd expects."""
         offs, nums, total = self._grad_views_layout()
         dev = self.device
         if not self._engine_stores_grads(node):
@@ -196,7 +231,7 @@ class NativeStateMixin:
             flat = self.__dict__["_grad_acc"] = torch.empty(total, dtype=torch.float32, device=dev)
             run(flat, False)
             torch.autograd.Variable._execution_engine.queue_callback(self._adopt_accumulated_grads)
-        return [None] * len(offs)
+        return self._pass_param_grads(node, flat)
 
     def refresh_weights(self) -> None:
         self.__dict__["_state_tensor_cache"] = None
@@ -211,7 +246,7 @@ class NativeStateMixin:
     # without native state and builds its own on first use, so two objects never own -- and free -- the same handle.
     _NATIVE_RESET = ("_h", "_h_key", "_wkey", "_packed", "_ws")
     _NATIVE_DROP = ("_state_tensor_cache", "_ws_pool", "_bwd_scratch", "_grad_acc", "_grad_task", "_gv_layout", "last_flat_grad",
-                    "_ws_bytes", "_op_key")
+                    "_ws_bytes", "_op_key", "_grad_views", "_ddp_wrappers")
 
     def __getstate__(self):
         state = self.__dict__.copy()
